@@ -7,6 +7,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 MAX_SCORERS = 8
 MAX_ENDPOINT_COLS = 4
+MAX_TOPK = 8
 
 SCORER = {"queue": 0, "kv": 1, "prefix": 2, "lora": 3, "running": 4, "latency": 5, "token_load": 6,
           "col0": 8, "col1": 9, "col2": 10, "col3": 11, "pair0": 16, "pair1": 17}
@@ -66,6 +67,10 @@ class Batch(C.Structure):
                 ("filter_mask_out", C.c_void_p)]
 
 
+class TopK(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("k", C.c_int32), ("endpoints", C.c_void_p), ("scores", C.c_void_p)]
+
+
 class Stats(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("M", C.c_int32), ("epoch", C.c_uint64), ("kernel_launches", C.c_uint64),
                 ("prefix_hashes", C.c_int64), ("prefix_live_hashes", C.c_int64), ("prefix_capacity", C.c_int64),
@@ -88,6 +93,7 @@ ABI_SYMBOLS = [
     ("eppscore_latency_params_default", None, [C.POINTER(LatencyParams)]),
     ("eppscore_set_latency_params", C.c_int32, [_P, C.POINTER(LatencyParams)]),
     ("eppscore_schedule_batch", C.c_int32, [_P, C.POINTER(Batch)]),
+    ("eppscore_schedule_batch_topk", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
     ("eppscore_hash_prompts", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     ("eppscore_count_fields", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
     ("eppscore_hash_prompts_host", C.c_int32, [C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32]),

@@ -14,9 +14,9 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libeppscore.so")
 SOURCES = ["capi.cu", "hash_kernel.cu", "prepare_kernel.cu", "score_generic.cu", "score_dense.cu", "pick_sparse.cu",
            "prefix_index.cu", "fields_kernel.cu", "host_path.cu"]
-# score_matrix.cu holds 56 instantiations of one kernel template: compiled as four objects (one (MASKED, DIAG) combination each,
-# -DEPP_MATRIX_PART=k) so that they build in parallel
-PART_SOURCES = [("score_matrix.cu", f"score_matrix_p{k}.o", [f"-DEPP_MATRIX_PART={k}"]) for k in range(4)]
+# score_matrix.cu holds 64 instantiations of one kernel template: compiled as eight objects (one (MASKED, DIAG) combination each,
+# with and without top-k lists, -DEPP_MATRIX_PART=k) so that they build in parallel
+PART_SOURCES = [("score_matrix.cu", f"score_matrix_p{k}.o", [f"-DEPP_MATRIX_PART={k}"]) for k in range(8)]
 # host-only C++ compiled by g++ directly (AVX-512 intrinsics: kept away from nvcc's front end); the ISA flags apply to this
 # file alone and its one entry point is only called after a run-time CPU check (host_path.cu)
 CPP_SOURCES = [("host_hash_simd.cpp", ["-mavx512f", "-mavx512dq"])]

@@ -93,10 +93,11 @@ struct eppscore_engine {
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
-        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask;
+        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s;
     void release() {
       DevBuf* all[] = {&s_prompts, &s_off, &s_len, &s_seed, &s_hashes, &s_nh, &s_adapter, &s_mask, &s_dense, &s_dtotal, &s_pick,
-                       &s_score, &s_tie, &s_match, &s_total, &s_scores, &s_intok, &s_tslo, &s_pslo, &s_pred, &s_fields, &s_fmask};
+                       &s_score, &s_tie, &s_match, &s_total, &s_scores, &s_intok, &s_tslo, &s_pslo, &s_pred, &s_fields, &s_fmask,
+                       &s_topk_m, &s_topk_s};
       for (DevBuf* b : all) b->release();
     }
   } sc[4];
@@ -251,6 +252,9 @@ struct DevBatch {  // all device pointers
   uint16_t* total_blocks;
   uint64_t* hashes_out;
   double* scores_out;
+  int32_t topk;          // > 0: topk_m / topk_score [R*topk] are written
+  int32_t* topk_m;
+  double* topk_score;
 };
 
 // The hot path on device-resident buffers: [hash kernel] + score/pick kernel, asynchronous on `s`.
@@ -305,6 +309,9 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   a.match_out = b.match_blocks;
   a.total_out = b.total_blocks;
   a.scores_out = b.scores_out;
+  a.topk = b.topk;
+  a.topk_m = b.topk_m;
+  a.topk_score = b.topk_score;
   if (dense && e->cfg.pick_mode != EPPSCORE_PICK_MAX_SCORE)
     return fail(e, EPPSCORE_ERR_INVALID, "the stochastic pickers are not available on dense feature rows");
   if (cfg_has(e->cfg, EPPSCORE_SCORER_LATENCY)) {
@@ -828,13 +835,24 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   return EPPSCORE_OK;
 }
 
-int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
+}  // extern "C"
+
+namespace {
+
+// eppscore_schedule_batch(_topk): t == nullptr ⇒ no top-k lists
+int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t) {
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  if (t) {
+    if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
+    if (t->k < 1 || t->k > EPPSCORE_MAX_TOPK) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
+    if (!t->endpoints || !t->scores) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
+  }
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
   int32_t rc = EPPSCORE_OK;
+  const int32_t tk = t ? t->k : 0;
   DevBatch d{};
   d.R = b->R;
   d.request_base = b->request_base;
@@ -864,6 +882,9 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
     d.total_blocks = b->total_blocks;
     d.hashes_out = b->hashes_out;
     d.scores_out = b->scores_out;
+    d.topk = tk;
+    d.topk_m = t ? t->endpoints : nullptr;
+    d.topk_score = t ? t->scores : nullptr;
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
     // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here)
     const bool sliceable = d.prompt_bytes && !d.hashes_in && !d.cand_mask && !d.dense_feat && !d.pred_out && !d.filter_mask_out &&
@@ -894,6 +915,10 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
       q.pick = d.pick + base;
       q.pick_score = d.pick_score + base;
       q.tie_count = d.tie_count + base;
+      if (tk) {
+        q.topk_m = d.topk_m + (size_t)base * tk;
+        q.topk_score = d.topk_score + (size_t)base * tk;
+      }
       if (d.total_blocks) q.total_blocks = d.total_blocks + base;
       if (d.hashes_out) q.hashes_out = d.hashes_out + (size_t)base * mbk;
       const int si = c % S;
@@ -930,9 +955,10 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
   if (diag || b->R < 2 * chunk) chunk = b->R;
   const int nstreams = chunk < b->R ? 2 : 1;
   if (nstreams == 2 && !e->stream2) CK(e, cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
-  // pinned staging: pick i32 | score f64 | tie i32 | total u16, each [R]
-  const size_t RR = (size_t)b->R;
-  const size_t o_score = (RR * 4 + 7) & ~(size_t)7, o_tie = o_score + RR * 8, o_total = o_tie + RR * 4, res_bytes = o_total + RR * 2;
+  // pinned staging: pick i32 | score f64 | tie i32 | total u16, each [R]; top-k endpoints i32 | scores f64, each [R*k]
+  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk;
+  const size_t o_score = (RR * 4 + 7) & ~(size_t)7, o_tie = o_score + RR * 8, o_total = o_tie + RR * 4;
+  const size_t o_tkm = (o_total + RR * 2 + 7) & ~(size_t)7, o_tks = (o_tkm + RK * 4 + 7) & ~(size_t)7, res_bytes = o_tks + RK * 8;
   if (e->h_res_bytes < res_bytes) {
     if (e->h_res) cudaFreeHost(e->h_res);
     e->h_res = nullptr;
@@ -945,6 +971,8 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
   double* hp_score = reinterpret_cast<double*>(hres + o_score);
   int32_t* hp_tie = reinterpret_cast<int32_t*>(hres + o_tie);
   uint16_t* hp_total = reinterpret_cast<uint16_t*>(hres + o_total);
+  int32_t* hp_tkm = reinterpret_cast<int32_t*>(hres + o_tkm);
+  double* hp_tks = reinterpret_cast<double*>(hres + o_tks);
   int ci = 0;
   for (int32_t r0 = 0; r0 < b->R; r0 += chunk, ci++) {
     const int32_t r1 = std::min(b->R, r0 + chunk);
@@ -999,6 +1027,13 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
     d.pick = sc.s_pick.as<int32_t>();
     d.pick_score = sc.s_score.as<double>();
     d.tie_count = sc.s_tie.as<int32_t>();
+    if (tk) {  // [R*k]: small, like the picks (the chunks keep overlapping)
+      CK(e, sc.s_topk_m.reserve(R * tk * 4));
+      CK(e, sc.s_topk_s.reserve(R * tk * 8));
+      d.topk = tk;
+      d.topk_m = sc.s_topk_m.as<int32_t>();
+      d.topk_score = sc.s_topk_s.as<double>();
+    }
     if (b->match_blocks) {
       CK(e, sc.s_match.reserve(R * M * 2));
       d.match_blocks = sc.s_match.as<uint16_t>();
@@ -1032,6 +1067,10 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
     if (b->pick) CK(e, cudaMemcpyAsync(hp_pick + r0, d.pick, R * 4, cudaMemcpyDeviceToHost, st));
     if (b->pick_score) CK(e, cudaMemcpyAsync(hp_score + r0, d.pick_score, R * 8, cudaMemcpyDeviceToHost, st));
     if (b->tie_count) CK(e, cudaMemcpyAsync(hp_tie + r0, d.tie_count, R * 4, cudaMemcpyDeviceToHost, st));
+    if (tk) {
+      CK(e, cudaMemcpyAsync(hp_tkm + (size_t)r0 * tk, d.topk_m, R * tk * 4, cudaMemcpyDeviceToHost, st));
+      CK(e, cudaMemcpyAsync(hp_tks + (size_t)r0 * tk, d.topk_score, R * tk * 8, cudaMemcpyDeviceToHost, st));
+    }
     if (b->match_blocks) CK(e, cudaMemcpyAsync(b->match_blocks + (size_t)r0 * M, d.match_blocks, R * M * 2, cudaMemcpyDeviceToHost, st));
     if (b->total_blocks) CK(e, cudaMemcpyAsync(hp_total + r0, d.total_blocks, R * 2, cudaMemcpyDeviceToHost, st));
     if (b->scores_out) CK(e, cudaMemcpyAsync(b->scores_out + (size_t)r0 * M, d.scores_out, R * M * 8, cudaMemcpyDeviceToHost, st));
@@ -1045,8 +1084,24 @@ int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) {
   if (b->pick_score) memcpy(b->pick_score, hp_score, RR * 8);
   if (b->tie_count) memcpy(b->tie_count, hp_tie, RR * 4);
   if (b->total_blocks) memcpy(b->total_blocks, hp_total, RR * 2);
+  if (tk) {
+    memcpy(t->endpoints, hp_tkm, RK * 4);
+    memcpy(t->scores, hp_tks, RK * 8);
+  }
   e->sched_pending = false;  // everything launched above has completed
   return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_schedule_batch(eppscore_engine* e, const eppscore_batch* b) { return schedule_batch(e, b, nullptr); }
+
+int32_t eppscore_schedule_batch_topk(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!t) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
+  return schedule_batch(e, b, t);
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,

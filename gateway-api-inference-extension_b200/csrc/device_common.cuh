@@ -161,6 +161,10 @@ __device__ __forceinline__ double neg_log(double u) {
   const double lnf = __dmul_rn(__dmul_rn(2.0, z), p);
   return -__dadd_rn(__dmul_rn((double)e, 0.6931471805599453), lnf);
 }
+// A-Res key of a candidate with score > 0 (weightedrandom/picker.go:121-152): U^(1/score) maximal <=> -ln(U)/score minimal
+__device__ __forceinline__ double ares_key(uint32_t prio, int m, double score) {
+  return -__ddiv_rn(neg_log(uniform01(prio, m)), score);
+}
 // arg-max of a key with the pair's weighted score carried along; lowest index on (improbable) key ties
 struct RBest {
   double key, score;
@@ -191,6 +195,106 @@ __device__ __forceinline__ void rbest_warp_reduce(RBest& b) {
     b.score = t ? os : b.score;
     b.m = t ? om : b.m;
     b.n += on;
+  }
+}
+
+// ---- top-k: maxNumOfEndpoints (picker/common.go:39-42) ----
+// Every pick mode is one total order: key descending, then tie descending, then endpoint index ascending.  Its first
+// element is what the arg-max states above pick:
+//   max-score        key = score, tie = tie_mode ? tie_prio : 0                     (best_update / best_merge)
+//   weighted-random  score > 0:  key = ares_key, tie = 2^32 (ahead of any priority)  (rb_pos of rbest_update)
+//                    score <= 0: key = -inf, tie = tie_prio                          (rb_all: the random picker)
+//   random           key = -inf, tie = tie_prio                                      (rb_all)
+// tie and index travel packed in one word, ord = tie << 14 | (16383 - m), so the order is (key, ord) descending
+// (m < 8192 = the largest max_endpoints); ord = 0 is an empty entry, after every endpoint.
+constexpr int kTopKMax = 8;  // EPPSCORE_MAX_TOPK
+constexpr unsigned long long kTopKIdx = 0x3FFF;
+__device__ __forceinline__ double neg_inf() { return __longlong_as_double((long long)0xfff0000000000000ULL); }
+__device__ __forceinline__ void topk_key(int pick_mode, int tie_mode, double score, uint32_t prio, int m, double& key,
+                                         unsigned long long& ord) {
+  unsigned long long tie;
+  if (pick_mode == 0) {
+    key = score;
+    tie = tie_mode ? prio : 0u;
+  } else if (pick_mode == 1 && score > 0.0) {
+    key = ares_key(prio, m, score);
+    tie = 1ULL << 32;
+  } else {
+    key = neg_inf();
+    tie = prio;
+  }
+  ord = (tie << 14) | (kTopKIdx - (unsigned long long)m);
+}
+__device__ __forceinline__ int topk_endpoint(unsigned long long ord) { return ord ? (int)(kTopKIdx - (ord & kTopKIdx)) : -1; }
+__device__ __forceinline__ bool topk_before(double ak, unsigned long long ao, double bk, unsigned long long bo) {
+  return ak > bk || (ak == bk && ao > bo);
+}
+// one lane's best entries, sorted, in registers (every index is a compile-time constant after unrolling)
+struct TopK {
+  double key[kTopKMax], score[kTopKMax];
+  unsigned long long ord[kTopKMax];
+};
+__device__ __forceinline__ void topk_clear(TopK& t) {
+#pragma unroll
+  for (int i = 0; i < kTopKMax; i++) {
+    t.key[i] = neg_inf();
+    t.score[i] = 0.0;
+    t.ord[i] = 0;
+  }
+}
+// keep the k best (k <= kTopKMax, warp-uniform)
+__device__ __forceinline__ void topk_insert(TopK& t, int k, double key, unsigned long long ord, double score) {
+  bool b[kTopKMax];
+#pragma unroll
+  for (int i = 0; i < kTopKMax; i++) b[i] = i < k && topk_before(key, ord, t.key[i], t.ord[i]);
+#pragma unroll
+  for (int i = kTopKMax - 1; i >= 0; i--) {
+    if (!b[i]) continue;
+    if (i > 0 && b[i - 1]) {  // the new entry goes further up: shift
+      t.key[i] = t.key[i - 1];
+      t.ord[i] = t.ord[i - 1];
+      t.score[i] = t.score[i - 1];
+    } else {
+      t.key[i] = key;
+      t.ord[i] = ord;
+      t.score[i] = score;
+    }
+  }
+}
+// k rounds of a warp arg-max over the list heads; the lane that owns the winner (lane = m & 31 in every kernel's endpoint
+// layout) pops its head.  Lane i returns the i-th entry of the warp's order (-1, 0.0 past the last candidate).
+__device__ __forceinline__ void topk_warp_merge(TopK& t, int k, int lane, int& out_m, double& out_score) {
+  out_m = -1;
+  out_score = 0.0;
+  for (int i = 0; i < k; i++) {
+    double bk = t.key[0];
+    unsigned long long bo = t.ord[0];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      const double ok = shfl_xor_f64(bk, o);
+      const unsigned long long oo = __shfl_xor_sync(0xffffffffu, bo, o);
+      if (topk_before(ok, oo, bk, bo)) {
+        bk = ok;
+        bo = oo;
+      }
+    }
+    if (bo == 0) break;  // (warp-uniform) no candidate left
+    const int m = topk_endpoint(bo), owner = m & 31;
+    const double s = shfl_f64(t.score[0], owner);
+    if (lane == i) {
+      out_m = m;
+      out_score = s;
+    }
+    if (lane == owner) {
+#pragma unroll
+      for (int j = 0; j < kTopKMax - 1; j++) {
+        t.key[j] = t.key[j + 1];
+        t.ord[j] = t.ord[j + 1];
+        t.score[j] = t.score[j + 1];
+      }
+      t.key[kTopKMax - 1] = neg_inf();
+      t.ord[kTopKMax - 1] = 0;
+    }
   }
 }
 

@@ -158,6 +158,9 @@ struct ScoreArgs {
   uint16_t* match_out;          // [R][M] or null
   uint16_t* total_out;          // [R] or null
   double* scores_out;           // [R][M] or null (diagnostics)
+  int32_t topk;                 // > 0: the first topk entries of each request's pick order (full-matrix / generic dense kernels)
+  int32_t* topk_m;              // [R][topk]
+  double* topk_score;           // [R][topk]
   LatArgs lat;
   // device-side filters of the latency profile (run before the scorers, on top of cand_mask): kind 1 prefix-cache-affinity
   // {threshold, explorationProbability, maxTTFTPenaltyMs}, kind 2 slo-headroom-tier {epsilonExploreNeg}

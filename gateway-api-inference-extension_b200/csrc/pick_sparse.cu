@@ -472,7 +472,7 @@ static int launch_sparse_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
 // Returns the number of launches: the sparse kernel plus the full-matrix kernel restricted to the requests it deferred.
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
   if (a.R <= 0) return 0;
-  if (!a.plan.sparse_ok || !a.summ || !a.tiemask || a.cand_mask || a.dense || a.match_out || a.scores_out) return 0;
+  if (!a.plan.sparse_ok || !a.summ || !a.tiemask || a.cand_mask || a.dense || a.match_out || a.scores_out || a.topk > 0) return 0;
   if (a.geo.Mpad > 65536) return 0;  // inline members are uint16
   int launched;
   switch (a.geo.J) {

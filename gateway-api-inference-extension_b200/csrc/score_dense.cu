@@ -150,7 +150,7 @@ constexpr uint32_t seq_of(int k, Rest... rest) {
 #define X STEP_PAIR
 // Unmasked batches without per-pair diagnostics only; returns 0 when no specialisation matches.
 int launch_score_dense_fast(const ScoreArgs& a, cudaStream_t s, int sm_count) {
-  if (a.R <= 0 || !a.dense || a.cand_mask || a.match_out || a.scores_out) return 0;
+  if (a.R <= 0 || !a.dense || a.cand_mask || a.match_out || a.scores_out || a.topk > 0) return 0;
   switch (a.plan.seq) {
     case seq_of(E): return launch_dense(score_dense_fast_kernel<E>, a, s, sm_count);
     case seq_of(E, P): return launch_dense(score_dense_fast_kernel<E, P>, a, s, sm_count);

@@ -15,7 +15,8 @@ constexpr int kScoreWarps = 8;
 
 // Dense rows: float4 {matchBlocks, lora class, pair0, pair1} per (request, endpoint), streamed with
 // coalesced 128-bit loads (lane l reads endpoint i*32+l); endpoint tile in shared memory.
-template <bool MASKED>
+// TOPK: the first a.topk entries of each request's max-score order are written too.
+template <bool MASKED, bool TOPK = false>
 __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(const __grid_constant__ ScoreArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const Plan& plan = a.plan;
@@ -81,6 +82,8 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
     }
     const uint32_t areq = tie_areq(a.request_base + r, plan.seed_lo);
     Best best = best_none();
+    TopK tk;
+    if (TOPK) topk_clear(tk);
     const float4* row = a.dense + (size_t)r * M;
 #pragma unroll 4
     for (int i = 0; i < nchunks; i++) {
@@ -125,8 +128,23 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
       }
       if (a.scores_out && m < M) a.scores_out[(size_t)r * M + m] = cand ? acc : nan64();
       if (cand) best_update(best, acc, m, tie_mode, areq, plan.seed_hi);
+      if (TOPK && cand) {
+        double key;
+        unsigned long long ord;
+        topk_key(0, tie_mode, acc, tie_prio(areq, m, plan.seed_hi), m, key, ord);
+        topk_insert(tk, a.topk, key, ord, acc);
+      }
     }
     best_group_reduce<32>(best, tie_mode);
+    if (TOPK) {
+      int tm;
+      double ts;
+      topk_warp_merge(tk, a.topk, lane, tm, ts);
+      if (lane < a.topk) {
+        a.topk_m[(size_t)r * a.topk + lane] = tm;
+        a.topk_score[(size_t)r * a.topk + lane] = ts;
+      }
+    }
     if (lane == 0) {
       a.pick[r] = best.m;
       a.pick_score[r] = best.m >= 0 ? best.score : 0.0;
@@ -157,6 +175,9 @@ int launch_score_pick(const ScoreArgs& a, bool dense, cudaStream_t s, int sm_cou
     const int MP = (a.geo.M + 31) & ~31;
     size_t smem = (size_t)a.plan.n_terms * MP * 8 + (masked ? 2 * (size_t)MP * 8 : 0) +
                   (size_t)kScoreWarps * (kLutMax + 1) * 8;
+    if (a.topk > 0)
+      return masked ? launch_with_smem(score_pick_dense_kernel<true, true>, a, smem, s, sm_count)
+                    : launch_with_smem(score_pick_dense_kernel<false, true>, a, smem, s, sm_count);
     if (masked) return launch_with_smem(score_pick_dense_kernel<true>, a, smem, s, sm_count);
     return launch_with_smem(score_pick_dense_kernel<false>, a, smem, s, sm_count);
   }

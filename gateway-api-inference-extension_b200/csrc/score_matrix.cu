@@ -50,9 +50,11 @@ __device__ __forceinline__ LatPair lat_pair(const double* tp, double tpot_genera
   return o;
 }
 
-// RND: the stochastic pickers (random / weighted-random) are compiled in; always for the runtime-generic SEQ == 0
-template <uint32_t SEQ, bool MASKED, bool DIAG, bool LAT, bool RND = (SEQ == 0)>
-__global__ void __launch_bounds__(kMatrixWarps * 32) score_matrix_kernel(const __grid_constant__ ScoreArgs a) {
+// RND: the stochastic pickers (random / weighted-random) are compiled in; always for the runtime-generic SEQ == 0.
+// TOPK: the first a.topk entries of each request's pick order are written too (runtime-generic SEQ == 0 only).  Those
+// variants ask for one resident CTA per SM, so ptxas keeps the per-lane lists in registers instead of spilling them.
+template <uint32_t SEQ, bool MASKED, bool DIAG, bool LAT, bool RND = (SEQ == 0), bool TOPK = false>
+__global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_kernel(const __grid_constant__ ScoreArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   pdl_wait();  // (no-op unless launched behind pick_sparse / the hash kernels with programmatic dependent launch)
   if (a.only_deferred) {  // the pass behind pick_sparse: normally nothing was deferred — leave before staging anything
@@ -540,6 +542,8 @@ __global__ void __launch_bounds__(kMatrixWarps * 32) score_matrix_kernel(const _
     Best best = best_none();
     RBest rb_pos = rbest_none(), rb_all = rbest_none();  // stochastic pickers (runtime-generic variants only)
     const int pick_mode = RND ? plan.pick_mode : 0;
+    TopK tk;
+    if (TOPK) topk_clear(tk);
 
     // ---------------- Score (scheduler_profile.go:151-174) + Pick (maxscore/picker.go:87-115) ----------------
     // per-step constants hoisted out of the pair loop (compile-time step index when SEQ != 0)
@@ -664,10 +668,16 @@ __global__ void __launch_bounds__(kMatrixWarps * 32) score_matrix_kernel(const _
           if (cand) {  // random: highest priority wins; weighted-random (A-Res): smallest -ln(U)/score among score > 0
             const uint32_t pr = tie_prio(areq, m, plan.seed_hi);
             rbest_update(rb_all, (double)pr, acc, m);
-            if (pick_mode == 1 && acc > 0.0) rbest_update(rb_pos, -__ddiv_rn(neg_log(uniform01(pr, m)), acc), acc, m);
+            if (pick_mode == 1 && acc > 0.0) rbest_update(rb_pos, ares_key(pr, m, acc), acc, m);
           }
         } else if (cand) {
           best_update(best, acc, m, tie_mode, areq, plan.seed_hi);
+        }
+        if (TOPK && cand) {
+          double key;
+          unsigned long long ord;
+          topk_key(pick_mode, tie_mode, acc, tie_prio(areq, m, plan.seed_hi), m, key, ord);
+          topk_insert(tk, a.topk, key, ord, acc);
         }
       }
       // re-zero exactly the counters this request touched
@@ -687,6 +697,15 @@ __global__ void __launch_bounds__(kMatrixWarps * 32) score_matrix_kernel(const _
       best.m = w.m;
       best.score = w.score;
       best.cnt = w.n;
+    }
+    if (TOPK) {  // (warp-uniform) the per-lane lists merged into the request's first a.topk entries, lane i writes entry i
+      int tm;
+      double ts;
+      topk_warp_merge(tk, a.topk, lane, tm, ts);
+      if (lane < a.topk) {
+        a.topk_m[(size_t)r * a.topk + lane] = tm;
+        a.topk_score[(size_t)r * a.topk + lane] = ts;
+      }
     }
     if (lane == 0) {
       a.pick[r] = best.m;
@@ -755,6 +774,14 @@ static int launch_matrix_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
                  : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false>, a, MASKED, false, s, sm_count);
   }
 }
+// top-k lists: the runtime-generic variants only, every pick mode
+template <bool MASKED, bool DIAG>
+static int launch_matrix_topk(const ScoreArgs& a, cudaStream_t s, int sm_count) {
+  bool lat = false;
+  for (int i = 0; i < a.plan.n_steps; i++) lat = lat || a.plan.kind[i] == STEP_LATENCY;
+  return lat ? launch_matrix(score_matrix_kernel<0, MASKED, DIAG, true, true, true>, a, MASKED, true, s, sm_count)
+             : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false, true, true>, a, MASKED, false, s, sm_count);
+}
 #undef MK
 #undef MKL
 #undef MKR
@@ -764,9 +791,9 @@ static int launch_matrix_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
 #undef L
 #undef Q
 
-// The file is compiled four times (build.py: -DEPP_MATRIX_PART=0..3), one (MASKED, DIAG) combination of the kernel per object,
-// so the 56 instantiations build in parallel (one translation unit took over three minutes); without the macro everything
-// lands in one object.  The kernels are the same instantiations either way.
+// The file is compiled eight times (build.py: -DEPP_MATRIX_PART=0..7), one (MASKED, DIAG) combination of the kernel per object
+// and the top-k variants apart (parts 4..7), so the 64 instantiations build in parallel (one translation unit took over three
+// minutes); without the macro everything lands in one object.  The kernels are the same instantiations either way.
 #ifndef EPP_MATRIX_PART
 #define EPP_MATRIX_PART -1
 #endif
@@ -774,6 +801,10 @@ int launch_matrix_part0(const ScoreArgs& a, cudaStream_t s, int sm_count);  // u
 int launch_matrix_part1(const ScoreArgs& a, cudaStream_t s, int sm_count);  // unmasked, diagnostics outputs
 int launch_matrix_part2(const ScoreArgs& a, cudaStream_t s, int sm_count);  // masked
 int launch_matrix_part3(const ScoreArgs& a, cudaStream_t s, int sm_count);  // masked, diagnostics outputs
+int launch_matrix_part4(const ScoreArgs& a, cudaStream_t s, int sm_count);  // parts 0..3 with top-k lists
+int launch_matrix_part5(const ScoreArgs& a, cudaStream_t s, int sm_count);
+int launch_matrix_part6(const ScoreArgs& a, cudaStream_t s, int sm_count);
+int launch_matrix_part7(const ScoreArgs& a, cudaStream_t s, int sm_count);
 #if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 0
 int launch_matrix_part0(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_seq<false, false>(a, s, sm_count); }
 #endif
@@ -786,12 +817,27 @@ int launch_matrix_part2(const ScoreArgs& a, cudaStream_t s, int sm_count) { retu
 #if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 3
 int launch_matrix_part3(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_seq<true, true>(a, s, sm_count); }
 #endif
+#if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 4
+int launch_matrix_part4(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_topk<false, false>(a, s, sm_count); }
+#endif
+#if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 5
+int launch_matrix_part5(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_topk<false, true>(a, s, sm_count); }
+#endif
+#if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 6
+int launch_matrix_part6(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_topk<true, false>(a, s, sm_count); }
+#endif
+#if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 7
+int launch_matrix_part7(const ScoreArgs& a, cudaStream_t s, int sm_count) { return launch_matrix_topk<true, true>(a, s, sm_count); }
+#endif
 
 #if EPP_MATRIX_PART == -1 || EPP_MATRIX_PART == 0
 // every (request, endpoint) pair scored; any plan without pair columns
 int launch_score_matrix(const ScoreArgs& a, cudaStream_t s, int sm_count) {
   if (a.R <= 0) return 0;
   const bool diag = a.match_out != nullptr || a.scores_out != nullptr || a.lat.pred_out != nullptr;  // diagnostics variants keep the R x M stores out of the hot loop
+  if (a.topk > 0)
+    return a.cand_mask ? (diag ? launch_matrix_part7(a, s, sm_count) : launch_matrix_part6(a, s, sm_count))
+                       : (diag ? launch_matrix_part5(a, s, sm_count) : launch_matrix_part4(a, s, sm_count));
   if (a.cand_mask) return diag ? launch_matrix_part3(a, s, sm_count) : launch_matrix_part2(a, s, sm_count);
   return diag ? launch_matrix_part1(a, s, sm_count) : launch_matrix_part0(a, s, sm_count);
 }

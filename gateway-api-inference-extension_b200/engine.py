@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 
 from . import _capi as capi
-from ._capi import Batch, Config, EppscoreError, LatencyParams, SCORER, Snapshot, Stats
+from ._capi import Batch, Config, EppscoreError, LatencyParams, SCORER, Snapshot, Stats, TopK
 
 
 def default_config(scorers=None, filters=(), **kw) -> Config:
@@ -159,11 +159,13 @@ class Engine:
                  n_hashes_in=None, hash_stride=0, adapter_id=None, cand_mask=None, dense_feat=None, dense_total=None,
                  block_chars=0, max_blocks=0, request_base=0, want_match=False, want_total=True, want_hashes=False,
                  want_scores=False, input_tokens=None, ttft_slo=None, tpot_slo=None, want_pred=False, want_filter_mask=False,
-                 device=False, stream=None, out=None):
+                 topk=0, device=False, stream=None, out=None):
         """Host mode (device=False): numpy in, returns dict of numpy outputs (copies inside the call).
         Device mode: CUDA tensors / raw pointers in; `out` must hold preallocated CUDA tensors
         (pick int32[R], pick_score float64[R], tie_count int32[R], optional match_blocks/total_blocks/hashes_out);
-        the call is asynchronous on `stream`."""
+        the call is asynchronous on `stream`.
+        topk=k (1..8): also the first k endpoints of every request's pick order (maxNumOfEndpoints, eppscore_topk):
+        topk_pick int32[R, k] (-1 padded) and topk_score float64[R, k]; in device mode `out` holds them."""
         a = _Args(device)
         b = Batch()
         b.struct_size = C.sizeof(Batch)
@@ -201,7 +203,11 @@ class Engine:
             b.scores_out = a.ptr(out.get("scores_out"), None)
             b.pred_out = a.ptr(out.get("pred_out"), None)
             b.filter_mask_out = a.ptr(out.get("filter_mask_out"), None)
-            self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
+            if topk:
+                t = self._topk(topk, a.ptr(out["topk_pick"], None), a.ptr(out["topk_score"], None))
+                self._check(self._lib.eppscore_schedule_batch_topk(self._h, C.byref(b), C.byref(t)))
+            else:
+                self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
             return out
         M = self.M
         mb = max_blocks or self.cfg.max_blocks
@@ -220,8 +226,23 @@ class Engine:
             res["filter_mask_out"] = np.zeros((R, max((M + 31) // 32, 1)), np.uint32)
         for k, v in res.items():
             setattr(b, k, v.ctypes.data)
-        self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
+        if topk:
+            res["topk_pick"] = np.full((R, topk), -1, np.int32)
+            res["topk_score"] = np.zeros((R, topk), np.float64)
+            t = self._topk(topk, res["topk_pick"].ctypes.data, res["topk_score"].ctypes.data)
+            self._check(self._lib.eppscore_schedule_batch_topk(self._h, C.byref(b), C.byref(t)))
+        else:
+            self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
         return res
+
+    @staticmethod
+    def _topk(k, endpoints, scores) -> TopK:
+        t = TopK()
+        t.struct_size = C.sizeof(TopK)
+        t.k = k
+        t.endpoints = endpoints
+        t.scores = scores
+        return t
 
     def hash_prompts(self, prompt_bytes, prompt_off, model_seed=None, prompt_len=None, block_chars=0, max_blocks=0):
         R = len(prompt_off) - 1

@@ -28,7 +28,15 @@
 #include "epp_types.hpp"
 #include "host_eval.hpp"
 
+// eppscore_schedule_batch_topk came after EPPSCORE_ABI_VERSION 3 without changing it, so an engine library of the same
+// version may lack it: the symbol is bound weakly and EngineHasTopK() tells.  Without it, maxNumOfEndpoints > 1 takes the
+// whole score map (max-score only, the route of k > 8); the stochastic pickers refuse k > 1.
+extern "C" int32_t eppscore_schedule_batch_topk(struct eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t)
+    __attribute__((weak));
+
 namespace epp {
+
+inline bool EngineHasTopK() { return &eppscore_schedule_batch_topk != nullptr; }
 
 // ---- plugins (descriptors) ----
 struct Scorer {
@@ -105,7 +113,8 @@ inline DeviceFilter SLOHeadroomTierFilter(double epsilonExploreNeg = 0.01) {
 }
 
 struct MaxScorePicker {
-  int MaxNumOfEndpoints = 1;  // picker.DefaultMaxNumOfEndpoints (picker/common.go:36); > 1: top-k from the engine's score rows
+  int MaxNumOfEndpoints = 1;  // picker.DefaultMaxNumOfEndpoints (picker/common.go:36); 2..8: the engine's top-k lists (every
+                              // mode), > 8: max-score only, from the engine's score rows
   int Mode = EPPSCORE_PICK_MAX_SCORE;
 };
 // weighted-random-picker (A-Res, picker/weightedrandom/picker.go:111-155) and random-picker (picker/random/picker.go:85-101):
@@ -167,8 +176,10 @@ class Scheduler {
     const auto& sc = cfg.Profile.scorers();
     if (sc.size() > EPPSCORE_MAX_SCORERS) throw SchedulingError("too many scorers in profile");
     if (cfg.Profile.picker().MaxNumOfEndpoints < 1) throw SchedulingError("maxNumOfEndpoints must be >= 1");
-    if (cfg.Profile.picker().MaxNumOfEndpoints > 1 && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE)
-      throw SchedulingError("maxNumOfEndpoints > 1 is supported for the max-score picker only");
+    if (cfg.Profile.picker().MaxNumOfEndpoints > EPPSCORE_MAX_TOPK && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE)
+      throw SchedulingError("maxNumOfEndpoints > 8 is supported for the max-score picker only");
+    if (cfg.Profile.picker().MaxNumOfEndpoints > 1 && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE && !EngineHasTopK())
+      throw SchedulingError("maxNumOfEndpoints > 1 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk");
     c.n_scorers = (int32_t)sc.size();
     {  // the small-batch CPU route applies to request-independent profiles only
       std::vector<int32_t> kinds;
@@ -374,12 +385,27 @@ class Scheduler {
     b.total_blocks = last_nh_.data();
     b.hashes_out = want_prefix ? last_hashes_.data() : nullptr;
     const int topk = cfg_.Profile.picker().MaxNumOfEndpoints;
+    const bool engine_topk = topk > 1 && topk <= EPPSCORE_MAX_TOPK && EngineHasTopK();
     std::vector<double> all_scores;
-    if (topk > 1) {  // the whole weightedScorePerEndpoint map, NaN for non-candidates (scheduler_profile.go:155-174)
-      all_scores.resize((size_t)R * Mx);
-      b.scores_out = all_scores.data();
+    std::vector<int32_t> topk_ids;
+    std::vector<double> topk_scores;
+    if (engine_topk) {  // the picker's first k endpoints, ordered on the device (eppscore_topk)
+      topk_ids.resize((size_t)R * topk);
+      topk_scores.resize((size_t)R * topk);
+      eppscore_topk t{};
+      t.struct_size = sizeof(t);
+      t.k = topk;
+      t.endpoints = topk_ids.data();
+      t.scores = topk_scores.data();
+      if (eppscore_schedule_batch_topk(eng_, &b, &t) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_schedule_batch_topk: ") + eppscore_last_error(eng_));
+    } else {
+      if (topk > 1) {  // k > 8, max-score: the whole weightedScorePerEndpoint map, NaN for non-candidates (scheduler_profile.go:155-174)
+        all_scores.resize((size_t)R * Mx);
+        b.scores_out = all_scores.data();
+      }
+      if (eppscore_schedule_batch(eng_, &b) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_schedule_batch: ") + eppscore_last_error(eng_));
     }
-    if (eppscore_schedule_batch(eng_, &b) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_schedule_batch: ") + eppscore_last_error(eng_));
     last_endpoints_ = &endpoints;
     last_ids_ = ids;
     last_rows_ = Mx;
@@ -396,7 +422,19 @@ class Scheduler {
       se.TieCount = ties[r];
       out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints.push_back(se);
       out[r].result.PrimaryProfileName = cfg_.ProfileName;
-      if (topk > 1) {  // picker/maxscore/picker.go:104-106: the next best candidates, descending score
+      if (engine_topk) {  // entries 1..k-1 of the picker's order (entry 0 is the pick); -1 past the last candidate
+        auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
+        for (int i = 1; i < topk; i++) {
+          const int32_t id = topk_ids[(size_t)r * topk + i];
+          if (id < 0) break;
+          if (id >= Mx || pos_of_id[(size_t)id] < 0) throw SchedulingError("engine listed an endpoint that is not in the candidate list");
+          ScoredEndpoint o2;
+          o2.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)id]];
+          o2.Index = pos_of_id[(size_t)id];
+          o2.Score = topk_scores[(size_t)r * topk + i];
+          te.push_back(o2);
+        }
+      } else if (topk > 1) {  // picker/maxscore/picker.go:104-106: the next best candidates, descending score
         auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
         for (const auto& pr : TopK(all_scores.data() + (size_t)r * Mx, Mx, topk)) {  // (id, score), NaN rows skipped
           const int pos = pos_of_id[(size_t)pr.first];

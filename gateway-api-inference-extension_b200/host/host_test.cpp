@@ -7,6 +7,7 @@
 //   TestPrefixPluginCompletion        .../approximateprefix/plugin_test.go:161-227 (via PreRequest)
 //   TestTokenLoadScorer               pkg/epp/framework/plugins/scheduling/scorer/tokenload/token_load_test.go:32-61
 //   TestPickWeightedRandomPicker      pkg/epp/framework/plugins/scheduling/picker/weightedrandom/picker_test.go:30-140
+//   TestPickRandomPicker (top-k)      pkg/epp/framework/plugins/scheduling/picker/random/picker_test.go:40-119
 //   TestScore* (latency-scorer)       pkg/epp/framework/plugins/scheduling/scorer/latency/plugin_test.go:52-208
 #include <cmath>
 #include <cstdio>
@@ -359,6 +360,48 @@ static void TestTopK() {
   CHECK(te[0].Score == 1 - 0.70 && te[1].Score == 1 - 0.75 && te[2].Score == 1 - 0.75);
 }
 
+// weighted-random and random pickers with maxNumOfEndpoints = 3: k distinct candidates per request, entry 0 the pick; the random
+// picker includes each of 5 endpoints with probability 3/5 (random/picker_test.go:40-119, +-5 %)
+static void TestTopKStochastic() {
+  if (!EngineHasTopK()) {
+    std::printf("top-k stochastic pickers: skipped (the engine library has no eppscore_schedule_batch_topk)\n");
+    return;
+  }
+  for (int mode = 0; mode < 2; mode++) {
+    SchedulerConfig c;
+    c.CpuBatchThreshold = g_cpu_threshold;
+    MaxScorePicker pk = mode == 0 ? MaxScorePicker(WeightedRandomPicker{}) : MaxScorePicker(RandomPicker{});
+    pk.MaxNumOfEndpoints = 3;
+    c.Profile.WithScorers({NewWeightedScorer(std::make_shared<KVCacheUtilizationScorer>(), 1)}).WithPicker(pk);
+    c.MaxEndpoints = 8;
+    c.TieSeed = 77;
+    Scheduler s(c);
+    std::vector<Endpoint> eps;
+    for (int i = 0; i < 5; i++) {
+      Metrics m;
+      m.KVCacheUsagePercent = 0.1 * (i + 1);  // scores 0.9 .. 0.5
+      eps.push_back(NewEndpoint("pod" + std::to_string(i + 1), m));
+    }
+    const int n = 4000;
+    std::vector<InferenceRequest> reqs(n, InferenceRequest{"t", "m", "", ""});
+    auto res = s.ScheduleBatch(reqs, eps);
+    int count[5] = {0, 0, 0, 0, 0};
+    for (auto& r : res) {
+      const auto& te = r.result.ProfileResults.at("default").TargetEndpoints;
+      CHECK(r.error.empty() && te.size() == 3);
+      if (te.size() != 3) continue;
+      CHECK(te[0].Index != te[1].Index && te[0].Index != te[2].Index && te[1].Index != te[2].Index);
+      for (const auto& se : te) {
+        CHECK(se.Index >= 0 && se.Index < 5 && se.Score == 1.0 - 0.1 * (se.Index + 1));
+        if (se.Index >= 0 && se.Index < 5) count[se.Index]++;
+      }
+    }
+    if (mode == 1)
+      for (int i = 0; i < 5; i++) CHECK(std::fabs(count[i] / (double)n - 0.6) <= 0.05);
+  }
+  std::printf("top-k stochastic pickers: checked\n");
+}
+
 // the coalescing front over the REAL scheduler: 32 caller threads, batches of up to 64, results handed back to their callers
 static void TestCoalescedSchedule() {
   SchedulerConfig c = DefaultFourScorerConfig();
@@ -401,6 +444,7 @@ int main() {
       TestLatencyScorer();
       TestWeightedRandomPicker();
       TestTopK();
+      TestTopKStochastic();
       std::printf("pass %d (CpuBatchThreshold = %d) done\n", pass, g_cpu_threshold);
     }
     TestCoalescedSchedule();

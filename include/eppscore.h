@@ -222,6 +222,26 @@ typedef struct eppscore_batch {
   uint32_t *filter_mask_out;   /* optional [R*ceil(M/32)]: the candidate set left by the device-side filters — diagnostics */
 } eppscore_batch;
 
+/* maxNumOfEndpoints (picker/common.go:39-42): the first k endpoints of each request's pick order, for
+ * eppscore_schedule_batch_topk.  Both arrays are [R*k], row r = request r, and live where batch.location says.
+ * Entry 0 is pick / pick_score; a request with fewer than k candidates is padded with endpoint -1, score 0.0.
+ * The order of each pick mode, on the weighted scores of the candidates:
+ *   max-score      score descending; then (TIE_SEEDED_RANDOM) tie priority descending; then endpoint ascending
+ *   weighted-random  candidates with score > 0 first, by A-Res key descending, then endpoint ascending; then the
+ *                  candidates with score <= 0 (key 0 in weightedrandom/picker.go:126-129), by priority descending, then
+ *                  endpoint ascending
+ *   random         priority descending, then endpoint ascending
+ * i.e. a shuffle inside each tie class (maxscore/picker.go:91-107), sampling without replacement
+ * (weightedrandom/picker.go:121-152) and the first k of a shuffle (random/picker.go:90-96), drawn from the counter-based
+ * generator of eppscore_pick_mode, so the lists do not depend on how a batch is cut into shards. */
+#define EPPSCORE_MAX_TOPK 8
+typedef struct eppscore_topk {
+  uint32_t struct_size;
+  int32_t k;                   /* 1..EPPSCORE_MAX_TOPK */
+  int32_t *endpoints;          /* [R*k] */
+  double *scores;              /* [R*k] ScoredEndpoint.Score of each entry */
+} eppscore_topk;
+
 typedef struct eppscore_stats {
   uint32_t struct_size;
   int32_t M;
@@ -268,6 +288,9 @@ int32_t eppscore_set_latency_params(struct eppscore_engine *e, const eppscore_la
 
 /* ---- the hot path: Filter(mask) → Score → Pick for R requests ---- */
 int32_t eppscore_schedule_batch(struct eppscore_engine *e, const eppscore_batch *b);
+/* The same, plus the first t->k endpoints of every request's pick order (see eppscore_topk).  These batches run on the
+ * full-matrix kernels.  ERR_INVALID: k outside [1, EPPSCORE_MAX_TOPK], a wrong struct_size or NULL arrays. */
+int32_t eppscore_schedule_batch_topk(struct eppscore_engine *e, const eppscore_batch *b, const eppscore_topk *t);
 
 /* ---- stand-alone stages (same kernels; for parity tests and hosts that only want one stage) ---- */
 /* hashPrompt for R prompts (hashing.go:34-98). hashes_out [R*max_blocks], n_hashes_out [R]. */
