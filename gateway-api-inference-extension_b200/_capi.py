@@ -107,6 +107,11 @@ ABI_SYMBOLS = [
     ("eppscore_prefix_lru_len", C.c_int32, [_P, C.c_int32]),
     ("eppscore_prefix_lru_keys", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_commit_picks_device", C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int64, _P]),
+    ("eppscore_estimate_tokens", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
+    ("eppscore_inflight_add", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P]),
+    ("eppscore_inflight_release", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P]),
+    ("eppscore_inflight_remove_endpoint", C.c_int32, [_P, C.c_int32]),
+    ("eppscore_inflight_get", C.c_int32, [_P, _P, _P, C.c_int32]),
     ("eppscore_host_alloc", _P, [C.c_size_t]),
     ("eppscore_host_free", None, [_P]),
 ]

@@ -89,6 +89,17 @@ struct eppscore_engine {
   bool sched_pending = false;
   DevBuf c_pick, c_hash, c_nh, c_ep, c_op;  // staging for the host-array forms of commit_picks / prefix_add / prefix_apply
 
+  // in-flight load producer (inflightload/producer.go): per-endpoint request and token counters, [Mpad] int64 each, zeroed at
+  // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens; the snapshot terms are then
+  // prepared again (with last_pa) after every counter mutation.  Mutations outside a CUDA-graph capture are ordered through
+  // ev_inflight, recorded after each one on its stream.
+  DevBuf inflight_req, inflight_tok, inflight_err;
+  DevBuf c_iep, c_itok, c_esize, c_ehint, c_echars, c_eout;  // staging for the host-array forms
+  cudaEvent_t ev_inflight = nullptr;
+  bool inflight_pending = false;
+  bool snapshot_has_tokens = false;  // the current snapshot carries inflight_tokens
+  PrepareArgs last_pa{};             // what the current snapshot was prepared with
+
   // scratch for host-location batches and internal hashes: two sets, so the chunks of a host batch can alternate
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
   struct Scratch {
@@ -144,6 +155,11 @@ bool cfg_has(const eppscore_config& c, int kind) {
   for (int i = 0; i < c.n_scorers; i++)
     if (c.scorer_kind[i] == kind) return true;
   return false;
+}
+
+// The token-load scorer reads the in-flight counters: the current snapshot's terms depend on them.
+bool counters_feed_scorer(const eppscore_engine* e) {
+  return e->have_snapshot && !e->snapshot_has_tokens && cfg_has(e->cfg, EPPSCORE_SCORER_TOKEN_LOAD);
 }
 
 // Translate the scorer list into kernel steps.  Leading request-independent scorers are folded into
@@ -222,6 +238,52 @@ int32_t index_begin(eppscore_engine* e) {
 }
 int32_t index_end(eppscore_engine* e) {
   CK(e, cudaEventRecord(e->ev_table, e->stream));
+  return EPPSCORE_OK;
+}
+
+// Prepares the snapshot terms from e->last_pa on `st` and publishes them: ev_snapshot is recorded behind the kernels so that
+// batches on other streams wait for the new terms (schedule_device).  The engine stream waits too, except while `st` is being
+// captured into a CUDA graph: a captured stream may not take dependencies from outside its capture, so inside one
+// ev_snapshot becomes a graph edge that other streams of the same capture join on, and in-stream order does the rest.
+int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st) {
+  e->launches += launch_prepare_snapshot(e->last_pa, st);
+  CK(e, cudaGetLastError());
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  unsigned long long cap_id = 0;
+  cudaStreamGetCaptureInfo(st, &cap, &cap_id);
+  CK(e, cudaEventRecord(e->ev_snapshot, st));
+  e->snapshot_stream = st;
+  if (cap == cudaStreamCaptureStatusNone) {
+    e->snapshot_capture_id = 0;
+    if (st != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_snapshot, 0));
+  } else {
+    e->snapshot_capture_id = cap_id;
+  }
+  return EPPSCORE_OK;
+}
+
+// Counter mutations: each one waits for the previous one (they do not all commute: remove_endpoint sets to zero), unless `st`
+// is being captured, where the caller's graph edges order them.
+int32_t inflight_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  cudaStreamIsCapturing(st, &cap);
+  *capturing = cap != cudaStreamCaptureStatusNone;
+  if (!*capturing && e->inflight_pending) CK(e, cudaStreamWaitEvent(st, e->ev_inflight, 0));
+  return EPPSCORE_OK;
+}
+// After a mutation: when the counters feed the token-load scorer, its term, the folded leading run and the per-adapter
+// summaries of the sparse path all change, so the snapshot is prepared again on the same stream, with eppscore_set_snapshot's
+// ordering (a device-location batch another stream launched against the current terms finishes reading them first).
+int32_t inflight_end(eppscore_engine* e, cudaStream_t st, bool capturing) {
+  if (counters_feed_scorer(e)) {
+    if (!capturing && e->sched_pending) CK(e, cudaStreamWaitEvent(st, e->ev_sched, 0));
+    const int32_t rc = prepare_snapshot(e, st);
+    if (rc != EPPSCORE_OK) return rc;
+  }
+  if (!capturing) {
+    CK(e, cudaEventRecord(e->ev_inflight, st));
+    e->inflight_pending = true;
+  }
   return EPPSCORE_OK;
 }
 
@@ -387,7 +449,8 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   if (launched == 0) launched = launch_score_pick(a, dense, s, e->sm_count);
   e->launches += launched;
   CK(e, cudaGetLastError());
-  if (!capturing && s != e->stream && a.table) {  // a later index mutation (engine stream) must wait for this batch
+  // a later index mutation (engine stream), or a counter mutation that prepares the terms again, must wait for this batch
+  if (!capturing && s != e->stream && (a.table || counters_feed_scorer(e))) {
     CK(e, cudaEventRecord(e->ev_sched, s));
     e->sched_pending = true;
   }
@@ -536,6 +599,14 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   CK(nullptr, ep->raw_max.reserve(mp * 4));
   for (int i = 0; i < 4; i++) CK(nullptr, ep->raw_col[i].reserve(mp * 8));
   CK(nullptr, ep->raw_tokens.reserve(mp * 8));
+  CK(nullptr, ep->inflight_req.reserve(mp * 8));
+  CK(nullptr, ep->inflight_tok.reserve(mp * 8));
+  CK(nullptr, ep->inflight_err.reserve(4));
+  CK(nullptr, cudaMemsetAsync(ep->inflight_req.p, 0, mp * 8, ep->stream));
+  CK(nullptr, cudaMemsetAsync(ep->inflight_tok.p, 0, mp * 8, ep->stream));
+  CK(nullptr, cudaMemsetAsync(ep->inflight_err.p, 0, 4, ep->stream));
+  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_inflight, cudaEventDisableTiming));
+  CK(nullptr, init_inflight_update());
   for (int which = 0; which < 2; which++)  // value buckets for the masked min/max of the queue / running scorers
     if (cfg_has(ep->cfg, which == 0 ? EPPSCORE_SCORER_QUEUE : EPPSCORE_SCORER_RUNNING)) {
       CK(nullptr, ep->qhdr[which].reserve(sizeof(QBucketHdr)));
@@ -596,7 +667,8 @@ void eppscore_destroy(eppscore_engine* e) {
   DevBuf* bufs[] = {&e->qhdr[0], &e->qhdr[1], &e->qbucket[0], &e->qbucket[1], &e->raw_min_tpot, &e->raw_dispatched, &e->raw_prefill, &e->raw_tokens, &e->lat_ep,
                     &e->raw_kv, &e->raw_queue, &e->raw_running, &e->raw_act, &e->raw_wait, &e->raw_nmodels, &e->raw_max,
                     &e->fold_unmasked, &e->fold_masked, &e->cls_lo, &e->cls_hi, &e->summ, &e->tiemask, &e->prefix_lut2d, &e->c_pick, &e->c_hash, &e->c_nh,
-                    &e->c_ep, &e->c_op};
+                    &e->c_ep, &e->c_op, &e->inflight_req, &e->inflight_tok, &e->inflight_err, &e->c_iep, &e->c_itok, &e->c_esize,
+                    &e->c_ehint, &e->c_echars, &e->c_eout};
   for (auto& x : e->sc) x.release();
   for (int i = 0; i < 3; i++) {
     if (e->split_stream[i]) {
@@ -615,6 +687,7 @@ void eppscore_destroy(eppscore_engine* e) {
   for (int i = 0; i < 4; i++) e->raw_col[i].release();
   for (int i = 0; i < kMaxSteps; i++) e->term[i].release();
   e->index.reset();
+  if (e->ev_inflight) cudaEventDestroy(e->ev_inflight);
   if (e->ev_sched) cudaEventDestroy(e->ev_sched);
   if (e->ev_caller) cudaEventDestroy(e->ev_caller);
   if (e->ev_snapshot) cudaEventDestroy(e->ev_snapshot);
@@ -747,7 +820,14 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
     pa.qhdr[which] = e->qhdr[which].as<QBucketHdr>();
     pa.qbucket[which] = e->qbucket[which].as<uint32_t>();
   }
-  pa.tokens = s->inflight_tokens ? (on_device ? s->inflight_tokens : e->raw_tokens.as<int64_t>()) : nullptr;
+  // InFlightLoad.Tokens: the snapshot's array when it carries one, else the in-flight counters (all 0 until the first
+  // eppscore_inflight_add, which scores exactly like an absent attribute, token_load.go:91-98)
+  pa.tokens = s->inflight_tokens ? (on_device ? s->inflight_tokens : e->raw_tokens.as<int64_t>()) : e->inflight_tok.as<int64_t>();
+  if (!s->inflight_tokens && e->inflight_pending) {  // the counters were last changed on another stream
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    cudaStreamIsCapturing(st, &cap);
+    if (cap == cudaStreamCaptureStatusNone) CK(e, cudaStreamWaitEvent(st, e->ev_inflight, 0));
+  }
   pa.token_threshold = e->cfg.token_load_threshold;
   e->lat_args = LatArgs{};
   if (e->lat_ep.p) {
@@ -815,22 +895,13 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   for (int t = 0; t < kMaxSteps; t++) pa.plan_term[t] = e->plan_unmasked.term_ptr[t];
   pa.summ = e->plan_unmasked.plan.sparse_ok ? e->summ.as<AdapterSummary>() : nullptr;
   pa.tiemask = e->tiemask.as<uint32_t>();
-  e->launches += launch_prepare_snapshot(pa, st);
-  CK(e, cudaGetLastError());
-  // Cross-stream ordering through an event — skipped while the caller's stream is being captured into a
-  // CUDA graph (a captured stream may not take dependencies from outside its capture; in-stream order suffices).
+  e->snapshot_has_tokens = s->inflight_tokens != nullptr;
+  e->last_pa = pa;
+  int32_t rc = prepare_snapshot(e, st);
+  if (rc != EPPSCORE_OK) return rc;
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  unsigned long long cap_id = 0;
-  cudaStreamGetCaptureInfo(st, &cap, &cap_id);
-  CK(e, cudaEventRecord(e->ev_snapshot, st));  // inside a capture this becomes a graph edge other captured streams can join on
-  e->snapshot_stream = st;
-  if (cap == cudaStreamCaptureStatusNone) {
-    e->snapshot_capture_id = 0;
-    if (st != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_snapshot, 0));
-    if (!on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
-  } else {
-    e->snapshot_capture_id = cap_id;
-  }
+  cudaStreamIsCapturing(st, &cap);
+  if (cap == cudaStreamCaptureStatusNone && !on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
   e->have_snapshot = true;
   return EPPSCORE_OK;
 }
@@ -1358,6 +1429,100 @@ int32_t eppscore_prefix_get(eppscore_engine* e, uint64_t hash, uint32_t* bitset_
   int32_t count = 0;
   CK(e, e->index->get(hash, bitset_out, bitset_out ? words : 0, &count, e->stream));
   return count;
+}
+
+// ---------------- in-flight load producer ----------------
+int32_t eppscore_estimate_tokens(eppscore_engine* e, int32_t R, int32_t location, const int64_t* request_size_bytes,
+                                 const int32_t* token_hint, const int32_t* prompt_chars, int64_t* out, void* stream) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (R < 0 || (R > 0 && !out)) return fail(e, EPPSCORE_ERR_INVALID, "estimate_tokens: R < 0 or out NULL");
+  if (R == 0) return EPPSCORE_OK;
+  CK(e, cudaSetDevice(e->device));
+  if (location == 1) {
+    e->launches += launch_estimate_tokens(request_size_bytes, token_hint, prompt_chars, R, out, stream ? (cudaStream_t)stream : e->stream);
+    CK(e, cudaGetLastError());
+    return EPPSCORE_OK;
+  }
+  const int64_t* d_size = nullptr;
+  const int32_t *d_hint = nullptr, *d_chars = nullptr;
+  int32_t rc;
+  if ((rc = h2d(e, e->c_esize, request_size_bytes, (size_t)R, &d_size)) != EPPSCORE_OK) return rc;
+  if ((rc = h2d(e, e->c_ehint, token_hint, (size_t)R, &d_hint)) != EPPSCORE_OK) return rc;
+  if ((rc = h2d(e, e->c_echars, prompt_chars, (size_t)R, &d_chars)) != EPPSCORE_OK) return rc;
+  CK(e, e->c_eout.reserve((size_t)R * 8));
+  e->launches += launch_estimate_tokens(d_size, d_hint, d_chars, R, e->c_eout.as<int64_t>(), e->stream);
+  CK(e, cudaGetLastError());
+  CK(e, cudaMemcpyAsync(out, e->c_eout.p, (size_t)R * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  return EPPSCORE_OK;
+}
+
+static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const int64_t* tokens,
+                               void* stream, int sign) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (R < 0 || (R > 0 && !endpoint)) return fail(e, EPPSCORE_ERR_INVALID, "inflight update: R < 0 or endpoint NULL");
+  if (R == 0) return EPPSCORE_OK;
+  CK(e, cudaSetDevice(e->device));
+  const bool on_device = location == 1;
+  cudaStream_t st = (on_device && stream) ? (cudaStream_t)stream : e->stream;
+  const int32_t* d_ep = endpoint;
+  const int64_t* d_tok = tokens;
+  if (!on_device) {
+    for (int32_t r = 0; r < R; r++)
+      if (endpoint[r] >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight update: endpoint >= max_endpoints");
+  }
+  bool capturing = false;
+  int32_t rc = inflight_begin(e, st, &capturing);
+  if (rc != EPPSCORE_OK) return rc;
+  if (!on_device) {
+    if ((rc = h2d(e, e->c_iep, endpoint, (size_t)R, &d_ep)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->c_itok, tokens, (size_t)R, &d_tok)) != EPPSCORE_OK) return rc;
+  }
+  e->launches += launch_inflight_update(d_ep, d_tok, R, e->cfg.max_endpoints, sign, e->inflight_req.as<int64_t>(),
+                                        e->inflight_tok.as<int64_t>(), e->inflight_err.as<uint32_t>(), st);
+  CK(e, cudaGetLastError());
+  if ((rc = inflight_end(e, st, capturing)) != EPPSCORE_OK) return rc;
+  if (!on_device) CK(e, cudaStreamSynchronize(st));  // the caller's host arrays may be reused
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_inflight_add(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const int64_t* tokens,
+                              void* stream) {
+  return inflight_update(e, R, location, endpoint, tokens, stream, 1);
+}
+
+int32_t eppscore_inflight_release(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const int64_t* tokens,
+                                  void* stream) {
+  return inflight_update(e, R, location, endpoint, tokens, stream, -1);
+}
+
+int32_t eppscore_inflight_remove_endpoint(eppscore_engine* e, int32_t endpoint) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (endpoint < 0 || endpoint >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight_remove_endpoint: endpoint out of range");
+  CK(e, cudaSetDevice(e->device));
+  bool capturing = false;
+  int32_t rc = inflight_begin(e, e->stream, &capturing);
+  if (rc != EPPSCORE_OK) return rc;
+  CK(e, cudaMemsetAsync(e->inflight_req.as<int64_t>() + endpoint, 0, 8, e->stream));
+  CK(e, cudaMemsetAsync(e->inflight_tok.as<int64_t>() + endpoint, 0, 8, e->stream));
+  return inflight_end(e, e->stream, capturing);
+}
+
+int32_t eppscore_inflight_get(eppscore_engine* e, int64_t* requests_out, int64_t* tokens_out, int32_t M) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (M < 0 || M > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight_get: M outside [0, max_endpoints]");
+  CK(e, cudaSetDevice(e->device));
+  if (e->inflight_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_inflight, 0));
+  uint32_t err = 0;
+  if (M > 0 && requests_out) CK(e, cudaMemcpyAsync(requests_out, e->inflight_req.p, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (M > 0 && tokens_out) CK(e, cudaMemcpyAsync(tokens_out, e->inflight_tok.p, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaMemcpyAsync(&err, e->inflight_err.p, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  if (err) {
+    CK(e, cudaMemsetAsync(e->inflight_err.p, 0, 4, e->stream));
+    return fail(e, EPPSCORE_ERR_INVALID, "an inflight update on device arrays named an endpoint >= max_endpoints (those entries were skipped)");
+  }
+  return EPPSCORE_OK;
 }
 
 void* eppscore_host_alloc(size_t bytes) {

@@ -241,5 +241,12 @@ int launch_score_pick(const ScoreArgs& a, bool dense, cudaStream_t s, int sm_cou
 int launch_score_matrix(const ScoreArgs& a, cudaStream_t s, int sm_count);             // every pair scored (masks, diagnostics)
 int launch_score_dense_fast(const ScoreArgs& a, cudaStream_t s, int sm_count);         // 0 if no specialisation applies
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count);              // 0 if not applicable
+// in-flight load producer (inflight_kernel.cu): requests[m] += sign * #{r : endpoint[r] == m}, token_sum[m] += sign * Σ tokens[r];
+// endpoint < 0 is skipped, endpoint >= n_ep (<= 8192) is skipped and sets *err.  init_* opts the kernel into the 16 bytes of
+// shared memory per endpoint it needs (once per device).
+cudaError_t init_inflight_update();
+int launch_inflight_update(const int32_t* endpoint, const int64_t* tokens, int R, int n_ep, int sign, int64_t* requests,
+                           int64_t* token_sum, uint32_t* err, cudaStream_t s);
+int launch_estimate_tokens(const int64_t* size, const int32_t* hint, const int32_t* chars, int R, int64_t* out, cudaStream_t s);
 
 }  // namespace eppscore

@@ -280,6 +280,45 @@ class Engine:
                                                     a.ptr(prompt_len, np.int32), out.ctypes.data, None))
         return out[:R]
 
+    # ------------------------------------------------------------------ in-flight load producer
+    def estimate_tokens(self, R, request_size_bytes=None, token_hint=None, prompt_chars=None, device=False, stream=None, out=None):
+        """SimpleTokenEstimator.Estimate per request (eppscore_estimate_tokens): int64[R].  Host mode: numpy in, numpy out.
+        Device mode: CUDA tensors / raw pointers in, `out` an int64[R] CUDA tensor, asynchronous on `stream`."""
+        a = _Args(device)
+        if device:
+            if out is None:
+                raise ValueError("device mode needs a preallocated out")
+            o_ptr = a.ptr(out, None)
+        else:
+            out = np.zeros(max(R, 1), np.int64)
+            o_ptr = out.ctypes.data
+        self._check(self._lib.eppscore_estimate_tokens(self._h, R, 1 if device else 0, a.ptr(request_size_bytes, np.int64),
+                                                       a.ptr(token_hint, np.int32), a.ptr(prompt_chars, np.int32), o_ptr, stream))
+        return out if device else out[:R]
+
+    def _inflight(self, fn, endpoint, tokens, device, stream):
+        a = _Args(device)
+        R = int(endpoint.shape[0]) if hasattr(endpoint, "shape") else len(endpoint)
+        self._check(fn(self._h, R, 1 if device else 0, a.ptr(endpoint, np.int32), a.ptr(tokens, np.int64), stream))
+
+    def inflight_add(self, endpoint, tokens=None, device=False, stream=None):
+        """PreRequest for a batch: requests[endpoint[r]] += 1, tokens[endpoint[r]] += tokens[r] (endpoint -1: skipped)."""
+        self._inflight(self._lib.eppscore_inflight_add, endpoint, tokens, device, stream)
+
+    def inflight_release(self, endpoint, tokens=None, device=False, stream=None):
+        """ResponseBody at end of stream: the reverse of inflight_add with the same estimates."""
+        self._inflight(self._lib.eppscore_inflight_release, endpoint, tokens, device, stream)
+
+    def inflight_remove_endpoint(self, endpoint):
+        self._check(self._lib.eppscore_inflight_remove_endpoint(self._h, endpoint))
+
+    def inflight_get(self, M=None):
+        """(requests int64[M], tokens int64[M]): the counters after every earlier update; M defaults to max_endpoints."""
+        M = self.cfg.max_endpoints if M is None else M
+        req, tok = np.zeros(max(M, 1), np.int64), np.zeros(max(M, 1), np.int64)
+        self._check(self._lib.eppscore_inflight_get(self._h, req.ctypes.data, tok.ctypes.data, M))
+        return req[:M], tok[:M]
+
     @staticmethod
     def model_seed(model, salt=b"") -> int:
         if isinstance(model, str):

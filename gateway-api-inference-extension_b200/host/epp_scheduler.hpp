@@ -16,6 +16,7 @@
 // itself happens in the CUDA kernels.  Filters run on the host exactly like the reference's filter chain and
 // become the per-request candidate mask.  One Scheduler owns one engine (one GPU).
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <map>
 #include <memory>
@@ -34,9 +35,25 @@
 extern "C" int32_t eppscore_schedule_batch_topk(struct eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t)
     __attribute__((weak));
 
+// The in-flight load producer's entry points came the same way: bound weakly, EngineHasInFlightLoad() tells.
+extern "C" int32_t eppscore_estimate_tokens(struct eppscore_engine* e, int32_t R, int32_t location, const int64_t* request_size_bytes,
+                                            const int32_t* token_hint, const int32_t* prompt_chars, int64_t* out, void* stream)
+    __attribute__((weak));
+extern "C" int32_t eppscore_inflight_add(struct eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint,
+                                         const int64_t* tokens, void* stream) __attribute__((weak));
+extern "C" int32_t eppscore_inflight_release(struct eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint,
+                                             const int64_t* tokens, void* stream) __attribute__((weak));
+extern "C" int32_t eppscore_inflight_remove_endpoint(struct eppscore_engine* e, int32_t endpoint) __attribute__((weak));
+extern "C" int32_t eppscore_inflight_get(struct eppscore_engine* e, int64_t* requests_out, int64_t* tokens_out, int32_t M)
+    __attribute__((weak));
+
 namespace epp {
 
 inline bool EngineHasTopK() { return &eppscore_schedule_batch_topk != nullptr; }
+inline bool EngineHasInFlightLoad() {
+  return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
+         &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
+}
 
 // ---- plugins (descriptors) ----
 struct Scorer {
@@ -79,6 +96,11 @@ struct PredictedLatencyProducer {
   };
   std::map<std::string, EndpointState> State;  // keyed by NamespacedName.String()
 };
+
+// inflight-load-producer (requestcontrol/dataproducer/inflightload/producer.go): requests and estimated tokens in flight per
+// endpoint, the InFlightLoad attribute the token-load scorer reads.  The counters live on the device (eppscore_inflight_*);
+// the plugin has no parameters (its factory, producer.go:40-47, uses SimpleTokenEstimator's defaults).
+struct InFlightLoadProducer {};
 
 struct WeightedScorer {
   std::shared_ptr<Scorer> Scorer_;
@@ -166,6 +188,10 @@ struct SchedulerConfig {
   // scorers, no device filters, max-score picker, lowest-index ties) are evaluated on the host (SmallBatchCpu): a launch
   // costs tens of microseconds, a 1 x 4 queue-scorer Schedule a fraction of one.  0 disables the route.
   int CpuBatchThreshold = 8;
+  // Opt-in, as the plugin is in the reference's config.  With it, PreRequest also counts each request on its target endpoint,
+  // ResponseComplete releases it, RemovePod drops the endpoint's counters, and a token-load scorer reads the counters
+  // (Endpoint::InFlightTokens is then not used).  Batches always take the engine route: the counters live on the device.
+  std::shared_ptr<InFlightLoadProducer> InFlightLoad;
 };
 
 class Scheduler {
@@ -180,6 +206,9 @@ class Scheduler {
       throw SchedulingError("maxNumOfEndpoints > 8 is supported for the max-score picker only");
     if (cfg.Profile.picker().MaxNumOfEndpoints > 1 && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE && !EngineHasTopK())
       throw SchedulingError("maxNumOfEndpoints > 1 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk");
+    if (cfg.InFlightLoad && !EngineHasInFlightLoad())
+      throw SchedulingError("the inflight-load-producer needs an engine library with eppscore_inflight_add");
+    inflight_ = cfg.InFlightLoad != nullptr;
     c.n_scorers = (int32_t)sc.size();
     {  // the small-batch CPU route applies to request-independent profiles only
       std::vector<int32_t> kinds;
@@ -191,13 +220,16 @@ class Scheduler {
       double thr = 4194304.0;
       for (auto& w : sc)
         if (auto* tl = dynamic_cast<TokenLoadScorer*>(w.Scorer_.get())) thr = (double)tl->QueueThresholdTokens;
-      cpu_route_ok_ = cfg.CpuBatchThreshold > 0 && cfg.Profile.device_filters().empty() && cfg.Profile.picker().Mode == EPPSCORE_PICK_MAX_SCORE &&
+      cpu_route_ok_ = cfg.CpuBatchThreshold > 0 && !inflight_ && cfg.Profile.device_filters().empty() && cfg.Profile.picker().Mode == EPPSCORE_PICK_MAX_SCORE &&
                       cfg.Profile.picker().MaxNumOfEndpoints == 1 && cfg.TieMode == EPPSCORE_TIE_LOWEST_INDEX && cpu_.Configure(kinds, weights, thr);
     }
     for (size_t i = 0; i < sc.size(); i++) {
       c.scorer_kind[i] = sc[i].Scorer_->Kind;
       c.scorer_weight[i] = sc[i].Weight();
-      if (auto* tl = dynamic_cast<TokenLoadScorer*>(sc[i].Scorer_.get())) c.token_load_threshold = (double)tl->QueueThresholdTokens;
+      if (auto* tl = dynamic_cast<TokenLoadScorer*>(sc[i].Scorer_.get())) {
+        c.token_load_threshold = (double)tl->QueueThresholdTokens;
+        token_load_ = true;
+      }
       if (auto* ls = dynamic_cast<LatencyScorer*>(sc[i].Scorer_.get())) latency_scorer_ = ls;
     }
     if (latency_scorer_ && !cfg.Profile.producer()) throw SchedulingError("latency-scorer needs a predicted-latency-producer");
@@ -357,6 +389,12 @@ class Scheduler {
     }
     off[R] = (int64_t)bytes.size();
     bytes.resize(bytes.size() + 64, 0);
+    if (inflight_) {  // the estimator's inputs, for PreRequest
+      last_size_.resize((size_t)R);
+      last_hint_.resize((size_t)R);
+      last_chars_.resize((size_t)R);
+      for (int r = 0; r < R; r++) EstimateInputs(requests[r], &last_size_[r], &last_hint_[r], &last_chars_[r]);
+    }
     const bool want_prefix = max_blocks > 0 && block_tokens > 0;
     std::vector<int32_t> pick((size_t)R), ties((size_t)R);
     std::vector<double> score((size_t)R);
@@ -452,29 +490,73 @@ class Scheduler {
   }
   uint64_t CpuRoutedRequests() const { return cpu_routed_; }
 
-  // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index.
+  // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index; with the
+  // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
+  // (inflightload/producer.go:101-120).
   void PreRequest(const std::vector<BatchItem>& results) {
-    if (!last_endpoints_ || last_hashes_.empty()) return;
+    if (!last_endpoints_ || (last_hashes_.empty() && !inflight_)) return;
     const int R = (int)results.size();
     std::vector<int32_t> pick((size_t)R, -1);
     for (int r = 0; r < R; r++)
       if (results[r].error.empty()) pick[r] = last_ids_[(size_t)results[r].result.ProfileResults.at(cfg_.ProfileName).TargetEndpoints[0].Index];
-    std::vector<int32_t> cap((size_t)last_rows_, 0);
-    for (size_t m = 0; m < last_endpoints_->size(); m++)  // makeserver, plugin.go:207-216
-      cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks > 0) ? (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks : 0;
-    if (eppscore_commit_picks(eng_, R, pick.data(), last_hashes_.data(), last_nh_.data(), last_stride_, cap.data()) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_commit_picks: ") + eppscore_last_error(eng_));
+    if (!last_hashes_.empty()) {
+      std::vector<int32_t> cap((size_t)last_rows_, 0);
+      for (size_t m = 0; m < last_endpoints_->size(); m++)  // makeserver, plugin.go:207-216
+        cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks > 0) ? (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks : 0;
+      if (eppscore_commit_picks(eng_, R, pick.data(), last_hashes_.data(), last_nh_.data(), last_stride_, cap.data()) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_commit_picks: ") + eppscore_last_error(eng_));
+    }
+    if (inflight_ && (int)last_size_.size() == R) {
+      std::vector<int64_t> est((size_t)R);
+      if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+      if (eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
+    }
+  }
+
+  // ResponseBody at end of stream (inflightload/producer.go:122-169) for a request PreRequest counted, given the result it was
+  // scheduled with (the reference reads it from request.SchedulingResult): its TargetEndpoints[0] gives back one request and the
+  // request's estimate.  Without the producer, or for a server that has left the pool since (its id may already be another
+  // server's), nothing happens.
+  void ResponseComplete(const InferenceRequest& request, const SchedulingResult& result) {
+    if (!inflight_) return;
+    auto pr = result.ProfileResults.find(cfg_.ProfileName);
+    if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
+    const int32_t id = ServerId(pr->second.TargetEndpoints[0].Endpoint_->GetMetadata()->NamespacedName_.String());
+    if (id < 0) return;
+    int64_t size = 0, est = 0;
+    int32_t hint = -1, chars = 0;
+    EstimateInputs(request, &size, &hint, &chars);
+    if (eppscore_estimate_tokens(eng_, 1, 0, &size, &hint, &chars, &est, nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+    if (eppscore_inflight_release(eng_, 1, 0, &id, &est, nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_inflight_release: ") + eppscore_last_error(eng_));
   }
 
   // indexer.RemovePod (indexer.go:167-182), called when a model server leaves the pool: its LRU and its memberships go, its
-  // id is free for the next new server.
+  // id is free for the next new server.  With the inflight-load-producer also DeleteEndpoint (producer.go:181-187), so the next
+  // server to get the id starts from 0.
   void RemovePod(const std::string& namespaced_name) {
     auto it = server_ids_.find(namespaced_name);
     if (it == server_ids_.end()) return;
     if (eppscore_prefix_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
       throw SchedulingError(std::string("eppscore_prefix_remove_endpoint: ") + eppscore_last_error(eng_));
+    if (inflight_ && eppscore_inflight_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_inflight_remove_endpoint: ") + eppscore_last_error(eng_));
     free_ids_.push_back(it->second);
     server_ids_.erase(it);
+  }
+
+  // PrepareRequestData's view (producer.go:90-99) of one server: {requests, tokens} in flight; {0, 0} without the producer or
+  // for a server never seen.
+  std::pair<int64_t, int64_t> InFlightLoad(const std::string& namespaced_name) {
+    const int id = ServerId(namespaced_name);
+    if (!inflight_ || id < 0) return {0, 0};
+    std::vector<int64_t> req((size_t)id + 1), tok((size_t)id + 1);
+    if (eppscore_inflight_get(eng_, req.data(), tok.data(), id + 1) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_inflight_get: ") + eppscore_last_error(eng_));
+    return {req[(size_t)id], tok[(size_t)id]};
   }
   int ServerId(const std::string& namespaced_name) const {  // -1: never seen (or removed)
     auto it = server_ids_.find(namespaced_name);
@@ -486,6 +568,13 @@ class Scheduler {
   eppscore_engine* engine() { return eng_; }
 
  private:
+  // SimpleTokenEstimator's inputs for one request (eppscore_estimate_tokens): the body is always present here
+  static void EstimateInputs(const InferenceRequest& q, int64_t* size, int32_t* hint, int32_t* chars) {
+    *size = q.RequestSizeBytes;
+    *hint = q.InputTokenCountHint;
+    *chars = (int32_t)std::min<size_t>(q.Prompt.size(), 0x7fffffff);
+  }
+
   // Metrics maps → the packed SoA snapshot; adapter names get dictionary ids in first-seen order.
   int IdOf(const std::string& namespaced_name) {
     auto it = server_ids_.find(namespaced_name);
@@ -592,7 +681,8 @@ class Scheduler {
     s.lora_waiting = wait.data();
     s.lora_nmodels = nm.data();
     s.lora_max = mx.data();
-    s.inflight_tokens = have_tokens ? tokens.data() : nullptr;
+    // with the producer, a token-load scorer reads the engine's in-flight counters (a snapshot array would take precedence)
+    s.inflight_tokens = (have_tokens && !(inflight_ && token_load_)) ? tokens.data() : nullptr;
     if (prod) {
       s.min_tpot_slo = min_tpot.data();
       s.dispatched = dispatched.data();
@@ -619,6 +709,10 @@ class Scheduler {
   std::unordered_map<std::string, int> server_ids_;  // ServerID (NamespacedName) -> stable endpoint id
   std::vector<int> free_ids_;
   uint64_t remapped_batches_ = 0;
+  bool inflight_ = false;    // SchedulerConfig::InFlightLoad
+  bool token_load_ = false;  // the profile has a token-load scorer
+  std::vector<int64_t> last_size_;  // estimator inputs of the last engine batch, per request
+  std::vector<int32_t> last_hint_, last_chars_;
 };
 
 inline Scheduler* NewSchedulerWithConfig(const SchedulerConfig& c) { return new Scheduler(c); }

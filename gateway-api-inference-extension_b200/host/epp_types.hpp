@@ -53,6 +53,11 @@ struct InferenceRequest {
   std::string Prompt;     // getUserInputBytes() output (hashing.go:106-135): Completions prompt or marshalled messages
   std::string CacheSalt;
   std::map<std::string, std::string> Headers;  // "x-slo-ttft-ms" / "x-slo-tpot-ms" feed the latency path
+  // SimpleTokenEstimator inputs (inflightload/token_estimator.go:48-72): the request body's size when known (> 0 wins), and
+  // Body.InputTokenCountHint() (>= 0: the exact input token count of token-ID prompts); otherwise len(Prompt) stands in for
+  // len(Body.PromptText())
+  int64_t RequestSizeBytes = 0;
+  int InputTokenCountHint = -1;
 };
 
 // len(strings.Fields(s)) (predictedlatency/plugin.go:286): runs of unicode.IsSpace separate fields.  Go decodes

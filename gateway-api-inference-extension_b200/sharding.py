@@ -59,3 +59,14 @@ def gather_commit_stream(dist, pick, n_hashes, hashes, g_pick, g_nh, g_hash):
     dist.all_gather_into_tensor(g_nh.view(torch.uint8), n_hashes.view(torch.uint8))
     dist.all_gather_into_tensor(g_hash, hashes)
     return g_pick, g_nh, g_hash
+
+
+def gather_inflight_stream(dist, endpoint, tokens, g_endpoint, g_tokens):
+    """The in-flight load counterpart (inflightload/producer.go:101-169): every rank contributes its shard's updates —
+    endpoint i32[R] (-1: none), estimated tokens i64[R] — and receives every shard's, which it applies with one
+    eppscore_inflight_add (or _release) of world*R entries.  The counters are sums of integer adds, so the order of the
+    gathered stream does not matter, only that the set is complete: every rank then holds the counters of one process that
+    applied all updates.  g_* are the preallocated [world*R] outputs."""
+    dist.all_gather_into_tensor(g_endpoint, endpoint)
+    dist.all_gather_into_tensor(g_tokens, tokens)
+    return g_endpoint, g_tokens

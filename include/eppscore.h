@@ -169,7 +169,8 @@ typedef struct eppscore_snapshot {
   const double *min_tpot_slo;    /* getEndpointMinTPOTSLO (predictedlatency/plugin.go:347-355)        [M] */
   const int32_t *dispatched;     /* getEndpointRunningRequestCount (plugin.go:357-363)                [M] */
   const uint8_t *prefill_role;   /* hasPrefillRole(EndpointRoleLabel, endpoint) (prediction.go:168-175) [M] */
-  const int64_t *inflight_tokens;/* InFlightLoad.Tokens attribute (token_load.go:91-95); NULL ⇒ absent [M] */
+  const int64_t *inflight_tokens;/* InFlightLoad.Tokens attribute (token_load.go:91-95); NULL ⇒ the engine's in-flight
+                                    counters (eppscore_inflight_add; all 0, i.e. absent, until the first add) [M] */
 } eppscore_snapshot;
 
 /* One batch = R concurrent Scheduler.Schedule() calls (pkg/epp/scheduling/scheduler.go:54). */
@@ -342,6 +343,42 @@ int32_t eppscore_prefix_lru_len(const struct eppscore_engine *e, int32_t endpoin
 int32_t eppscore_prefix_lru_keys(const struct eppscore_engine *e, int32_t endpoint, uint64_t *out, int32_t cap); /* oldest first */
 /* Replication across GPUs: the index is a deterministic function of the ordered commit stream, so every rank applies the
  * same eppscore_commit_picks[_device] calls (the shards' picks all-gathered in global request order) — SURVEY §8e. */
+
+/* ---- in-flight load producer (requestcontrol/dataproducer/inflightload/producer.go) ----
+ * Two DEVICE-RESIDENT int64 counters per endpoint, requests and estimated tokens, zeroed by eppscore_create: the reference's
+ * InFlightLoad attribute.  They feed EPPSCORE_SCORER_TOKEN_LOAD whenever the snapshot carries no inflight_tokens (a snapshot
+ * that carries it keeps precedence); untouched counters are 0, which scores exactly like an absent attribute.  Every
+ * mutation below prepares the current snapshot's terms again on its stream, with eppscore_set_snapshot's cross-stream
+ * ordering (legal inside a CUDA-graph capture), so the next batch sees the new load; a batch sees one load view, as it sees
+ * one index state.  Updates are integer adds: a batch's order does not matter, and replicas across GPUs only have to apply
+ * the same SET of updates (sharding.gather_inflight_stream).  Device-location calls are asynchronous on `stream`
+ * (NULL = engine stream); host-location calls return when the update is done. */
+/* SimpleTokenEstimator.Estimate with its defaults, 4.0 characters per token and output ratio 1.5 (token_estimator.go:36-72),
+ * for R requests, in integer arithmetic (equal to the reference for every input below 2^52 tokens):
+ *   request_size_bytes[r] > 0   input = max(size / 4, 1)
+ *   prompt_chars[r] < 0         Body == nil: the estimate is 0
+ *   token_hint[r] >= 0          input = hint (Body.InputTokenCountHint())
+ *   otherwise                   input = max(1, round(chars / 4.0)), chars = len(Body.PromptText())
+ *   out[r] = input + round(1.5 * input), rounding half away from zero (math.Round).
+ * Any input array may be NULL: size 0, hint -1, chars 0 (body present) respectively.  out [R]. */
+int32_t eppscore_estimate_tokens(struct eppscore_engine *e, int32_t R, int32_t location, const int64_t *request_size_bytes,
+                                 const int32_t *token_hint, const int32_t *prompt_chars, int64_t *out, void *stream);
+/* PreRequest for a batch (producer.go:101-120): for every r with endpoint[r] >= 0, requests += 1 and tokens += tokens[r]
+ * (tokens NULL: 0).  ERR_INVALID for an endpoint >= max_endpoints; device arrays cannot be checked before the launch: such
+ * entries are skipped and the next eppscore_inflight_get returns ERR_INVALID. */
+int32_t eppscore_inflight_add(struct eppscore_engine *e, int32_t R, int32_t location, const int32_t *endpoint,
+                              const int64_t *tokens, void *stream);
+/* ResponseBody at end of stream (producer.go:122-169): the same with the signs reversed.  Pass the estimate that was added:
+ * the reference estimates the same request again and gets the same number. */
+int32_t eppscore_inflight_release(struct eppscore_engine *e, int32_t R, int32_t location, const int32_t *endpoint,
+                                  const int64_t *tokens, void *stream);
+/* DeleteEndpoint (producer.go:181-187): both counters of `endpoint` to 0, so a recycled endpoint id starts from 0.  A later
+ * release makes them negative, as in the reference (concurrencyTracker.add recreates the counter holding the delta); the
+ * token-load scorer maps a load <= 0 to 1.0. */
+int32_t eppscore_inflight_remove_endpoint(struct eppscore_engine *e, int32_t endpoint);
+/* PrepareRequestData's view (producer.go:90-99): the first M counters, read synchronously on the engine stream after every
+ * earlier mutation.  Either output may be NULL. */
+int32_t eppscore_inflight_get(struct eppscore_engine *e, int64_t *requests_out, int64_t *tokens_out, int32_t M);
 
 /* pinned host memory for callers that want the fast copy path (cudaHostAlloc / cudaFreeHost) */
 void *eppscore_host_alloc(size_t bytes);
