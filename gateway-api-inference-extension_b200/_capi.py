@@ -112,6 +112,11 @@ ABI_SYMBOLS = [
     ("eppscore_inflight_release", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P]),
     ("eppscore_inflight_remove_endpoint", C.c_int32, [_P, C.c_int32]),
     ("eppscore_inflight_get", C.c_int32, [_P, _P, _P, C.c_int32]),
+    ("eppscore_running_add", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
+    ("eppscore_running_remove", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P]),
+    ("eppscore_running_remove_endpoint", C.c_int32, [_P, C.c_int32]),
+    ("eppscore_running_get", C.c_int32, [_P, _P, _P, C.c_int32]),
+    ("eppscore_running_reserve", C.c_int32, [_P, C.c_int64]),
     ("eppscore_host_alloc", _P, [C.c_size_t]),
     ("eppscore_host_free", None, [_P]),
 ]

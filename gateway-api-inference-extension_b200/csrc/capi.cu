@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -89,16 +90,35 @@ struct eppscore_engine {
   bool sched_pending = false;
   DevBuf c_pick, c_hash, c_nh, c_ep, c_op;  // staging for the host-array forms of commit_picks / prefix_add / prefix_apply
 
+  // Producer state the scorers read: mutations of either producer below prepare the snapshot terms again (with last_pa) when
+  // the state feeds the current snapshot.  Mutations outside a CUDA-graph capture are ordered through ev_producer, recorded
+  // after each one on its stream, so the two families never rewrite the terms concurrently (producer_begin / producer_end).
+  cudaEvent_t ev_producer = nullptr;
+  bool producer_pending = false;
+  PrepareArgs last_pa{};  // what the current snapshot was prepared with
+
   // in-flight load producer (inflightload/producer.go): per-endpoint request and token counters, [Mpad] int64 each, zeroed at
-  // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens; the snapshot terms are then
-  // prepared again (with last_pa) after every counter mutation.  Mutations outside a CUDA-graph capture are ordered through
-  // ev_inflight, recorded after each one on its stream.
+  // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens.
   DevBuf inflight_req, inflight_tok, inflight_err;
   DevBuf c_iep, c_itok, c_esize, c_ehint, c_echars, c_eout;  // staging for the host-array forms
-  cudaEvent_t ev_inflight = nullptr;
-  bool inflight_pending = false;
   bool snapshot_has_tokens = false;  // the current snapshot carries inflight_tokens
-  PrepareArgs last_pa{};             // what the current snapshot was prepared with
+
+  // predicted-latency producer's running-request queues (running_kernel.cu): the (endpoint, key) -> tpot table and the
+  // per-endpoint count / minimum.  They feed the latency fold-in when the snapshot lacks min_tpot_slo or dispatched.
+  DevBuf run_tab[8];  // two tables of run_cap slots (slot, tpot, owner, rm each): the table and its spare, in either role
+  DevBuf run_desc;    // the device descriptor (RunDev) every running kernel reads the tables and the scratch through
+  RunDev run_host{};  // its host copy (re-read before a change: the device-side compaction swaps the two tables)
+  DevBuf run_count, run_min_bits, run_min_cnt, run_min_view, run_dirty, run_rc_min, run_rc_cnt, run_ctr;
+  DevBuf c_rep, c_rkey, c_rtpot, c_rslot, c_rwon;  // staging for host arrays and the per-call [R] scratch
+  int64_t run_cap = 0;
+  // host upper bounds of the live entries and tombstones: the counters copied back behind the last mutation (h_run,
+  // ev_run_copy) once that copy has landed, plus R per call issued since
+  int64_t run_bound_live = 0;
+  RunCounters* h_run = nullptr;
+  cudaEvent_t ev_run_copy = nullptr;
+  bool run_copy_issued = false;
+  bool run_captured = false;  // a mutation was captured since the last exact read: its replays are invisible to the bound
+  bool snapshot_has_min_tpot = false, snapshot_has_dispatched = false;
 
   // scratch for host-location batches and internal hashes: two sets, so the chunks of a host batch can alternate
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
@@ -161,6 +181,11 @@ bool cfg_has(const eppscore_config& c, int kind) {
 bool counters_feed_scorer(const eppscore_engine* e) {
   return e->have_snapshot && !e->snapshot_has_tokens && cfg_has(e->cfg, EPPSCORE_SCORER_TOKEN_LOAD);
 }
+// The latency fold-in reads the running-request queues (the per-endpoint minimum, or the count, or both).
+bool running_feeds_scorer(const eppscore_engine* e) {
+  return e->have_snapshot && e->lat_ep.p && (!e->snapshot_has_min_tpot || !e->snapshot_has_dispatched);
+}
+bool producers_feed_scorer(const eppscore_engine* e) { return counters_feed_scorer(e) || running_feeds_scorer(e); }
 
 // Translate the scorer list into kernel steps.  Leading request-independent scorers are folded into
 // one precomputed array ((0.0+t0)+t1)+… — exact, because the kernel adds in the same order.
@@ -262,27 +287,29 @@ int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st) {
   return EPPSCORE_OK;
 }
 
-// Counter mutations: each one waits for the previous one (they do not all commute: remove_endpoint sets to zero), unless `st`
-// is being captured, where the caller's graph edges order them.
-int32_t inflight_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
+// Producer mutations (in-flight counters and running-request queues alike): each one waits for the previous one of either
+// family (they do not all commute: remove_endpoint sets to zero, and both families prepare the same snapshot terms again),
+// unless `st` is being captured, where the caller's graph edges order them.
+int32_t producer_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
   *capturing = cap != cudaStreamCaptureStatusNone;
-  if (!*capturing && e->inflight_pending) CK(e, cudaStreamWaitEvent(st, e->ev_inflight, 0));
+  if (!*capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
   return EPPSCORE_OK;
 }
-// After a mutation: when the counters feed the token-load scorer, its term, the folded leading run and the per-adapter
-// summaries of the sparse path all change, so the snapshot is prepared again on the same stream, with eppscore_set_snapshot's
-// ordering (a device-location batch another stream launched against the current terms finishes reading them first).
-int32_t inflight_end(eppscore_engine* e, cudaStream_t st, bool capturing) {
-  if (counters_feed_scorer(e)) {
+// After a mutation: when the producer's state feeds the current snapshot (`feeds`), the terms that read it — the token-load
+// term, the latency fold-in's endpoint arrays, the folded leading run and the per-adapter summaries of the sparse path —
+// change, so the snapshot is prepared again on the same stream, with eppscore_set_snapshot's ordering (a device-location batch
+// another stream launched against the current terms finishes reading them first).
+int32_t producer_end(eppscore_engine* e, cudaStream_t st, bool capturing, bool feeds) {
+  if (feeds) {
     if (!capturing && e->sched_pending) CK(e, cudaStreamWaitEvent(st, e->ev_sched, 0));
     const int32_t rc = prepare_snapshot(e, st);
     if (rc != EPPSCORE_OK) return rc;
   }
   if (!capturing) {
-    CK(e, cudaEventRecord(e->ev_inflight, st));
-    e->inflight_pending = true;
+    CK(e, cudaEventRecord(e->ev_producer, st));
+    e->producer_pending = true;
   }
   return EPPSCORE_OK;
 }
@@ -449,8 +476,8 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   if (launched == 0) launched = launch_score_pick(a, dense, s, e->sm_count);
   e->launches += launched;
   CK(e, cudaGetLastError());
-  // a later index mutation (engine stream), or a counter mutation that prepares the terms again, must wait for this batch
-  if (!capturing && s != e->stream && (a.table || counters_feed_scorer(e))) {
+  // a later index mutation (engine stream), or a producer mutation that prepares the terms again, must wait for this batch
+  if (!capturing && s != e->stream && (a.table || producers_feed_scorer(e))) {
     CK(e, cudaEventRecord(e->ev_sched, s));
     e->sched_pending = true;
   }
@@ -465,6 +492,46 @@ int32_t h2d(eppscore_engine* e, DevBuf& buf, const T* src, size_t count, const T
   CK(e, cudaMemcpyAsync(buf.p, src, count * sizeof(T), cudaMemcpyHostToDevice, st ? st : e->stream));
   *out = buf.as<T>();
   return EPPSCORE_OK;
+}
+
+constexpr int64_t kRunInitialSlots = 4096;
+
+// A running-request table of `slots` slots (a power of two), empty: slots {0, 0}, no bids.  tpot needs no initial value.
+cudaError_t run_alloc_table(eppscore_engine* e, int64_t slots, DevBuf* slot, DevBuf* tpot, DevBuf* owner, DevBuf* rm, cudaStream_t st) {
+  (void)e;
+  const size_t n = (size_t)slots;
+  cudaError_t c;
+  if ((c = slot->reserve(n * sizeof(RunSlot))) != cudaSuccess) return c;
+  if ((c = tpot->reserve(n * 8)) != cudaSuccess) return c;
+  if ((c = owner->reserve(n * 8)) != cudaSuccess) return c;
+  if ((c = rm->reserve(n * 8)) != cudaSuccess) return c;
+  if ((c = cudaMemsetAsync(slot->p, 0, n * sizeof(RunSlot), st)) != cudaSuccess) return c;
+  if ((c = cudaMemsetAsync(owner->p, 0xff, n * 8, st)) != cudaSuccess) return c;
+  return cudaMemsetAsync(rm->p, 0xff, n * 8, st);
+}
+
+// The descriptor as created: tab[0..3] the table, tab[4..7] its spare, the per-endpoint arrays, the scratch.
+void run_init_desc(eppscore_engine* e) {
+  RunDev& d = e->run_host;
+  d.slot = e->run_tab[0].as<RunSlot>();
+  d.tpot = e->run_tab[1].as<unsigned long long>();
+  d.owner = e->run_tab[2].as<unsigned long long>();
+  d.rm = e->run_tab[3].as<unsigned long long>();
+  d.spare_slot = e->run_tab[4].as<RunSlot>();
+  d.spare_tpot = e->run_tab[5].as<unsigned long long>();
+  d.spare_owner = e->run_tab[6].as<unsigned long long>();
+  d.spare_rm = e->run_tab[7].as<unsigned long long>();
+  d.mask = (unsigned long long)e->run_cap - 1;
+  d.count = e->run_count.as<int>();
+  d.min_bits = e->run_min_bits.as<unsigned long long>();
+  d.min_cnt = e->run_min_cnt.as<int>();
+  d.min_view = e->run_min_view.as<double>();
+  d.dirty = e->run_dirty.as<unsigned>();
+  d.rc_min = e->run_rc_min.as<unsigned long long>();
+  d.rc_cnt = e->run_rc_cnt.as<int>();
+  d.ctr = e->run_ctr.as<RunCounters>();
+  d.slot_of = e->c_rslot.as<int32_t>();
+  d.won = e->c_rwon.as<uint8_t>();
 }
 
 }  // namespace
@@ -605,8 +672,40 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   CK(nullptr, cudaMemsetAsync(ep->inflight_req.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_tok.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_err.p, 0, 4, ep->stream));
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_inflight, cudaEventDisableTiming));
+  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_producer, cudaEventDisableTiming));
   CK(nullptr, init_inflight_update());
+  {  // running-request queues: every endpoint empty, a small table (grown by the first calls that need room)
+    CK(nullptr, ep->run_count.reserve(mp * 4));
+    CK(nullptr, ep->run_min_bits.reserve(mp * 8));
+    CK(nullptr, ep->run_min_cnt.reserve(mp * 4));
+    CK(nullptr, ep->run_min_view.reserve(mp * 8));
+    CK(nullptr, ep->run_dirty.reserve(mp * 4));
+    CK(nullptr, ep->run_rc_min.reserve(mp * 8));
+    CK(nullptr, ep->run_rc_cnt.reserve(mp * 4));
+    CK(nullptr, ep->run_ctr.reserve(sizeof(RunCounters)));
+    CK(nullptr, cudaMemsetAsync(ep->run_count.p, 0, mp * 4, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_min_bits.p, 0xff, mp * 8, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_min_cnt.p, 0, mp * 4, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_min_view.p, 0, mp * 8, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_dirty.p, 0, mp * 4, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_rc_min.p, 0xff, mp * 8, ep->stream));
+    CK(nullptr, cudaMemsetAsync(ep->run_rc_cnt.p, 0, mp * 4, ep->stream));
+    RunCounters c0{};
+    c0.gen = 1;  // owner words of slots that predate every call are 0 (gen 0)
+    CK(nullptr, cudaMemcpyAsync(ep->run_ctr.p, &c0, sizeof(c0), cudaMemcpyHostToDevice, ep->stream));
+    CK(nullptr, cudaHostAlloc(&ep->h_run, sizeof(RunCounters), cudaHostAllocDefault));
+    memset(ep->h_run, 0, sizeof(RunCounters));
+    CK(nullptr, cudaEventCreateWithFlags(&ep->ev_run_copy, cudaEventDisableTiming));
+    CK(nullptr, run_alloc_table(ep, kRunInitialSlots, &ep->run_tab[0], &ep->run_tab[1], &ep->run_tab[2], &ep->run_tab[3], ep->stream));
+    CK(nullptr, run_alloc_table(ep, kRunInitialSlots, &ep->run_tab[4], &ep->run_tab[5], &ep->run_tab[6], &ep->run_tab[7], ep->stream));
+    ep->run_cap = kRunInitialSlots;
+    CK(nullptr, ep->c_rslot.reserve(kRunInitialSlots * 4));
+    CK(nullptr, ep->c_rwon.reserve(kRunInitialSlots));
+    CK(nullptr, ep->run_desc.reserve(sizeof(RunDev)));
+    run_init_desc(ep);
+    CK(nullptr, cudaMemcpyAsync(ep->run_desc.p, &ep->run_host, sizeof(RunDev), cudaMemcpyHostToDevice, ep->stream));
+    CK(nullptr, init_running_kernels());
+  }
   for (int which = 0; which < 2; which++)  // value buckets for the masked min/max of the queue / running scorers
     if (cfg_has(ep->cfg, which == 0 ? EPPSCORE_SCORER_QUEUE : EPPSCORE_SCORER_RUNNING)) {
       CK(nullptr, ep->qhdr[which].reserve(sizeof(QBucketHdr)));
@@ -668,8 +767,11 @@ void eppscore_destroy(eppscore_engine* e) {
                     &e->raw_kv, &e->raw_queue, &e->raw_running, &e->raw_act, &e->raw_wait, &e->raw_nmodels, &e->raw_max,
                     &e->fold_unmasked, &e->fold_masked, &e->cls_lo, &e->cls_hi, &e->summ, &e->tiemask, &e->prefix_lut2d, &e->c_pick, &e->c_hash, &e->c_nh,
                     &e->c_ep, &e->c_op, &e->inflight_req, &e->inflight_tok, &e->inflight_err, &e->c_iep, &e->c_itok, &e->c_esize,
-                    &e->c_ehint, &e->c_echars, &e->c_eout};
+                    &e->c_ehint, &e->c_echars, &e->c_eout, &e->run_desc, &e->run_count,
+                    &e->run_min_bits, &e->run_min_cnt, &e->run_min_view, &e->run_dirty, &e->run_rc_min, &e->run_rc_cnt, &e->run_ctr,
+                    &e->c_rep, &e->c_rkey, &e->c_rtpot, &e->c_rslot, &e->c_rwon};
   for (auto& x : e->sc) x.release();
+  for (auto& x : e->run_tab) x.release();
   for (int i = 0; i < 3; i++) {
     if (e->split_stream[i]) {
       cudaStreamSynchronize(e->split_stream[i]);
@@ -687,7 +789,9 @@ void eppscore_destroy(eppscore_engine* e) {
   for (int i = 0; i < 4; i++) e->raw_col[i].release();
   for (int i = 0; i < kMaxSteps; i++) e->term[i].release();
   e->index.reset();
-  if (e->ev_inflight) cudaEventDestroy(e->ev_inflight);
+  if (e->ev_producer) cudaEventDestroy(e->ev_producer);
+  if (e->ev_run_copy) cudaEventDestroy(e->ev_run_copy);
+  if (e->h_run) cudaFreeHost(e->h_run);
   if (e->ev_sched) cudaEventDestroy(e->ev_sched);
   if (e->ev_caller) cudaEventDestroy(e->ev_caller);
   if (e->ev_snapshot) cudaEventDestroy(e->ev_snapshot);
@@ -823,10 +927,11 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   // InFlightLoad.Tokens: the snapshot's array when it carries one, else the in-flight counters (all 0 until the first
   // eppscore_inflight_add, which scores exactly like an absent attribute, token_load.go:91-98)
   pa.tokens = s->inflight_tokens ? (on_device ? s->inflight_tokens : e->raw_tokens.as<int64_t>()) : e->inflight_tok.as<int64_t>();
-  if (!s->inflight_tokens && e->inflight_pending) {  // the counters were last changed on another stream
+  const bool reads_running = e->lat_ep.p && (!s->min_tpot_slo || !s->dispatched);
+  if ((!s->inflight_tokens || reads_running) && e->producer_pending) {  // producer state last changed on another stream
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cap);
-    if (cap == cudaStreamCaptureStatusNone) CK(e, cudaStreamWaitEvent(st, e->ev_inflight, 0));
+    if (cap == cudaStreamCaptureStatusNone) CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
   }
   pa.token_threshold = e->cfg.token_load_threshold;
   e->lat_args = LatArgs{};
@@ -835,8 +940,11 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
     // per-request / per-pair terms (LatArgs); the weight normalisations are single IEEE divides
     // (scorer/latency/plugin.go:325-333,373-379) done here on the host (-ffp-contract=off).
     const eppscore_latency_params& lp = e->lat_params;
-    pa.min_tpot = s->min_tpot_slo ? (on_device ? s->min_tpot_slo : e->raw_min_tpot.as<double>()) : nullptr;
-    pa.dispatched = s->dispatched ? (on_device ? s->dispatched : e->raw_dispatched.as<int32_t>()) : nullptr;
+    // getEndpointMinTPOTSLO / getEndpointRunningRequestCount: the snapshot's arrays when it carries them, field by field,
+    // else the running-request queues (min 0 and count 0 until the first eppscore_running_add, which score exactly like
+    // absent arrays)
+    pa.min_tpot = s->min_tpot_slo ? (on_device ? s->min_tpot_slo : e->raw_min_tpot.as<double>()) : e->run_min_view.as<double>();
+    pa.dispatched = s->dispatched ? (on_device ? s->dispatched : e->raw_dispatched.as<int32_t>()) : e->run_count.as<int32_t>();
     pa.prefill = s->prefill_role ? (on_device ? s->prefill_role : e->raw_prefill.as<uint8_t>()) : nullptr;
     const double coef[8] = {lp.ttft_intercept, lp.ttft_kv, lp.ttft_waiting, lp.ttft_running,
                             lp.tpot_intercept, lp.tpot_kv, lp.tpot_waiting, lp.tpot_running};
@@ -896,6 +1004,8 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   pa.summ = e->plan_unmasked.plan.sparse_ok ? e->summ.as<AdapterSummary>() : nullptr;
   pa.tiemask = e->tiemask.as<uint32_t>();
   e->snapshot_has_tokens = s->inflight_tokens != nullptr;
+  e->snapshot_has_min_tpot = s->min_tpot_slo != nullptr;
+  e->snapshot_has_dispatched = s->dispatched != nullptr;
   e->last_pa = pa;
   int32_t rc = prepare_snapshot(e, st);
   if (rc != EPPSCORE_OK) return rc;
@@ -1472,7 +1582,7 @@ static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, 
       if (endpoint[r] >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight update: endpoint >= max_endpoints");
   }
   bool capturing = false;
-  int32_t rc = inflight_begin(e, st, &capturing);
+  int32_t rc = producer_begin(e, st, &capturing);
   if (rc != EPPSCORE_OK) return rc;
   if (!on_device) {
     if ((rc = h2d(e, e->c_iep, endpoint, (size_t)R, &d_ep)) != EPPSCORE_OK) return rc;
@@ -1481,7 +1591,7 @@ static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, 
   e->launches += launch_inflight_update(d_ep, d_tok, R, e->cfg.max_endpoints, sign, e->inflight_req.as<int64_t>(),
                                         e->inflight_tok.as<int64_t>(), e->inflight_err.as<uint32_t>(), st);
   CK(e, cudaGetLastError());
-  if ((rc = inflight_end(e, st, capturing)) != EPPSCORE_OK) return rc;
+  if ((rc = producer_end(e, st, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
   if (!on_device) CK(e, cudaStreamSynchronize(st));  // the caller's host arrays may be reused
   return EPPSCORE_OK;
 }
@@ -1501,18 +1611,18 @@ int32_t eppscore_inflight_remove_endpoint(eppscore_engine* e, int32_t endpoint) 
   if (endpoint < 0 || endpoint >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight_remove_endpoint: endpoint out of range");
   CK(e, cudaSetDevice(e->device));
   bool capturing = false;
-  int32_t rc = inflight_begin(e, e->stream, &capturing);
+  int32_t rc = producer_begin(e, e->stream, &capturing);
   if (rc != EPPSCORE_OK) return rc;
   CK(e, cudaMemsetAsync(e->inflight_req.as<int64_t>() + endpoint, 0, 8, e->stream));
   CK(e, cudaMemsetAsync(e->inflight_tok.as<int64_t>() + endpoint, 0, 8, e->stream));
-  return inflight_end(e, e->stream, capturing);
+  return producer_end(e, e->stream, capturing, counters_feed_scorer(e));
 }
 
 int32_t eppscore_inflight_get(eppscore_engine* e, int64_t* requests_out, int64_t* tokens_out, int32_t M) {
   if (!e) return EPPSCORE_ERR_INVALID;
   if (M < 0 || M > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight_get: M outside [0, max_endpoints]");
   CK(e, cudaSetDevice(e->device));
-  if (e->inflight_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_inflight, 0));
+  if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
   uint32_t err = 0;
   if (M > 0 && requests_out) CK(e, cudaMemcpyAsync(requests_out, e->inflight_req.p, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
   if (M > 0 && tokens_out) CK(e, cudaMemcpyAsync(tokens_out, e->inflight_tok.p, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
@@ -1523,6 +1633,236 @@ int32_t eppscore_inflight_get(eppscore_engine* e, int64_t* requests_out, int64_t
     return fail(e, EPPSCORE_ERR_INVALID, "an inflight update on device arrays named an endpoint >= max_endpoints (those entries were skipped)");
   }
   return EPPSCORE_OK;
+}
+
+}  // extern "C"
+
+// ---------------- running-request queues (predicted-latency producer) ----------------
+namespace {
+
+// The live / tombstone counters as of every mutation ordered before `st`'s current end: read synchronously.  This also
+// re-bases the bounds after graph replays, which the host does not see.
+int32_t run_read_exact(eppscore_engine* e, cudaStream_t st) {
+  CK(e, cudaMemcpyAsync(e->h_run, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
+  CK(e, cudaStreamSynchronize(st));
+  e->run_bound_live = (int64_t)e->h_run->live;
+  e->run_copy_issued = false;
+  e->run_captured = false;
+  return EPPSCORE_OK;
+}
+
+// The device descriptor the kernels read the table and the scratch through.  The compaction kernels swap the table with its
+// spare on the device, so the host reads the descriptor back before it changes it.  Both run synchronously on `st`.
+int32_t run_desc_download(eppscore_engine* e, cudaStream_t st) {
+  CK(e, cudaStreamSynchronize(st));
+  CK(e, cudaMemcpyAsync(&e->run_host, e->run_desc.p, sizeof(RunDev), cudaMemcpyDeviceToHost, st));
+  CK(e, cudaStreamSynchronize(st));
+  return EPPSCORE_OK;
+}
+int32_t run_desc_upload(eppscore_engine* e, cudaStream_t st) {
+  CK(e, cudaMemcpyAsync(e->run_desc.p, &e->run_host, sizeof(RunDev), cudaMemcpyHostToDevice, st));
+  CK(e, cudaStreamSynchronize(st));
+  return EPPSCORE_OK;
+}
+
+// Grows the table to `slots` slots on `st` (outside a capture): a new table and spare, the live entries moved into it, the
+// descriptor pointed at it.  Graphs captured earlier read the table through the descriptor and the grid-stride passes loop
+// over its capacity, so they stay valid.
+int32_t run_grow(eppscore_engine* e, cudaStream_t st, int64_t slots) {
+  DevBuf nb[8];
+  cudaError_t c = run_alloc_table(e, slots, &nb[0], &nb[1], &nb[2], &nb[3], st);
+  if (c == cudaSuccess) c = run_alloc_table(e, slots, &nb[4], &nb[5], &nb[6], &nb[7], st);
+  if (c != cudaSuccess) {
+    for (DevBuf& b : nb) b.release();
+    return cuda_fail(e, c, "running-request table allocation");
+  }
+  int32_t rc = run_desc_download(e, st);
+  if (rc != EPPSCORE_OK) return rc;
+  const RunDev src = e->run_host;
+  RunDev& d = e->run_host;
+  d.slot = nb[0].as<RunSlot>();
+  d.tpot = nb[1].as<unsigned long long>();
+  d.owner = nb[2].as<unsigned long long>();
+  d.rm = nb[3].as<unsigned long long>();
+  d.spare_slot = nb[4].as<RunSlot>();
+  d.spare_tpot = nb[5].as<unsigned long long>();
+  d.spare_owner = nb[6].as<unsigned long long>();
+  d.spare_rm = nb[7].as<unsigned long long>();
+  d.mask = (unsigned long long)slots - 1;
+  e->launches += launch_running_rebuild(src, d, e->sm_count, st);  // also zeroes the tombstone count
+  CK(e, cudaGetLastError());
+  if ((rc = run_desc_upload(e, st)) != EPPSCORE_OK) return rc;
+  for (int i = 0; i < 8; i++) {
+    e->run_tab[i].release();
+    e->run_tab[i] = nb[i];
+  }
+  e->run_cap = slots;
+  return EPPSCORE_OK;
+}
+
+// Room for R more entries before an add.  Tombstones are the device's business (the compaction launched before every add),
+// so the host only guarantees live + R <= capacity / 2, from its upper bound on the live entries: the counters copied back
+// behind an earlier call once that copy has landed, plus R per add issued since.  Outside a capture the bound is held to a
+// quarter, so that compactions stay rare; when it does not hold, the exact count decides whether the table doubles (only
+// while live + R exceed a quarter of the slots: churn never grows it).  Inside a capture nothing can grow.
+int32_t run_make_room(eppscore_engine* e, cudaStream_t st, int64_t R, bool capturing) {
+  if (capturing) {
+    if (e->run_bound_live + R <= e->run_cap / 2) return EPPSCORE_OK;
+    return fail(e, EPPSCORE_ERR_CAPACITY, "running_add under CUDA-graph capture: the table may not have room for R more entries "
+                                          "(size it with eppscore_running_reserve before the capture)");
+  }
+  bool exact = false;
+  if (e->run_captured) {  // graph replays may have changed the counters since: read them once
+    int32_t rc = run_read_exact(e, st);
+    if (rc != EPPSCORE_OK) return rc;
+    exact = true;
+  } else if (e->run_copy_issued && cudaEventQuery(e->ev_run_copy) == cudaSuccess) {
+    e->run_bound_live = (int64_t)e->h_run->live;
+    e->run_copy_issued = false;
+  }
+  if (e->run_bound_live + R <= e->run_cap / 4) return EPPSCORE_OK;
+  if (!exact) {
+    int32_t rc = run_read_exact(e, st);
+    if (rc != EPPSCORE_OK) return rc;
+  }
+  int64_t slots = e->run_cap;
+  while (e->run_bound_live + R > slots / 4) slots *= 2;
+  return slots == e->run_cap ? EPPSCORE_OK : run_grow(e, st, slots);
+}
+
+// Per-call scratch of at least R entries.  Under a capture it cannot be allocated; outside one a larger scratch replaces the
+// old one in the descriptor.
+int32_t run_scratch(eppscore_engine* e, cudaStream_t st, int64_t R, bool capturing) {
+  if ((size_t)R * 4 <= e->c_rslot.bytes && (size_t)R <= e->c_rwon.bytes) return EPPSCORE_OK;
+  if (capturing)
+    return fail(e, EPPSCORE_ERR_CAPACITY, "running update under CUDA-graph capture: R exceeds the scratch sized by "
+                                          "eppscore_running_reserve");
+  int32_t rc = run_desc_download(e, st);
+  if (rc != EPPSCORE_OK) return rc;
+  CK(e, e->c_rslot.reserve((size_t)R * 4));
+  CK(e, e->c_rwon.reserve((size_t)R));
+  e->run_host.slot_of = e->c_rslot.as<int32_t>();
+  e->run_host.won = e->c_rwon.as<uint8_t>();
+  return run_desc_upload(e, st);
+}
+
+// Behind every mutation outside a capture: the counters are copied back asynchronously, for the next room check.
+int32_t run_copy_back(eppscore_engine* e, cudaStream_t st, bool capturing) {
+  if (capturing) {
+    e->run_captured = true;
+    return EPPSCORE_OK;
+  }
+  CK(e, cudaMemcpyAsync(e->h_run, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
+  CK(e, cudaEventRecord(e->ev_run_copy, st));
+  e->run_copy_issued = true;
+  return EPPSCORE_OK;
+}
+
+int32_t running_update(eppscore_engine* e, int op, int32_t R, int32_t location, const int32_t* endpoint, const uint64_t* key,
+                       const double* tpot, uint8_t* out, void* stream) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (R < 0 || (R > 0 && (!endpoint || !key))) return fail(e, EPPSCORE_ERR_INVALID, "running update: R < 0, or endpoint / request_key NULL");
+  if (R == 0) return EPPSCORE_OK;
+  CK(e, cudaSetDevice(e->device));
+  const bool on_device = location == 1;
+  cudaStream_t st = (on_device && stream) ? (cudaStream_t)stream : e->stream;
+  if (!on_device) {
+    for (int32_t r = 0; r < R; r++) {
+      if (endpoint[r] >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "running update: endpoint >= max_endpoints");
+      if (tpot && std::isnan(tpot[r])) return fail(e, EPPSCORE_ERR_INVALID, "running_add: tpot_slo is NaN");
+    }
+  }
+  bool capturing = false;
+  int32_t rc = producer_begin(e, st, &capturing);
+  if (rc != EPPSCORE_OK) return rc;
+  if (op == 0 && (rc = run_make_room(e, st, R, capturing)) != EPPSCORE_OK) return rc;
+  if ((rc = run_scratch(e, st, R, capturing)) != EPPSCORE_OK) return rc;
+  const int32_t* d_ep = endpoint;
+  const uint64_t* d_key = key;
+  const double* d_tpot = tpot;
+  if (!on_device) {
+    if ((rc = h2d(e, e->c_rep, endpoint, (size_t)R, &d_ep, st)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->c_rkey, key, (size_t)R, &d_key, st)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->c_rtpot, tpot, (size_t)R, &d_tpot, st)) != EPPSCORE_OK) return rc;
+  }
+  e->launches += launch_running_update(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, op, d_ep, d_key,
+                                        op == 0 ? d_tpot : nullptr, R, e->cfg.max_endpoints, on_device ? out : nullptr,
+                                        e->sm_count, st);
+  CK(e, cudaGetLastError());
+  if (!on_device && out) CK(e, cudaMemcpyAsync(out, e->c_rwon.p, (size_t)R, cudaMemcpyDeviceToHost, st));
+  if (op == 0) e->run_bound_live += R;
+  if ((rc = run_copy_back(e, st, capturing)) != EPPSCORE_OK) return rc;
+  if ((rc = producer_end(e, st, capturing, running_feeds_scorer(e))) != EPPSCORE_OK) return rc;
+  if (!on_device) CK(e, cudaStreamSynchronize(st));  // the caller's host arrays may be reused
+  return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_running_add(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const uint64_t* request_key,
+                             const double* tpot_slo, uint8_t* added_out, void* stream) {
+  return running_update(e, 0, R, location, endpoint, request_key, tpot_slo, added_out, stream);
+}
+
+int32_t eppscore_running_remove(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint,
+                                const uint64_t* request_key, uint8_t* removed_out, void* stream) {
+  return running_update(e, 1, R, location, endpoint, request_key, nullptr, removed_out, stream);
+}
+
+int32_t eppscore_running_remove_endpoint(eppscore_engine* e, int32_t endpoint) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (endpoint < 0 || endpoint >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "running_remove_endpoint: endpoint out of range");
+  CK(e, cudaSetDevice(e->device));
+  bool capturing = false;
+  int32_t rc = producer_begin(e, e->stream, &capturing);
+  if (rc != EPPSCORE_OK) return rc;
+  e->launches += launch_running_drop_endpoint(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, endpoint,
+                                              e->cfg.max_endpoints, e->sm_count, e->stream);
+  CK(e, cudaGetLastError());
+  if ((rc = run_copy_back(e, e->stream, capturing)) != EPPSCORE_OK) return rc;
+  if ((rc = producer_end(e, e->stream, capturing, running_feeds_scorer(e))) != EPPSCORE_OK) return rc;
+  // the live count only goes down: the host bound stays an upper bound
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_running_get(eppscore_engine* e, double* min_tpot_out, int32_t* count_out, int32_t M) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (M < 0 || M > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "running_get: M outside [0, max_endpoints]");
+  CK(e, cudaSetDevice(e->device));
+  if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
+  if (M > 0 && min_tpot_out) CK(e, cudaMemcpyAsync(min_tpot_out, e->run_min_view.p, (size_t)M * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (M > 0 && count_out) CK(e, cudaMemcpyAsync(count_out, e->run_count.p, (size_t)M * 4, cudaMemcpyDeviceToHost, e->stream));
+  int32_t rc = run_read_exact(e, e->stream);
+  if (rc != EPPSCORE_OK) return rc;
+  const unsigned err = e->h_run->err;
+  if (err) {
+    CK(e, cudaMemsetAsync(&e->run_ctr.as<RunCounters>()->err, 0, 4, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    if (err & kRunErrCapacity)
+      return fail(e, EPPSCORE_ERR_CAPACITY, "a running_add found no empty slot (a graph was replayed past the room "
+                                            "eppscore_running_reserve made); those entries were not added");
+    return fail(e, EPPSCORE_ERR_INVALID, "a running update on device arrays named an endpoint >= max_endpoints or a NaN "
+                                         "tpot (those entries were skipped)");
+  }
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_running_reserve(eppscore_engine* e, int64_t live_entries) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (live_entries < 0 || live_entries > (int64_t)1 << 29) return fail(e, EPPSCORE_ERR_INVALID, "running_reserve: live_entries outside [0, 2^29]");
+  if (live_entries > 0) {
+    CK(e, cudaSetDevice(e->device));
+    if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
+    int32_t rc = run_read_exact(e, e->stream);
+    if (rc != EPPSCORE_OK) return rc;
+    int64_t slots = e->run_cap;
+    while (live_entries > slots / 2) slots *= 2;
+    if (slots != e->run_cap && (rc = run_grow(e, e->stream, slots)) != EPPSCORE_OK) return rc;
+    if ((rc = run_scratch(e, e->stream, live_entries, false)) != EPPSCORE_OK) return rc;
+  }
+  return (int32_t)(e->run_cap / 2);
 }
 
 void* eppscore_host_alloc(size_t bytes) {

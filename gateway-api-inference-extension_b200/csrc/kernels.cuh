@@ -249,4 +249,44 @@ int launch_inflight_update(const int32_t* endpoint, const int64_t* tokens, int R
                            int64_t* token_sum, uint32_t* err, cudaStream_t s);
 int launch_estimate_tokens(const int64_t* size, const int32_t* hint, const int32_t* chars, int R, int64_t* out, cudaStream_t s);
 
+// predicted-latency producer's running-request queues (running_kernel.cu).  Table slot: {key, meta}, meta = endpoint + 1
+// (| kRunTomb once removed), {0, 0} empty; tpot[] holds the entry's tpot bits, owner[] / rm[] the (gen << 32 | r) bids of
+// an add / remove call (~0 when none).  Per endpoint: count, min_bits (kRunMinNone when empty), min_cnt = live entries
+// equal to min_bits, min_view = what the scorer reads (the minimum as a double, 0 when empty).
+struct __align__(16) RunSlot {
+  unsigned long long key, meta;
+};
+constexpr unsigned long long kRunTomb = 1ull << 32;
+constexpr unsigned long long kRunMinNone = ~0ull;
+constexpr unsigned kRunErrInvalid = 1u, kRunErrCapacity = 2u;
+struct RunCounters {
+  unsigned long long live, tomb;  // live entries, tombstones
+  unsigned gen, any_dirty, err, pad;
+};
+struct RunDev {
+  RunSlot* slot;
+  unsigned long long *tpot, *owner, *rm;
+  unsigned long long mask;  // capacity - 1 (a power of two)
+  int* count;
+  unsigned long long* min_bits;
+  int* min_cnt;
+  double* min_view;
+  unsigned* dirty;
+  unsigned long long* rc_min;  // recompute scratch: kRunMinNone / 0 between calls
+  int* rc_cnt;
+  RunCounters* ctr;
+  RunSlot* spare_slot;  // a second table of the same capacity: the target of the device-side compaction
+  unsigned long long *spare_tpot, *spare_owner, *spare_rm;
+  int32_t* slot_of;  // per-call scratch, [scratch capacity]
+  uint8_t* won;
+};
+cudaError_t init_running_kernels();
+// The kernels of a call read the table through the DEVICE-resident descriptor `dp` (so captured graphs follow a table that
+// grows or compacts later); `cap` only sizes the grid-stride passes.  op 0 = add (tpot may be NULL: 0), op 1 = remove;
+// out: optional [R] added / removed flags.
+int launch_running_update(RunDev* dp, unsigned long long cap, int op, const int32_t* endpoint, const uint64_t* key,
+                          const double* tpot, int R, int n_ep, uint8_t* out, int sm_count, cudaStream_t s);
+int launch_running_drop_endpoint(RunDev* dp, unsigned long long cap, int m, int n_ep, int sm_count, cudaStream_t s);
+int launch_running_rebuild(const RunDev& src, const RunDev& dst, int sm_count, cudaStream_t s);
+
 }  // namespace eppscore

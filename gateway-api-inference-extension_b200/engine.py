@@ -319,6 +319,47 @@ class Engine:
         self._check(self._lib.eppscore_inflight_get(self._h, req.ctypes.data, tok.ctypes.data, M))
         return req[:M], tok[:M]
 
+    # ------------------------------------------------------------------ running-request queues (predicted-latency producer)
+    def _running(self, fn, endpoint, request_key, tpot_slo, device, stream, out, want_out, extra):
+        a = _Args(device)
+        R = int(endpoint.shape[0]) if hasattr(endpoint, "shape") else len(endpoint)
+        if device:
+            o_ptr = a.ptr(out, None)
+        else:
+            out = np.zeros(max(R, 1), np.uint8) if want_out else None
+            o_ptr = out.ctypes.data if want_out else None
+        args = [a.ptr(endpoint, np.int32), a.ptr(request_key, np.uint64)]
+        if extra:
+            args.append(a.ptr(tpot_slo, np.float64))
+        self._check(fn(self._h, R, 1 if device else 0, *args, o_ptr, stream))
+        if device:
+            return out
+        return out[:R].astype(bool) if want_out else None
+
+    def running_add(self, endpoint, request_key, tpot_slo=None, device=False, stream=None, out=None, want_added=True):
+        """PreRequest for a batch (eppscore_running_add): adds (endpoint[r], request_key[r], tpot_slo[r]); endpoint -1 is
+        skipped.  Host mode returns added bool[R]; device mode writes `out` (a uint8[R] CUDA tensor) when given."""
+        return self._running(self._lib.eppscore_running_add, endpoint, request_key, tpot_slo, device, stream, out, want_added, True)
+
+    def running_remove(self, endpoint, request_key, device=False, stream=None, out=None, want_removed=True):
+        """End of stream / TTL expiry for a batch (eppscore_running_remove); host mode returns removed bool[R]."""
+        return self._running(self._lib.eppscore_running_remove, endpoint, request_key, None, device, stream, out, want_removed, False)
+
+    def running_remove_endpoint(self, endpoint):
+        self._check(self._lib.eppscore_running_remove_endpoint(self._h, endpoint))
+
+    def running_get(self, M=None):
+        """(min_tpot float64[M], count int32[M]): the queues' view after every earlier update; M defaults to max_endpoints."""
+        M = self.cfg.max_endpoints if M is None else M
+        mn, cnt = np.zeros(max(M, 1), np.float64), np.zeros(max(M, 1), np.int32)
+        self._check(self._lib.eppscore_running_get(self._h, mn.ctypes.data, cnt.ctypes.data, M))
+        return mn[:M], cnt[:M]
+
+    def running_reserve(self, live_entries=0):
+        """Room for live_entries entries (and calls of up to that many) before a graph capture; returns the capacity in
+        entries (live_entries 0: only the query)."""
+        return self._check(self._lib.eppscore_running_reserve(self._h, int(live_entries)))
+
     @staticmethod
     def model_seed(model, salt=b"") -> int:
         if isinstance(model, str):

@@ -47,8 +47,23 @@ extern "C" int32_t eppscore_inflight_remove_endpoint(struct eppscore_engine* e, 
 extern "C" int32_t eppscore_inflight_get(struct eppscore_engine* e, int64_t* requests_out, int64_t* tokens_out, int32_t M)
     __attribute__((weak));
 
+// The running-request queues of the predicted-latency producer came the same way: EngineHasRunningQueues() tells.
+extern "C" int32_t eppscore_running_add(struct eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint,
+                                        const uint64_t* request_key, const double* tpot_slo, uint8_t* added_out, void* stream)
+    __attribute__((weak));
+extern "C" int32_t eppscore_running_remove(struct eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint,
+                                           const uint64_t* request_key, uint8_t* removed_out, void* stream) __attribute__((weak));
+extern "C" int32_t eppscore_running_remove_endpoint(struct eppscore_engine* e, int32_t endpoint) __attribute__((weak));
+extern "C" int32_t eppscore_running_get(struct eppscore_engine* e, double* min_tpot_out, int32_t* count_out, int32_t M)
+    __attribute__((weak));
+extern "C" int32_t eppscore_running_reserve(struct eppscore_engine* e, int64_t live_entries) __attribute__((weak));
+
 namespace epp {
 
+inline bool EngineHasRunningQueues() {
+  return &eppscore_running_add != nullptr && &eppscore_running_remove != nullptr && &eppscore_running_remove_endpoint != nullptr &&
+         &eppscore_running_get != nullptr && &eppscore_running_reserve != nullptr;
+}
 inline bool EngineHasTopK() { return &eppscore_schedule_batch_topk != nullptr; }
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
@@ -95,6 +110,11 @@ struct PredictedLatencyProducer {
     int RunningRequests = 0; // getEndpointRunningRequestCount
   };
   std::map<std::string, EndpointState> State;  // keyed by NamespacedName.String()
+  // Opt-in: the Scheduler keeps the running-request queues itself, on the device (eppscore_running_*), as the reference's
+  // producer does (requestcontrol_hooks.go:73-86,219, plugin.go:190-196): PreRequest adds each scheduled request with its
+  // x-slo-tpot-ms to its TargetEndpoints[0], ResponseComplete and RequestExpired remove it, RemovePod empties the endpoint.
+  // State is then not read.  A request with an empty RequestId is not tracked (requestcontrol_hooks.go:66-69).
+  bool TrackRunningRequests = false;
 };
 
 // inflight-load-producer (requestcontrol/dataproducer/inflightload/producer.go): requests and estimated tokens in flight per
@@ -209,6 +229,9 @@ class Scheduler {
     if (cfg.InFlightLoad && !EngineHasInFlightLoad())
       throw SchedulingError("the inflight-load-producer needs an engine library with eppscore_inflight_add");
     inflight_ = cfg.InFlightLoad != nullptr;
+    running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
+    if (running_ && !EngineHasRunningQueues())
+      throw SchedulingError("TrackRunningRequests needs an engine library with eppscore_running_add");
     c.n_scorers = (int32_t)sc.size();
     {  // the small-batch CPU route applies to request-independent profiles only
       std::vector<int32_t> kinds;
@@ -220,7 +243,7 @@ class Scheduler {
       double thr = 4194304.0;
       for (auto& w : sc)
         if (auto* tl = dynamic_cast<TokenLoadScorer*>(w.Scorer_.get())) thr = (double)tl->QueueThresholdTokens;
-      cpu_route_ok_ = cfg.CpuBatchThreshold > 0 && !inflight_ && cfg.Profile.device_filters().empty() && cfg.Profile.picker().Mode == EPPSCORE_PICK_MAX_SCORE &&
+      cpu_route_ok_ = cfg.CpuBatchThreshold > 0 && !inflight_ && !running_ && cfg.Profile.device_filters().empty() && cfg.Profile.picker().Mode == EPPSCORE_PICK_MAX_SCORE &&
                       cfg.Profile.picker().MaxNumOfEndpoints == 1 && cfg.TieMode == EPPSCORE_TIE_LOWEST_INDEX && cpu_.Configure(kinds, weights, thr);
     }
     for (size_t i = 0; i < sc.size(); i++) {
@@ -363,17 +386,18 @@ class Scheduler {
       in_tokens.resize((size_t)R);
       ttft_slo.assign((size_t)R, 0.0);
       tpot_slo.assign((size_t)R, 0.0);
-      auto header = [](const InferenceRequest& q, const char* key) {
-        auto it = q.Headers.find(key);
-        if (it == q.Headers.end()) return 0.0;
-        char* end = nullptr;
-        const double v = strtod(it->second.c_str(), &end);
-        return (end && *end == 0 && end != it->second.c_str()) ? v : 0.0;  // parse error ⇒ 0 (logged only)
-      };
       for (int r = 0; r < R; r++) {
         in_tokens[r] = CountFields(requests[r].Prompt);
-        ttft_slo[r] = header(requests[r], "x-slo-ttft-ms");
-        tpot_slo[r] = header(requests[r], "x-slo-tpot-ms");
+        ttft_slo[r] = SloHeader(requests[r], "x-slo-ttft-ms");
+        tpot_slo[r] = SloHeader(requests[r], "x-slo-tpot-ms");
+      }
+    }
+    if (running_) {  // PreRequest's inputs: the request id and avgTPOTSLO, the same header rule
+      last_rid_.resize((size_t)R);
+      last_tpot_.resize((size_t)R);
+      for (int r = 0; r < R; r++) {
+        last_rid_[r] = requests[r].RequestId;
+        last_tpot_[r] = SloHeader(requests[r], "x-slo-tpot-ms");
       }
     }
     std::vector<uint64_t> seed((size_t)R);
@@ -494,7 +518,7 @@ class Scheduler {
   // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
   // (inflightload/producer.go:101-120).
   void PreRequest(const std::vector<BatchItem>& results) {
-    if (!last_endpoints_ || (last_hashes_.empty() && !inflight_)) return;
+    if (!last_endpoints_ || (last_hashes_.empty() && !inflight_ && !running_)) return;
     const int R = (int)results.size();
     std::vector<int32_t> pick((size_t)R, -1);
     for (int r = 0; r < R; r++)
@@ -513,13 +537,35 @@ class Scheduler {
       if (eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr) != EPPSCORE_OK)
         throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
     }
+    if (running_ && (int)last_rid_.size() == R) {  // requestcontrol_hooks.go:73-86
+      std::vector<int32_t> ep((size_t)R, -1);
+      std::vector<uint64_t> key((size_t)R, 0);
+      for (int r = 0; r < R; r++) {
+        if (pick[r] < 0 || last_rid_[r].empty()) continue;  // no target / missing x-request-id: not tracked
+        ep[r] = pick[r];
+        key[r] = KeyFor(last_rid_[r]);
+      }
+      std::vector<uint8_t> added((size_t)R, 0);
+      if (eppscore_running_add(eng_, R, 0, ep.data(), key.data(), last_tpot_.data(), added.data(), nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_running_add: ") + eppscore_last_error(eng_));
+      for (int r = 0; r < R; r++)
+        if (ep[r] >= 0) {
+          if (added[r]) running_keys_[last_rid_[r]].endpoints.push_back(ep[r]);
+          else ReleaseKeyIfUnused(last_rid_[r]);  // refused (already live there, or a negative tpot)
+        }
+    }
   }
+
+  // Context TTL expiry (predictedlatency/plugin.go:190-196) for a request PreRequest added: removed from its endpoint's
+  // running-request queue, as at the end of the stream.  The caller owns the TTL clock.
+  void RequestExpired(const InferenceRequest& request, const SchedulingResult& result) { RunningRemove(request, result); }
 
   // ResponseBody at end of stream (inflightload/producer.go:122-169) for a request PreRequest counted, given the result it was
   // scheduled with (the reference reads it from request.SchedulingResult): its TargetEndpoints[0] gives back one request and the
   // request's estimate.  Without the producer, or for a server that has left the pool since (its id may already be another
   // server's), nothing happens.
   void ResponseComplete(const InferenceRequest& request, const SchedulingResult& result) {
+    RunningRemove(request, result);  // requestcontrol_hooks.go:219
     if (!inflight_) return;
     auto pr = result.ProfileResults.find(cfg_.ProfileName);
     if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
@@ -544,6 +590,15 @@ class Scheduler {
       throw SchedulingError(std::string("eppscore_prefix_remove_endpoint: ") + eppscore_last_error(eng_));
     if (inflight_ && eppscore_inflight_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
       throw SchedulingError(std::string("eppscore_inflight_remove_endpoint: ") + eppscore_last_error(eng_));
+    if (running_) {  // the engine's one divergence: the recycled id's queue starts empty (include/eppscore.h)
+      if (eppscore_running_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_running_remove_endpoint: ") + eppscore_last_error(eng_));
+      for (auto k = running_keys_.begin(); k != running_keys_.end();) {
+        auto& v = k->second.endpoints;
+        v.erase(std::remove(v.begin(), v.end(), it->second), v.end());
+        k = v.empty() ? running_keys_.erase(k) : std::next(k);
+      }
+    }
     free_ids_.push_back(it->second);
     server_ids_.erase(it);
   }
@@ -558,6 +613,18 @@ class Scheduler {
       throw SchedulingError(std::string("eppscore_inflight_get: ") + eppscore_last_error(eng_));
     return {req[(size_t)id], tok[(size_t)id]};
   }
+  // getEndpointMinTPOTSLO / getEndpointRunningRequestCount (plugin.go:347-363) of one server from the engine's queues:
+  // {0, 0} without TrackRunningRequests or for a server never seen.
+  std::pair<double, int32_t> RunningRequests(const std::string& namespaced_name) {
+    const int id = ServerId(namespaced_name);
+    if (!running_ || id < 0) return {0.0, 0};
+    std::vector<double> mn((size_t)id + 1);
+    std::vector<int32_t> cnt((size_t)id + 1);
+    if (eppscore_running_get(eng_, mn.data(), cnt.data(), id + 1) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_running_get: ") + eppscore_last_error(eng_));
+    return {mn[(size_t)id], cnt[(size_t)id]};
+  }
+  size_t TrackedRequestIds() const { return running_keys_.size(); }  // ids with a live queue entry (their keys are kept)
   int ServerId(const std::string& namespaced_name) const {  // -1: never seen (or removed)
     auto it = server_ids_.find(namespaced_name);
     return it == server_ids_.end() ? -1 : it->second;
@@ -568,6 +635,50 @@ class Scheduler {
   eppscore_engine* engine() { return eng_; }
 
  private:
+  // x-slo-ttft-ms / x-slo-tpot-ms (predictedlatency/plugin.go:276-290): a parse error gives 0 (logged only)
+  static double SloHeader(const InferenceRequest& q, const char* key) {
+    auto it = q.Headers.find(key);
+    if (it == q.Headers.end()) return 0.0;
+    char* end = nullptr;
+    const double v = strtod(it->second.c_str(), &end);
+    return (end && *end == 0 && end != it->second.c_str()) ? v : 0.0;
+  }
+
+  // Exact request keys: x-request-id -> uint64 from 1, kept while the id has a live queue entry on some endpoint (the same id
+  // may be live on two endpoints, as queues are per endpoint in the reference).
+  struct KeyUse {
+    uint64_t key;
+    std::vector<int32_t> endpoints;  // where the id is live
+  };
+  uint64_t KeyFor(const std::string& rid) {
+    auto it = running_keys_.find(rid);
+    if (it != running_keys_.end()) return it->second.key;
+    const uint64_t k = next_key_++;
+    running_keys_.emplace(rid, KeyUse{k, {}});
+    return k;
+  }
+  void ReleaseKeyIfUnused(const std::string& rid) {
+    auto it = running_keys_.find(rid);
+    if (it != running_keys_.end() && it->second.endpoints.empty()) running_keys_.erase(it);
+  }
+  // removes (TargetEndpoints[0], request id) from the queues; nothing for an untracked id or a server that has left
+  void RunningRemove(const InferenceRequest& request, const SchedulingResult& result) {
+    if (!running_ || request.RequestId.empty()) return;
+    auto k = running_keys_.find(request.RequestId);
+    if (k == running_keys_.end()) return;
+    auto pr = result.ProfileResults.find(cfg_.ProfileName);
+    if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
+    const int32_t id = ServerId(pr->second.TargetEndpoints[0].Endpoint_->GetMetadata()->NamespacedName_.String());
+    auto& v = k->second.endpoints;
+    if (id < 0 || std::find(v.begin(), v.end(), id) == v.end()) return;
+    const uint64_t key = k->second.key;
+    uint8_t removed = 0;
+    if (eppscore_running_remove(eng_, 1, 0, &id, &key, &removed, nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_running_remove: ") + eppscore_last_error(eng_));
+    v.erase(std::find(v.begin(), v.end(), id));
+    if (v.empty()) running_keys_.erase(k);
+  }
+
   // SimpleTokenEstimator's inputs for one request (eppscore_estimate_tokens): the body is always present here
   static void EstimateInputs(const InferenceRequest& q, int64_t* size, int32_t* hint, int32_t* chars) {
     *size = q.RequestSizeBytes;
@@ -684,8 +795,9 @@ class Scheduler {
     // with the producer, a token-load scorer reads the engine's in-flight counters (a snapshot array would take precedence)
     s.inflight_tokens = (have_tokens && !(inflight_ && token_load_)) ? tokens.data() : nullptr;
     if (prod) {
-      s.min_tpot_slo = min_tpot.data();
-      s.dispatched = dispatched.data();
+      // with TrackRunningRequests the engine's queues feed the latency fold-in: the arrays stay NULL
+      s.min_tpot_slo = running_ ? nullptr : min_tpot.data();
+      s.dispatched = running_ ? nullptr : dispatched.data();
       s.prefill_role = prefill.data();
     }
     s.epoch = ++epoch_;
@@ -713,6 +825,11 @@ class Scheduler {
   bool token_load_ = false;  // the profile has a token-load scorer
   std::vector<int64_t> last_size_;  // estimator inputs of the last engine batch, per request
   std::vector<int32_t> last_hint_, last_chars_;
+  bool running_ = false;  // PredictedLatencyProducer::TrackRunningRequests
+  std::vector<std::string> last_rid_;  // PreRequest's inputs of the last engine batch, per request
+  std::vector<double> last_tpot_;
+  std::unordered_map<std::string, KeyUse> running_keys_;
+  uint64_t next_key_ = 1;
 };
 
 inline Scheduler* NewSchedulerWithConfig(const SchedulerConfig& c) { return new Scheduler(c); }

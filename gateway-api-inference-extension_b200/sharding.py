@@ -70,3 +70,19 @@ def gather_inflight_stream(dist, endpoint, tokens, g_endpoint, g_tokens):
     dist.all_gather_into_tensor(g_endpoint, endpoint)
     dist.all_gather_into_tensor(g_tokens, tokens)
     return g_endpoint, g_tokens
+
+
+def gather_running_stream(dist, endpoint, request_key, g_endpoint, g_key, tpot_slo=None, g_tpot=None):
+    """The running-request queue counterpart (predictedlatency/requestcontrol_hooks.go:73-86,219): every rank contributes its
+    shard's adds — endpoint i32[R] (-1: none), request key u64[R], tpot_slo f64[R] — or its removes (tpot_slo None), and
+    receives every shard's in rank order, which it applies with one eppscore_running_add (or _remove) of world*R entries.
+    Unlike the in-flight counters these updates do not commute when keys repeat (the first add of a key wins, a remove before
+    an add finds nothing), so every replica must apply the same concatenation in global request order, as the commit stream
+    does: shard r's requests are global requests [r*R, (r+1)*R).  Keys must be unique across shards; the caller assigns them
+    (e.g. rank in the top bits, or a key derived from the globally unique x-request-id).  g_* are the preallocated [world*R]
+    outputs; the keys travel as int64 (same bits)."""
+    dist.all_gather_into_tensor(g_endpoint, endpoint)
+    dist.all_gather_into_tensor(g_key, request_key)
+    if tpot_slo is not None:
+        dist.all_gather_into_tensor(g_tpot, tpot_slo)
+    return g_endpoint, g_key, g_tpot

@@ -380,6 +380,57 @@ int32_t eppscore_inflight_remove_endpoint(struct eppscore_engine *e, int32_t end
  * earlier mutation.  Either output may be NULL. */
 int32_t eppscore_inflight_get(struct eppscore_engine *e, int64_t *requests_out, int64_t *tokens_out, int32_t M);
 
+/* ---- running-request queues of the predicted-latency producer (predictedlatency/running_request_tpot_slo_queue.go) ----
+ * Per endpoint, the multiset of live requests (request key, tpot SLO), DEVICE-RESIDENT, empty at create.  Its view feeds the
+ * latency fold-in wherever the snapshot lacks the array (field by field; a snapshot array keeps precedence):
+ *   min_tpot_slo[m] = the smallest live tpot, 0 without a live entry   (getEndpointMinTPOTSLO, plugin.go:347-355)
+ *   dispatched[m]   = the number of live entries                        (getEndpointRunningRequestCount, plugin.go:357-363)
+ * Empty queues give 0 and 0, which score exactly like absent arrays.  Every mutation prepares the current snapshot's terms
+ * again on its stream when the queues feed them, with eppscore_set_snapshot's cross-stream ordering (legal inside a CUDA-graph
+ * capture); mutations of these queues and of the in-flight counters are ordered with each other in call order.
+ * Request keys are the caller's exact stand-ins for x-request-id (not hashes); 0 stands for an empty id.  The same key may be
+ * live on two endpoints, as queues are per endpoint in the reference.
+ * Order inside one call: equal to applying the R entries one by one in request order — of two adds of the same
+ * (endpoint, key) the lower r is added and keeps its tpot, of two removes the second finds nothing.  Between calls: stream
+ * order.  Entries with endpoint < 0 (unscheduled requests, pick -1) are skipped.  On host arrays an endpoint >= max_endpoints
+ * or a NaN tpot is ERR_INVALID before anything changes; on device arrays such an entry is skipped and the next
+ * eppscore_running_get returns ERR_INVALID.
+ * tpot: finite or +Inf.  0 is a live entry like any other (no x-slo-tpot-ms header): it becomes its endpoint's minimum, and a
+ * minimum of 0 turns the tightening of bufferedTPOT off (prediction.go:152, podMinTPOTSLO > 0).  -0.0 is accepted and stored
+ * as +0.0; every consumer compares with > 0, so this is not observable.
+ * Capacity: one open-addressing table of all live entries, at most half full counting tombstones.  Every add first compacts
+ * the table on the device when live + tombstones + R would pass half the slots (the live entries move into a spare table of
+ * the same size), so tombstones never run out, inside a replayed graph as well.  The kernels read the table through a
+ * device-resident descriptor: a call outside a capture may double the table (only while live + R exceed a quarter of the
+ * slots, so churn does not grow it), and graphs captured earlier keep working against the grown table.  A running_add under
+ * CUDA-graph capture cannot grow it and fails with ERR_CAPACITY unless live + R fits half the slots
+ * (eppscore_running_reserve makes room beforehand); replays must keep the live set within that room, or their adds are
+ * skipped and the next eppscore_running_get returns ERR_CAPACITY.  The first call outside a capture after a captured one
+ * reads the live count synchronously, as graph replays are invisible to the host.  Device-location calls are asynchronous
+ * on `stream` (NULL = engine stream); host-location calls return when the update is done. */
+/* PreRequest for a batch (requestcontrol_hooks.go:73-86): add (endpoint[r], request_key[r], tpot_slo[r]) for every r.  Refused
+ * (added_out[r] = 0, nothing changes) for key 0, tpot < 0, and an (endpoint, key) already live (its first tpot stays:
+ * running_request_tpot_slo_queue.go:127-137).  tpot_slo NULL: 0 for every entry.  added_out: optional [R], where the other
+ * arrays live.  A device-resident loop passes the batch's pick and tpot_slo buffers straight in. */
+int32_t eppscore_running_add(struct eppscore_engine *e, int32_t R, int32_t location, const int32_t *endpoint,
+                             const uint64_t *request_key, const double *tpot_slo, uint8_t *added_out, void *stream);
+/* End of stream (requestcontrol_hooks.go:219) or TTL expiry (plugin.go:190-196): remove each live (endpoint, key);
+ * removed_out[r] = 1 for the entries that removed one.  Absent pairs change nothing. */
+int32_t eppscore_running_remove(struct eppscore_engine *e, int32_t R, int32_t location, const int32_t *endpoint,
+                                const uint64_t *request_key, uint8_t *removed_out, void *stream);
+/* Empties `endpoint`'s queue, for a caller that recycles endpoint ids.  The reference has no counterpart: its queues are keyed
+ * by pod name and outlive the pod, so this is the one place the engine differs — a pod that leaves while requests still run on
+ * it and comes back under the same name starts empty here. */
+int32_t eppscore_running_remove_endpoint(struct eppscore_engine *e, int32_t endpoint);
+/* The view of the first M endpoints (min tpot as above, live count), read synchronously on the engine stream after every
+ * earlier mutation.  Either output may be NULL.  ERR_INVALID reports skipped device-array entries (see above); ERR_CAPACITY
+ * reports adds that found no room (a graph replayed past what eppscore_running_reserve provided). */
+int32_t eppscore_running_get(struct eppscore_engine *e, double *min_tpot_out, int32_t *count_out, int32_t M);
+/* Sizes the table so that it holds live_entries live entries (half its slots), and the per-call scratch for calls of up to
+ * live_entries entries: do this before capturing running calls into a CUDA graph.  Returns that capacity in entries (> 0),
+ * or a negative status; live_entries 0 only queries it. */
+int32_t eppscore_running_reserve(struct eppscore_engine *e, int64_t live_entries);
+
 /* pinned host memory for callers that want the fast copy path (cudaHostAlloc / cudaFreeHost) */
 void *eppscore_host_alloc(size_t bytes);
 void eppscore_host_free(void *p);
