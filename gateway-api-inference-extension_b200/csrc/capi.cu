@@ -4,15 +4,18 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/eppscore.h"
+#include "cuda_owners.hpp"
 #include "kernels.cuh"
 #include "prefix_index.hpp"
 #include "xxh64.cuh"
@@ -23,31 +26,16 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct DevBuf {
-  void* p = nullptr;
-  size_t bytes = 0;
-  cudaError_t reserve(size_t n) {
-    if (n <= bytes) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    bytes = 0;
-    size_t want = n + n / 8;  // a little slack so slowly growing batches do not reallocate every call
-    cudaError_t e = cudaMalloc(&p, want);
-    if (e == cudaSuccess) bytes = want;
-    return e;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    bytes = 0;
-  }
-  template <typename T>
-  T* as() const { return static_cast<T*>(p); }
-};
-
 struct PlanSet {
   Plan plan;
   const double* term_ptr[kMaxSteps];
+};
+
+// The last device-location batch a caller stream ran outside a capture (pending_record / pending_wait).
+struct PendingBatch {
+  cudaStream_t stream = nullptr;
+  Event done;          // recorded behind that batch
+  bool armed = false;  // the batch may not have completed
 };
 
 }  // namespace
@@ -58,8 +46,7 @@ struct eppscore_engine {
   eppscore_config cfg{};
   Geo geo{};
   int32_t A_cap = 64;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_snapshot = nullptr, ev_table = nullptr, ev_caller = nullptr;
+  Event ev_snapshot, ev_table, ev_caller;
   cudaStream_t snapshot_stream = nullptr;        // stream the last snapshot preparation ran on
   unsigned long long snapshot_capture_id = 0;    // != 0: ev_snapshot was recorded inside that CUDA-graph capture
   std::string err;
@@ -86,36 +73,37 @@ struct eppscore_engine {
 
   // prefix index: hashToPods + the per-endpoint LRUs, both device-resident (prefix_index.hpp); mutated on `stream`
   std::unique_ptr<DeviceIndex> index;
-  cudaEvent_t ev_sched = nullptr;   // last device-location schedule on a caller stream (index mutations wait for it)
-  bool sched_pending = false;
-  DevBuf c_pick, c_hash, c_nh, c_ep, c_op;  // staging for the host-array forms of commit_picks / prefix_add / prefix_apply
+  // device-location batches on caller streams that may still read the table, the terms or sc[0] (pending_record)
+  std::vector<PendingBatch> pending;
+  // Staging for the synchronous host-array calls: slot i holds the call's i-th array.  Each of those calls runs on `stream`
+  // and synchronises it before it returns, so one set serves them all.
+  DevBuf stage[6];
 
   // Producer state the scorers read: mutations of either producer below prepare the snapshot terms again (with last_pa) when
   // the state feeds the current snapshot.  Mutations outside a CUDA-graph capture are ordered through ev_producer, recorded
   // after each one on its stream, so the two families never rewrite the terms concurrently (producer_begin / producer_end).
-  cudaEvent_t ev_producer = nullptr;
+  Event ev_producer;
   bool producer_pending = false;
   PrepareArgs last_pa{};  // what the current snapshot was prepared with
 
   // in-flight load producer (inflightload/producer.go): per-endpoint request and token counters, [Mpad] int64 each, zeroed at
   // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens.
   DevBuf inflight_req, inflight_tok, inflight_err;
-  DevBuf c_iep, c_itok, c_esize, c_ehint, c_echars, c_eout;  // staging for the host-array forms
   bool snapshot_has_tokens = false;  // the current snapshot carries inflight_tokens
 
   // predicted-latency producer's running-request queues (running_kernel.cu): the (endpoint, key) -> tpot table and the
   // per-endpoint count / minimum.  They feed the latency fold-in when the snapshot lacks min_tpot_slo or dispatched.
-  DevBuf run_tab[8];  // two tables of run_cap slots (slot, tpot, owner, rm each): the table and its spare, in either role
+  std::array<DevBuf, 8> run_tab;  // two tables of run_cap slots (slot, tpot, owner, rm each): the table and its spare, in either role
   DevBuf run_desc;    // the device descriptor (RunDev) every running kernel reads the tables and the scratch through
   RunDev run_host{};  // its host copy (re-read before a change: the device-side compaction swaps the two tables)
   DevBuf run_count, run_min_bits, run_min_cnt, run_min_view, run_dirty, run_rc_min, run_rc_cnt, run_ctr;
-  DevBuf c_rep, c_rkey, c_rtpot, c_rslot, c_rwon;  // staging for host arrays and the per-call [R] scratch
+  DevBuf c_rslot, c_rwon;  // the per-call [R] scratch
   int64_t run_cap = 0;
   // host upper bounds of the live entries and tombstones: the counters copied back behind the last mutation (h_run,
   // ev_run_copy) once that copy has landed, plus R per call issued since
   int64_t run_bound_live = 0;
-  RunCounters* h_run = nullptr;
-  cudaEvent_t ev_run_copy = nullptr;
+  PinnedBuf h_run;  // RunCounters
+  Event ev_run_copy;
   bool run_copy_issued = false;
   bool run_captured = false;  // a mutation was captured since the last exact read: its replays are invisible to the bound
   bool snapshot_has_min_tpot = false, snapshot_has_dispatched = false;
@@ -125,25 +113,22 @@ struct eppscore_engine {
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
         s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s;
-    void release() {
-      DevBuf* all[] = {&s_prompts, &s_off, &s_len, &s_seed, &s_hashes, &s_nh, &s_adapter, &s_mask, &s_dense, &s_dtotal, &s_pick,
-                       &s_score, &s_tie, &s_match, &s_total, &s_scores, &s_intok, &s_tslo, &s_pslo, &s_pred, &s_fields, &s_fmask,
-                       &s_topk_m, &s_topk_s};
-      for (DevBuf* b : all) b->release();
-    }
   } sc[4];
   // pinned staging for the small per-request results of a host batch: a D2H copy into the caller's (usually pageable)
   // arrays would block the host after every chunk and serialise the pipeline
-  void* h_res = nullptr;
-  size_t h_res_bytes = 0;
-  cudaStream_t stream2 = nullptr;   // second copy/compute stream of the chunked host path
+  PinnedBuf h_res;
   int32_t host_chunk = 8192;        // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
   // (eppscore_set_debug keys 5 and 6)
   int32_t dev_split = 1, dev_streams = 2;
-  cudaStream_t split_stream[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t ev_fork = nullptr, ev_join[3] = {nullptr, nullptr, nullptr};
+  Event ev_fork, ev_join[3];
+
+  // The streams come last: members are destroyed in reverse order, and a Stream synchronises before it is destroyed, so
+  // every buffer above is freed only after the work queued on these streams has finished.
+  Stream stream;           // the engine stream
+  Stream stream2;          // second copy/compute stream of the chunked host path
+  Stream split_stream[3];  // the internal streams of a sliced device-location batch
 };
 using Scratch = eppscore_engine::Scratch;
 
@@ -162,6 +147,48 @@ int32_t cuda_fail(eppscore_engine* e, cudaError_t c, const char* what) {
     cudaError_t _c = (call);                                   \
     if (_c != cudaSuccess) return cuda_fail((e), _c, #call);   \
   } while (0)
+
+// Whether `st` is being captured into a CUDA graph; *id (when given) receives the capture's id, 0 outside a capture.
+bool is_capturing(cudaStream_t st, unsigned long long* id = nullptr) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  unsigned long long cap_id = 0;
+  cudaStreamGetCaptureInfo(st, &cap, &cap_id);
+  const bool capturing = cap != cudaStreamCaptureStatusNone;
+  if (id) *id = capturing ? cap_id : 0;
+  return capturing;
+}
+
+// A device-location batch on caller stream `s` may still read the index table, the snapshot terms and the scratch set sc[0]
+// when its call returns.  Outside a capture its stream's event is recorded again behind it, so the set of pending batches
+// holds one event per caller stream.  Whatever rewrites those first waits for all of them (pending_wait).  Inside a capture
+// the graph's edges order this instead, and the engine stream orders itself.
+int32_t pending_record(eppscore_engine* e, cudaStream_t s) {
+  if (s == e->stream || is_capturing(s)) return EPPSCORE_OK;
+  PendingBatch* slot = nullptr;
+  for (PendingBatch& p : e->pending) {
+    if (p.armed && p.stream == s) {
+      slot = &p;
+      break;
+    }
+    if (!p.armed && !slot) slot = &p;
+  }
+  if (!slot) slot = &e->pending.emplace_back();
+  if (!slot->done) CK(e, make(slot->done));
+  CK(e, cudaEventRecord(slot->done, s));
+  slot->stream = s;
+  slot->armed = true;
+  return EPPSCORE_OK;
+}
+// `st` waits for every pending batch.  A batch leaves the set once it has completed, not when a stream waits for it: the wait
+// orders only `st`, and a later rewrite on another stream must still wait.
+int32_t pending_wait(eppscore_engine* e, cudaStream_t st) {
+  for (PendingBatch& p : e->pending) {
+    if (!p.armed) continue;
+    if (cudaEventQuery(p.done) == cudaSuccess) p.armed = false;
+    else CK(e, cudaStreamWaitEvent(st, p.done, 0));
+  }
+  return EPPSCORE_OK;
+}
 
 bool is_endpoint_term_kind(int k, bool masked) {
   if (k == EPPSCORE_SCORER_KV_CACHE || k == EPPSCORE_SCORER_TOKEN_LOAD) return true;
@@ -185,7 +212,6 @@ bool counters_feed_scorer(const eppscore_engine* e) {
 bool running_feeds_scorer(const eppscore_engine* e) {
   return e->have_snapshot && e->lat_ep.p && (!e->snapshot_has_min_tpot || !e->snapshot_has_dispatched);
 }
-bool producers_feed_scorer(const eppscore_engine* e) { return counters_feed_scorer(e) || running_feeds_scorer(e); }
 
 // Translate the scorer list into kernel steps.  Leading request-independent scorers are folded into
 // one precomputed array ((0.0+t0)+t1)+… — exact, because the kernel adds in the same order.
@@ -254,13 +280,7 @@ void build_plan(eppscore_engine* e, bool masked, PlanSet* ps) {
 
 // Index mutations run on the engine stream.  They must not overtake scoring kernels that other streams launched
 // earlier against the same table, and later scoring on other streams waits for ev_table.
-int32_t index_begin(eppscore_engine* e) {
-  if (e->sched_pending) {
-    CK(e, cudaStreamWaitEvent(e->stream, e->ev_sched, 0));
-    e->sched_pending = false;
-  }
-  return EPPSCORE_OK;
-}
+int32_t index_begin(eppscore_engine* e) { return pending_wait(e, e->stream); }
 int32_t index_end(eppscore_engine* e) {
   CK(e, cudaEventRecord(e->ev_table, e->stream));
   return EPPSCORE_OK;
@@ -273,17 +293,12 @@ int32_t index_end(eppscore_engine* e) {
 int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st) {
   e->launches += launch_prepare_snapshot(e->last_pa, st);
   CK(e, cudaGetLastError());
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   unsigned long long cap_id = 0;
-  cudaStreamGetCaptureInfo(st, &cap, &cap_id);
+  const bool capturing = is_capturing(st, &cap_id);
   CK(e, cudaEventRecord(e->ev_snapshot, st));
   e->snapshot_stream = st;
-  if (cap == cudaStreamCaptureStatusNone) {
-    e->snapshot_capture_id = 0;
-    if (st != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_snapshot, 0));
-  } else {
-    e->snapshot_capture_id = cap_id;
-  }
+  e->snapshot_capture_id = cap_id;
+  if (!capturing && st != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_snapshot, 0));
   return EPPSCORE_OK;
 }
 
@@ -291,9 +306,7 @@ int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st) {
 // family (they do not all commute: remove_endpoint sets to zero, and both families prepare the same snapshot terms again),
 // unless `st` is being captured, where the caller's graph edges order them.
 int32_t producer_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cap);
-  *capturing = cap != cudaStreamCaptureStatusNone;
+  *capturing = is_capturing(st);
   if (!*capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
   return EPPSCORE_OK;
 }
@@ -303,8 +316,8 @@ int32_t producer_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
 // another stream launched against the current terms finishes reading them first).
 int32_t producer_end(eppscore_engine* e, cudaStream_t st, bool capturing, bool feeds) {
   if (feeds) {
-    if (!capturing && e->sched_pending) CK(e, cudaStreamWaitEvent(st, e->ev_sched, 0));
-    const int32_t rc = prepare_snapshot(e, st);
+    int32_t rc = capturing ? EPPSCORE_OK : pending_wait(e, st);
+    if (rc == EPPSCORE_OK) rc = prepare_snapshot(e, st);
     if (rc != EPPSCORE_OK) return rc;
   }
   if (!capturing) {
@@ -359,10 +372,8 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   // The hash kernels depend on neither, so the snapshot wait is issued only before the pick kernel: a caller
   // may prepare the snapshot on a second stream concurrently with the hashing of the batch.
   // Under CUDA-graph capture a stream may only wait on events recorded inside the SAME capture.
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   unsigned long long cap_id = 0;
-  cudaStreamGetCaptureInfo(s, &cap, &cap_id);
-  const bool capturing = cap != cudaStreamCaptureStatusNone;
+  const bool capturing = is_capturing(s, &cap_id);
   if (!capturing && s != e->stream) CK(e, cudaStreamWaitEvent(s, e->ev_table, 0));
   const bool wait_snapshot = capturing ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
                                        : (e->snapshot_capture_id == 0 && s != e->snapshot_stream);
@@ -476,11 +487,6 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   if (launched == 0) launched = launch_score_pick(a, dense, s, e->sm_count);
   e->launches += launched;
   CK(e, cudaGetLastError());
-  // a later index mutation (engine stream), or a producer mutation that prepares the terms again, must wait for this batch
-  if (!capturing && s != e->stream && (a.table || producers_feed_scorer(e))) {
-    CK(e, cudaEventRecord(e->ev_sched, s));
-    e->sched_pending = true;
-  }
   return EPPSCORE_OK;
 }
 
@@ -494,20 +500,42 @@ int32_t h2d(eppscore_engine* e, DevBuf& buf, const T* src, size_t count, const T
   return EPPSCORE_OK;
 }
 
+// Copies the bytes of prompts [r0, r1) from the host to `buf` on `st`; *out is the device base that the caller's offsets
+// index into.  The extent comes from prompt_off (and prompt_len when given).  The copy starts at a 16-byte aligned source
+// offset so every prompt keeps its alignment (the fast hash path needs 16-byte aligned starts), and is padded by 64 B so
+// 16-byte vector loads of the last block never leave the allocation.
+int32_t stage_prompts(eppscore_engine* e, DevBuf& buf, const uint8_t* bytes, const int64_t* off, const int32_t* len, int32_t r0,
+                      int32_t r1, cudaStream_t st, const uint8_t** out) {
+  size_t lo = (size_t)off[r0], hi = (size_t)off[r1];
+  if (len) {
+    lo = SIZE_MAX;
+    hi = 0;
+    for (int32_t r = r0; r < r1; r++) {
+      lo = std::min(lo, (size_t)off[r]);
+      hi = std::max(hi, (size_t)off[r] + (size_t)len[r]);
+    }
+    if (lo > hi) lo = hi = 0;
+  }
+  const size_t start = lo & ~(size_t)15;
+  CK(e, buf.reserve(hi - start + 64));
+  if (hi > start) CK(e, cudaMemcpyAsync(buf.p, bytes + start, hi - start, cudaMemcpyHostToDevice, st));
+  *out = buf.as<uint8_t>() - start;
+  return EPPSCORE_OK;
+}
+
 constexpr int64_t kRunInitialSlots = 4096;
 
-// A running-request table of `slots` slots (a power of two), empty: slots {0, 0}, no bids.  tpot needs no initial value.
-cudaError_t run_alloc_table(eppscore_engine* e, int64_t slots, DevBuf* slot, DevBuf* tpot, DevBuf* owner, DevBuf* rm, cudaStream_t st) {
-  (void)e;
+// A running-request table of `slots` slots (a power of two) in t[0..3] (slot, tpot, owner, rm), empty: slots {0, 0}, no
+// bids.  tpot needs no initial value.
+cudaError_t run_alloc_table(int64_t slots, DevBuf* t, cudaStream_t st) {
   const size_t n = (size_t)slots;
   cudaError_t c;
-  if ((c = slot->reserve(n * sizeof(RunSlot))) != cudaSuccess) return c;
-  if ((c = tpot->reserve(n * 8)) != cudaSuccess) return c;
-  if ((c = owner->reserve(n * 8)) != cudaSuccess) return c;
-  if ((c = rm->reserve(n * 8)) != cudaSuccess) return c;
-  if ((c = cudaMemsetAsync(slot->p, 0, n * sizeof(RunSlot), st)) != cudaSuccess) return c;
-  if ((c = cudaMemsetAsync(owner->p, 0xff, n * 8, st)) != cudaSuccess) return c;
-  return cudaMemsetAsync(rm->p, 0xff, n * 8, st);
+  if ((c = t[0].reserve(n * sizeof(RunSlot))) != cudaSuccess) return c;
+  for (int i = 1; i < 4; i++)
+    if ((c = t[i].reserve(n * 8)) != cudaSuccess) return c;
+  if ((c = cudaMemsetAsync(t[0].p, 0, n * sizeof(RunSlot), st)) != cudaSuccess) return c;
+  if ((c = cudaMemsetAsync(t[2].p, 0xff, n * 8, st)) != cudaSuccess) return c;
+  return cudaMemsetAsync(t[3].p, 0xff, n * 8, st);
 }
 
 // The descriptor as created: tab[0..3] the table, tab[4..7] its spare, the per-endpoint arrays, the scratch.
@@ -652,9 +680,10 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
     const char* fg = getenv("EPPSCORE_FORCE_GENERIC");
     ep->force_generic = fg && fg[0] == '1';
   }
-  CK(nullptr, cudaStreamCreateWithFlags(&ep->stream, cudaStreamNonBlocking));
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_snapshot, cudaEventDisableTiming));
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_table, cudaEventDisableTiming));
+  // every failure below frees what was allocated before it (the engine's members own it)
+  CK(nullptr, make(ep->stream));
+  CK(nullptr, make(ep->ev_snapshot));
+  CK(nullptr, make(ep->ev_table));
   // endpoint tile buffers
   const size_t mp = (size_t)ep->geo.Mpad;
   CK(nullptr, ep->raw_kv.reserve(mp * 8));
@@ -672,7 +701,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   CK(nullptr, cudaMemsetAsync(ep->inflight_req.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_tok.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_err.p, 0, 4, ep->stream));
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_producer, cudaEventDisableTiming));
+  CK(nullptr, make(ep->ev_producer));
   CK(nullptr, init_inflight_update());
   {  // running-request queues: every endpoint empty, a small table (grown by the first calls that need room)
     CK(nullptr, ep->run_count.reserve(mp * 4));
@@ -693,11 +722,11 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
     RunCounters c0{};
     c0.gen = 1;  // owner words of slots that predate every call are 0 (gen 0)
     CK(nullptr, cudaMemcpyAsync(ep->run_ctr.p, &c0, sizeof(c0), cudaMemcpyHostToDevice, ep->stream));
-    CK(nullptr, cudaHostAlloc(&ep->h_run, sizeof(RunCounters), cudaHostAllocDefault));
-    memset(ep->h_run, 0, sizeof(RunCounters));
-    CK(nullptr, cudaEventCreateWithFlags(&ep->ev_run_copy, cudaEventDisableTiming));
-    CK(nullptr, run_alloc_table(ep, kRunInitialSlots, &ep->run_tab[0], &ep->run_tab[1], &ep->run_tab[2], &ep->run_tab[3], ep->stream));
-    CK(nullptr, run_alloc_table(ep, kRunInitialSlots, &ep->run_tab[4], &ep->run_tab[5], &ep->run_tab[6], &ep->run_tab[7], ep->stream));
+    CK(nullptr, ep->h_run.reserve(sizeof(RunCounters)));
+    memset(ep->h_run.p, 0, sizeof(RunCounters));
+    CK(nullptr, make(ep->ev_run_copy));
+    CK(nullptr, run_alloc_table(kRunInitialSlots, &ep->run_tab[0], ep->stream));
+    CK(nullptr, run_alloc_table(kRunInitialSlots, &ep->run_tab[4], ep->stream));
     ep->run_cap = kRunInitialSlots;
     CK(nullptr, ep->c_rslot.reserve(kRunInitialSlots * 4));
     CK(nullptr, ep->c_rwon.reserve(kRunInitialSlots));
@@ -747,8 +776,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
     break;
   }
   // prefix index (device-resident: slot table + per-endpoint LRUs; the LRU regions are allocated by the first Add)
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_sched, cudaEventDisableTiming));
-  CK(nullptr, cudaEventCreateWithFlags(&ep->ev_caller, cudaEventDisableTiming));
+  CK(nullptr, make(ep->ev_caller));
   ep->index = std::make_unique<DeviceIndex>(ep->geo.Mpad, ep->geo.Mpad / 32, ep->cfg.prefix_capacity, ep->cfg.lru_capacity_default,
                                             ep->cfg.lru_capacity_max);
   CK(nullptr, ep->index->init(ep->stream));
@@ -762,42 +790,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
 void eppscore_destroy(eppscore_engine* e) {
   if (!e) return;
   cudaSetDevice(e->device);
-  cudaStreamSynchronize(e->stream);
-  DevBuf* bufs[] = {&e->qhdr[0], &e->qhdr[1], &e->qbucket[0], &e->qbucket[1], &e->raw_min_tpot, &e->raw_dispatched, &e->raw_prefill, &e->raw_tokens, &e->lat_ep,
-                    &e->raw_kv, &e->raw_queue, &e->raw_running, &e->raw_act, &e->raw_wait, &e->raw_nmodels, &e->raw_max,
-                    &e->fold_unmasked, &e->fold_masked, &e->cls_lo, &e->cls_hi, &e->summ, &e->tiemask, &e->prefix_lut2d, &e->c_pick, &e->c_hash, &e->c_nh,
-                    &e->c_ep, &e->c_op, &e->inflight_req, &e->inflight_tok, &e->inflight_err, &e->c_iep, &e->c_itok, &e->c_esize,
-                    &e->c_ehint, &e->c_echars, &e->c_eout, &e->run_desc, &e->run_count,
-                    &e->run_min_bits, &e->run_min_cnt, &e->run_min_view, &e->run_dirty, &e->run_rc_min, &e->run_rc_cnt, &e->run_ctr,
-                    &e->c_rep, &e->c_rkey, &e->c_rtpot, &e->c_rslot, &e->c_rwon};
-  for (auto& x : e->sc) x.release();
-  for (auto& x : e->run_tab) x.release();
-  for (int i = 0; i < 3; i++) {
-    if (e->split_stream[i]) {
-      cudaStreamSynchronize(e->split_stream[i]);
-      cudaStreamDestroy(e->split_stream[i]);
-    }
-    if (e->ev_join[i]) cudaEventDestroy(e->ev_join[i]);
-  }
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->h_res) cudaFreeHost(e->h_res);
-  if (e->stream2) {
-    cudaStreamSynchronize(e->stream2);
-    cudaStreamDestroy(e->stream2);
-  }
-  for (DevBuf* b : bufs) b->release();
-  for (int i = 0; i < 4; i++) e->raw_col[i].release();
-  for (int i = 0; i < kMaxSteps; i++) e->term[i].release();
-  e->index.reset();
-  if (e->ev_producer) cudaEventDestroy(e->ev_producer);
-  if (e->ev_run_copy) cudaEventDestroy(e->ev_run_copy);
-  if (e->h_run) cudaFreeHost(e->h_run);
-  if (e->ev_sched) cudaEventDestroy(e->ev_sched);
-  if (e->ev_caller) cudaEventDestroy(e->ev_caller);
-  if (e->ev_snapshot) cudaEventDestroy(e->ev_snapshot);
-  if (e->ev_table) cudaEventDestroy(e->ev_table);
-  if (e->stream) cudaStreamDestroy(e->stream);
-  delete e;
+  delete e;  // the engine's streams synchronise first, then everything else is freed (eppscore_engine's member order)
 }
 
 const char* eppscore_last_error(const eppscore_engine* e) { return e ? e->err.c_str() : g_create_error.c_str(); }
@@ -865,12 +858,11 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   cudaStream_t st = (on_device && s->stream) ? (cudaStream_t)s->stream : e->stream;
   const size_t M = (size_t)s->M;
   const bool have_lora = s->lora_active && s->lora_waiting && s->lora_words > 0;
-  {  // the term / class-plane / summary buffers are rewritten below: a device-location batch that another stream launched
-     // against the previous snapshot must have finished with them (inside a capture the graph's own edges order this)
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cap);
-    if (cap == cudaStreamCaptureStatusNone && e->sched_pending) CK(e, cudaStreamWaitEvent(st, e->ev_sched, 0));
-  }
+  const bool capturing = is_capturing(st);
+  int32_t rc;
+  // the term / class-plane / summary buffers are rewritten below: a device-location batch that another stream launched
+  // against the previous snapshot must have finished with them (inside a capture the graph's own edges order this)
+  if (!capturing && (rc = pending_wait(e, st)) != EPPSCORE_OK) return rc;
   // Host snapshots are copied into the engine's tile buffers; device snapshots (e.g. the buffer an NCCL
   // broadcast just filled) are used IN PLACE — they must stay valid until the next set_snapshot.
   if (!on_device) {
@@ -928,11 +920,8 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   // eppscore_inflight_add, which scores exactly like an absent attribute, token_load.go:91-98)
   pa.tokens = s->inflight_tokens ? (on_device ? s->inflight_tokens : e->raw_tokens.as<int64_t>()) : e->inflight_tok.as<int64_t>();
   const bool reads_running = e->lat_ep.p && (!s->min_tpot_slo || !s->dispatched);
-  if ((!s->inflight_tokens || reads_running) && e->producer_pending) {  // producer state last changed on another stream
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cap);
-    if (cap == cudaStreamCaptureStatusNone) CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
-  }
+  if ((!s->inflight_tokens || reads_running) && e->producer_pending && !capturing)  // producer state last changed on another stream
+    CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
   pa.token_threshold = e->cfg.token_load_threshold;
   e->lat_args = LatArgs{};
   if (e->lat_ep.p) {
@@ -1007,11 +996,8 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   e->snapshot_has_min_tpot = s->min_tpot_slo != nullptr;
   e->snapshot_has_dispatched = s->dispatched != nullptr;
   e->last_pa = pa;
-  int32_t rc = prepare_snapshot(e, st);
-  if (rc != EPPSCORE_OK) return rc;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cap);
-  if (cap == cudaStreamCaptureStatusNone && !on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
+  if ((rc = prepare_snapshot(e, st)) != EPPSCORE_OK) return rc;
+  if (!capturing && !on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
   e->have_snapshot = true;
   return EPPSCORE_OK;
 }
@@ -1073,13 +1059,16 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     int K = e->dev_split;
     if (!sliceable || e->dev_streams < 2) K = 1;
     while (K > 1 && b->R / K < 2048) K--;
-    if (K <= 1) return schedule_device(e, d, cs, e->sc[0]);
+    if (K <= 1) {
+      if ((rc = schedule_device(e, d, cs, e->sc[0])) != EPPSCORE_OK) return rc;
+      return pending_record(e, cs);
+    }
     // fork: the internal streams join the caller's stream (also inside a CUDA-graph capture), slice c goes to stream c mod S
     const int S = e->dev_streams < K ? e->dev_streams : K;
-    if (!e->ev_fork) CK(e, cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
+    if (!e->ev_fork) CK(e, make(e->ev_fork));
     for (int i = 0; i < S - 1; i++) {
-      if (!e->split_stream[i]) CK(e, cudaStreamCreateWithFlags(&e->split_stream[i], cudaStreamNonBlocking));
-      if (!e->ev_join[i]) CK(e, cudaEventCreateWithFlags(&e->ev_join[i], cudaEventDisableTiming));
+      if (!e->split_stream[i]) CK(e, make(e->split_stream[i]));
+      if (!e->ev_join[i]) CK(e, make(e->ev_join[i]));
     }
     CK(e, cudaEventRecord(e->ev_fork, cs));
     for (int i = 0; i < S - 1; i++) CK(e, cudaStreamWaitEvent(e->split_stream[i], e->ev_fork, 0));
@@ -1111,13 +1100,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
       cudaStreamWaitEvent(cs, e->ev_join[i], 0);
     }
     if (rc != EPPSCORE_OK) return rc;
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(cs, &cap);
-    if (cap == cudaStreamCaptureStatusNone && cs != e->stream) {
-      CK(e, cudaEventRecord(e->ev_sched, cs));
-      e->sched_pending = true;
-    }
-    return EPPSCORE_OK;
+    return pending_record(e, cs);
   }
   // ---- host buffers: H2D, kernels, D2H, all inside this call ----
   // The batch is cut into chunks that alternate between two streams (each with its own scratch set): the H2D copy of
@@ -1135,19 +1118,16 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   int32_t chunk = e->host_chunk > 0 ? e->host_chunk : b->R;
   if (diag || b->R < 2 * chunk) chunk = b->R;
   const int nstreams = chunk < b->R ? 2 : 1;
-  if (nstreams == 2 && !e->stream2) CK(e, cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
+  if (nstreams == 2 && !e->stream2) CK(e, make(e->stream2));
+  // the chunks reuse sc[0] / sc[1], which a device-location batch may still hold
+  if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
+  if (nstreams == 2 && (rc = pending_wait(e, e->stream2)) != EPPSCORE_OK) return rc;
   // pinned staging: pick i32 | score f64 | tie i32 | total u16, each [R]; top-k endpoints i32 | scores f64, each [R*k]
   const size_t RR = (size_t)b->R, RK = RR * (size_t)tk;
   const size_t o_score = (RR * 4 + 7) & ~(size_t)7, o_tie = o_score + RR * 8, o_total = o_tie + RR * 4;
   const size_t o_tkm = (o_total + RR * 2 + 7) & ~(size_t)7, o_tks = (o_tkm + RK * 4 + 7) & ~(size_t)7, res_bytes = o_tks + RK * 8;
-  if (e->h_res_bytes < res_bytes) {
-    if (e->h_res) cudaFreeHost(e->h_res);
-    e->h_res = nullptr;
-    e->h_res_bytes = 0;
-    CK(e, cudaHostAlloc(&e->h_res, res_bytes + res_bytes / 4, cudaHostAllocDefault));
-    e->h_res_bytes = res_bytes + res_bytes / 4;
-  }
-  unsigned char* hres = static_cast<unsigned char*>(e->h_res);
+  CK(e, e->h_res.reserve(res_bytes));
+  unsigned char* hres = e->h_res.as<unsigned char>();
   int32_t* hp_pick = reinterpret_cast<int32_t*>(hres);
   double* hp_score = reinterpret_cast<double*>(hres + o_score);
   int32_t* hp_tie = reinterpret_cast<int32_t*>(hres + o_tie);
@@ -1166,25 +1146,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     d.hash_stride = b->hash_stride;
     d.block_chars = b->block_chars;
     d.max_blocks = b->max_blocks;
-    if (b->prompt_bytes) {
-      // byte range of the chunk; the device copy starts at a 16-byte aligned source offset so every prompt keeps its
-      // alignment (the fast hash path needs 16-byte aligned starts), and the kernel keeps using the caller's offsets
-      size_t lo = (size_t)b->prompt_off[r0], hi = (size_t)b->prompt_off[r1];
-      if (b->prompt_len) {
-        lo = SIZE_MAX;
-        hi = 0;
-        for (int32_t r = r0; r < r1; r++) {
-          lo = std::min(lo, (size_t)b->prompt_off[r]);
-          hi = std::max(hi, (size_t)b->prompt_off[r] + (size_t)b->prompt_len[r]);
-        }
-        if (lo > hi) lo = hi = 0;
-      }
-      const size_t start = lo & ~(size_t)15;
-      // pad the device copy so 16-byte vector loads of the last block never leave the allocation
-      CK(e, sc.s_prompts.reserve(hi - start + 64));
-      if (hi > start) CK(e, cudaMemcpyAsync(sc.s_prompts.p, b->prompt_bytes + start, hi - start, cudaMemcpyHostToDevice, st));
-      d.prompt_bytes = sc.s_prompts.as<uint8_t>() - start;
-      if ((rc = h2d(e, sc.s_off, b->prompt_off + r0, R + 1, &d.prompt_off, st)) != EPPSCORE_OK) return rc;
+    if (b->prompt_bytes) {  // the kernels keep using the caller's offsets
+      if ((rc = stage_prompts(e, sc.s_prompts, b->prompt_bytes, b->prompt_off, b->prompt_len, r0, r1, st, &d.prompt_bytes)) != EPPSCORE_OK ||
+          (rc = h2d(e, sc.s_off, b->prompt_off + r0, R + 1, &d.prompt_off, st)) != EPPSCORE_OK)
+        return rc;
     }
 #define H2D(buf, field, per) \
   if ((rc = h2d(e, sc.buf, b->field ? b->field + (size_t)r0 * (per) : b->field, R * (per), &d.field, st)) != EPPSCORE_OK) return rc;
@@ -1269,7 +1234,6 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     memcpy(t->endpoints, hp_tkm, RK * 4);
     memcpy(t->scores, hp_tks, RK * 8);
   }
-  e->sched_pending = false;  // everything launched above has completed
   return EPPSCORE_OK;
 }
 
@@ -1296,13 +1260,13 @@ int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, c
   const int32_t mb = max_blocks > 0 ? max_blocks : e->cfg.max_blocks;
   if (mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
   CK(e, cudaSetDevice(e->device));
-  HashArgs h{};
-  h.R = R;
-  h.block_chars = bc;
-  h.max_blocks = mb;
-  h.stride = mb;
-  h.stage_mask = e->hash_stage_mask;
   if (location == 1) {
+    HashArgs h{};
+    h.R = R;
+    h.block_chars = bc;
+    h.max_blocks = mb;
+    h.stride = mb;
+    h.stage_mask = e->hash_stage_mask;
     h.bytes = prompt_bytes;
     h.off = prompt_off;
     h.len = prompt_len;
@@ -1313,27 +1277,25 @@ int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, c
     CK(e, cudaGetLastError());
     return EPPSCORE_OK;
   }
+  // host arrays: staged, hashed by the device form on the engine stream, copied back
+  const uint8_t* d_bytes;
+  const int64_t* d_off;
+  const int32_t* d_len;
+  const uint64_t* d_seed;
   int32_t rc;
-  size_t total = (size_t)prompt_off[R];
-  if (prompt_len) {
-    total = 0;
-    for (int32_t r = 0; r < R; r++) total = std::max(total, (size_t)prompt_off[r] + (size_t)prompt_len[r]);
-  }
-  CK(e, e->sc[0].s_prompts.reserve(total + 64));
-  if (total) CK(e, cudaMemcpyAsync(e->sc[0].s_prompts.p, prompt_bytes, total, cudaMemcpyHostToDevice, e->stream));
-  h.bytes = e->sc[0].s_prompts.as<uint8_t>();
-  if ((rc = h2d(e, e->sc[0].s_off, prompt_off, (size_t)R + 1, &h.off)) != EPPSCORE_OK) return rc;
-  if ((rc = h2d(e, e->sc[0].s_len, prompt_len, (size_t)R, &h.len)) != EPPSCORE_OK) return rc;
-  if ((rc = h2d(e, e->sc[0].s_seed, model_seed, (size_t)R, &h.seed)) != EPPSCORE_OK) return rc;
-  CK(e, e->sc[0].s_hashes.reserve((size_t)R * mb * 8));
-  CK(e, e->sc[0].s_nh.reserve((size_t)R * 2));
-  CK(e, cudaMemsetAsync(e->sc[0].s_hashes.p, 0, (size_t)R * mb * 8, e->stream));
-  h.hashes = e->sc[0].s_hashes.as<uint64_t>();
-  h.n_hashes = e->sc[0].s_nh.as<uint16_t>();
-  e->launches += launch_hash_prompts(h, e->stream, e->sm_count);
-  CK(e, cudaGetLastError());
-  CK(e, cudaMemcpyAsync(hashes_out, h.hashes, (size_t)R * mb * 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaMemcpyAsync(n_hashes_out, h.n_hashes, (size_t)R * 2, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = stage_prompts(e, e->stage[0], prompt_bytes, prompt_off, prompt_len, 0, R, e->stream, &d_bytes)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], prompt_off, (size_t)R + 1, &d_off)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], prompt_len, (size_t)R, &d_len)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[3], model_seed, (size_t)R, &d_seed)) != EPPSCORE_OK)
+    return rc;
+  CK(e, e->stage[4].reserve((size_t)R * mb * 8));
+  CK(e, e->stage[5].reserve((size_t)R * 2));
+  CK(e, cudaMemsetAsync(e->stage[4].p, 0, (size_t)R * mb * 8, e->stream));  // entries past n_hashes[r] are zero
+  rc = eppscore_hash_prompts(e, R, 1, d_bytes, d_off, d_len, d_seed, bc, mb, e->stage[4].as<uint64_t>(), e->stage[5].as<uint16_t>(),
+                             e->stream);
+  if (rc != EPPSCORE_OK) return rc;
+  CK(e, cudaMemcpyAsync(hashes_out, e->stage[4].p, (size_t)R * mb * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaMemcpyAsync(n_hashes_out, e->stage[5].p, (size_t)R * 2, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
   return EPPSCORE_OK;
 }
@@ -1361,22 +1323,18 @@ int32_t eppscore_count_fields(eppscore_engine* e, int32_t R, int32_t location, c
     CK(e, cudaGetLastError());
     return EPPSCORE_OK;
   }
-  size_t total = (size_t)prompt_off[R];
-  if (prompt_len) {
-    total = 0;
-    for (int32_t r = 0; r < R; r++) total = std::max(total, (size_t)prompt_off[r] + (size_t)prompt_len[r]);
-  }
-  CK(e, e->sc[0].s_prompts.reserve(total + 64));
-  if (total) CK(e, cudaMemcpyAsync(e->sc[0].s_prompts.p, prompt_bytes, total, cudaMemcpyHostToDevice, e->stream));
-  const int64_t* d_off = nullptr;
-  const int32_t* d_len = nullptr;
+  // host arrays: staged, counted by the device form on the engine stream, copied back
+  const uint8_t* d_bytes;
+  const int64_t* d_off;
+  const int32_t* d_len;
   int32_t rc;
-  if ((rc = h2d(e, e->sc[0].s_off, prompt_off, (size_t)R + 1, &d_off)) != EPPSCORE_OK) return rc;
-  if ((rc = h2d(e, e->sc[0].s_len, prompt_len, (size_t)R, &d_len)) != EPPSCORE_OK) return rc;
-  CK(e, e->sc[0].s_fields.reserve((size_t)R * 4));
-  e->launches += launch_count_fields(e->sc[0].s_prompts.as<uint8_t>(), d_off, d_len, R, e->sc[0].s_fields.as<int32_t>(), e->stream, e->sm_count);
-  CK(e, cudaGetLastError());
-  CK(e, cudaMemcpyAsync(out, e->sc[0].s_fields.p, (size_t)R * 4, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = stage_prompts(e, e->stage[0], prompt_bytes, prompt_off, prompt_len, 0, R, e->stream, &d_bytes)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], prompt_off, (size_t)R + 1, &d_off)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], prompt_len, (size_t)R, &d_len)) != EPPSCORE_OK)
+    return rc;
+  CK(e, e->stage[3].reserve((size_t)R * 4));
+  if ((rc = eppscore_count_fields(e, R, 1, d_bytes, d_off, d_len, e->stage[3].as<int32_t>(), e->stream)) != EPPSCORE_OK) return rc;
+  CK(e, cudaMemcpyAsync(out, e->stage[3].p, (size_t)R * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
   return EPPSCORE_OK;
 }
@@ -1420,14 +1378,15 @@ int32_t eppscore_commit_picks(eppscore_engine* e, int32_t R, const int32_t* pick
   int32_t rc = pad_caps(e, lru_capacity, &caps);
   if (rc != EPPSCORE_OK) return rc;
   if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
-  CK(e, e->c_pick.reserve((size_t)R * 4));
-  CK(e, e->c_hash.reserve((size_t)R * hash_stride * 8));
-  CK(e, e->c_nh.reserve((size_t)R * 2));
-  CK(e, cudaMemcpyAsync(e->c_pick.p, pick, (size_t)R * 4, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->c_hash.p, hashes, (size_t)R * hash_stride * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->c_nh.p, n_hashes, (size_t)R * 2, cudaMemcpyHostToDevice, e->stream));
-  rc = index_status(e, e->index->commit(R, e->c_pick.as<int32_t>(), e->c_hash.as<uint64_t>(), e->c_nh.as<uint16_t>(), hash_stride,
-                                        caps.empty() ? nullptr : caps.data(), 0, lo, hi - lo + 1, std::max<int64_t>(touches, 1), e->stream),
+  const int32_t* d_pick;
+  const uint64_t* d_hash;
+  const uint16_t* d_nh;
+  if ((rc = h2d(e, e->stage[0], pick, (size_t)R, &d_pick)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], n_hashes, (size_t)R, &d_nh)) != EPPSCORE_OK)
+    return rc;
+  rc = index_status(e, e->index->commit(R, d_pick, d_hash, d_nh, hash_stride, caps.empty() ? nullptr : caps.data(), 0, lo, hi - lo + 1,
+                                        std::max<int64_t>(touches, 1), e->stream),
                     "commit_picks");
   if (rc != EPPSCORE_OK) return rc;
   CK(e, cudaStreamSynchronize(e->stream));  // the caller's host arrays (pageable) may be reused
@@ -1471,14 +1430,14 @@ int32_t eppscore_prefix_add(eppscore_engine* e, const uint64_t* hashes, int32_t 
   if (rc != EPPSCORE_OK) return rc;
   const int32_t stride = n > 0 ? n : 1;
   const uint16_t nh = (uint16_t)n;
-  CK(e, e->c_pick.reserve(4));
-  CK(e, e->c_hash.reserve((size_t)stride * 8));
-  CK(e, e->c_nh.reserve(2));
-  CK(e, cudaMemcpyAsync(e->c_pick.p, &endpoint, 4, cudaMemcpyHostToDevice, e->stream));
-  if (n) CK(e, cudaMemcpyAsync(e->c_hash.p, hashes, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->c_nh.p, &nh, 2, cudaMemcpyHostToDevice, e->stream));
-  rc = index_status(e, e->index->commit(1, e->c_pick.as<int32_t>(), e->c_hash.as<uint64_t>(), e->c_nh.as<uint16_t>(), stride, nullptr,
-                                        lru_capacity, endpoint, 1, std::max(n, 1), e->stream),
+  CK(e, e->stage[0].reserve(4));
+  CK(e, e->stage[1].reserve((size_t)stride * 8));
+  CK(e, e->stage[2].reserve(2));
+  CK(e, cudaMemcpyAsync(e->stage[0].p, &endpoint, 4, cudaMemcpyHostToDevice, e->stream));
+  if (n) CK(e, cudaMemcpyAsync(e->stage[1].p, hashes, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+  CK(e, cudaMemcpyAsync(e->stage[2].p, &nh, 2, cudaMemcpyHostToDevice, e->stream));
+  rc = index_status(e, e->index->commit(1, e->stage[0].as<int32_t>(), e->stage[1].as<uint64_t>(), e->stage[2].as<uint16_t>(), stride,
+                                        nullptr, lru_capacity, endpoint, 1, std::max(n, 1), e->stream),
                     "prefix_add");
   if (rc != EPPSCORE_OK) return rc;
   CK(e, cudaStreamSynchronize(e->stream));
@@ -1494,13 +1453,13 @@ int32_t eppscore_prefix_apply(eppscore_engine* e, int64_t n, const uint64_t* has
   CK(e, cudaSetDevice(e->device));
   int32_t rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
-  CK(e, e->c_hash.reserve((size_t)n * 8));
-  CK(e, e->c_ep.reserve((size_t)n * 4));
-  CK(e, e->c_op.reserve((size_t)n));
-  CK(e, cudaMemcpyAsync(e->c_hash.p, hash, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->c_ep.p, endpoint, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->c_op.p, op, (size_t)n, cudaMemcpyHostToDevice, e->stream));
-  rc = index_status(e, e->index->apply(n, e->c_hash.as<uint64_t>(), e->c_ep.as<int32_t>(), e->c_op.as<uint8_t>(), e->stream), "prefix_apply");
+  const uint64_t* d_hash;
+  const int32_t* d_ep;
+  const uint8_t* d_op;
+  if ((rc = h2d(e, e->stage[0], hash, (size_t)n, &d_hash)) != EPPSCORE_OK || (rc = h2d(e, e->stage[1], endpoint, (size_t)n, &d_ep)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], op, (size_t)n, &d_op)) != EPPSCORE_OK)
+    return rc;
+  rc = index_status(e, e->index->apply(n, d_hash, d_ep, d_op, e->stream), "prefix_apply");
   if (rc != EPPSCORE_OK) return rc;
   CK(e, cudaStreamSynchronize(e->stream));
   return index_end(e);
@@ -1553,16 +1512,17 @@ int32_t eppscore_estimate_tokens(eppscore_engine* e, int32_t R, int32_t location
     CK(e, cudaGetLastError());
     return EPPSCORE_OK;
   }
-  const int64_t* d_size = nullptr;
-  const int32_t *d_hint = nullptr, *d_chars = nullptr;
+  // host arrays: staged, estimated by the device form on the engine stream, copied back
+  const int64_t* d_size;
+  const int32_t *d_hint, *d_chars;
   int32_t rc;
-  if ((rc = h2d(e, e->c_esize, request_size_bytes, (size_t)R, &d_size)) != EPPSCORE_OK) return rc;
-  if ((rc = h2d(e, e->c_ehint, token_hint, (size_t)R, &d_hint)) != EPPSCORE_OK) return rc;
-  if ((rc = h2d(e, e->c_echars, prompt_chars, (size_t)R, &d_chars)) != EPPSCORE_OK) return rc;
-  CK(e, e->c_eout.reserve((size_t)R * 8));
-  e->launches += launch_estimate_tokens(d_size, d_hint, d_chars, R, e->c_eout.as<int64_t>(), e->stream);
-  CK(e, cudaGetLastError());
-  CK(e, cudaMemcpyAsync(out, e->c_eout.p, (size_t)R * 8, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = h2d(e, e->stage[0], request_size_bytes, (size_t)R, &d_size)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], token_hint, (size_t)R, &d_hint)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], prompt_chars, (size_t)R, &d_chars)) != EPPSCORE_OK)
+    return rc;
+  CK(e, e->stage[3].reserve((size_t)R * 8));
+  if ((rc = eppscore_estimate_tokens(e, R, 1, d_size, d_hint, d_chars, e->stage[3].as<int64_t>(), e->stream)) != EPPSCORE_OK) return rc;
+  CK(e, cudaMemcpyAsync(out, e->stage[3].p, (size_t)R * 8, cudaMemcpyDeviceToHost, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
   return EPPSCORE_OK;
 }
@@ -1585,8 +1545,8 @@ static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, 
   int32_t rc = producer_begin(e, st, &capturing);
   if (rc != EPPSCORE_OK) return rc;
   if (!on_device) {
-    if ((rc = h2d(e, e->c_iep, endpoint, (size_t)R, &d_ep)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->c_itok, tokens, (size_t)R, &d_tok)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->stage[0], endpoint, (size_t)R, &d_ep)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->stage[1], tokens, (size_t)R, &d_tok)) != EPPSCORE_OK) return rc;
   }
   e->launches += launch_inflight_update(d_ep, d_tok, R, e->cfg.max_endpoints, sign, e->inflight_req.as<int64_t>(),
                                         e->inflight_tok.as<int64_t>(), e->inflight_err.as<uint32_t>(), st);
@@ -1643,9 +1603,9 @@ namespace {
 // The live / tombstone counters as of every mutation ordered before `st`'s current end: read synchronously.  This also
 // re-bases the bounds after graph replays, which the host does not see.
 int32_t run_read_exact(eppscore_engine* e, cudaStream_t st) {
-  CK(e, cudaMemcpyAsync(e->h_run, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
+  CK(e, cudaMemcpyAsync(e->h_run.p, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
   CK(e, cudaStreamSynchronize(st));
-  e->run_bound_live = (int64_t)e->h_run->live;
+  e->run_bound_live = (int64_t)e->h_run.as<RunCounters>()->live;
   e->run_copy_issued = false;
   e->run_captured = false;
   return EPPSCORE_OK;
@@ -1669,13 +1629,10 @@ int32_t run_desc_upload(eppscore_engine* e, cudaStream_t st) {
 // descriptor pointed at it.  Graphs captured earlier read the table through the descriptor and the grid-stride passes loop
 // over its capacity, so they stay valid.
 int32_t run_grow(eppscore_engine* e, cudaStream_t st, int64_t slots) {
-  DevBuf nb[8];
-  cudaError_t c = run_alloc_table(e, slots, &nb[0], &nb[1], &nb[2], &nb[3], st);
-  if (c == cudaSuccess) c = run_alloc_table(e, slots, &nb[4], &nb[5], &nb[6], &nb[7], st);
-  if (c != cudaSuccess) {
-    for (DevBuf& b : nb) b.release();
-    return cuda_fail(e, c, "running-request table allocation");
-  }
+  std::array<DevBuf, 8> nb;
+  cudaError_t c = run_alloc_table(slots, &nb[0], st);
+  if (c == cudaSuccess) c = run_alloc_table(slots, &nb[4], st);
+  if (c != cudaSuccess) return cuda_fail(e, c, "running-request table allocation");
   int32_t rc = run_desc_download(e, st);
   if (rc != EPPSCORE_OK) return rc;
   const RunDev src = e->run_host;
@@ -1692,10 +1649,7 @@ int32_t run_grow(eppscore_engine* e, cudaStream_t st, int64_t slots) {
   e->launches += launch_running_rebuild(src, d, e->sm_count, st);  // also zeroes the tombstone count
   CK(e, cudaGetLastError());
   if ((rc = run_desc_upload(e, st)) != EPPSCORE_OK) return rc;
-  for (int i = 0; i < 8; i++) {
-    e->run_tab[i].release();
-    e->run_tab[i] = nb[i];
-  }
+  e->run_tab = std::move(nb);  // nb takes the old tables and frees them
   e->run_cap = slots;
   return EPPSCORE_OK;
 }
@@ -1717,7 +1671,7 @@ int32_t run_make_room(eppscore_engine* e, cudaStream_t st, int64_t R, bool captu
     if (rc != EPPSCORE_OK) return rc;
     exact = true;
   } else if (e->run_copy_issued && cudaEventQuery(e->ev_run_copy) == cudaSuccess) {
-    e->run_bound_live = (int64_t)e->h_run->live;
+    e->run_bound_live = (int64_t)e->h_run.as<RunCounters>()->live;
     e->run_copy_issued = false;
   }
   if (e->run_bound_live + R <= e->run_cap / 4) return EPPSCORE_OK;
@@ -1752,7 +1706,7 @@ int32_t run_copy_back(eppscore_engine* e, cudaStream_t st, bool capturing) {
     e->run_captured = true;
     return EPPSCORE_OK;
   }
-  CK(e, cudaMemcpyAsync(e->h_run, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
+  CK(e, cudaMemcpyAsync(e->h_run.p, e->run_ctr.p, sizeof(RunCounters), cudaMemcpyDeviceToHost, st));
   CK(e, cudaEventRecord(e->ev_run_copy, st));
   e->run_copy_issued = true;
   return EPPSCORE_OK;
@@ -1781,9 +1735,9 @@ int32_t running_update(eppscore_engine* e, int op, int32_t R, int32_t location, 
   const uint64_t* d_key = key;
   const double* d_tpot = tpot;
   if (!on_device) {
-    if ((rc = h2d(e, e->c_rep, endpoint, (size_t)R, &d_ep, st)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->c_rkey, key, (size_t)R, &d_key, st)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->c_rtpot, tpot, (size_t)R, &d_tpot, st)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->stage[0], endpoint, (size_t)R, &d_ep, st)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->stage[1], key, (size_t)R, &d_key, st)) != EPPSCORE_OK) return rc;
+    if ((rc = h2d(e, e->stage[2], tpot, (size_t)R, &d_tpot, st)) != EPPSCORE_OK) return rc;
   }
   e->launches += launch_running_update(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, op, d_ep, d_key,
                                         op == 0 ? d_tpot : nullptr, R, e->cfg.max_endpoints, on_device ? out : nullptr,
@@ -1836,7 +1790,7 @@ int32_t eppscore_running_get(eppscore_engine* e, double* min_tpot_out, int32_t* 
   if (M > 0 && count_out) CK(e, cudaMemcpyAsync(count_out, e->run_count.p, (size_t)M * 4, cudaMemcpyDeviceToHost, e->stream));
   int32_t rc = run_read_exact(e, e->stream);
   if (rc != EPPSCORE_OK) return rc;
-  const unsigned err = e->h_run->err;
+  const unsigned err = e->h_run.as<RunCounters>()->err;
   if (err) {
     CK(e, cudaMemsetAsync(&e->run_ctr.as<RunCounters>()->err, 0, 4, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
