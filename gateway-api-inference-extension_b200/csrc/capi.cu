@@ -485,6 +485,10 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   int launched = 0;
   if (!e->force_generic) launched = dense ? launch_score_dense_fast(a, s, e->sm_count) : launch_pick_sparse(a, s, e->sm_count);
   if (launched == 0) launched = launch_score_pick(a, dense, s, e->sm_count);
+  if (launched < 0) {
+    cudaGetLastError();  // (a failed launch is not sticky: clear it so the next call does not report it again)
+    return cuda_fail(e, (cudaError_t)-launched, "scoring kernel launch");
+  }
   e->launches += launched;
   CK(e, cudaGetLastError());
   return EPPSCORE_OK;

@@ -30,6 +30,32 @@ inline cudaError_t launch_maybe_pdl(bool pdl, void (*kernel)(KArgs...), dim3 gri
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
+// Shared-memory plan of a CTA with up to max_warps warps: `staged` bytes of arrays the kernel can also read from global
+// memory, `fixed` bytes per CTA and `per_warp` bytes per warp, within the device's opt-in limit.  Fewer warps come first;
+// the staged arrays stay in global memory (only when the kernel can read them there: may_unstage) when not even one warp
+// fits beside them.
+inline cudaError_t fit_cta_smem(size_t staged, size_t fixed, size_t per_warp, int max_warps, bool may_unstage, int* warps,
+                                int32_t* stage, size_t* smem) {
+  int dev = 0, optin = 0;
+  cudaError_t c = cudaGetDevice(&dev);
+  if (c == cudaSuccess) c = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (c != cudaSuccess) return c;
+  for (int st = 1; st >= (may_unstage ? 0 : 1); st--)
+    for (int w = max_warps; w >= 1; w--) {
+      const size_t need = fixed + (st ? staged : 0) + (size_t)w * per_warp;
+      if (need <= (size_t)optin) {
+        *warps = w;
+        *stage = st;
+        *smem = need;
+        return cudaSuccess;
+      }
+    }
+  return cudaErrorInvalidConfiguration;
+}
+
+// a launcher's result for one kernel launch: 1, or -(cudaError_t) when it failed
+inline int launched_one(cudaError_t c) { return c == cudaSuccess ? 1 : -(int)c; }
+
 __device__ __forceinline__ double clamp01(double s) {  // enforceScoreRange, scheduler_profile.go:194-202
   if (s < 0.0) return 0.0;
   if (s > 1.0) return 1.0;

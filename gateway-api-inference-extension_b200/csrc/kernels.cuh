@@ -170,6 +170,8 @@ struct ScoreArgs {
   uint32_t* filter_mask_out;    // [R][mask_words] or null: the candidate set after the filter chain
   int32_t only_deferred;        // full-matrix kernel: score only the requests the sparse kernel marked pick == kPickDeferred
   int32_t pdl;                  // launch the pick kernels with programmatic dependent launch (they follow the hash kernels)
+  int32_t stage_terms;          // full-matrix / generic dense kernels: the term and min/max arrays sit in shared memory (set by
+                                // their launchers; 0: they did not fit, the kernel reads them from global memory)
 };
 constexpr int32_t kPickDeferred = -2;
 
@@ -232,7 +234,8 @@ struct PrepareArgs {
   uint32_t* tiemask;
 };
 
-// launchers. Each returns the number of kernels it launched (for gpu_launches).
+// launchers. Each returns the number of kernels it launched (for gpu_launches); the scoring launchers return -(cudaError_t)
+// when a launch failed.
 int launch_hash_prompts(const HashArgs& a, cudaStream_t s, int sm_count);
 int launch_prepare_snapshot(const PrepareArgs& a, cudaStream_t s);
 int launch_count_fields(const uint8_t* bytes, const int64_t* off, const int32_t* len, int R, int32_t* out, cudaStream_t s,

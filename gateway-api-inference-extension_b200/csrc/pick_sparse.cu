@@ -449,8 +449,7 @@ static int launch_sparse_inst(const ScoreArgs& a, cudaStream_t s, int sm_count) 
   const int need = (a.R + per_block - 1) / per_block;
   if (blocks > need) blocks = need;
   if (blocks < 1) blocks = 1;
-  launch_maybe_pdl(a.pdl != 0, kernel, dim3(blocks), dim3(kSparseWarps * 32), 0, s, a);
-  return 1;
+  return launched_one(launch_maybe_pdl(a.pdl != 0, kernel, dim3(blocks), dim3(kSparseWarps * 32), 0, s, a));
 }
 
 constexpr uint32_t sparse_seq() { return 0; }
@@ -481,10 +480,12 @@ int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
     case 4: launched = launch_sparse_seq<4>(a, s, sm_count); break;
     default: launched = launch_sparse_seq<8>(a, s, sm_count); break;
   }
-  if (a.table && a.hashes) {  // only a request with prefix matches can overflow its exception table
+  if (launched > 0 && a.table && a.hashes) {  // only a request with prefix matches can overflow its exception table
     ScoreArgs d = a;
     d.only_deferred = 1;
-    launched += launch_score_matrix(d, s, sm_count);
+    const int deferred = launch_score_matrix(d, s, sm_count);
+    if (deferred < 0) return deferred;
+    launched += deferred;
   }
   return launched;
 }

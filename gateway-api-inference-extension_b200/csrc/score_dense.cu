@@ -126,7 +126,8 @@ template <typename K>
 static int launch_dense(K kernel, const ScoreArgs& a, cudaStream_t s, int sm_count) {
   const int MP = (a.geo.M + 31) & ~31;
   const size_t smem = (size_t)a.plan.n_terms * MP * 8 + kMaxSteps * 4 * 8 + (size_t)kDenseWarps * (kLutMax + 1) * 8;
-  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const cudaError_t c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (c != cudaSuccess) return -(int)c;
   int occ = 1;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kDenseWarps * 32, smem);
   if (occ < 1) occ = 1;
@@ -134,8 +135,7 @@ static int launch_dense(K kernel, const ScoreArgs& a, cudaStream_t s, int sm_cou
   const int need = (a.R + kDenseWarps - 1) / kDenseWarps;
   if (blocks > need) blocks = need;
   if (blocks < 1) blocks = 1;
-  kernel<<<blocks, kDenseWarps * 32, smem, s>>>(a);
-  return 1;
+  return launched_one(launch_maybe_pdl(false, kernel, dim3(blocks), dim3(kDenseWarps * 32), smem, s, a));
 }
 
 constexpr uint32_t seq_of() { return 0; }

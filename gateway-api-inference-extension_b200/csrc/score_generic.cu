@@ -22,29 +22,38 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
   const Plan& plan = a.plan;
   const int M = a.geo.M;
   const int MP = (M + 31) & ~31;
-  double* s_term = reinterpret_cast<double*>(smem_raw);
-  long long* s_q = reinterpret_cast<long long*>(s_term + (size_t)plan.n_terms * MP);
-  double* s_lut = reinterpret_cast<double*>(s_q + (MASKED ? 2 * MP : 0));
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int t = 0; t < plan.n_terms; t++)
-    for (int m = threadIdx.x; m < MP; m += blockDim.x) s_term[(size_t)t * MP + m] = m < M ? a.term[t][m] : 0.0;
-  if (MASKED)
-    for (int which = 0; which < 2; which++)
-      for (int m = threadIdx.x; m < MP; m += blockDim.x)
-        s_q[which * MP + m] = (a.minmax_q[which] && m < M) ? a.minmax_q[which][m] : 0;
-  __syncthreads();
-
-  double* lut = s_lut + warp * (kLutMax + 1);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, NWARPS = blockDim.x >> 5;
   int lut_total = -1, prefix_step = -1;
   bool has_minmax[2] = {false, false};
   for (int s = 0; s < plan.n_steps; s++) {
     if (plan.kind[s] == STEP_PREFIX && prefix_step < 0) prefix_step = s;
     if (plan.kind[s] == STEP_MINMAX) has_minmax[plan.arg[s]] = true;
   }
+  // term and min/max arrays: staged in shared memory, or read from global memory when they do not fit (launch_score_pick)
+  const bool stage = a.stage_terms != 0;
+  const bool q_smem = stage && MASKED && (has_minmax[0] || has_minmax[1]);
+  double* s_term = reinterpret_cast<double*>(smem_raw);
+  long long* s_q = reinterpret_cast<long long*>(s_term + (stage ? (size_t)plan.n_terms * MP : 0));
+  double* s_lut = reinterpret_cast<double*>(s_q + (q_smem ? 2 * MP : 0));
+  if (stage)
+    for (int t = 0; t < plan.n_terms; t++)
+      for (int m = threadIdx.x; m < MP; m += blockDim.x) s_term[(size_t)t * MP + m] = m < M ? a.term[t][m] : 0.0;
+  if (q_smem)
+    for (int which = 0; which < 2; which++)
+      for (int m = threadIdx.x; m < MP; m += blockDim.x)
+        s_q[which * MP + m] = (a.minmax_q[which] && m < M) ? a.minmax_q[which][m] : 0;
+  __syncthreads();
+  auto qval = [&](int which, int m) -> long long {  // raw queue / running value of endpoint m (0 past M)
+    if (q_smem) return s_q[which * MP + m];
+    const long long* q = reinterpret_cast<const long long*>(a.minmax_q[which]);
+    return (q && m < M) ? __ldg(q + m) : 0LL;
+  };
+
+  double* lut = s_lut + warp * (kLutMax + 1);
   const int tie_mode = plan.tie_mode;
   const int nchunks = MP >> 5;
 
-  const int gw = blockIdx.x * kScoreWarps + warp, nw = gridDim.x * kScoreWarps;
+  const int gw = blockIdx.x * NWARPS + warp, nw = gridDim.x * NWARPS;
   for (int r = gw; r < a.R; r += nw) {
     const int total = a.dense_total ? a.dense_total[r] : 0;
     if (prefix_step >= 0 && total != lut_total) {
@@ -65,7 +74,7 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
         if (((__ldg(mrow + i) >> lane) & 1u) && m < M) {
 #pragma unroll
           for (int which = 0; which < 2; which++) {
-            const long long v = s_q[which * MP + m];
+            const long long v = qval(which, m);
             mn[which] = v < mn[which] ? v : mn[which];
             mx[which] = v > mx[which] ? v : mx[which];
           }
@@ -99,7 +108,7 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
       for (int s = 0; s < plan.n_steps; s++) {
         double term;
         switch (plan.kind[s]) {
-          case STEP_EP_TERM: term = s_term[(size_t)plan.arg[s] * MP + m]; break;
+          case STEP_EP_TERM: term = stage ? s_term[(size_t)plan.arg[s] * MP + m] : __ldg(a.term[plan.arg[s]] + m); break;
           case STEP_PREFIX: {
             const int cc = c < 65535 ? c : 65535;
             term = (s == prefix_step && total <= kLutMax && cc <= total) ? lut[cc]
@@ -118,7 +127,7 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
             const int which = plan.arg[s];
             double sc = 1.0;
             if (MASKED && mx[which] != mn[which])
-              sc = __ddiv_rn(__ll2double_rn(mx[which] - s_q[which * MP + m]), __ll2double_rn(mx[which] - mn[which]));
+              sc = __ddiv_rn(__ll2double_rn(mx[which] - qval(which, m)), __ll2double_rn(mx[which] - mn[which]));
             term = __dmul_rn(clamp01(sc), plan.weight[s]);
             break;
           }
@@ -155,31 +164,36 @@ __global__ void __launch_bounds__(kScoreWarps * 32) score_pick_dense_kernel(cons
 }
 
 template <typename K>
-static int launch_with_smem(K kernel, const ScoreArgs& a, size_t smem, cudaStream_t s, int sm_count) {
-  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+static int launch_dense_generic(K kernel, const ScoreArgs& args, bool masked, cudaStream_t s, int sm_count) {
+  ScoreArgs a = args;
+  const int MP = (a.geo.M + 31) & ~31;
+  bool minmax = false;
+  for (int i = 0; i < a.plan.n_steps; i++) minmax = minmax || a.plan.kind[i] == STEP_MINMAX;
+  const size_t staged = (size_t)a.plan.n_terms * MP * 8 + (masked && minmax ? 2 * (size_t)MP * 8 : 0);
+  int warps = 0;
+  size_t smem = 0;
+  cudaError_t c = fit_cta_smem(staged, 0, (size_t)(kLutMax + 1) * 8, kScoreWarps, true, &warps, &a.stage_terms, &smem);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (c != cudaSuccess) return -(int)c;
   int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kScoreWarps * 32, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, warps * 32, smem);
   if (occ < 1) occ = 1;
-  const int need = (a.R + kScoreWarps - 1) / kScoreWarps;
+  const int need = (a.R + warps - 1) / warps;
   int blocks = sm_count * occ;  // persistent: one wave, warps stride over requests
   if (blocks > need) blocks = need;
   if (blocks < 1) blocks = 1;
-  kernel<<<blocks, kScoreWarps * 32, smem, s>>>(a);
-  return 1;
+  return launched_one(launch_maybe_pdl(false, kernel, dim3(blocks), dim3(warps * 32), smem, s, a));
 }
 
 int launch_score_pick(const ScoreArgs& a, bool dense, cudaStream_t s, int sm_count) {
   if (a.R <= 0) return 0;
   const bool masked = a.cand_mask != nullptr;
   if (dense) {
-    const int MP = (a.geo.M + 31) & ~31;
-    size_t smem = (size_t)a.plan.n_terms * MP * 8 + (masked ? 2 * (size_t)MP * 8 : 0) +
-                  (size_t)kScoreWarps * (kLutMax + 1) * 8;
     if (a.topk > 0)
-      return masked ? launch_with_smem(score_pick_dense_kernel<true, true>, a, smem, s, sm_count)
-                    : launch_with_smem(score_pick_dense_kernel<false, true>, a, smem, s, sm_count);
-    if (masked) return launch_with_smem(score_pick_dense_kernel<true>, a, smem, s, sm_count);
-    return launch_with_smem(score_pick_dense_kernel<false>, a, smem, s, sm_count);
+      return masked ? launch_dense_generic(score_pick_dense_kernel<true, true>, a, masked, s, sm_count)
+                    : launch_dense_generic(score_pick_dense_kernel<false, true>, a, masked, s, sm_count);
+    if (masked) return launch_dense_generic(score_pick_dense_kernel<true>, a, masked, s, sm_count);
+    return launch_dense_generic(score_pick_dense_kernel<false>, a, masked, s, sm_count);
   }
   return launch_score_matrix(a, s, sm_count);  // score_matrix.cu
 }

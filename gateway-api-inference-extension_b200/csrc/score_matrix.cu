@@ -50,6 +50,10 @@ __device__ __forceinline__ LatPair lat_pair(const double* tp, double tpot_genera
   return o;
 }
 
+__host__ __device__ constexpr bool seq_has_minmax(uint32_t seq) {
+  return seq != 0 && ((int)(seq & 15u) - 1 == STEP_MINMAX || seq_has_minmax(seq >> 4));
+}
+
 // RND: the stochastic pickers (random / weighted-random) are compiled in; always for the runtime-generic SEQ == 0.
 // TOPK: the first a.topk entries of each request's pick order are written too (runtime-generic SEQ == 0 only).  Those
 // variants ask for one resident CTA per SM, so ptxas keeps the per-lane lists in registers instead of spilling them.
@@ -57,9 +61,10 @@ template <uint32_t SEQ, bool MASKED, bool DIAG, bool LAT, bool RND = (SEQ == 0),
 __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_kernel(const __grid_constant__ ScoreArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   pdl_wait();  // (no-op unless launched behind pick_sparse / the hash kernels with programmatic dependent launch)
+  const int NWARPS = blockDim.x >> 5;  // kMatrixWarps, or fewer when that many do not fit in shared memory (launch_matrix)
   if (a.only_deferred) {  // the pass behind pick_sparse: normally nothing was deferred — leave before staging anything
     bool any = false;
-    const int gw0 = blockIdx.x * kMatrixWarps + (threadIdx.x >> 5), nw0 = gridDim.x * kMatrixWarps;
+    const int gw0 = blockIdx.x * NWARPS + (threadIdx.x >> 5), nw0 = gridDim.x * NWARPS;
     for (long long r = gw0 + (long long)(threadIdx.x & 31) * nw0; r < a.R; r += 32LL * nw0) any |= a.pick[r] == kPickDeferred;
     if (!__syncthreads_or(any ? 1 : 0)) return;
   }
@@ -68,41 +73,6 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
   const int RW = a.geo.row_words;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const bool wide_cnt = a.hash_stride > 256;  // counters: 8-bit (0 decodes as 256 for touched slots) or 16-bit
-
-  // ---- shared memory carve-up ----
-  double* s_term = reinterpret_cast<double*>(smem_raw);
-  long long* s_q = reinterpret_cast<long long*>(s_term + (size_t)plan.n_terms * MPAD);
-  double* s_lora = reinterpret_cast<double*>(s_q + (MASKED ? 2 * MPAD : 0));
-  double* s_latw = s_lora + kMaxSteps * 4;
-  double* s_lut = s_latw + (LAT ? kLatW : 0);
-  constexpr int NLUT = LAT ? 3 : 2;
-  double* lut_p = s_lut + (size_t)warp * NLUT * (kLutMax + 1);
-  double* lut_q = lut_p + (kLutMax + 1);
-  double* lut_l = lut_q + (LAT ? (kLutMax + 1) : 0);  // coef * (c/total) of the prediction / composite
-  unsigned char* s_cnt_all = reinterpret_cast<unsigned char*>(s_lut + (size_t)kMatrixWarps * NLUT * (kLutMax + 1));
-  const int cnt_bytes = MPAD * (wide_cnt ? 2 : 1) + RW * 4;  // match counters + the permuted bitmap of touched endpoints
-  unsigned char* cnt_raw = s_cnt_all + (size_t)warp * cnt_bytes;
-  uint32_t* tperm = reinterpret_cast<uint32_t*>(cnt_raw + MPAD * (wide_cnt ? 2 : 1));
-  uint8_t* cnt8 = cnt_raw;
-  uint16_t* cnt16 = reinterpret_cast<uint16_t*>(cnt_raw);
-
-  for (int t = 0; t < plan.n_terms; t++)
-    for (int m = threadIdx.x; m < MPAD; m += blockDim.x) s_term[(size_t)t * MPAD + m] = a.term[t][m];
-  if (MASKED)
-    for (int which = 0; which < 2; which++)
-      for (int m = threadIdx.x; m < MPAD; m += blockDim.x)
-        s_q[which * MPAD + m] = (a.minmax_q[which] && m < M) ? a.minmax_q[which][m] : 0;
-  if (threadIdx.x < kMaxSteps * 4) s_lora[threadIdx.x] = plan.lora_term[threadIdx.x >> 2][threadIdx.x & 3];
-  int lat_step = -1;
-  if (LAT) {
-    for (int s = 0; s < plan.n_steps; s++)
-      if (plan.kind[s] == STEP_LATENCY && lat_step < 0) lat_step = s;
-    // scores[ep] = w / wMax (plugin.go:306, :360), clamped and weighted like any scorer (scheduler_profile.go:168)
-    if (threadIdx.x < kLatW)
-      s_latw[threadIdx.x] = __dmul_rn(clamp01(__ddiv_rn((double)threadIdx.x, 100.0)), plan.weight[lat_step < 0 ? 0 : lat_step]);
-  }
-  for (int i = threadIdx.x; i < (kMatrixWarps * cnt_bytes) / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(s_cnt_all)[i] = 0;
-  __syncthreads();
 
   // ---- plan facts (warp-uniform) ----
   int prefix_step = -1, q_step = -1;
@@ -114,11 +84,58 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
       if (q_step < 0) q_step = s;  // the first min/max scorer gets the per-row LUT
     }
   }
+
+  // ---- shared memory carve-up ----
+  // The term and min/max arrays are staged unless they do not fit beside one warp's counters (a.stage_terms == 0, only at
+  // large Mpad with many terms); they are then read from global memory, where they stay L2-resident.  The specialised
+  // sequences have at most one term array, which always fits: only the runtime-generic variants carry the global path.
+  const bool stage = SEQ != 0 || a.stage_terms != 0;
+  const bool q_smem = MASKED && (SEQ != 0 ? seq_has_minmax(SEQ) : (stage && (has_minmax[0] || has_minmax[1])));
+  double* s_term = reinterpret_cast<double*>(smem_raw);
+  long long* s_q = reinterpret_cast<long long*>(s_term + (stage ? (size_t)plan.n_terms * MPAD : 0));
+  double* s_lora = reinterpret_cast<double*>(s_q + (q_smem ? 2 * MPAD : 0));
+  double* s_latw = s_lora + kMaxSteps * 4;
+  double* s_lut = s_latw + (LAT ? kLatW : 0);
+  constexpr int NLUT = LAT ? 3 : 2;
+  double* lut_p = s_lut + (size_t)warp * NLUT * (kLutMax + 1);
+  double* lut_q = lut_p + (kLutMax + 1);
+  double* lut_l = lut_q + (LAT ? (kLutMax + 1) : 0);  // coef * (c/total) of the prediction / composite
+  unsigned char* s_cnt_all = reinterpret_cast<unsigned char*>(s_lut + (size_t)NWARPS * NLUT * (kLutMax + 1));
+  const int cnt_bytes = MPAD * (wide_cnt ? 2 : 1) + RW * 4;  // match counters + the permuted bitmap of touched endpoints
+  unsigned char* cnt_raw = s_cnt_all + (size_t)warp * cnt_bytes;
+  uint32_t* tperm = reinterpret_cast<uint32_t*>(cnt_raw + MPAD * (wide_cnt ? 2 : 1));
+  uint8_t* cnt8 = cnt_raw;
+  uint16_t* cnt16 = reinterpret_cast<uint16_t*>(cnt_raw);
+
+  if (stage)
+    for (int t = 0; t < plan.n_terms; t++)
+      for (int m = threadIdx.x; m < MPAD; m += blockDim.x) s_term[(size_t)t * MPAD + m] = a.term[t][m];
+  if (q_smem)
+    for (int which = 0; which < 2; which++)
+      for (int m = threadIdx.x; m < MPAD; m += blockDim.x)
+        s_q[which * MPAD + m] = (a.minmax_q[which] && m < M) ? a.minmax_q[which][m] : 0;
+  auto qval = [&](int which, int m) -> long long {  // raw queue / running value of endpoint m (0 past M)
+    if (q_smem) return s_q[which * MPAD + m];
+    const long long* q = reinterpret_cast<const long long*>(a.minmax_q[which]);
+    return (q && m < M) ? __ldg(q + m) : 0LL;
+  };
+  if (threadIdx.x < kMaxSteps * 4) s_lora[threadIdx.x] = plan.lora_term[threadIdx.x >> 2][threadIdx.x & 3];
+  int lat_step = -1;
+  if (LAT) {
+    for (int s = 0; s < plan.n_steps; s++)
+      if (plan.kind[s] == STEP_LATENCY && lat_step < 0) lat_step = s;
+    // scores[ep] = w / wMax (plugin.go:306, :360), clamped and weighted like any scorer (scheduler_profile.go:168)
+    if (threadIdx.x < kLatW)
+      s_latw[threadIdx.x] = __dmul_rn(clamp01(__ddiv_rn((double)threadIdx.x, 100.0)), plan.weight[lat_step < 0 ? 0 : lat_step]);
+  }
+  for (int i = threadIdx.x; i < (NWARPS * cnt_bytes) / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(s_cnt_all)[i] = 0;
+  __syncthreads();
+
   const bool want_prefix = prefix_step >= 0 || a.match_out != nullptr || a.total_out != nullptr || (LAT && lat_step >= 0);
   const int tie_mode = plan.tie_mode;
   int lut_total = -1, lutl_total = -1;
 
-  const int gw = blockIdx.x * kMatrixWarps + warp, nw = gridDim.x * kMatrixWarps;
+  const int gw = blockIdx.x * NWARPS + warp, nw = gridDim.x * NWARPS;
   for (int r = gw; r < a.R; r += nw) {
     if (a.only_deferred && a.pick[r] != kPickDeferred) continue;  // (warp-uniform) the sparse kernel already scored it
     // ---------------- matchLongestPrefix into the shared-memory counters ----------------
@@ -290,7 +307,7 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
 #pragma unroll
             for (int which = 0; which < 2; which++) {
               if (scanned[which]) continue;
-              const long long v = s_q[which * MPAD + m];
+              const long long v = qval(which, m);
               mn[which] = v < mn[which] ? v : mn[which];
               mx[which] = v > mx[which] ? v : mx[which];
             }
@@ -502,7 +519,6 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
         l_pok = l_rgP > eps;
         l_rT = l_tok ? __drcp_rn(l_rgT) : 0.0;                                  // fast path of the normalisation, see below
         l_rP = l_pok ? __drcp_rn(l_rgP) : 0.0;
-        l_fast = l_alpha >= 0.0 && l_alpha <= 1.0 && l_beta >= 0.0 && l_beta <= 1.0;
         l_alpha = L.alpha;
         l_beta = L.beta;
         if (!l_tok && l_pok) {                                                  // plugin.go:275-279
@@ -512,6 +528,7 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
           l_alpha = 1.0;
           l_beta = 0.0;
         }
+        l_fast = l_alpha >= 0.0 && l_alpha <= 1.0 && l_beta >= 0.0 && l_beta <= 1.0;
       } else {
         // composite fallback: maxQ over the candidates, starting from 0 (plugin.go:338-344)
         long long mq = 0;
@@ -551,7 +568,8 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
     double wq[8];
 #pragma unroll
     for (int s = 0; s < 8; s++) {
-      tptr[s] = s_term + (size_t)(s < plan.n_steps && plan.kind[s] == STEP_EP_TERM ? plan.arg[s] : 0) * MPAD;
+      const int ta = s < plan.n_steps && plan.kind[s] == STEP_EP_TERM ? plan.arg[s] : 0;
+      tptr[s] = stage ? s_term + (size_t)ta * MPAD : a.term[ta];
       wq[s] = s < plan.n_steps ? plan.weight[s] : 0.0;
     }
     const bool q_flat = !MASKED || q_step < 0 || mx[plan.arg[q_step < 0 ? 0 : q_step]] == mn[plan.arg[q_step < 0 ? 0 : q_step]];
@@ -590,11 +608,11 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
             if (s == q_step ? q_flat : (!MASKED || mx[which] == mn[which])) {
               term = __dmul_rn(1.0, wq[s]);                                  // queue.go:95-98
             } else if (s == q_step && qlut_ok) {
-              long long d = mx[which] - s_q[which * MPAD + m];
+              long long d = mx[which] - qval(which, m);
               d = d < 0 ? 0 : (d > kLutMax ? kLutMax : d);                   // (non-candidates only)
               term = lut_q[(int)d];
             } else {
-              const double sc = __ddiv_rn(__ll2double_rn(mx[which] - s_q[which * MPAD + m]),
+              const double sc = __ddiv_rn(__ll2double_rn(mx[which] - qval(which, m)),
                                           __ll2double_rn(mx[which] - mn[which]));  // queue.go:99
               term = __dmul_rn(clamp01(sc), wq[s]);
             }
@@ -607,7 +625,7 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
             const double pt = llut_ok ? lut_l[c] : __dmul_rn(L.has_predictions ? L.ttft_prefix : L.wpref,
                                                              total ? __ddiv_rn((double)c, (double)total) : 0.0);
             const double* tp = L.ep + (size_t)t * 256 + lane;
-            int w = 0;
+            long long w = 0;  // Go's int: 64-bit, so no v below 2^63 saturates or wraps
             if (L.has_predictions) {
               const LatPair lp = lat_pair(tp, L.tpot_generated, pt, l_x, l_y, l_tslo, l_buf);
               if (DIAG && L.pred_out && m < M) {
@@ -621,12 +639,12 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
               const double v = most ? __dmul_rn(comb, 100.0) : __dmul_rn(__dsub_rn(1.0, comb), 100.0);
               const int vn = __double2int_rn(v);
               const bool in_tier = lp.rank == l_sel;
-              w = in_tier ? __double2int_rz(v) + 1 : 0;                        // float64(int(x) + minWeight + 1); 0 outside the tier
+              w = in_tier ? __double2ll_rz(v) + 1 : 0;                         // float64(int(x) + minWeight + 1); 0 outside the tier
               const bool redo = in_tier && (!l_fast || fabs(__dsub_rn(v, (double)vn)) < 1e-9);
               if (__any_sync(0xffffffffu, redo)) {                             // warp-uniform: scoreBucket, plugin.go:281-306, exactly
                 const double eT = l_tok ? __ddiv_rn(dT, l_rgT) : 0.5, eP = l_pok ? __ddiv_rn(dP, l_rgP) : 0.5;
                 const double ec = __dadd_rn(__dmul_rn(l_alpha, eT), __dmul_rn(l_beta, eP));
-                const int we = __double2int_rz(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1;
+                const long long we = __double2ll_rz(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1;
                 w = redo ? we : w;
               }
             } else {                                                           // compositeScores, plugin.go:346-360
@@ -636,11 +654,11 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
               const double ck = __ldg(tp);
               const double v = __dmul_rn(100.0, __dadd_rn(__dadd_rn(ck, __dmul_rn(L.wq, rel)), pt));
               const double fl = floor(v);
-              w = (int)__double2ll_rz(round(v));                               // int(math.Round(0 + 100*composite))
+              w = __double2ll_rz(round(v));                                    // int(math.Round(0 + 100*composite))
               const bool redo = !l_fast || !(fabs(v) < 1e4) || fabs(__dsub_rn(__dsub_rn(v, fl), 0.5)) < 1e-9;
               if (__any_sync(0xffffffffu, redo)) {
                 const double er = l_maxq > 0 ? __ddiv_rn(dq, l_qrange) : 1.0;
-                const int we = (int)__double2ll_rz(round(__dmul_rn(100.0, __dadd_rn(__dadd_rn(ck, __dmul_rn(L.wq, er)), pt))));
+                const long long we = __double2ll_rz(round(__dmul_rn(100.0, __dadd_rn(__dadd_rn(ck, __dmul_rn(L.wq, er)), pt))));
                 w = redo ? we : w;
               }
               if (DIAG && L.pred_out && m < M) {
@@ -648,7 +666,8 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
                 L.pred_out[((size_t)r * M + m) * 2 + 1] = nan64();
               }
             }
-            term = (unsigned)w < (unsigned)kLatW ? s_latw[w] : __dmul_rn(clamp01(__ddiv_rn((double)w, 100.0)), wq[s]);
+            term = (unsigned long long)w < (unsigned long long)kLatW ? s_latw[w]
+                                                                     : __dmul_rn(clamp01(__ddiv_rn(__ll2double_rn(w), 100.0)), wq[s]);
           } else {
             term = __dmul_rn(0.0, wq[s]);                                    // pair columns absent: score 0
           }
@@ -718,22 +737,30 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
 }
 
 template <typename K>
-static int launch_matrix(K kernel, const ScoreArgs& a, bool masked, bool lat, cudaStream_t s, int sm_count) {
+static int launch_matrix(K kernel, const ScoreArgs& args, bool masked, bool lat, bool generic, cudaStream_t s, int sm_count) {
+  ScoreArgs a = args;
   const int MPAD = a.geo.Mpad;
   const bool wide = a.hash_stride > 256;
-  const size_t smem = (size_t)a.plan.n_terms * MPAD * 8 + (masked ? 2 * (size_t)MPAD * 8 : 0) + kMaxSteps * 4 * 8 +
-                      (lat ? kLatW * 8 : 0) + (size_t)kMatrixWarps * (lat ? 3 : 2) * (kLutMax + 1) * 8 +
-                      (size_t)kMatrixWarps * ((size_t)MPAD * (wide ? 2 : 1) + (size_t)a.geo.row_words * 4);
-  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  bool minmax = false;
+  for (int i = 0; i < a.plan.n_steps; i++) minmax = minmax || a.plan.kind[i] == STEP_MINMAX;
+  // the kernel's carve-up: term arrays [+ min/max values], LoRA terms [+ latency weights], then per warp the LUTs, the
+  // match counters and the touched-endpoint bitmap
+  const size_t staged = (size_t)a.plan.n_terms * MPAD * 8 + (masked && minmax ? 2 * (size_t)MPAD * 8 : 0);
+  const size_t fixed = kMaxSteps * 4 * 8 + (lat ? kLatW * 8 : 0);
+  const size_t per_warp = (size_t)(lat ? 3 : 2) * (kLutMax + 1) * 8 + (size_t)MPAD * (wide ? 2 : 1) + (size_t)a.geo.row_words * 4;
+  int warps = 0;
+  size_t smem = 0;
+  cudaError_t c = fit_cta_smem(staged, fixed, per_warp, kMatrixWarps, generic, &warps, &a.stage_terms, &smem);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (c != cudaSuccess) return -(int)c;
   int occ = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kMatrixWarps * 32, smem);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, warps * 32, smem);
   if (occ < 1) occ = 1;
-  const int need = (a.R + kMatrixWarps - 1) / kMatrixWarps;
+  const int need = (a.R + warps - 1) / warps;
   int blocks = sm_count * occ;  // persistent: one wave, warps stride over requests
   if (blocks > need) blocks = need;
   if (blocks < 1) blocks = 1;
-  launch_maybe_pdl(a.pdl != 0, kernel, dim3(blocks), dim3(kMatrixWarps * 32), smem, s, a);
-  return 1;
+  return launched_one(launch_maybe_pdl(a.pdl != 0, kernel, dim3(blocks), dim3(warps * 32), smem, s, a));
 }
 
 constexpr uint32_t mseq() { return 0; }
@@ -747,9 +774,9 @@ constexpr uint32_t mseq(int k, Rest... rest) {
 #define L STEP_LORA
 #define Q STEP_MINMAX
 #define T STEP_LATENCY
-#define MK(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, false>, a, MASKED, false, s, sm_count)
-#define MKL(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, true>, a, MASKED, true, s, sm_count)
-#define MKR(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, false, true>, a, MASKED, false, s, sm_count)
+#define MK(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, false>, a, MASKED, false, false, s, sm_count)
+#define MKL(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, true>, a, MASKED, true, false, s, sm_count)
+#define MKR(...) launch_matrix(score_matrix_kernel<mseq(__VA_ARGS__), MASKED, DIAG, false, true>, a, MASKED, false, false, s, sm_count)
 template <bool MASKED, bool DIAG>
 static int launch_matrix_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
   bool lat = false;
@@ -770,8 +797,8 @@ static int launch_matrix_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
     case mseq(T): return MKL(T);          // the latency profile of the reference chart (config/charts/epplib/templates/_config.yaml:66-75)
     case mseq(T, L): return MKL(T, L);
     default:
-      return lat ? launch_matrix(score_matrix_kernel<0, MASKED, DIAG, true>, a, MASKED, true, s, sm_count)
-                 : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false>, a, MASKED, false, s, sm_count);
+      return lat ? launch_matrix(score_matrix_kernel<0, MASKED, DIAG, true>, a, MASKED, true, true, s, sm_count)
+                 : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false>, a, MASKED, false, true, s, sm_count);
   }
 }
 // top-k lists: the runtime-generic variants only, every pick mode
@@ -779,8 +806,8 @@ template <bool MASKED, bool DIAG>
 static int launch_matrix_topk(const ScoreArgs& a, cudaStream_t s, int sm_count) {
   bool lat = false;
   for (int i = 0; i < a.plan.n_steps; i++) lat = lat || a.plan.kind[i] == STEP_LATENCY;
-  return lat ? launch_matrix(score_matrix_kernel<0, MASKED, DIAG, true, true, true>, a, MASKED, true, s, sm_count)
-             : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false, true, true>, a, MASKED, false, s, sm_count);
+  return lat ? launch_matrix(score_matrix_kernel<0, MASKED, DIAG, true, true, true>, a, MASKED, true, true, s, sm_count)
+             : launch_matrix(score_matrix_kernel<0, MASKED, DIAG, false, true, true>, a, MASKED, false, true, s, sm_count);
 }
 #undef MK
 #undef MKL
