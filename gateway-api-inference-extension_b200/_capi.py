@@ -76,7 +76,7 @@ class Stats(C.Structure):
                 ("prefix_hashes", C.c_int64), ("prefix_live_hashes", C.c_int64), ("prefix_capacity", C.c_int64),
                 ("prefix_table_bytes", C.c_int64), ("lru_entries", C.c_int64), ("lru_bytes", C.c_int64),
                 ("prefix_overflow_rows", C.c_int64), ("prefix_rebuilds", C.c_int64), ("index_error", C.c_uint32),
-                ("reserved", C.c_uint32)]
+                ("probe_resolved", C.c_uint32)]
 
 
 # every symbol include/eppscore.h declares: (name, restype, argtypes)

@@ -89,6 +89,8 @@ struct eppscore_engine {
   // in-flight load producer (inflightload/producer.go): per-endpoint request and token counters, [Mpad] int64 each, zeroed at
   // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens.
   DevBuf inflight_req, inflight_tok, inflight_err;
+  // requests the probing hash kernel has resolved since creation (u64; eppscore_stats.probe_resolved, modulo 2^32)
+  DevBuf probe_resolved;
   bool snapshot_has_tokens = false;  // the current snapshot carries inflight_tokens
 
   // predicted-latency producer's running-request queues (running_kernel.cu): the (endpoint, key) -> tpot table and the
@@ -112,7 +114,7 @@ struct eppscore_engine {
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
-        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s;
+        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe;
   } sc[4];
   // pinned staging for the small per-request results of a host batch: a D2H copy into the caller's (usually pageable)
   // arrays would block the host after every chunk and serialise the pipeline
@@ -468,6 +470,16 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
         h.n_hashes = sc.s_nh.as<uint16_t>();
         h.stage_mask = e->hash_stage_mask;
         h.pdl = e->use_pdl ? 1 : 0;
+        // the sparse pick kernel follows and would probe the index: the hash kernel probes it instead while it holds the
+        // hashes, and leaves the rows it resolved out of the hash buffer.  Not when the caller wants every row (hashes_out,
+        // the closed loop's commit input): then no write is saved, and on H100 the schedule call measured slower that way.
+        if (!e->force_generic && !b.hashes_out && hash_probe_applies(h) && pick_sparse_probes(a)) {
+          CK(e, sc.s_probe.reserve((size_t)b.R * sizeof(ProbeRec)));
+          h.table = e->index->view();
+          h.probe = sc.s_probe.as<ProbeRec>();
+          h.resolved = e->probe_resolved.as<unsigned long long>();
+          a.probe = h.probe;
+        }
         e->launches += launch_hash_prompts(h, s, e->sm_count);
         hashed_here = true;
         a.hashes = hashes;
@@ -705,6 +717,8 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   CK(nullptr, cudaMemsetAsync(ep->inflight_req.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_tok.p, 0, mp * 8, ep->stream));
   CK(nullptr, cudaMemsetAsync(ep->inflight_err.p, 0, 4, ep->stream));
+  CK(nullptr, ep->probe_resolved.reserve(8));
+  CK(nullptr, cudaMemsetAsync(ep->probe_resolved.p, 0, 8, ep->stream));
   CK(nullptr, make(ep->ev_producer));
   CK(nullptr, init_inflight_update());
   {  // running-request queues: every endpoint empty, a small table (grown by the first calls that need room)
@@ -819,6 +833,9 @@ int32_t eppscore_get_stats(const eppscore_engine* ce, eppscore_stats* out) {
   out->prefix_overflow_rows = st.ovf_rows;
   out->prefix_rebuilds = st.rebuilds;
   out->index_error = st.error;
+  unsigned long long resolved = 0;  // (the caller has waited for its batches)
+  CK(e, cudaMemcpy(&resolved, e->probe_resolved.p, 8, cudaMemcpyDeviceToHost));
+  out->probe_resolved = (uint32_t)resolved;
   return EPPSCORE_OK;
 }
 

@@ -83,6 +83,25 @@ __device__ __forceinline__ double shfl_f64(double v, int src) {
 }
 __device__ __forceinline__ long long shfl_xor_i64(long long v, int o) { return __shfl_xor_sync(0xffffffffu, v, o); }
 __device__ __forceinline__ uint4 ldg16(const void* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+
+// indexer.Get (indexer.go:86-102) on the prefix index, continued from the first load: lo holds the first 16 bytes of slot idx
+// ({key.lo, key.hi, cnt, ep0 | ep1 << 16}).  Walks the linear probe to h's slot or to a never-used one and returns whether h
+// is present with a non-empty set (an emptied set == a deleted key); idx / lo are left at the last slot loaded.
+__device__ __forceinline__ bool table_find(const TSlot* slots, uint64_t mask, uint64_t h, uint64_t& idx, uint4& lo) {
+  for (;;) {
+    if (lo.z == kCntFree) return false;
+    if ((((uint64_t)lo.y << 32) | lo.x) == h) return (lo.z & kCntMask) != 0;
+    idx = (idx + 1) & mask;
+    lo = ldg16(&slots[idx]);
+  }
+}
+// do two inline sets with the same raw cnt word (not rows) have the same members?  Slots are kept CANONICAL by the index
+// program (members sorted, unused entries 0xFFFF: prefix_table.cuh set_member / clear_member) and the second half of a slot
+// is loaded for neither or both (same count), so equal sets are equal words.  A stale entry could only make two equal sets
+// look different, which sends the request through its exception table — slower, never wrong.
+__device__ __forceinline__ bool same_inline_set(uint32_t w0, const uint4& h0, uint32_t w1, const uint4& h1) {
+  return ((w0 ^ w1) | (h0.x ^ h1.x) | (h0.y ^ h1.y) | (h0.z ^ h1.z) | (h0.w ^ h1.w)) == 0;
+}
 __device__ __forceinline__ double nan64() { return __longlong_as_double(0x7ff8000000000000LL); }
 
 // clamp(match/total)*w, prefix/plugin.go:108-110 + scheduler_profile.go:168 (the slow, LUT-less form)

@@ -457,21 +457,33 @@ __global__ void __launch_bounds__(kFusedWarps * 32, 5) hash_fused_kernel(HashArg
 // ---------------------------------------------------------------------------------------------
 // hash_warp_kernel: both stages in one kernel WITHOUT any CTA-level synchronisation.  A WARP owns a tile of 32 requests:
 //   A  lane = block: the stripe states of 32 blocks of one request after the other go to the warp's shared-memory tile
-//      [request][block]; the next request's 64 bytes per lane are requested before the current block is digested;
+//      [request][block]; the next TWO requests' 64 bytes per lane are in flight while the current block is digested
+//      (one ahead left the warps latency bound: 68 us for the plain form, 78 us with the probe, against 68 us now, H100);
 //   B  lane = request: the serial chain over the tile's rows, in place (32 chains in flight per warp);
 //   C  lane = block: the finished hashes leave the tile, 256 contiguous bytes per request.
 // Only __syncwarp between the phases: no warp ever waits for another one, the chain phases of some warps overlap the HBM
 // stream of the others, the 8-byte body states never travel through HBM and the second launch is gone.
+// PROBE (schedule_device, when pick_sparse_kernel follows): between B and C each lane also runs indexer.Get over its request's
+// new hashes while the tile holds them, exactly as pick_sparse_kernel would, and a request whose matched blocks all carry its
+// first hit's inline set is RESOLVED: its ProbeRec holds the count and the set, and its row of hashes is not written (nothing
+// reads it).  The index is not snapshot data, so this kernel still runs concurrently with a snapshot preparation.
 // ---------------------------------------------------------------------------------------------
 constexpr int kWarpTileWarps = 8;
+constexpr int kProbeU = 4;     // PROBE: hashes probed per lane at a time (independent loads in flight)
 
-template <int BC>
-__global__ void __launch_bounds__(kWarpTileWarps * 32, 3) hash_warp_kernel(HashArgs a) {
+template <int BC, bool PROBE>
+__global__ void __launch_bounds__(kWarpTileWarps * 32, 2) hash_warp_kernel(HashArgs a) {
   extern __shared__ __align__(16) unsigned char hw_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint64_t(*tile)[33] = reinterpret_cast<uint64_t(*)[33]>(hw_smem) + (size_t)warp * 32;
   const int bc = BC ? BC : a.block_chars;
   const int ntiles = (a.R + 31) / 32;
+  const TSlot* slots = nullptr;
+  uint64_t slot_mask = 0;
+  if (PROBE) {
+    slots = a.table->slots;
+    slot_mask = a.table->mask;
+  }
   for (int t = blockIdx.x * kWarpTileWarps + warp; t < ntiles; t += gridDim.x * kWarpTileWarps) {
     const int base = t * 32, r = base + lane;
     ReqDesc d;
@@ -486,40 +498,42 @@ __global__ void __launch_bounds__(kWarpTileWarps * 32, 3) hash_warp_kernel(HashA
 #pragma unroll
     for (int o = 16; o; o >>= 1) maxfull = max(maxfull, __shfl_xor_sync(0xffffffffu, maxfull, o));
     uint64_t prev = d.seed;
+    // PROBE state of this lane's request (pick_sparse's matchLongestPrefix without the table): p_ok = resolvable so far
+    // (the fast path without a trailing partial block: the others need hash_slow_kernel's hashes), p_open = still walking
+    bool p_ok = PROBE && r < a.R && d.fast && d.rem == 0;
+    bool p_open = p_ok && nf_mine > 0;
+    uint32_t p_n = 0, ref_raw = 0, ref_w = 0;
+    uint4 ref_hi = make_uint4(0u, 0u, 0u, 0u);
     for (int c0 = 0; c0 < maxfull; c0 += 32) {
       const int blk = c0 + lane;
       // ---- A: body states ----
       if (BC == 64) {
-        uint4 cur[4], nxt[4];
-        bool con, non = false;
-        {
-          const int nf = __shfl_sync(0xffffffffu, nf_mine, 0);
-          const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), 0);
-          con = blk < nf;
-          if (con) {
+        uint4 buf[3][4];  // a ring: request rq digested while rq+1 and rq+2 are in flight (indices compile-time after unrolling)
+        bool on[3];
+        auto fetch = [&](int rq, uint4 (&dst)[4], bool& o) {
+          const int nf = __shfl_sync(0xffffffffu, nf_mine, rq);
+          const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq);
+          o = blk < nf;
+          if (o) {
             const uint8_t* q = reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * 64;
 #pragma unroll
-            for (int k = 0; k < 4; k++) cur[k] = ldg16(q + 16 * k);
+            for (int k = 0; k < 4; k++) dst[k] = ldg16(q + 16 * k);
           }
-        }
+        };
+        fetch(0, buf[0], on[0]);
+        fetch(1, buf[1], on[1]);
 #pragma unroll 1
-        for (int rq = 0; rq < 32; rq++) {
-          if (rq + 1 < 32) {
-            const int nf = __shfl_sync(0xffffffffu, nf_mine, rq + 1);
-            const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq + 1);
-            non = blk < nf;
-            if (non) {
-              const uint8_t* q = reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * 64;
+        for (int rq0 = 0; rq0 < 32; rq0 += 3) {
 #pragma unroll
-              for (int k = 0; k < 4; k++) nxt[k] = ldg16(q + 16 * k);
+          for (int j = 0; j < 3; j++) {
+            const int rq = rq0 + j;
+            if (rq < 32) {
+              const int ns = (j + 2) % 3;
+              on[ns] = false;
+              if (rq + 2 < 32) fetch(rq + 2, buf[ns], on[ns]);
+              if (on[j]) tile[rq][lane] = body_state_64(buf[j]);
             }
-          } else {
-            non = false;
           }
-          if (con) tile[rq][lane] = body_state_64(cur);
-#pragma unroll
-          for (int k = 0; k < 4; k++) cur[k] = nxt[k];
-          con = non;
         }
       } else {
 #pragma unroll 1
@@ -531,23 +545,78 @@ __global__ void __launch_bounds__(kWarpTileWarps * 32, 3) hash_warp_kernel(HashA
       }
       __syncwarp();
       // ---- B: the chain, lane = request ----
-      {
-        const int nb = min(32, nf_mine - c0);
-        for (int i = 0; i < nb; i++) {
-          prev = xchain_aligned(tile[lane][i], prev);
-          tile[lane][i] = prev;
-        }
+      const int nb = min(32, nf_mine - c0);
+      for (int i = 0; i < nb; i++) {
+        prev = xchain_aligned(tile[lane][i], prev);
+        tile[lane][i] = prev;
       }
+      // ---- PROBE: indexer.Get on the lane's own row, kProbeU blocks at a time, up to the first miss ----
+      if (PROBE) {
+        for (int i0 = 0; __any_sync(0xffffffffu, p_open && i0 < nb); i0 += kProbeU) {
+          uint64_t h[kProbeU], idx[kProbeU];
+          uint4 lo[kProbeU];
+          bool act[kProbeU], hit[kProbeU];
+#pragma unroll
+          for (int u = 0; u < kProbeU; u++) {
+            act[u] = p_open && i0 + u < nb;
+            h[u] = act[u] ? tile[lane][i0 + u] : 0ULL;
+            idx[u] = h[u] & slot_mask;
+          }
+#pragma unroll
+          for (int u = 0; u < kProbeU; u++) {
+            lo[u] = make_uint4(0u, 0u, kCntFree, 0u);
+            if (act[u]) lo[u] = ldg16(&slots[idx[u]]);
+          }
+#pragma unroll
+          for (int u = 0; u < kProbeU; u++) hit[u] = act[u] && table_find(slots, slot_mask, h[u], idx[u], lo[u]);
+#pragma unroll
+          for (int u = 0; u < kProbeU; u++) {
+            if (!act[u] || !p_open) continue;
+            if (!hit[u]) {
+              p_open = false;                                   // the first miss ends the matched prefix
+              continue;
+            }
+            // members 2..9 (the slot's second half, same 32-byte sector as the first), loaded as pick_sparse_kernel loads them
+            uint4 hi = make_uint4(0u, 0u, 0u, 0u);
+            if (!(lo[u].z & kCntRow) && (lo[u].z & kCntMask) > 2u) hi = ldg16(reinterpret_cast<const uint4*>(&slots[idx[u]]) + 1);
+            if (c0 + i0 + u == 0) {
+              ref_raw = lo[u].z;                                // the first hit: the reference set
+              ref_w = lo[u].w;
+              ref_hi = hi;
+              p_n = 1;
+              if (ref_raw & kCntRow) p_ok = p_open = false;     // a bitset row: pick_sparse's exception table
+            } else if (lo[u].z != ref_raw || !same_inline_set(ref_w, ref_hi, lo[u].w, hi)) {
+              p_ok = p_open = false;                            // a different set: pick_sparse's exception table
+            } else {
+              p_n++;
+            }
+          }
+        }
+        if (c0 + 32 >= nf_mine) p_open = false;                 // the whole row matched
+      }
+      // a resolved row whose walk is over is not written: nothing reads it
+      const int nf_out = (PROBE && p_ok && !p_open) ? 0 : nf_mine;
       __syncwarp();
       // ---- C: hashes out ----
 #pragma unroll 4
       for (int rq = 0; rq < 32; rq++) {
-        const int nf = __shfl_sync(0xffffffffu, nf_mine, rq);
+        const int nf = __shfl_sync(0xffffffffu, nf_out, rq);
         if (blk < nf) a.hashes[(size_t)(base + rq) * a.stride + blk] = tile[rq][lane];
       }
       __syncwarp();
     }
-    if (r < a.R) a.n_hashes[r] = (uint16_t)(d.nfull + (d.rem > 0 ? 1 : 0));
+    if (PROBE) {
+      const uint32_t res = __ballot_sync(0xffffffffu, p_ok);
+      if (lane == 0 && res) atomicAdd(a.resolved, (unsigned long long)__popc(res));
+    }
+    if (r < a.R) {
+      a.n_hashes[r] = (uint16_t)(d.nfull + (d.rem > 0 ? 1 : 0));
+      if (PROBE) {
+        uint4* q = reinterpret_cast<uint4*>(a.probe + r);
+        q[0] = make_uint4(ref_raw, ref_w, p_ok ? p_n : kProbeUnresolved, 0u);
+        q[1] = ref_hi;
+      }
+    }
   }
 }
 
@@ -627,24 +696,35 @@ __global__ void __launch_bounds__(256) hash_slow_kernel(HashArgs a) {
   if (d.rem > 0) out[d.nfull] = link_slow(d.p + (size_t)d.nfull * bc, (uint32_t)d.rem, prev);
 }
 
+constexpr int kDefaultStages = 27;
+
+// the probing form exists for the default form (the warp-tile kernel) only
+bool hash_probe_applies(const HashArgs& a) {
+  return a.block_chars > 0 && (a.block_chars & 31) == 0 && (a.stage_mask == 0 || a.stage_mask == kDefaultStages);
+}
+
+template <int BC, bool PROBE>
+static void launch_warp_tile(const HashArgs& a, int blocks, size_t smem, cudaStream_t s) {
+  cudaFuncSetAttribute(hash_warp_kernel<BC, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  hash_warp_kernel<BC, PROBE><<<blocks, kWarpTileWarps * 32, smem, s>>>(a);
+}
+
 int launch_hash_prompts(const HashArgs& a, cudaStream_t s, int sm_count) {
   if (a.R <= 0) return 0;
   // default 27: the warp-tile fused kernel where the block size allows it (on H100 the step is 7 % faster than with the
   // two-kernel form), otherwise bodies + the CTA-tile chain kernel
-  const int stages0 = a.stage_mask ? a.stage_mask : 27;
+  const int stages0 = a.stage_mask ? a.stage_mask : kDefaultStages;
   if ((stages0 & 8) && a.block_chars > 0 && (a.block_chars & 31) == 0) {  // the warp-tile fused kernel
     const int ntiles = (a.R + 31) / 32;
-    int blocks = sm_count * 3;
+    int blocks = sm_count * 2;  // (the register budget of two requests in flight per warp: 2 CTAs per SM)
     const int need = (ntiles + kWarpTileWarps - 1) / kWarpTileWarps;
     if (blocks > need) blocks = need;
     const size_t smem = (size_t)kWarpTileWarps * 32 * 33 * 8;
-    if (a.block_chars == 64) {
-      cudaFuncSetAttribute(hash_warp_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      hash_warp_kernel<64><<<blocks, kWarpTileWarps * 32, smem, s>>>(a);
-    } else {
-      cudaFuncSetAttribute(hash_warp_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      hash_warp_kernel<0><<<blocks, kWarpTileWarps * 32, smem, s>>>(a);
-    }
+    const bool probe = a.probe != nullptr;  // (set only where hash_probe_applies)
+    if (a.block_chars == 64)
+      probe ? launch_warp_tile<64, true>(a, blocks, smem, s) : launch_warp_tile<64, false>(a, blocks, smem, s);
+    else
+      probe ? launch_warp_tile<0, true>(a, blocks, smem, s) : launch_warp_tile<0, false>(a, blocks, smem, s);
     hash_slow_kernel<<<(a.R + 255) / 256, 256, 0, s>>>(a);
     return 2;
   }

@@ -123,6 +123,15 @@ struct QBucketHdr {
 };
 constexpr int kQBuckets = 256;
 
+// What the hashing kernel found in the prefix index for one request, when it probed the index itself (hash_warp_kernel<BC,
+// true>): the request's n matched blocks are all hits carrying one inline set, {raw cnt word, ep0 | ep1 << 16, hi = ep2..ep9}
+// exactly as pick_sparse_kernel loads a slot; n == kProbeUnresolved sends the request through pick_sparse's own probe.
+struct __align__(16) ProbeRec {
+  uint32_t raw, w, n, pad;
+  uint4 hi;
+};
+constexpr uint32_t kProbeUnresolved = 0xFFFFFFFFu;
+
 struct ScoreArgs {
   Geo geo;
   Plan plan;
@@ -148,6 +157,7 @@ struct ScoreArgs {
   const uint16_t* n_hashes;     // [R]
   int32_t hash_stride;
   const TableView* table;       // device pointer to the prefix index's view (null: no table) — stable across rebuilds
+  const ProbeRec* probe;        // [R] or null: the hashing kernel's probe of this batch (pick_sparse skips the resolved rows)
   // dense rows
   const float4* dense;          // [R][M]
   const uint16_t* dense_total;  // [R]
@@ -188,6 +198,10 @@ struct HashArgs {
   uint16_t* n_hashes;       // [R]
   int32_t pdl;              // launch the chain kernel with programmatic dependent launch
   int32_t stage_mask;       // diagnostics: eppscore_set_debug key 2 (include/eppscore.h); 0 = the default form
+  // probe the prefix index too (hash_probe_applies): one record per request; the rows it resolves never reach `hashes`
+  const TableView* table;
+  ProbeRec* probe;          // [R] or null
+  unsigned long long* resolved;  // with probe: += the requests resolved (one atomic per warp tile)
 };
 
 struct PrepareArgs {
@@ -237,6 +251,7 @@ struct PrepareArgs {
 // launchers. Each returns the number of kernels it launched (for gpu_launches); the scoring launchers return -(cudaError_t)
 // when a launch failed.
 int launch_hash_prompts(const HashArgs& a, cudaStream_t s, int sm_count);
+bool hash_probe_applies(const HashArgs& a);   // launch_hash_prompts can probe the index for this batch (a.probe)
 int launch_prepare_snapshot(const PrepareArgs& a, cudaStream_t s);
 int launch_count_fields(const uint8_t* bytes, const int64_t* off, const int32_t* len, int R, int32_t* out, cudaStream_t s,
                         int sm_count);  // len(strings.Fields(prompt)) per request
@@ -244,6 +259,7 @@ int launch_score_pick(const ScoreArgs& a, bool dense, cudaStream_t s, int sm_cou
 int launch_score_matrix(const ScoreArgs& a, cudaStream_t s, int sm_count);             // every pair scored (masks, diagnostics)
 int launch_score_dense_fast(const ScoreArgs& a, cudaStream_t s, int sm_count);         // 0 if no specialisation applies
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count);              // 0 if not applicable
+bool pick_sparse_probes(const ScoreArgs& a);  // launch_pick_sparse takes the batch and probes the index for it (plan, outputs and geometry set; table and hashes are not looked at)
 // in-flight load producer (inflight_kernel.cu): requests[m] += sign * #{r : endpoint[r] == m}, token_sum[m] += sign * Σ tokens[r];
 // endpoint < 0 is skipped, endpoint >= n_ep (<= 8192) is skipped and sets *err.  init_* opts the kernel into the 16 bytes of
 // shared memory per endpoint it needs (once per device).

@@ -117,13 +117,6 @@ __device__ __forceinline__ uint32_t slot_member(uint32_t w, const uint4& hi, uin
   const uint32_t x = k < 2 ? w : (k < 4 ? hi.x : (k < 6 ? hi.y : (k < 8 ? hi.z : hi.w)));
   return (k & 1) ? (x >> 16) : (x & 0xFFFFu);
 }
-// do two inline sets with the same raw cnt word (not rows) have the same members?  Slots are kept CANONICAL by the index
-// program (members sorted, unused entries 0xFFFF: prefix_table.cuh set_member / clear_member) and the second half of a slot
-// is loaded for neither or both (same count), so equal sets are equal words.  A stale entry could only make two equal sets
-// look different, which sends the request through its exception table — slower, never wrong.
-__device__ __forceinline__ bool same_inline_set(uint32_t w0, const uint4& h0, uint32_t w1, const uint4& h1) {
-  return ((w0 ^ w1) | (h0.x ^ h1.x) | (h0.y ^ h1.y) | (h0.z ^ h1.z) | (h0.w ^ h1.w)) == 0;
-}
 // order-independent form of best_update (the exceptions of a lane arrive in table order, not ascending)
 __device__ __forceinline__ void best_update_any(Best& b, double s, int m, int tie_mode, uint32_t areq, uint32_t seed_hi) {
   const bool first = b.m < 0;
@@ -196,8 +189,13 @@ __global__ void __launch_bounds__(kSparseWarps * 32, EPP_SPARSE_MINBLOCKS) pick_
     bool use_table = false;                    // uniform within the request's lane group
     int n_same = 0;                            // matched blocks so far, all carrying the reference set
     if (have_table) {
+      // a request the hashing kernel resolved (ProbeRec) skips the probe: it takes part in the rounds of the other requests of
+      // its warp without a hit (no table, no count), and takes its count and set from the record afterwards
+      // (only the count is held across the probe rounds: the set is loaded after them, which keeps the registers as they were)
+      const uint32_t rec_n = (a.probe && valid) ? __ldg(&a.probe[r].n) : kProbeUnresolved;
+      const bool resolved = rec_n != kProbeUnresolved;  // (uniform in the request's lane group)
       constexpr int U = 4;            // hashes probed per lane per round (independent loads in flight)
-      bool stop = n == 0;
+      bool stop = n == 0 || resolved;
       int c0 = 0;
       while (__any_sync(0xffffffffu, !stop)) {
         uint64_t h[U], idx[U];
@@ -216,20 +214,7 @@ __global__ void __launch_bounds__(kSparseWarps * 32, EPP_SPARSE_MINBLOCKS) pick_
           if (act[u]) lo[u] = ldg16(&slots[idx[u]]);
         }
 #pragma unroll
-        for (int u = 0; u < U; u++) {                           // indexer.Get, indexer.go:86-102
-          hit[u] = false;
-          if (act[u]) {
-            for (;;) {
-              if (lo[u].z == kCntFree) break;                   // never-used slot: hash unknown
-              if ((((uint64_t)lo[u].y << 32) | lo[u].x) == h[u]) {
-                hit[u] = (lo[u].z & kCntMask) != 0;             // emptied set == deleted key
-                break;
-              }
-              idx[u] = (idx[u] + 1) & slot_mask;
-              lo[u] = ldg16(&slots[idx[u]]);
-            }
-          }
-        }
+        for (int u = 0; u < U; u++) hit[u] = act[u] && table_find(slots, slot_mask, h[u], idx[u], lo[u]);
         int nh_total = 0;   // blocks matched in this round before the first global miss
         bool open = !stop;
 #pragma unroll
@@ -256,7 +241,7 @@ __global__ void __launch_bounds__(kSparseWarps * 32, EPP_SPARSE_MINBLOCKS) pick_
         // i.e. all hits carry the same inline set as the request's first hit.  Then the exceptions are that set's members,
         // each with the number of matched blocks — no table needed.  The first hit that differs switches the request to the
         // table: the reference set is entered with the count so far, every later hit adds 1 to its own members.
-        if (c0 == 0) {  // the first hit of the request: lane 0 of the group, sub-round 0
+        if (c0 == 0) {  // the first hit of the request: lane 0 of the group, sub-round 0 (a resolved request takes its own below)
           ref_raw = __shfl_sync(0xffffffffu, hit[0] ? lo[0].z : 0u, gi * G);
           ref_w = __shfl_sync(0xffffffffu, lo[0].w, gi * G);
           ref_hi.x = __shfl_sync(0xffffffffu, hi[0].x, gi * G);
@@ -299,6 +284,14 @@ __global__ void __launch_bounds__(kSparseWarps * 32, EPP_SPARSE_MINBLOCKS) pick_
         }
         c0 += U * G;
         if (nh_total < U * G || c0 >= n) stop = true;
+      }
+      if (resolved) {
+        const uint2 set = __ldg(reinterpret_cast<const uint2*>(&a.probe[r].raw));
+        n_same = (int)rec_n;
+        ref_raw = set.x;
+        ref_w = set.y;
+        ref_hi = make_uint4(0u, 0u, 0u, 0u);  // members 2..9 exist only in sets of more than two
+        if ((ref_raw & kCntMask) > 2u) ref_hi = ldg16(&a.probe[r].hi);
       }
       __syncwarp();
     }
@@ -469,10 +462,21 @@ static int launch_sparse_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
 
 // Applicable when: unmasked, not dense, no per-pair diagnostics, plan flagged sparse_ok, summaries present.
 // Returns the number of launches: the sparse kernel plus the full-matrix kernel restricted to the requests it deferred.
+static bool sparse_applies(const ScoreArgs& a) {
+  if (a.R <= 0) return false;
+  if (!a.plan.sparse_ok || !a.summ || !a.tiemask || a.cand_mask || a.dense || a.match_out || a.scores_out || a.topk > 0) return false;
+  return a.geo.Mpad <= 65536;  // inline members are uint16
+}
+
+bool pick_sparse_probes(const ScoreArgs& a) {
+  if (!sparse_applies(a)) return false;
+  for (int s = 0; s < a.plan.n_steps; s++)
+    if (a.plan.kind[s] == STEP_PREFIX) return true;
+  return false;
+}
+
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
-  if (a.R <= 0) return 0;
-  if (!a.plan.sparse_ok || !a.summ || !a.tiemask || a.cand_mask || a.dense || a.match_out || a.scores_out || a.topk > 0) return 0;
-  if (a.geo.Mpad > 65536) return 0;  // inline members are uint16
+  if (!sparse_applies(a)) return 0;
   int launched;
   switch (a.geo.J) {
     case 1: launched = launch_sparse_seq<1>(a, s, sm_count); break;

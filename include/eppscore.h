@@ -257,7 +257,8 @@ typedef struct eppscore_stats {
   int64_t prefix_overflow_rows; /* sets of more than 10 endpoints (bitset rows in use) */
   int64_t prefix_rebuilds;      /* table rebuilds so far */
   uint32_t index_error;         /* sticky device-side error flags of the index (0 = healthy) */
-  uint32_t reserved;
+  uint32_t probe_resolved;      /* requests whose prefix match the hashing kernel settled itself, so the pick kernel skipped
+                                   their index probe; since creation, modulo 2^32 (diagnostics: read after the batches finished) */
 } eppscore_stats;
 
 /* ---- lifecycle ---- */

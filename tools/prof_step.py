@@ -1,5 +1,8 @@
 """Times the kernels of the headline step one by one (device-resident inputs, rotating input sets > L2) and the host-buffer
-call at several chunk sizes.  usage: python tools/prof_step.py [what ...]   what in {hash, hash2, pick, step, split, e2e, commit}"""
+call at several chunk sizes.  usage: python tools/prof_step.py [what ...]   what in {hash, hash2, pick, step, probe, split, e2e, commit}
+probe: the step's kernels one by one as the step runs them (the probing hash kernel, pick_sparse fed by its records), from a
+torch.profiler trace of CUDA-graph replays over the rotating input sets, and the shares of resolved / table-path / deferred
+requests: resolved counted by the engine (eppscore_stats.probe_resolved), deferred from the oracle's match counts."""
 import os
 import sys
 import time
@@ -105,6 +108,49 @@ if "pick" in what:
     assert np.array_equal(out["pick"][:4096].cpu().numpy(), want["pick"]) and np.array_equal(out["pick_score"][:4096].cpu().numpy(), want["pick_score"])
 if "step" in what:
     print(f"hash + pick     : {timeit(step):8.2f} us (direct launches, snapshot not re-prepared)")
+if "probe" in what:
+    from torch.profiler import ProfilerActivity, profile
+    from tests.score_constants import score_constants
+    for i in range(NS):
+        step(i)
+    torch.cuda.synchronize()
+    gs = []
+    for i in range(NS):
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=stream):
+            step(i)
+        gs.append(g)
+    for i in range(8):
+        gs[i % NS].replay()
+    torch.cuda.synchronize()
+    iters = 40
+    with profile(activities=[ProfilerActivity.CUDA]) as tr:
+        for i in range(iters):
+            gs[i % NS].replay()
+        torch.cuda.synchronize()
+    per = {}
+    for ev in tr.key_averages():
+        if ev.device_type.name == "CUDA" and ev.count > 0:
+            per[ev.key] = (ev.self_device_time_total if hasattr(ev, "self_device_time_total") else ev.self_cuda_time_total, ev.count)
+    for k, (tot, n) in sorted(per.items(), key=lambda kv: -kv[1][0]):
+        print(f"  {k[:90]:90s}: {tot / iters:8.2f} us per step ({n // iters} per step)")
+    print(f"hash + pick     : {timeit(step):8.2f} us (graph, no profiler)")
+    resolved = []
+    for i in range(NS):
+        r0 = eng.stats().probe_resolved
+        step(i)
+        torch.cuda.synchronize()
+        resolved.append((eng.stats().probe_resolved - r0) % (1 << 32))
+    kx = score_constants().exc_max
+    full = o.schedule_batch(osnap, prof, idx, R, prompt_bytes=host[0][0], prompt_off=host[0][1], model_seed=np.full(R, seed, np.uint64),
+                            adapter_id=host[0][2], block_chars=bench.BLOCK_CHARS, max_blocks=bench.MAX_BLOCKS, n_threads=os.cpu_count(),
+                            want_match=True)
+    deferred = int(((full["match_blocks"] > 0).sum(axis=1) > kx).sum())
+    step(0)
+    torch.cuda.synchronize()
+    assert np.array_equal(out["pick"].cpu().numpy(), full["pick"]) and np.array_equal(out["pick_score"].cpu().numpy(), full["pick_score"])
+    print(f"resolved by the hash kernel: {resolved} of {R} per set; set 0: resolved {resolved[0] / R:.4f}, "
+          f"deferred {deferred / R:.4f}, table path {(R - resolved[0] - deferred) / R:.4f}")
 if "split" in what:
     # the body kernel's two forms, then the device-resident batch cut into slices over several streams (debug keys 5 / 6)
     for mask, name in ((1, "bodies, one-shot"), (33, "bodies, pipelined (exp.)")):
