@@ -94,6 +94,7 @@ ABI_SYMBOLS = [
     ("eppscore_set_latency_params", C.c_int32, [_P, C.POINTER(LatencyParams)]),
     ("eppscore_schedule_batch", C.c_int32, [_P, C.POINTER(Batch)]),
     ("eppscore_schedule_batch_topk", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
+    ("eppscore_schedule_batch_topk_wide", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
     ("eppscore_hash_prompts", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     ("eppscore_count_fields", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
     ("eppscore_hash_prompts_host", C.c_int32, [C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32]),

@@ -119,7 +119,12 @@ struct eppscore_engine {
   // pinned staging for the small per-request results of a host batch: a D2H copy into the caller's (usually pageable)
   // arrays would block the host after every chunk and serialise the pipeline
   PinnedBuf h_res;
-  int32_t host_chunk = 8192;        // requests per chunk of a host-location batch (eppscore_set_debug key 3)
+  // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide): slot 0 serves device-location
+  // batches and the engine stream's host chunks, slot 1 the chunks on stream2.  Allocated by the first call that needs one
+  // and never reallocated, so a graph captured after that call keeps pointing at live memory.
+  DevBuf wide_scores[2];
+  int32_t wide_rows = 0;
+  int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
   // (eppscore_set_debug keys 5 and 6)
@@ -506,6 +511,115 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   return EPPSCORE_OK;
 }
 
+// Rows per slice of a wide top-k batch: a fixed byte budget of score rows.  Step 2 reads the slice right after step 1 wrote
+// it, so a slice that fits the H100's 50 MB L2 is read from L2 instead of HBM.  Measured with tools/prof_topk_wide.py at the
+// headline shape (64K x 1024, k = 16, H100 80GB HBM3 at 700 W): 32 MiB (16 slices) 1.96 / 2.57 / 2.06 ms for max-score /
+// weighted-random / random, 512 MiB (one slice, -DEPP_WIDE_SLICE_BYTES) 1.70 / 2.32 / 1.85 ms.  The L2 reuse does not pay
+// for the per-slice launches; 32 MiB stays because the large budget costs 16x the memory (two 512 MiB slots plus a hash
+// scratch for 64K rows) for about 12 %.
+#ifndef EPP_WIDE_SLICE_BYTES
+#define EPP_WIDE_SLICE_BYTES (32ull << 20)
+#endif
+constexpr unsigned long long kWideSliceBytes = EPP_WIDE_SLICE_BYTES;
+
+// Rows [base, base + n) of a device batch (every per-request array offset; prompt_bytes stays, the offsets index into it).
+DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t mw, size_t mb, size_t k) {
+  DevBatch q = d;
+  q.R = n;
+  q.request_base = d.request_base + base;
+  const size_t b = (size_t)base;
+  auto off = [b](auto* p, size_t per) { return p ? p + b * per : p; };
+  q.prompt_off = off(d.prompt_off, 1);
+  q.prompt_len = off(d.prompt_len, 1);
+  q.model_seed = off(d.model_seed, 1);
+  q.hashes_in = off(d.hashes_in, (size_t)d.hash_stride);
+  q.n_hashes_in = off(d.n_hashes_in, 1);
+  q.adapter_id = off(d.adapter_id, 1);
+  q.cand_mask = off(d.cand_mask, mw);
+  q.dense_feat = off(d.dense_feat, M * 4);
+  q.dense_total = off(d.dense_total, 1);
+  q.input_tokens = off(d.input_tokens, 1);
+  q.ttft_slo = off(d.ttft_slo, 1);
+  q.tpot_slo = off(d.tpot_slo, 1);
+  q.pred_out = off(d.pred_out, M * 2);
+  q.filter_mask_out = off(d.filter_mask_out, mw);
+  q.pick = off(d.pick, 1);
+  q.pick_score = off(d.pick_score, 1);
+  q.tie_count = off(d.tie_count, 1);
+  q.match_blocks = off(d.match_blocks, M);
+  q.total_blocks = off(d.total_blocks, 1);
+  q.hashes_out = off(d.hashes_out, mb);
+  q.scores_out = off(d.scores_out, M);
+  q.topk_m = off(d.topk_m, k);
+  q.topk_score = off(d.topk_score, k);
+  return q;
+}
+
+// eppscore_schedule_batch_topk_wide on device buffers, asynchronous on `s`, in two steps per slice of rows:
+//   1. the batch's scores_out route (the diagnostics variants of the full-matrix and generic dense kernels) writes the slice's
+//      weighted scores, NaN for non-candidates, into wide_scores[slot] (or into the caller's scores_out, which then needs no
+//      slicing), together with pick / pick_score / tie_count;
+//   2. topk_select_kernel turns the rows into the lists d.topk_m / d.topk_score [R][k].
+// The slices run in order on `s` (the scratch holds one slice), whatever the slicing keys 5 / 6 say.
+int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStream_t s, Scratch& sc, int slot) {
+  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch before set_snapshot");
+  if (d.R <= 0) return EPPSCORE_OK;
+  const size_t M = (size_t)e->M, mw = (M + 31) / 32;
+  const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
+  auto select = [&](const DevBatch& q, const double* scores) -> int32_t {
+    TopKSelectArgs t{};
+    t.scores = scores;
+    t.R = q.R;
+    t.M = e->M;
+    t.k = k;
+    t.pick_mode = e->cfg.pick_mode;
+    t.tie_mode = e->cfg.tie_mode;
+    t.seed_lo = (uint32_t)e->cfg.tie_seed;
+    t.seed_hi = (uint32_t)(e->cfg.tie_seed >> 32);
+    t.request_base = q.request_base;
+    t.out_m = q.topk_m;
+    t.out_s = q.topk_score;
+    const int launched = launch_topk_select(t, s);
+    if (launched < 0) {
+      cudaGetLastError();
+      return cuda_fail(e, (cudaError_t)-launched, "topk_select_kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
+    return EPPSCORE_OK;
+  };
+  int32_t rc;
+  if (d.scores_out) {
+    DevBatch q = d;
+    q.topk = 0;
+    if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
+    return select(d, d.scores_out);
+  }
+  DevBuf& buf = e->wide_scores[slot];
+  if (!buf.p) {
+    if (is_capturing(s))
+      return fail(e, EPPSCORE_ERR_CAPACITY,
+                  "the first eppscore_schedule_batch_topk_wide allocates the engine's score scratch: make one wide call outside "
+                  "the CUDA-graph capture first");
+    CK(e, buf.reserve((size_t)e->wide_rows * e->geo.Mpad * 8));
+  }
+  // the per-slice hash scratch is sized for a whole slice up front, so a larger wide call later does not move it under a
+  // captured graph
+  if (d.prompt_bytes && !d.hashes_in && !d.hashes_out) {
+    CK(e, sc.s_hashes.reserve((size_t)e->wide_rows * mb * 8));
+    CK(e, sc.s_nh.reserve((size_t)e->wide_rows * 2));
+  }
+  if (d.prompt_bytes && !d.input_tokens && cfg_has(e->cfg, EPPSCORE_SCORER_LATENCY)) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
+  for (int32_t base = 0; base < d.R; base += e->wide_rows) {
+    DevBatch q = slice_rows(d, base, std::min(e->wide_rows, d.R - base), M, mw, (size_t)mb, (size_t)k);
+    q.topk = 0;
+    q.scores_out = buf.as<double>();
+    if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
+    if ((rc = select(q, q.scores_out)) != EPPSCORE_OK) return rc;
+  }
+  return EPPSCORE_OK;
+}
+
 template <typename T>
 int32_t h2d(eppscore_engine* e, DevBuf& buf, const T* src, size_t count, const T** out, cudaStream_t st = nullptr) {
   *out = nullptr;
@@ -684,6 +798,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   eppscore_latency_params_default(&e->lat_params);
   e->geo = make_geo(e->cfg.max_endpoints);
   e->A_cap = (e->cfg.max_adapters + 63) / 64 * 64;
+  e->wide_rows = (int32_t)std::max<unsigned long long>(1, kWideSliceBytes / ((unsigned long long)e->geo.Mpad * 8));
   if (e->cfg.lru_capacity_max < 0) return fail(nullptr, EPPSCORE_ERR_INVALID, "lru_capacity_max < 0");
   eppscore_engine* ep = e.get();
   CK(nullptr, cudaSetDevice(device));
@@ -1027,13 +1142,14 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
 
 namespace {
 
-// eppscore_schedule_batch(_topk): t == nullptr ⇒ no top-k lists
-int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t) {
+// eppscore_schedule_batch(_topk, _topk_wide): t == nullptr ⇒ no top-k lists; wide: any k up to max_endpoints (schedule_wide)
+int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t, bool wide = false) {
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
   if (t) {
     if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
-    if (t->k < 1 || t->k > EPPSCORE_MAX_TOPK) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
+    if (wide && (t->k < 1 || t->k > e->cfg.max_endpoints)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, max_endpoints]");
+    if (!wide && (t->k < 1 || t->k > EPPSCORE_MAX_TOPK)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
     if (!t->endpoints || !t->scores) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
   }
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
@@ -1074,6 +1190,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     d.topk_m = t ? t->endpoints : nullptr;
     d.topk_score = t ? t->scores : nullptr;
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
+    if (wide) {
+      if ((rc = schedule_wide(e, d, tk, cs, e->sc[0], 0)) != EPPSCORE_OK) return rc;
+      return pending_record(e, cs);
+    }
     // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here)
     const bool sliceable = d.prompt_bytes && !d.hashes_in && !d.cand_mask && !d.dense_feat && !d.pred_out && !d.filter_mask_out &&
                            !d.match_blocks && !d.scores_out && !d.input_tokens && !d.ttft_slo && !d.tpot_slo;
@@ -1229,7 +1349,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
       hashes_dev = sc.s_hashes.as<uint64_t>();
       d.hashes_out = hashes_dev;
     }
-    rc = schedule_device(e, d, st, sc);
+    rc = wide ? schedule_wide(e, d, tk, st, sc, ci & 1) : schedule_device(e, d, st, sc);
     if (rc != EPPSCORE_OK) return rc;
     if (b->pick) CK(e, cudaMemcpyAsync(hp_pick + r0, d.pick, R * 4, cudaMemcpyDeviceToHost, st));
     if (b->pick_score) CK(e, cudaMemcpyAsync(hp_score + r0, d.pick_score, R * 8, cudaMemcpyDeviceToHost, st));
@@ -1268,6 +1388,12 @@ int32_t eppscore_schedule_batch_topk(eppscore_engine* e, const eppscore_batch* b
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!t) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
   return schedule_batch(e, b, t);
+}
+
+int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!t) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
+  return schedule_batch(e, b, t, true);
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,

@@ -260,6 +260,19 @@ int launch_score_matrix(const ScoreArgs& a, cudaStream_t s, int sm_count);      
 int launch_score_dense_fast(const ScoreArgs& a, cudaStream_t s, int sm_count);         // 0 if no specialisation applies
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count);              // 0 if not applicable
 bool pick_sparse_probes(const ScoreArgs& a);  // launch_pick_sparse takes the batch and probes the index for it (plan, outputs and geometry set; table and hashes are not looked at)
+
+// top-k lists of any length from weighted score rows (topk_select.cu): row r of `scores` ([R][M], NaN = not a candidate) is
+// request request_base + r; the first k entries of its pick order (device_common.cuh topk_key) go to out_m / out_s [R][k]
+struct TopKSelectArgs {
+  const double* scores;
+  int32_t R, M, k;
+  int32_t pick_mode, tie_mode;
+  uint32_t seed_lo, seed_hi;
+  int64_t request_base;
+  int32_t* out_m;
+  double* out_s;
+};
+int launch_topk_select(const TopKSelectArgs& a, cudaStream_t s);  // M <= 8192
 // in-flight load producer (inflight_kernel.cu): requests[m] += sign * #{r : endpoint[r] == m}, token_sum[m] += sign * Σ tokens[r];
 // endpoint < 0 is skipped, endpoint >= n_ep (<= 8192) is skipped and sets *err.  init_* opts the kernel into the 16 bytes of
 // shared memory per endpoint it needs (once per device).

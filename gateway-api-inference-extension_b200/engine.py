@@ -159,13 +159,18 @@ class Engine:
                  n_hashes_in=None, hash_stride=0, adapter_id=None, cand_mask=None, dense_feat=None, dense_total=None,
                  block_chars=0, max_blocks=0, request_base=0, want_match=False, want_total=True, want_hashes=False,
                  want_scores=False, input_tokens=None, ttft_slo=None, tpot_slo=None, want_pred=False, want_filter_mask=False,
-                 topk=0, device=False, stream=None, out=None):
+                 topk=0, topk_wide=0, device=False, stream=None, out=None):
         """Host mode (device=False): numpy in, returns dict of numpy outputs (copies inside the call).
         Device mode: CUDA tensors / raw pointers in; `out` must hold preallocated CUDA tensors
         (pick int32[R], pick_score float64[R], tie_count int32[R], optional match_blocks/total_blocks/hashes_out);
         the call is asynchronous on `stream`.
         topk=k (1..8): also the first k endpoints of every request's pick order (maxNumOfEndpoints, eppscore_topk):
-        topk_pick int32[R, k] (-1 padded) and topk_score float64[R, k]; in device mode `out` holds them."""
+        topk_pick int32[R, k] (-1 padded) and topk_score float64[R, k]; in device mode `out` holds them.
+        topk_wide=k (1..max_endpoints): the same lists for any k (eppscore_schedule_batch_topk_wide), returned the same way."""
+        if topk and topk_wide:
+            raise ValueError("topk and topk_wide are exclusive")
+        call, topk = ((self._lib.eppscore_schedule_batch_topk_wide, topk_wide) if topk_wide else
+                      (self._lib.eppscore_schedule_batch_topk, topk))
         a = _Args(device)
         b = Batch()
         b.struct_size = C.sizeof(Batch)
@@ -205,7 +210,7 @@ class Engine:
             b.filter_mask_out = a.ptr(out.get("filter_mask_out"), None)
             if topk:
                 t = self._topk(topk, a.ptr(out["topk_pick"], None), a.ptr(out["topk_score"], None))
-                self._check(self._lib.eppscore_schedule_batch_topk(self._h, C.byref(b), C.byref(t)))
+                self._check(call(self._h, C.byref(b), C.byref(t)))
             else:
                 self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
             return out
@@ -230,7 +235,7 @@ class Engine:
             res["topk_pick"] = np.full((R, topk), -1, np.int32)
             res["topk_score"] = np.zeros((R, topk), np.float64)
             t = self._topk(topk, res["topk_pick"].ctypes.data, res["topk_score"].ctypes.data)
-            self._check(self._lib.eppscore_schedule_batch_topk(self._h, C.byref(b), C.byref(t)))
+            self._check(call(self._h, C.byref(b), C.byref(t)))
         else:
             self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
         return res

@@ -34,6 +34,10 @@
 // whole score map (max-score only, the route of k > 8); the stochastic pickers refuse k > 1.
 extern "C" int32_t eppscore_schedule_batch_topk(struct eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t)
     __attribute__((weak));
+// eppscore_schedule_batch_topk_wide (lists longer than 8) came the same way: EngineHasTopKWide() tells.  Without it, the
+// stochastic pickers refuse k > 8 and max-score k > 8 takes the score map.
+extern "C" int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t)
+    __attribute__((weak));
 
 // The in-flight load producer's entry points came the same way: bound weakly, EngineHasInFlightLoad() tells.
 extern "C" int32_t eppscore_estimate_tokens(struct eppscore_engine* e, int32_t R, int32_t location, const int64_t* request_size_bytes,
@@ -65,6 +69,7 @@ inline bool EngineHasRunningQueues() {
          &eppscore_running_get != nullptr && &eppscore_running_reserve != nullptr;
 }
 inline bool EngineHasTopK() { return &eppscore_schedule_batch_topk != nullptr; }
+inline bool EngineHasTopKWide() { return &eppscore_schedule_batch_topk_wide != nullptr; }
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
          &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
@@ -156,7 +161,8 @@ inline DeviceFilter SLOHeadroomTierFilter(double epsilonExploreNeg = 0.01) {
 
 struct MaxScorePicker {
   int MaxNumOfEndpoints = 1;  // picker.DefaultMaxNumOfEndpoints (picker/common.go:36); 2..8: the engine's top-k lists (every
-                              // mode), > 8: max-score only, from the engine's score rows
+                              // mode); > 8: the engine's wide lists (every mode; max-score with TIE_SEEDED_RANDOM, or an
+                              // engine without the wide call: max-score only, from the engine's score rows)
   int Mode = EPPSCORE_PICK_MAX_SCORE;
 };
 // weighted-random-picker (A-Res, picker/weightedrandom/picker.go:111-155) and random-picker (picker/random/picker.go:85-101):
@@ -222,8 +228,9 @@ class Scheduler {
     const auto& sc = cfg.Profile.scorers();
     if (sc.size() > EPPSCORE_MAX_SCORERS) throw SchedulingError("too many scorers in profile");
     if (cfg.Profile.picker().MaxNumOfEndpoints < 1) throw SchedulingError("maxNumOfEndpoints must be >= 1");
-    if (cfg.Profile.picker().MaxNumOfEndpoints > EPPSCORE_MAX_TOPK && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE)
-      throw SchedulingError("maxNumOfEndpoints > 8 is supported for the max-score picker only");
+    if (cfg.Profile.picker().MaxNumOfEndpoints > EPPSCORE_MAX_TOPK && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE &&
+        !EngineHasTopKWide())
+      throw SchedulingError("maxNumOfEndpoints > 8 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk_wide");
     if (cfg.Profile.picker().MaxNumOfEndpoints > 1 && cfg.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE && !EngineHasTopK())
       throw SchedulingError("maxNumOfEndpoints > 1 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk");
     if (cfg.InFlightLoad && !EngineHasInFlightLoad())
@@ -447,22 +454,28 @@ class Scheduler {
     b.total_blocks = last_nh_.data();
     b.hashes_out = want_prefix ? last_hashes_.data() : nullptr;
     const int topk = cfg_.Profile.picker().MaxNumOfEndpoints;
-    const bool engine_topk = topk > 1 && topk <= EPPSCORE_MAX_TOPK && EngineHasTopK();
+    // k > 8: the wide lists, except max-score with seeded-random ties, whose device order puts positions >= 1 of a tie class
+    // in priority order where the score map's route has ascending index
+    const bool engine_wide = topk > EPPSCORE_MAX_TOPK && EngineHasTopKWide() &&
+                             (cfg_.Profile.picker().Mode != EPPSCORE_PICK_MAX_SCORE || cfg_.TieMode == EPPSCORE_TIE_LOWEST_INDEX);
+    const bool engine_topk = (topk > 1 && topk <= EPPSCORE_MAX_TOPK && EngineHasTopK()) || engine_wide;
+    const int klist = engine_wide ? std::min(topk, cfg_.MaxEndpoints) : topk;  // entries past max_endpoints would all be -1
     std::vector<double> all_scores;
     std::vector<int32_t> topk_ids;
     std::vector<double> topk_scores;
     if (engine_topk) {  // the picker's first k endpoints, ordered on the device (eppscore_topk)
-      topk_ids.resize((size_t)R * topk);
-      topk_scores.resize((size_t)R * topk);
+      topk_ids.resize((size_t)R * klist);
+      topk_scores.resize((size_t)R * klist);
       eppscore_topk t{};
       t.struct_size = sizeof(t);
-      t.k = topk;
+      t.k = klist;
       t.endpoints = topk_ids.data();
       t.scores = topk_scores.data();
-      if (eppscore_schedule_batch_topk(eng_, &b, &t) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_schedule_batch_topk: ") + eppscore_last_error(eng_));
+      const char* what = engine_wide ? "eppscore_schedule_batch_topk_wide: " : "eppscore_schedule_batch_topk: ";
+      if ((engine_wide ? eppscore_schedule_batch_topk_wide(eng_, &b, &t) : eppscore_schedule_batch_topk(eng_, &b, &t)) != EPPSCORE_OK)
+        throw SchedulingError(std::string(what) + eppscore_last_error(eng_));
     } else {
-      if (topk > 1) {  // k > 8, max-score: the whole weightedScorePerEndpoint map, NaN for non-candidates (scheduler_profile.go:155-174)
+      if (topk > 1) {  // k > 8, max-score (seeded-random ties or no wide call): the whole weightedScorePerEndpoint map, NaN for non-candidates (scheduler_profile.go:155-174)
         all_scores.resize((size_t)R * Mx);
         b.scores_out = all_scores.data();
       }
@@ -486,14 +499,14 @@ class Scheduler {
       out[r].result.PrimaryProfileName = cfg_.ProfileName;
       if (engine_topk) {  // entries 1..k-1 of the picker's order (entry 0 is the pick); -1 past the last candidate
         auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
-        for (int i = 1; i < topk; i++) {
-          const int32_t id = topk_ids[(size_t)r * topk + i];
+        for (int i = 1; i < klist; i++) {
+          const int32_t id = topk_ids[(size_t)r * klist + i];
           if (id < 0) break;
           if (id >= Mx || pos_of_id[(size_t)id] < 0) throw SchedulingError("engine listed an endpoint that is not in the candidate list");
           ScoredEndpoint o2;
           o2.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)id]];
           o2.Index = pos_of_id[(size_t)id];
-          o2.Score = topk_scores[(size_t)r * topk + i];
+          o2.Score = topk_scores[(size_t)r * klist + i];
           te.push_back(o2);
         }
       } else if (topk > 1) {  // picker/maxscore/picker.go:104-106: the next best candidates, descending score

@@ -238,7 +238,7 @@ typedef struct eppscore_batch {
 #define EPPSCORE_MAX_TOPK 8
 typedef struct eppscore_topk {
   uint32_t struct_size;
-  int32_t k;                   /* 1..EPPSCORE_MAX_TOPK */
+  int32_t k;                   /* 1..EPPSCORE_MAX_TOPK (eppscore_schedule_batch_topk_wide: 1..max_endpoints) */
   int32_t *endpoints;          /* [R*k] */
   double *scores;              /* [R*k] ScoredEndpoint.Score of each entry */
 } eppscore_topk;
@@ -293,6 +293,17 @@ int32_t eppscore_schedule_batch(struct eppscore_engine *e, const eppscore_batch 
 /* The same, plus the first t->k endpoints of every request's pick order (see eppscore_topk).  These batches run on the
  * full-matrix kernels.  ERR_INVALID: k outside [1, EPPSCORE_MAX_TOPK], a wrong struct_size or NULL arrays. */
 int32_t eppscore_schedule_batch_topk(struct eppscore_engine *e, const eppscore_batch *b, const eppscore_topk *t);
+/* The same lists for any k in [1, config.max_endpoints] (maxNumOfEndpoints has no upper bound in the reference), in the
+ * order documented above eppscore_topk, on the device for every pick mode.  pick, pick_score and tie_count are those of
+ * eppscore_schedule_batch, entry 0 is the pick, short lists are padded with -1 / 0.0, and for k <= EPPSCORE_MAX_TOPK the lists
+ * equal eppscore_schedule_batch_topk's bit for bit.  It accepts the batches eppscore_schedule_batch_topk accepts and refuses
+ * the others with the same status.  Per slice of requests, the batch's scores_out route writes the weighted scores into an
+ * engine-owned scratch (a fixed byte budget of rows: its size depends on max_endpoints only), and a selection kernel orders
+ * each row.  The scratch is allocated by the first wide call and never reallocated: a wide call inside a CUDA-graph capture
+ * before any wide call outside one fails with ERR_CAPACITY.  A caller that passes scores_out gets the rows there and no
+ * scratch is used.  The slices of a device-location batch run in order on its stream (debug keys 5 / 6 do not cut it).
+ * ERR_INVALID: k outside [1, max_endpoints], a wrong struct_size or NULL arrays. */
+int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppscore_batch *b, const eppscore_topk *t);
 
 /* ---- stand-alone stages (same kernels; for parity tests and hosts that only want one stage) ---- */
 /* hashPrompt for R prompts (hashing.go:34-98). hashes_out [R*max_blocks], n_hashes_out [R]. */
