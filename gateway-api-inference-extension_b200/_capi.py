@@ -8,6 +8,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 MAX_SCORERS = 8
 MAX_ENDPOINT_COLS = 4
 MAX_TOPK = 8
+MAX_PROFILES = 4
 
 SCORER = {"queue": 0, "kv": 1, "prefix": 2, "lora": 3, "running": 4, "latency": 5, "token_load": 6,
           "col0": 8, "col1": 9, "col2": 10, "col3": 11, "pair0": 16, "pair1": 17}
@@ -31,6 +32,18 @@ class Config(C.Structure):
                 ("max_adapters", C.c_int32), ("prefix_capacity", C.c_int64), ("lru_capacity_default", C.c_int32),
                 ("lru_capacity_max", C.c_int32), ("token_load_threshold", C.c_double), ("pick_mode", C.c_int32), ("n_filters", C.c_int32),
                 ("filter_kind", C.c_int32 * 4), ("filter_param", (C.c_double * 3) * 4)]
+
+
+class Profile(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("n_scorers", C.c_int32), ("scorer_kind", C.c_int32 * MAX_SCORERS),
+                ("scorer_weight", C.c_double * MAX_SCORERS), ("pick_mode", C.c_int32), ("n_filters", C.c_int32),
+                ("filter_kind", C.c_int32 * 4), ("filter_param", (C.c_double * 3) * 4)]
+
+
+class ProfileRun(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("profile", C.c_int32), ("cand_mask", C.c_void_p), ("pick", C.c_void_p),
+                ("pick_score", C.c_void_p), ("tie_count", C.c_void_p), ("scores_out", C.c_void_p), ("pred_out", C.c_void_p),
+                ("filter_mask_out", C.c_void_p)]
 
 
 class LatencyParams(C.Structure):
@@ -95,12 +108,17 @@ ABI_SYMBOLS = [
     ("eppscore_schedule_batch", C.c_int32, [_P, C.POINTER(Batch)]),
     ("eppscore_schedule_batch_topk", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
     ("eppscore_schedule_batch_topk_wide", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
+    ("eppscore_add_profile", C.c_int32, [_P, C.POINTER(Profile), C.POINTER(C.c_int32)]),
+    ("eppscore_set_profile_endpoints", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
+    ("eppscore_schedule_batch_profiles", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun)]),
     ("eppscore_hash_prompts", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     ("eppscore_count_fields", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
     ("eppscore_hash_prompts_host", C.c_int32, [C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32]),
     ("eppscore_model_seed", C.c_uint64, [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]),
     ("eppscore_xxh64", C.c_uint64, [C.c_char_p, C.c_size_t, C.c_uint64]),
     ("eppscore_commit_picks", C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P]),
+    ("eppscore_commit_picks_profiles", C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), _P, _P, C.c_int32, _P,
+                                                   C.c_int32, C.c_int64, _P]),
     ("eppscore_prefix_add", C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32]),
     ("eppscore_prefix_apply", C.c_int32, [_P, C.c_int64, _P, _P, _P]),
     ("eppscore_prefix_remove_endpoint", C.c_int32, [_P, C.c_int32]),

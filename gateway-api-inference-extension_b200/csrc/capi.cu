@@ -38,6 +38,19 @@ struct PendingBatch {
   bool armed = false;  // the batch may not have completed
 };
 
+// One scheduler profile (eppscore_add_profile): its configuration and everything prepared for it from the shared snapshot.
+struct Profile {
+  eppscore_config cfg{};  // the engine's config with this profile's scorers, picker and filters, and its own tie seed
+  DevBuf term[kMaxSteps], fold_unmasked, fold_masked, summ, tiemask, prefix_lut2d, qhdr[2], qbucket[2];
+  bool have_lut2d = false;
+  PlanSet plan_unmasked{}, plan_masked{};
+  PrepareArgs pa{};  // what the current snapshot was prepared with
+  // endpoint subset: natural-order [Mpad/32] and permuted [row_words] bit rows, live (what the current snapshot was prepared with)
+  // and next (eppscore_set_profile_endpoints, copied to live by the next set_snapshot)
+  DevBuf member_nat, member_perm, next_nat, next_perm;
+  bool subset = false, next_subset = false;
+};
+
 }  // namespace
 
 struct eppscore_engine {
@@ -60,16 +73,17 @@ struct eppscore_engine {
   int32_t M = 0, A = 0, lora_words = 0;
   uint64_t epoch = 0;
   DevBuf raw_kv, raw_queue, raw_running, raw_act, raw_wait, raw_nmodels, raw_max, raw_col[4];
-  DevBuf raw_min_tpot, raw_dispatched, raw_prefill, raw_tokens, lat_ep, qhdr[2], qbucket[2];
+  DevBuf raw_min_tpot, raw_dispatched, raw_prefill, raw_tokens, lat_ep;
   eppscore_latency_params lat_params{};  // pending: applied by the next set_snapshot
   LatArgs lat_args{};                    // what the current snapshot was prepared with
   bool have_col[4] = {false, false, false, false};
   bool have_running = false;
   const int64_t* cur_queue = nullptr;    // raw WaitingQueueSize / RunningRequestsSize of the current snapshot
   const int64_t* cur_running = nullptr;  // (engine copy for host snapshots, the caller's buffer for device ones)
-  DevBuf term[kMaxSteps], fold_unmasked, fold_masked, cls_lo, cls_hi, summ, tiemask, prefix_lut2d;
-  bool have_lut2d = false;
-  PlanSet plan_unmasked{}, plan_masked{};
+  DevBuf cls_lo, cls_hi;                 // LoRA class planes (snapshot only: every profile's adapter kernel writes the same)
+  Profile prof[EPPSCORE_MAX_PROFILES];
+  int32_t n_prof = 0;
+  PrepareArgs base_pa{};                 // the profile-independent part of the current snapshot's preparation
 
   // prefix index: hashToPods + the per-endpoint LRUs, both device-resident (prefix_index.hpp); mutated on `stream`
   std::unique_ptr<DeviceIndex> index;
@@ -79,12 +93,11 @@ struct eppscore_engine {
   // and synchronises it before it returns, so one set serves them all.
   DevBuf stage[6];
 
-  // Producer state the scorers read: mutations of either producer below prepare the snapshot terms again (with last_pa) when
-  // the state feeds the current snapshot.  Mutations outside a CUDA-graph capture are ordered through ev_producer, recorded
-  // after each one on its stream, so the two families never rewrite the terms concurrently (producer_begin / producer_end).
+  // Producer state the scorers read: mutations of either producer below prepare the terms of the profiles that read the state
+  // again (with their Profile::pa).  Mutations outside a CUDA-graph capture are ordered through ev_producer, recorded after
+  // each one on its stream, so the two families never rewrite the terms concurrently (producer_begin / producer_end).
   Event ev_producer;
   bool producer_pending = false;
-  PrepareArgs last_pa{};  // what the current snapshot was prepared with
 
   // in-flight load producer (inflightload/producer.go): per-endpoint request and token counters, [Mpad] int64 each, zeroed at
   // create.  They feed the token-load scorer when the snapshot carries no inflight_tokens.
@@ -114,7 +127,8 @@ struct eppscore_engine {
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
-        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe;
+        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe,
+        s_subset;  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
   } sc[4];
   // pinned staging for the small per-request results of a host batch: a D2H copy into the caller's (usually pageable)
   // arrays would block the host after every chunk and serialise the pipeline
@@ -211,26 +225,35 @@ bool cfg_has(const eppscore_config& c, int kind) {
   return false;
 }
 
-// The token-load scorer reads the in-flight counters: the current snapshot's terms depend on them.
-bool counters_feed_scorer(const eppscore_engine* e) {
-  return e->have_snapshot && !e->snapshot_has_tokens && cfg_has(e->cfg, EPPSCORE_SCORER_TOKEN_LOAD);
+// Bit p: profile p has a scorer of this kind.
+unsigned profiles_with(const eppscore_engine* e, int kind) {
+  unsigned bits = 0;
+  for (int p = 0; p < e->n_prof; p++)
+    if (cfg_has(e->prof[p].cfg, kind)) bits |= 1u << p;
+  return bits;
 }
-// The latency fold-in reads the running-request queues (the per-endpoint minimum, or the count, or both).
-bool running_feeds_scorer(const eppscore_engine* e) {
-  return e->have_snapshot && e->lat_ep.p && (!e->snapshot_has_min_tpot || !e->snapshot_has_dispatched);
+// The profiles whose current terms read the in-flight counters (token-load scorers).
+unsigned counters_feed_scorer(const eppscore_engine* e) {
+  return (e->have_snapshot && !e->snapshot_has_tokens) ? profiles_with(e, EPPSCORE_SCORER_TOKEN_LOAD) : 0u;
+}
+// The profiles whose latency fold-in reads the running-request queues (the per-endpoint minimum, or the count, or both).
+unsigned running_feeds_scorer(const eppscore_engine* e) {
+  return (e->have_snapshot && e->lat_ep.p && (!e->snapshot_has_min_tpot || !e->snapshot_has_dispatched))
+             ? profiles_with(e, EPPSCORE_SCORER_LATENCY)
+             : 0u;
 }
 
 // Translate the scorer list into kernel steps.  Leading request-independent scorers are folded into
 // one precomputed array ((0.0+t0)+t1)+… — exact, because the kernel adds in the same order.
-void build_plan(eppscore_engine* e, bool masked, PlanSet* ps) {
+void build_plan(Profile& P, bool masked, PlanSet* ps) {
   Plan& p = ps->plan;
   memset(&p, 0, sizeof(p));
-  const eppscore_config& c = e->cfg;
+  const eppscore_config& c = P.cfg;
   int lead = 0;
   while (lead < c.n_scorers && is_endpoint_term_kind(c.scorer_kind[lead], masked)) lead++;
   int nt = 0, ns = 0;
   if (lead > 0) {
-    ps->term_ptr[nt] = (masked ? e->fold_masked : e->fold_unmasked).as<double>();
+    ps->term_ptr[nt] = (masked ? P.fold_masked : P.fold_unmasked).as<double>();
     p.kind[ns] = STEP_EP_TERM;
     p.arg[ns] = nt++;
     ns++;
@@ -240,7 +263,7 @@ void build_plan(eppscore_engine* e, bool masked, PlanSet* ps) {
     const double w = c.scorer_weight[s];
     p.weight[ns] = w;
     if (is_endpoint_term_kind(k, masked)) {
-      ps->term_ptr[nt] = e->term[s].as<double>();
+      ps->term_ptr[nt] = P.term[s].as<double>();
       p.kind[ns] = STEP_EP_TERM;
       p.arg[ns] = nt++;
     } else if (k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING) {
@@ -293,12 +316,14 @@ int32_t index_end(eppscore_engine* e) {
   return EPPSCORE_OK;
 }
 
-// Prepares the snapshot terms from e->last_pa on `st` and publishes them: ev_snapshot is recorded behind the kernels so that
-// batches on other streams wait for the new terms (schedule_device).  The engine stream waits too, except while `st` is being
-// captured into a CUDA graph: a captured stream may not take dependencies from outside its capture, so inside one
-// ev_snapshot becomes a graph edge that other streams of the same capture join on, and in-stream order does the rest.
-int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st) {
-  e->launches += launch_prepare_snapshot(e->last_pa, st);
+// Prepares the terms of the profiles in `which` (bit p: profile p) from their Profile::pa on `st` and publishes them:
+// ev_snapshot is recorded behind the kernels so that batches on other streams wait for the new terms (schedule_device).  The
+// engine stream waits too, except while `st` is being captured into a CUDA graph: a captured stream may not take dependencies
+// from outside its capture, so inside one ev_snapshot becomes a graph edge that other streams of the same capture join on, and
+// in-stream order does the rest.
+int32_t prepare_snapshot(eppscore_engine* e, cudaStream_t st, unsigned which) {
+  for (int p = 0; p < e->n_prof; p++)
+    if (which & (1u << p)) e->launches += launch_prepare_snapshot(e->prof[p].pa, st);
   CK(e, cudaGetLastError());
   unsigned long long cap_id = 0;
   const bool capturing = is_capturing(st, &cap_id);
@@ -317,14 +342,14 @@ int32_t producer_begin(eppscore_engine* e, cudaStream_t st, bool* capturing) {
   if (!*capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(st, e->ev_producer, 0));
   return EPPSCORE_OK;
 }
-// After a mutation: when the producer's state feeds the current snapshot (`feeds`), the terms that read it — the token-load
-// term, the latency fold-in's endpoint arrays, the folded leading run and the per-adapter summaries of the sparse path —
-// change, so the snapshot is prepared again on the same stream, with eppscore_set_snapshot's ordering (a device-location batch
-// another stream launched against the current terms finishes reading them first).
-int32_t producer_end(eppscore_engine* e, cudaStream_t st, bool capturing, bool feeds) {
+// After a mutation: for the profiles whose terms read the producer's state (`feeds`, bit p: profile p), the terms that read it
+// — the token-load term, the latency fold-in's endpoint arrays, the folded leading run and the per-adapter summaries of the
+// sparse path — change, so those profiles are prepared again on the same stream, with eppscore_set_snapshot's ordering (a
+// device-location batch another stream launched against the current terms finishes reading them first).
+int32_t producer_end(eppscore_engine* e, cudaStream_t st, bool capturing, unsigned feeds) {
   if (feeds) {
     int32_t rc = capturing ? EPPSCORE_OK : pending_wait(e, st);
-    if (rc == EPPSCORE_OK) rc = prepare_snapshot(e, st);
+    if (rc == EPPSCORE_OK) rc = prepare_snapshot(e, st, feeds);
     if (rc != EPPSCORE_OK) return rc;
   }
   if (!capturing) {
@@ -333,6 +358,18 @@ int32_t producer_end(eppscore_engine* e, cudaStream_t st, bool capturing, bool f
   }
   return EPPSCORE_OK;
 }
+
+// One profile's share of a batch (eppscore_profile_run): its host-side filter result and outputs, device pointers.
+struct DevRun {
+  int32_t profile;
+  const uint32_t* cand_mask;
+  int32_t* pick;
+  double* pick_score;
+  int32_t* tie_count;
+  double* scores_out;
+  double* pred_out;
+  uint32_t* filter_mask_out;
+};
 
 struct DevBatch {  // all device pointers
   int32_t R;
@@ -346,34 +383,27 @@ struct DevBatch {  // all device pointers
   int32_t hash_stride;
   int32_t block_chars, max_blocks;
   const int32_t* adapter_id;
-  const uint32_t* cand_mask;
   const float* dense_feat;
   const uint16_t* dense_total;
   const int32_t* input_tokens;
   const double* ttft_slo;
   const double* tpot_slo;
-  double* pred_out;
-  uint32_t* filter_mask_out;
-  int32_t* pick;
-  double* pick_score;
-  int32_t* tie_count;
-  uint16_t* match_blocks;
+  uint16_t* match_blocks;   // profile-independent outputs, written by the kernels of run 0
   uint16_t* total_blocks;
   uint64_t* hashes_out;
-  double* scores_out;
-  int32_t topk;          // > 0: topk_m / topk_score [R*topk] are written
+  int32_t topk;          // > 0 (single run only): topk_m / topk_score [R*topk] are written
   int32_t* topk_m;
   double* topk_score;
+  int32_t n_runs;
+  DevRun run[EPPSCORE_MAX_PROFILES];
 };
 
-// The hot path on device-resident buffers: [hash kernel] + score/pick kernel, asynchronous on `s`.
+// The hot path on device-resident buffers: [hash kernel] + each run's score/pick kernels, asynchronous on `s`.  The hash stage
+// runs once for all runs.
 int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, Scratch& sc) {
   if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch before set_snapshot");
   if (b.R <= 0) return EPPSCORE_OK;
-  if (!b.pick || !b.pick_score || !b.tie_count) return fail(e, EPPSCORE_ERR_INVALID, "pick/pick_score/tie_count required");
   const bool dense = b.dense_feat != nullptr;
-  const bool masked = b.cand_mask != nullptr;
-  const PlanSet& ps = masked ? e->plan_masked : e->plan_unmasked;
 
   // Ordering against the snapshot preparation and the table flush, which may have run on other streams.
   // The hash kernels depend on neither, so the snapshot wait is issued only before the pick kernel: a caller
@@ -385,129 +415,212 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   const bool wait_snapshot = capturing ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
                                        : (e->snapshot_capture_id == 0 && s != e->snapshot_stream);
 
-  bool hashed_here = false;
-  ScoreArgs a{};
-  a.geo = e->geo;
-  a.geo.M = e->M;
-  a.plan = ps.plan;
-  a.R = b.R;
-  a.request_base = b.request_base;
-  for (int t = 0; t < ps.plan.n_terms; t++) a.term[t] = ps.term_ptr[t];
-  a.minmax_q[0] = e->cur_queue;
-  a.minmax_q[1] = e->cur_running;
-  for (int which = 0; which < 2; which++) {
-    a.qhdr[which] = e->qhdr[which].as<QBucketHdr>();
-    a.qbucket[which] = e->qbucket[which].as<uint32_t>();
+  // Per run: its profile's arguments.  A run on a profile with an endpoint subset and no cand_mask stays on the sparse path with
+  // the member bitmap when that path takes it; every other run on such a profile is scored by the masked kernels on rows
+  // subset ∧ cand_mask (`via_rows`).
+  ScoreArgs a[EPPSCORE_MAX_PROFILES];
+  bool via_rows[EPPSCORE_MAX_PROFILES] = {};
+  bool any_lat = false, want_prefix = b.match_blocks || b.total_blocks || b.hashes_out;
+  for (int i = 0; i < b.n_runs; i++) {
+    const DevRun& run = b.run[i];
+    Profile& P = e->prof[run.profile];
+    if (!run.pick || !run.pick_score || !run.tie_count) return fail(e, EPPSCORE_ERR_INVALID, "pick/pick_score/tie_count required");
+    if (dense && P.cfg.pick_mode != EPPSCORE_PICK_MAX_SCORE)
+      return fail(e, EPPSCORE_ERR_INVALID, "the stochastic pickers are not available on dense feature rows");
+    ScoreArgs& x = a[i];
+    x = ScoreArgs{};
+    x.geo = e->geo;
+    x.geo.M = e->M;
+    x.R = b.R;
+    x.request_base = b.request_base;
+    for (int which = 0; which < 2; which++) {
+      x.minmax_q[which] = which == 0 ? e->cur_queue : e->cur_running;
+      x.qhdr[which] = P.qhdr[which].as<QBucketHdr>();
+      x.qbucket[which] = P.qbucket[which].as<uint32_t>();
+    }
+    x.cls_lo = e->cls_lo.as<uint32_t>();
+    x.cls_hi = e->cls_hi.as<uint32_t>();
+    x.prefix_lut2d = P.have_lut2d ? P.prefix_lut2d.as<double>() : nullptr;
+    x.A = e->A;
+    x.adapter_id = b.adapter_id;
+    x.mask_words = (e->M + 31) / 32;
+    x.dense = reinterpret_cast<const float4*>(b.dense_feat);
+    x.dense_total = b.dense_total;
+    x.pick = run.pick;
+    x.pick_score = run.pick_score;
+    x.tie_count = run.tie_count;
+    x.scores_out = run.scores_out;
+    if (i == 0) {
+      x.match_out = b.match_blocks;
+      x.total_out = b.total_blocks;
+      x.topk = b.topk;
+      x.topk_m = b.topk_m;
+      x.topk_score = b.topk_score;
+    }
+    if (cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY)) {
+      if (dense) return fail(e, EPPSCORE_ERR_INVALID, "the latency scorer is not available on dense feature rows");
+      if (!e->lat_args.enabled) return fail(e, EPPSCORE_ERR_INVALID, "latency scorer configured but the snapshot was prepared without latency params");
+      any_lat = true;
+      x.lat = e->lat_args;
+      x.lat.input_tokens = b.input_tokens;
+      x.lat.ttft_slo = b.ttft_slo;
+      x.lat.tpot_slo = b.tpot_slo;
+      x.lat.pred_out = run.pred_out;
+      x.n_filters = P.cfg.n_filters;
+      for (int f = 0; f < P.cfg.n_filters; f++) {
+        x.filter_kind[f] = P.cfg.filter_kind[f];
+        for (int q = 0; q < 3; q++) x.filter_param[f][q] = P.cfg.filter_param[f][q];
+      }
+      x.filter_mask_out = run.filter_mask_out;
+    }
+    if (cfg_has(P.cfg, EPPSCORE_SCORER_PREFIX) || cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY)) want_prefix = true;
+    // the unmasked form first: it decides whether the sparse path takes the run
+    const PlanSet& pu = P.plan_unmasked;
+    x.plan = pu.plan;
+    for (int t = 0; t < pu.plan.n_terms; t++) x.term[t] = pu.term_ptr[t];
+    x.summ = pu.plan.sparse_ok ? P.summ.as<AdapterSummary>() : nullptr;
+    x.tiemask = pu.plan.sparse_ok ? P.tiemask.as<uint32_t>() : nullptr;
+    x.member = P.subset ? P.member_perm.as<uint32_t>() : nullptr;
+    x.cand_mask = run.cand_mask;
+    if (P.subset && (run.cand_mask || dense || e->force_generic || !pick_sparse_applies(x))) {
+      via_rows[i] = true;
+      x.member = nullptr;
+      x.cand_mask = nullptr;  // the rows in sc.s_subset (reserved below, before the first launch)
+    }
+    if (run.cand_mask || via_rows[i]) {
+      const PlanSet& pm = P.plan_masked;
+      x.plan = pm.plan;
+      for (int t = 0; t < kMaxSteps; t++) x.term[t] = t < pm.plan.n_terms ? pm.term_ptr[t] : nullptr;
+      x.summ = nullptr;
+      x.tiemask = nullptr;
+    }
   }
-  a.cls_lo = e->cls_lo.as<uint32_t>();
-  a.cls_hi = e->cls_hi.as<uint32_t>();
-  a.summ = ps.plan.sparse_ok ? e->summ.as<AdapterSummary>() : nullptr;
-  a.tiemask = ps.plan.sparse_ok ? e->tiemask.as<uint32_t>() : nullptr;
-  a.prefix_lut2d = e->have_lut2d ? e->prefix_lut2d.as<double>() : nullptr;
-  a.A = e->A;
-  a.adapter_id = b.adapter_id;
-  a.cand_mask = b.cand_mask;
-  a.mask_words = (e->M + 31) / 32;
-  a.dense = reinterpret_cast<const float4*>(b.dense_feat);
-  a.dense_total = b.dense_total;
-  a.pick = b.pick;
-  a.pick_score = b.pick_score;
-  a.tie_count = b.tie_count;
-  a.match_out = b.match_blocks;
-  a.total_out = b.total_blocks;
-  a.scores_out = b.scores_out;
-  a.topk = b.topk;
-  a.topk_m = b.topk_m;
-  a.topk_score = b.topk_score;
-  if (dense && e->cfg.pick_mode != EPPSCORE_PICK_MAX_SCORE)
-    return fail(e, EPPSCORE_ERR_INVALID, "the stochastic pickers are not available on dense feature rows");
-  if (cfg_has(e->cfg, EPPSCORE_SCORER_LATENCY)) {
-    if (dense) return fail(e, EPPSCORE_ERR_INVALID, "the latency scorer is not available on dense feature rows");
-    if (!e->lat_args.enabled) return fail(e, EPPSCORE_ERR_INVALID, "latency scorer configured but the snapshot was prepared without latency params");
-    a.lat = e->lat_args;
-    a.lat.input_tokens = b.input_tokens;
-    if (!b.input_tokens && b.prompt_bytes && b.prompt_off) {  // count the fields of the prompt bytes on the device
-      CK(e, sc.s_fields.reserve((size_t)b.R * 4));
-      e->launches += launch_count_fields(b.prompt_bytes, b.prompt_off, b.prompt_len, b.R, sc.s_fields.as<int32_t>(), s, e->sm_count);
-      a.lat.input_tokens = sc.s_fields.as<int32_t>();
+  const size_t rows_bytes = (size_t)b.R * ((e->M + 31) / 32) * 4;
+  for (int i = 0; i < b.n_runs; i++)
+    if (via_rows[i] || e->prof[b.run[i].profile].subset) {  // (a sparse run on a subset may defer requests to member rows)
+      CK(e, sc.s_subset.reserve(rows_bytes));
+      break;
     }
-    a.lat.ttft_slo = b.ttft_slo;
-    a.lat.tpot_slo = b.tpot_slo;
-    a.lat.pred_out = b.pred_out;
-    a.n_filters = e->cfg.n_filters;
-    for (int f = 0; f < e->cfg.n_filters; f++) {
-      a.filter_kind[f] = e->cfg.filter_kind[f];
-      for (int q = 0; q < 3; q++) a.filter_param[f][q] = e->cfg.filter_param[f][q];
-    }
-    a.filter_mask_out = b.filter_mask_out;
+  for (int i = 0; i < b.n_runs; i++)
+    if (via_rows[i]) a[i].cand_mask = sc.s_subset.as<uint32_t>();
+  if (any_lat && !b.input_tokens && b.prompt_bytes && b.prompt_off) {  // count the fields of the prompt bytes on the device
+    CK(e, sc.s_fields.reserve((size_t)b.R * 4));
+    e->launches += launch_count_fields(b.prompt_bytes, b.prompt_off, b.prompt_len, b.R, sc.s_fields.as<int32_t>(), s, e->sm_count);
+    for (int i = 0; i < b.n_runs; i++)
+      if (a[i].lat.enabled) a[i].lat.input_tokens = sc.s_fields.as<int32_t>();
   }
 
-  if (!dense) {
-    const bool want_prefix = cfg_has(e->cfg, EPPSCORE_SCORER_PREFIX) || cfg_has(e->cfg, EPPSCORE_SCORER_LATENCY) ||
-                             b.match_blocks || b.total_blocks || b.hashes_out;
-    if (want_prefix && (b.hashes_in || b.prompt_bytes)) {
-      if (b.hashes_in) {
-        if (!b.n_hashes_in || b.hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "hashes_in needs n_hashes_in and hash_stride");
-        a.hashes = b.hashes_in;
-        a.n_hashes = b.n_hashes_in;
-        a.hash_stride = b.hash_stride;
-      } else {
-        const int32_t bc = b.block_chars > 0 ? b.block_chars : e->cfg.block_chars;
-        const int32_t mb = b.max_blocks > 0 ? b.max_blocks : e->cfg.max_blocks;
-        if (mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
-        if (!b.prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
-        uint64_t* hashes = b.hashes_out;
-        if (!hashes) {
-          CK(e, sc.s_hashes.reserve((size_t)b.R * mb * 8));
-          hashes = sc.s_hashes.as<uint64_t>();
-        }
-        CK(e, sc.s_nh.reserve((size_t)b.R * 2));
-        HashArgs h{};
-        h.R = b.R;
-        h.bytes = b.prompt_bytes;
-        h.off = b.prompt_off;
-        h.len = b.prompt_len;
-        h.seed = b.model_seed;
-        h.block_chars = bc;
-        h.max_blocks = mb;
-        h.hashes = hashes;
-        h.stride = mb;
-        h.n_hashes = sc.s_nh.as<uint16_t>();
-        h.stage_mask = e->hash_stage_mask;
-        h.pdl = e->use_pdl ? 1 : 0;
-        // the sparse pick kernel follows and would probe the index: the hash kernel probes it instead while it holds the
-        // hashes, and leaves the rows it resolved out of the hash buffer.  Not when the caller wants every row (hashes_out,
-        // the closed loop's commit input): then no write is saved, and on H100 the schedule call measured slower that way.
-        if (!e->force_generic && !b.hashes_out && hash_probe_applies(h) && pick_sparse_probes(a)) {
-          CK(e, sc.s_probe.reserve((size_t)b.R * sizeof(ProbeRec)));
-          h.table = e->index->view();
-          h.probe = sc.s_probe.as<ProbeRec>();
-          h.resolved = e->probe_resolved.as<unsigned long long>();
-          a.probe = h.probe;
-        }
-        e->launches += launch_hash_prompts(h, s, e->sm_count);
-        hashed_here = true;
-        a.hashes = hashes;
-        a.n_hashes = h.n_hashes;
-        a.hash_stride = mb;
+  bool hashed_here = false;
+  const uint64_t* hashes = nullptr;
+  const uint16_t* n_hashes = nullptr;
+  int32_t hash_stride = 0;
+  const ProbeRec* probe = nullptr;
+  const TableView* table = nullptr;
+  if (!dense && want_prefix && (b.hashes_in || b.prompt_bytes)) {
+    if (b.hashes_in) {
+      if (!b.n_hashes_in || b.hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "hashes_in needs n_hashes_in and hash_stride");
+      hashes = b.hashes_in;
+      n_hashes = b.n_hashes_in;
+      hash_stride = b.hash_stride;
+    } else {
+      const int32_t bc = b.block_chars > 0 ? b.block_chars : e->cfg.block_chars;
+      const int32_t mb = b.max_blocks > 0 ? b.max_blocks : e->cfg.max_blocks;
+      if (mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
+      if (!b.prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
+      uint64_t* hout = b.hashes_out;
+      if (!hout) {
+        CK(e, sc.s_hashes.reserve((size_t)b.R * mb * 8));
+        hout = sc.s_hashes.as<uint64_t>();
       }
-      a.table = e->index->view();
+      CK(e, sc.s_nh.reserve((size_t)b.R * 2));
+      HashArgs h{};
+      h.R = b.R;
+      h.bytes = b.prompt_bytes;
+      h.off = b.prompt_off;
+      h.len = b.prompt_len;
+      h.seed = b.model_seed;
+      h.block_chars = bc;
+      h.max_blocks = mb;
+      h.hashes = hout;
+      h.stride = mb;
+      h.n_hashes = sc.s_nh.as<uint16_t>();
+      h.stage_mask = e->hash_stage_mask;
+      h.pdl = e->use_pdl ? 1 : 0;
+      // the sparse pick kernel follows and would probe the index: the hash kernel probes it instead while it holds the
+      // hashes, and leaves the rows it resolved out of the hash buffer.  Not when the caller wants every row (hashes_out,
+      // the closed loop's commit input): then no write is saved, and on H100 the schedule call measured slower that way.
+      // With several runs, every run that reads the hashes must be one that takes the records.
+      bool probe_ok = !e->force_generic && !b.hashes_out && hash_probe_applies(h), probes = false;
+      for (int i = 0; i < b.n_runs && probe_ok; i++) {
+        const Plan& pl = a[i].plan;
+        bool reads = a[i].match_out || a[i].total_out;
+        for (int t = 0; t < pl.n_steps; t++) reads = reads || pl.kind[t] == STEP_PREFIX || pl.kind[t] == STEP_LATENCY;
+        const bool takes = pick_sparse_probes(a[i]);
+        if (reads && !takes) probe_ok = false;
+        probes = probes || takes;
+      }
+      if (probe_ok && probes) {
+        CK(e, sc.s_probe.reserve((size_t)b.R * sizeof(ProbeRec)));
+        h.table = e->index->view();
+        h.probe = sc.s_probe.as<ProbeRec>();
+        h.resolved = e->probe_resolved.as<unsigned long long>();
+        probe = h.probe;
+      }
+      e->launches += launch_hash_prompts(h, s, e->sm_count);
+      hashed_here = true;
+      hashes = hout;
+      n_hashes = h.n_hashes;
+      hash_stride = mb;
     }
+    table = e->index->view();
   }
   if (wait_snapshot) CK(e, cudaStreamWaitEvent(s, e->ev_snapshot, 0));
-  // programmatic dependent launch when the previous kernel of the stream is this batch's hash kernel (the snapshot event,
-  // when there is one, stays a full dependency of the pick kernel)
-  a.pdl = (e->use_pdl && hashed_here) ? 1 : 0;
-  // dispatch: specialised fast paths first, the fully general kernels otherwise
-  int launched = 0;
-  if (!e->force_generic) launched = dense ? launch_score_dense_fast(a, s, e->sm_count) : launch_pick_sparse(a, s, e->sm_count);
-  if (launched == 0) launched = launch_score_pick(a, dense, s, e->sm_count);
-  if (launched < 0) {
-    cudaGetLastError();  // (a failed launch is not sticky: clear it so the next call does not report it again)
-    return cuda_fail(e, (cudaError_t)-launched, "scoring kernel launch");
+  for (int i = 0; i < b.n_runs; i++) {
+    ScoreArgs& x = a[i];
+    const Profile& P = e->prof[b.run[i].profile];
+    x.hashes = hashes;
+    x.n_hashes = n_hashes;
+    x.hash_stride = hash_stride;
+    x.table = table;
+    x.probe = pick_sparse_probes(x) ? probe : nullptr;
+    if (via_rows[i]) {
+      e->launches += launch_subset_mask(P.member_nat.as<uint32_t>(), b.run[i].cand_mask, b.R, x.mask_words, nullptr,
+                                        sc.s_subset.as<uint32_t>(), s, e->sm_count);
+      CK(e, cudaGetLastError());
+    }
+    // programmatic dependent launch when the previous kernel of the stream is this batch's hash kernel (the snapshot event,
+    // when there is one, stays a full dependency of the pick kernel)
+    x.pdl = (e->use_pdl && hashed_here && i == 0 && !via_rows[i]) ? 1 : 0;
+    // dispatch: specialised fast paths first, the fully general kernels otherwise
+    int launched = 0;
+    if (!e->force_generic) launched = dense ? launch_score_dense_fast(x, s, e->sm_count) : launch_pick_sparse(x, s, e->sm_count);
+    const bool sparse = launched > 0 && !dense;
+    if (launched == 0) launched = launch_score_pick(x, dense, s, e->sm_count);
+    if (launched > 0 && sparse && x.member && x.table && x.hashes) {
+      // the requests the sparse kernel deferred: the masked full-matrix kernel on their member rows
+      e->launches += launch_subset_mask(P.member_nat.as<uint32_t>(), nullptr, b.R, x.mask_words, x.pick, sc.s_subset.as<uint32_t>(),
+                                        s, e->sm_count);
+      ScoreArgs d = x;
+      const PlanSet& pm = P.plan_masked;
+      d.plan = pm.plan;
+      for (int t = 0; t < kMaxSteps; t++) d.term[t] = t < pm.plan.n_terms ? pm.term_ptr[t] : nullptr;
+      d.summ = nullptr;
+      d.tiemask = nullptr;
+      d.member = nullptr;
+      d.probe = nullptr;
+      d.cand_mask = sc.s_subset.as<uint32_t>();
+      d.only_deferred = 1;
+      d.pdl = 0;
+      const int deferred = launch_score_matrix(d, s, e->sm_count);
+      launched = deferred < 0 ? deferred : launched + deferred;
+    }
+    if (launched < 0) {
+      cudaGetLastError();  // (a failed launch is not sticky: clear it so the next call does not report it again)
+      return cuda_fail(e, (cudaError_t)-launched, "scoring kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
   }
-  e->launches += launched;
-  CK(e, cudaGetLastError());
   return EPPSCORE_OK;
 }
 
@@ -535,21 +648,25 @@ DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t
   q.hashes_in = off(d.hashes_in, (size_t)d.hash_stride);
   q.n_hashes_in = off(d.n_hashes_in, 1);
   q.adapter_id = off(d.adapter_id, 1);
-  q.cand_mask = off(d.cand_mask, mw);
   q.dense_feat = off(d.dense_feat, M * 4);
   q.dense_total = off(d.dense_total, 1);
   q.input_tokens = off(d.input_tokens, 1);
   q.ttft_slo = off(d.ttft_slo, 1);
   q.tpot_slo = off(d.tpot_slo, 1);
-  q.pred_out = off(d.pred_out, M * 2);
-  q.filter_mask_out = off(d.filter_mask_out, mw);
-  q.pick = off(d.pick, 1);
-  q.pick_score = off(d.pick_score, 1);
-  q.tie_count = off(d.tie_count, 1);
+  for (int i = 0; i < d.n_runs; i++) {
+    const DevRun& x = d.run[i];
+    DevRun& y = q.run[i];
+    y.cand_mask = off(x.cand_mask, mw);
+    y.pred_out = off(x.pred_out, M * 2);
+    y.filter_mask_out = off(x.filter_mask_out, mw);
+    y.pick = off(x.pick, 1);
+    y.pick_score = off(x.pick_score, 1);
+    y.tie_count = off(x.tie_count, 1);
+    y.scores_out = off(x.scores_out, M);
+  }
   q.match_blocks = off(d.match_blocks, M);
   q.total_blocks = off(d.total_blocks, 1);
   q.hashes_out = off(d.hashes_out, mb);
-  q.scores_out = off(d.scores_out, M);
   q.topk_m = off(d.topk_m, k);
   q.topk_score = off(d.topk_score, k);
   return q;
@@ -566,16 +683,17 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStre
   if (d.R <= 0) return EPPSCORE_OK;
   const size_t M = (size_t)e->M, mw = (M + 31) / 32;
   const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
+  const Profile& P = e->prof[d.run[0].profile];
   auto select = [&](const DevBatch& q, const double* scores) -> int32_t {
     TopKSelectArgs t{};
     t.scores = scores;
     t.R = q.R;
     t.M = e->M;
     t.k = k;
-    t.pick_mode = e->cfg.pick_mode;
-    t.tie_mode = e->cfg.tie_mode;
-    t.seed_lo = (uint32_t)e->cfg.tie_seed;
-    t.seed_hi = (uint32_t)(e->cfg.tie_seed >> 32);
+    t.pick_mode = P.cfg.pick_mode;
+    t.tie_mode = P.cfg.tie_mode;
+    t.seed_lo = (uint32_t)P.cfg.tie_seed;
+    t.seed_hi = (uint32_t)(P.cfg.tie_seed >> 32);
     t.request_base = q.request_base;
     t.out_m = q.topk_m;
     t.out_s = q.topk_score;
@@ -589,11 +707,11 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStre
     return EPPSCORE_OK;
   };
   int32_t rc;
-  if (d.scores_out) {
+  if (d.run[0].scores_out) {
     DevBatch q = d;
     q.topk = 0;
     if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
-    return select(d, d.scores_out);
+    return select(d, d.run[0].scores_out);
   }
   DevBuf& buf = e->wide_scores[slot];
   if (!buf.p) {
@@ -609,13 +727,14 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStre
     CK(e, sc.s_hashes.reserve((size_t)e->wide_rows * mb * 8));
     CK(e, sc.s_nh.reserve((size_t)e->wide_rows * 2));
   }
-  if (d.prompt_bytes && !d.input_tokens && cfg_has(e->cfg, EPPSCORE_SCORER_LATENCY)) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
+  if (d.prompt_bytes && !d.input_tokens && cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY)) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
+  if (P.subset) CK(e, sc.s_subset.reserve((size_t)e->wide_rows * mw * 4));
   for (int32_t base = 0; base < d.R; base += e->wide_rows) {
     DevBatch q = slice_rows(d, base, std::min(e->wide_rows, d.R - base), M, mw, (size_t)mb, (size_t)k);
     q.topk = 0;
-    q.scores_out = buf.as<double>();
+    q.run[0].scores_out = buf.as<double>();
     if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
-    if ((rc = select(q, q.scores_out)) != EPPSCORE_OK) return rc;
+    if ((rc = select(q, q.run[0].scores_out)) != EPPSCORE_OK) return rc;
   }
   return EPPSCORE_OK;
 }
@@ -692,6 +811,117 @@ void run_init_desc(eppscore_engine* e) {
   d.won = e->c_rwon.as<uint8_t>();
 }
 
+// The per-profile fields of a config (eppscore_create, eppscore_add_profile): nullptr when they are valid, else the reason.
+const char* profile_error(const eppscore_config& c) {
+  if (c.n_scorers < 0 || c.n_scorers > EPPSCORE_MAX_SCORERS) return "n_scorers out of range";
+  int nlat = 0;
+  for (int i = 0; i < c.n_scorers; i++) {
+    const int k = c.scorer_kind[i];
+    const bool ok = (k >= 0 && k <= 6) || (k >= 8 && k < 12) || (k >= 16 && k < 18);
+    if (!ok) return "unknown scorer kind";
+    nlat += k == EPPSCORE_SCORER_LATENCY;
+  }
+  if (nlat > 1) return "at most one latency scorer per profile";
+  if (c.pick_mode < 0 || c.pick_mode > EPPSCORE_PICK_RANDOM) return "unknown pick_mode";
+  if (c.n_filters < 0 || c.n_filters > EPPSCORE_MAX_FILTERS) return "n_filters out of range";
+  if (c.n_filters > 0) {
+    if (!cfg_has(c, EPPSCORE_SCORER_LATENCY)) return "device-side filters need the latency scorer in the profile";
+    if (cfg_has(c, EPPSCORE_SCORER_QUEUE) || cfg_has(c, EPPSCORE_SCORER_RUNNING))
+      return "device-side filters cannot be combined with the queue / running scorers";
+    for (int f = 0; f < c.n_filters; f++) {
+      const int k = c.filter_kind[f];
+      const double* par = c.filter_param[f];
+      if (k == EPPSCORE_FILTER_PREFIX_AFFINITY) {  // prefixcacheaffinity/plugin.go:80-91
+        if (par[0] > 1.0 || par[1] < 0 || par[1] > 1.0 || par[2] < 0) return "prefix-cache-affinity-filter: invalid parameters";
+      } else if (k == EPPSCORE_FILTER_SLO_HEADROOM_TIER) {  // sloheadroomtier/plugin.go:66-68
+        if (par[0] < 0 || par[0] > 1.0) return "slo-headroom-tier-filter: epsilonExploreNeg must be in [0, 1]";
+      } else {
+        return "unknown filter kind";
+      }
+    }
+  }
+  return nullptr;
+}
+
+// Sizes profile p's buffers (and the engine's latency buffers when it is the first latency profile), builds its plans and its
+// prefix term table, synchronously on the engine stream.  `ef` receives the error (nullptr inside eppscore_create).
+int32_t profile_init(eppscore_engine* e, eppscore_engine* ef, int32_t p) {
+  Profile& P = e->prof[p];
+  const size_t mp = (size_t)e->geo.Mpad;
+  for (int which = 0; which < 2; which++)  // value buckets for the masked min/max of the queue / running scorers
+    if (cfg_has(P.cfg, which == 0 ? EPPSCORE_SCORER_QUEUE : EPPSCORE_SCORER_RUNNING)) {
+      CK(ef, P.qhdr[which].reserve(sizeof(QBucketHdr)));
+      CK(ef, P.qbucket[which].reserve((size_t)kQBuckets * (mp / 32) * 4));
+      CK(ef, cudaMemsetAsync(P.qhdr[which].p, 0, sizeof(QBucketHdr), e->stream));
+    }
+  if (cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY) && !e->lat_ep.p) {
+    CK(ef, e->raw_min_tpot.reserve(mp * 8));
+    CK(ef, e->raw_dispatched.reserve(mp * 4));
+    CK(ef, e->raw_prefill.reserve(mp));
+    CK(ef, e->lat_ep.reserve(mp * 8 * kLatArrays));
+  }
+  for (int i = 0; i < kMaxSteps; i++) CK(ef, P.term[i].reserve(mp * 8));
+  CK(ef, P.fold_unmasked.reserve(mp * 8));
+  CK(ef, P.fold_masked.reserve(mp * 8));
+  CK(ef, P.summ.reserve((size_t)(e->A_cap + 1) * sizeof(AdapterSummary)));
+  CK(ef, P.tiemask.reserve((size_t)(e->A_cap + 1) * e->geo.row_words * 4));
+  for (DevBuf* b : {&P.member_nat, &P.next_nat}) CK(ef, b->reserve(mp / 32 * 4));
+  for (DevBuf* b : {&P.member_perm, &P.next_perm}) CK(ef, b->reserve((size_t)e->geo.row_words * 4));
+  build_plan(P, false, &P.plan_unmasked);
+  build_plan(P, true, &P.plan_masked);
+  // prefix term table for the sparse path: lut2d[total][c] = clamp(c/total) * w  (prefix/plugin.go:108-110,
+  // scheduler_profile.go:168) — one IEEE divide and one multiply per entry, computed here on the host (no contraction:
+  // this file is compiled with -ffp-contract=off)
+  for (int sidx = 0; sidx < P.plan_unmasked.plan.n_steps; sidx++) {
+    if (P.plan_unmasked.plan.kind[sidx] != STEP_PREFIX) continue;
+    const double w = P.plan_unmasked.plan.weight[sidx];
+    std::vector<double> lut((size_t)(kLutMax + 1) * (kLutMax + 1), 0.0);
+    for (int total = 0; total <= kLutMax; total++)
+      for (int c = 0; c <= kLutMax; c++) {
+        volatile double sc = 0.0;
+        if (total != 0) sc = (double)c / (double)total;
+        volatile double cl = clamp01_host(sc);
+        lut[(size_t)total * (kLutMax + 1) + c] = cl * w;
+      }
+    CK(ef, P.prefix_lut2d.reserve(lut.size() * 8));
+    CK(ef, cudaMemcpy(P.prefix_lut2d.p, lut.data(), lut.size() * 8, cudaMemcpyHostToDevice));
+    P.have_lut2d = true;
+    break;
+  }
+  return EPPSCORE_OK;
+}
+
+// Profile p's preparation arguments: the snapshot's shared part (e->base_pa) and the profile's own scorers, buffers and subset.
+void profile_pa(eppscore_engine* e, int32_t p) {
+  Profile& P = e->prof[p];
+  PrepareArgs pa = e->base_pa;
+  const eppscore_config& c = P.cfg;
+  pa.n_scorers = c.n_scorers;
+  for (int i = 0; i < c.n_scorers; i++) {
+    pa.kind[i] = c.scorer_kind[i];
+    pa.weight[i] = c.scorer_weight[i];
+    pa.term[i] = is_endpoint_term_kind(pa.kind[i], false) ? P.term[i].as<double>() : nullptr;
+  }
+  for (int which = 0; which < 2; which++) {
+    pa.qhdr[which] = P.qhdr[which].as<QBucketHdr>();
+    pa.qbucket[which] = P.qbucket[which].as<uint32_t>();
+  }
+  if (!cfg_has(c, EPPSCORE_SCORER_LATENCY)) pa.lat_ep = nullptr;  // (the latency profiles write the engine's arrays)
+  int lead_u = 0, lead_m = 0;
+  while (lead_u < c.n_scorers && is_endpoint_term_kind(c.scorer_kind[lead_u], false)) lead_u++;
+  while (lead_m < c.n_scorers && is_endpoint_term_kind(c.scorer_kind[lead_m], true)) lead_m++;
+  pa.fold_unmasked = lead_u ? P.fold_unmasked.as<double>() : nullptr;
+  pa.fold_unmasked_n = lead_u;
+  pa.fold_masked = lead_m ? P.fold_masked.as<double>() : nullptr;
+  pa.fold_masked_n = lead_m;
+  pa.plan_u = P.plan_unmasked.plan;
+  for (int t = 0; t < kMaxSteps; t++) pa.plan_term[t] = P.plan_unmasked.term_ptr[t];
+  pa.summ = P.plan_unmasked.plan.sparse_ok ? P.summ.as<AdapterSummary>() : nullptr;
+  pa.tiemask = P.tiemask.as<uint32_t>();
+  pa.member = P.subset ? P.member_nat.as<uint32_t>() : nullptr;
+  P.pa = pa;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -748,35 +978,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   *out = nullptr;
   if (!cfg || cfg->struct_size != sizeof(eppscore_config))
     return fail(nullptr, EPPSCORE_ERR_INVALID, "config NULL or struct_size mismatch");
-  if (cfg->n_scorers < 0 || cfg->n_scorers > EPPSCORE_MAX_SCORERS) return fail(nullptr, EPPSCORE_ERR_INVALID, "n_scorers out of range");
-  for (int i = 0; i < cfg->n_scorers; i++) {
-    const int k = cfg->scorer_kind[i];
-    const bool ok = (k >= 0 && k <= 6) || (k >= 8 && k < 12) || (k >= 16 && k < 18);
-    if (!ok) return fail(nullptr, EPPSCORE_ERR_INVALID, "unknown scorer kind");
-  }
-  {
-    int nlat = 0;
-    for (int i = 0; i < cfg->n_scorers; i++) nlat += cfg->scorer_kind[i] == EPPSCORE_SCORER_LATENCY;
-    if (nlat > 1) return fail(nullptr, EPPSCORE_ERR_INVALID, "at most one latency scorer per profile");
-  }
-  if (cfg->pick_mode < 0 || cfg->pick_mode > EPPSCORE_PICK_RANDOM) return fail(nullptr, EPPSCORE_ERR_INVALID, "unknown pick_mode");
-  if (cfg->n_filters < 0 || cfg->n_filters > EPPSCORE_MAX_FILTERS) return fail(nullptr, EPPSCORE_ERR_INVALID, "n_filters out of range");
-  if (cfg->n_filters > 0) {
-    if (!cfg_has(*cfg, EPPSCORE_SCORER_LATENCY)) return fail(nullptr, EPPSCORE_ERR_INVALID, "device-side filters need the latency scorer in the profile");
-    if (cfg_has(*cfg, EPPSCORE_SCORER_QUEUE) || cfg_has(*cfg, EPPSCORE_SCORER_RUNNING))
-      return fail(nullptr, EPPSCORE_ERR_INVALID, "device-side filters cannot be combined with the queue / running scorers");
-    for (int f = 0; f < cfg->n_filters; f++) {
-      const int k = cfg->filter_kind[f];
-      const double* par = cfg->filter_param[f];
-      if (k == EPPSCORE_FILTER_PREFIX_AFFINITY) {  // prefixcacheaffinity/plugin.go:80-91
-        if (par[0] > 1.0 || par[1] < 0 || par[1] > 1.0 || par[2] < 0) return fail(nullptr, EPPSCORE_ERR_INVALID, "prefix-cache-affinity-filter: invalid parameters");
-      } else if (k == EPPSCORE_FILTER_SLO_HEADROOM_TIER) {  // sloheadroomtier/plugin.go:66-68
-        if (par[0] < 0 || par[0] > 1.0) return fail(nullptr, EPPSCORE_ERR_INVALID, "slo-headroom-tier-filter: epsilonExploreNeg must be in [0, 1]");
-      } else {
-        return fail(nullptr, EPPSCORE_ERR_INVALID, "unknown filter kind");
-      }
-    }
-  }
+  if (const char* why = profile_error(*cfg)) return fail(nullptr, EPPSCORE_ERR_INVALID, why);
   if (cfg->max_endpoints < 1 || cfg->max_endpoints > 8192)
     return fail(nullptr, EPPSCORE_ERR_CAPACITY, "max_endpoints must be in [1, 8192]");
   if (cfg->max_blocks < 0 || cfg->max_blocks > EPPSCORE_MAX_BLOCKS) return fail(nullptr, EPPSCORE_ERR_CAPACITY, "max_blocks out of range");
@@ -868,46 +1070,11 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
     CK(nullptr, cudaMemcpyAsync(ep->run_desc.p, &ep->run_host, sizeof(RunDev), cudaMemcpyHostToDevice, ep->stream));
     CK(nullptr, init_running_kernels());
   }
-  for (int which = 0; which < 2; which++)  // value buckets for the masked min/max of the queue / running scorers
-    if (cfg_has(ep->cfg, which == 0 ? EPPSCORE_SCORER_QUEUE : EPPSCORE_SCORER_RUNNING)) {
-      CK(nullptr, ep->qhdr[which].reserve(sizeof(QBucketHdr)));
-      CK(nullptr, ep->qbucket[which].reserve((size_t)kQBuckets * (mp / 32) * 4));
-      CK(nullptr, cudaMemsetAsync(ep->qhdr[which].p, 0, sizeof(QBucketHdr), ep->stream));
-    }
-  if (cfg_has(ep->cfg, EPPSCORE_SCORER_LATENCY)) {
-    CK(nullptr, ep->raw_min_tpot.reserve(mp * 8));
-    CK(nullptr, ep->raw_dispatched.reserve(mp * 4));
-    CK(nullptr, ep->raw_prefill.reserve(mp));
-    CK(nullptr, ep->lat_ep.reserve(mp * 8 * kLatArrays));
-  }
-  for (int i = 0; i < kMaxSteps; i++) CK(nullptr, ep->term[i].reserve(mp * 8));
-  CK(nullptr, ep->fold_unmasked.reserve(mp * 8));
-  CK(nullptr, ep->fold_masked.reserve(mp * 8));
   CK(nullptr, ep->cls_lo.reserve((size_t)(ep->A_cap + 1) * ep->geo.row_words * 4));
   CK(nullptr, ep->cls_hi.reserve((size_t)(ep->A_cap + 1) * ep->geo.row_words * 4));
-  CK(nullptr, ep->summ.reserve((size_t)(ep->A_cap + 1) * sizeof(AdapterSummary)));
-  CK(nullptr, ep->tiemask.reserve((size_t)(ep->A_cap + 1) * ep->geo.row_words * 4));
-  build_plan(ep, false, &ep->plan_unmasked);
-  build_plan(ep, true, &ep->plan_masked);
-  // engine-wide prefix term table for the sparse path: lut2d[total][c] = clamp(c/total) * w  (prefix/plugin.go:108-110,
-  // scheduler_profile.go:168) — one IEEE divide and one multiply per entry, computed here on the host (no contraction:
-  // this file is compiled with -ffp-contract=off)
-  for (int sidx = 0; sidx < ep->plan_unmasked.plan.n_steps; sidx++) {
-    if (ep->plan_unmasked.plan.kind[sidx] != STEP_PREFIX) continue;
-    const double w = ep->plan_unmasked.plan.weight[sidx];
-    std::vector<double> lut((size_t)(kLutMax + 1) * (kLutMax + 1), 0.0);
-    for (int total = 0; total <= kLutMax; total++)
-      for (int c = 0; c <= kLutMax; c++) {
-        volatile double sc = 0.0;
-        if (total != 0) sc = (double)c / (double)total;
-        volatile double cl = clamp01_host(sc);
-        lut[(size_t)total * (kLutMax + 1) + c] = cl * w;
-      }
-    CK(nullptr, ep->prefix_lut2d.reserve(lut.size() * 8));
-    CK(nullptr, cudaMemcpy(ep->prefix_lut2d.p, lut.data(), lut.size() * 8, cudaMemcpyHostToDevice));
-    ep->have_lut2d = true;
-    break;
-  }
+  ep->prof[0].cfg = ep->cfg;
+  ep->n_prof = 1;
+  if (int32_t rc = profile_init(ep, nullptr, 0)) return rc;
   // prefix index (device-resident: slot table + per-endpoint LRUs; the LRU regions are allocated by the first Add)
   CK(nullptr, make(ep->ev_caller));
   ep->index = std::make_unique<DeviceIndex>(ep->geo.Mpad, ep->geo.Mpad / 32, ep->cfg.prefix_capacity, ep->cfg.lru_capacity_default,
@@ -1033,12 +1200,6 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   PrepareArgs pa{};
   pa.geo = e->geo;
   pa.geo.M = s->M;
-  pa.n_scorers = e->cfg.n_scorers;
-  for (int i = 0; i < e->cfg.n_scorers; i++) {
-    pa.kind[i] = e->cfg.scorer_kind[i];
-    pa.weight[i] = e->cfg.scorer_weight[i];
-    pa.term[i] = is_endpoint_term_kind(pa.kind[i], false) ? e->term[i].as<double>() : nullptr;
-  }
   pa.kv = on_device ? s->kv_usage : e->raw_kv.as<double>();
   pa.queue = e->cur_queue;
   pa.running = e->cur_running;
@@ -1048,10 +1209,6 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   pa.maxm = s->lora_max ? (on_device ? s->lora_max : e->raw_max.as<int32_t>()) : nullptr;
   for (int i = 0; i < 4; i++)
     pa.col[i] = s->endpoint_col[i] ? (on_device ? s->endpoint_col[i] : e->raw_col[i].as<double>()) : nullptr;
-  for (int which = 0; which < 2; which++) {
-    pa.qhdr[which] = e->qhdr[which].as<QBucketHdr>();
-    pa.qbucket[which] = e->qbucket[which].as<uint32_t>();
-  }
   // InFlightLoad.Tokens: the snapshot's array when it carries one, else the in-flight counters (all 0 until the first
   // eppscore_inflight_add, which scores exactly like an absent attribute, token_load.go:91-98)
   pa.tokens = s->inflight_tokens ? (on_device ? s->inflight_tokens : e->raw_tokens.as<int64_t>()) : e->inflight_tok.as<int64_t>();
@@ -1115,24 +1272,23 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
   }
   pa.lora_words = e->lora_words;
   pa.A = e->A;
-  int lead_u = 0, lead_m = 0;
-  while (lead_u < e->cfg.n_scorers && is_endpoint_term_kind(e->cfg.scorer_kind[lead_u], false)) lead_u++;
-  while (lead_m < e->cfg.n_scorers && is_endpoint_term_kind(e->cfg.scorer_kind[lead_m], true)) lead_m++;
-  pa.fold_unmasked = lead_u ? e->fold_unmasked.as<double>() : nullptr;
-  pa.fold_unmasked_n = lead_u;
-  pa.fold_masked = lead_m ? e->fold_masked.as<double>() : nullptr;
-  pa.fold_masked_n = lead_m;
   pa.cls_lo = e->cls_lo.as<uint32_t>();
   pa.cls_hi = e->cls_hi.as<uint32_t>();
-  pa.plan_u = e->plan_unmasked.plan;
-  for (int t = 0; t < kMaxSteps; t++) pa.plan_term[t] = e->plan_unmasked.term_ptr[t];
-  pa.summ = e->plan_unmasked.plan.sparse_ok ? e->summ.as<AdapterSummary>() : nullptr;
-  pa.tiemask = e->tiemask.as<uint32_t>();
   e->snapshot_has_tokens = s->inflight_tokens != nullptr;
   e->snapshot_has_min_tpot = s->min_tpot_slo != nullptr;
   e->snapshot_has_dispatched = s->dispatched != nullptr;
-  e->last_pa = pa;
-  if ((rc = prepare_snapshot(e, st)) != EPPSCORE_OK) return rc;
+  e->base_pa = pa;
+  // every profile: its endpoint subset as set since (eppscore_set_profile_endpoints), then its terms
+  for (int p = 0; p < e->n_prof; p++) {
+    Profile& P = e->prof[p];
+    P.subset = P.next_subset;
+    if (P.subset) {
+      CK(e, cudaMemcpyAsync(P.member_nat.p, P.next_nat.p, P.next_nat.bytes, cudaMemcpyDeviceToDevice, st));
+      CK(e, cudaMemcpyAsync(P.member_perm.p, P.next_perm.p, P.next_perm.bytes, cudaMemcpyDeviceToDevice, st));
+    }
+    profile_pa(e, p);
+  }
+  if ((rc = prepare_snapshot(e, st, (1u << e->n_prof) - 1)) != EPPSCORE_OK) return rc;
   if (!capturing && !on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
   e->have_snapshot = true;
   return EPPSCORE_OK;
@@ -1142,10 +1298,10 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
 
 namespace {
 
-// eppscore_schedule_batch(_topk, _topk_wide): t == nullptr ⇒ no top-k lists; wide: any k up to max_endpoints (schedule_wide)
-int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t, bool wide = false) {
-  if (!e) return EPPSCORE_ERR_INVALID;
-  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+// eppscore_schedule_batch(_topk, _topk_wide, _profiles): the runs (profile + per-profile filter result and outputs) of one
+// batch; t == nullptr ⇒ no top-k lists (top-k: one run); wide: any k up to max_endpoints (schedule_wide)
+int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
+                       const eppscore_topk* t, bool wide = false) {
   if (t) {
     if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
     if (wide && (t->k < 1 || t->k > e->cfg.max_endpoints)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, max_endpoints]");
@@ -1163,6 +1319,8 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   d.hash_stride = b->hash_stride;
   d.block_chars = b->block_chars;
   d.max_blocks = b->max_blocks;
+  d.n_runs = n_runs;
+  for (int i = 0; i < n_runs; i++) d.run[i].profile = runs[i].profile;
   if (b->location == 1) {
     d.prompt_bytes = b->prompt_bytes;
     d.prompt_off = b->prompt_off;
@@ -1171,32 +1329,38 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     d.hashes_in = b->hashes_in;
     d.n_hashes_in = b->n_hashes_in;
     d.adapter_id = b->adapter_id;
-    d.cand_mask = b->cand_mask;
     d.dense_feat = b->dense_feat;
     d.dense_total = b->dense_total;
     d.input_tokens = b->input_tokens;
     d.ttft_slo = b->ttft_slo;
     d.tpot_slo = b->tpot_slo;
-    d.pred_out = b->pred_out;
-    d.filter_mask_out = b->filter_mask_out;
-    d.pick = b->pick;
-    d.pick_score = b->pick_score;
-    d.tie_count = b->tie_count;
     d.match_blocks = b->match_blocks;
     d.total_blocks = b->total_blocks;
     d.hashes_out = b->hashes_out;
-    d.scores_out = b->scores_out;
     d.topk = tk;
     d.topk_m = t ? t->endpoints : nullptr;
     d.topk_score = t ? t->scores : nullptr;
+    bool per_pair = false;  // R x M outputs or masks on some run
+    for (int i = 0; i < n_runs; i++) {
+      const eppscore_profile_run& x = runs[i];
+      DevRun& y = d.run[i];
+      y.cand_mask = x.cand_mask;
+      y.pick = x.pick;
+      y.pick_score = x.pick_score;
+      y.tie_count = x.tie_count;
+      y.scores_out = x.scores_out;
+      y.pred_out = x.pred_out;
+      y.filter_mask_out = x.filter_mask_out;
+      per_pair = per_pair || x.cand_mask || x.scores_out || x.pred_out || x.filter_mask_out;
+    }
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
     if (wide) {
       if ((rc = schedule_wide(e, d, tk, cs, e->sc[0], 0)) != EPPSCORE_OK) return rc;
       return pending_record(e, cs);
     }
     // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here)
-    const bool sliceable = d.prompt_bytes && !d.hashes_in && !d.cand_mask && !d.dense_feat && !d.pred_out && !d.filter_mask_out &&
-                           !d.match_blocks && !d.scores_out && !d.input_tokens && !d.ttft_slo && !d.tpot_slo;
+    const bool sliceable = d.prompt_bytes && !d.hashes_in && !per_pair && !d.dense_feat && !d.match_blocks && !d.input_tokens &&
+                           !d.ttft_slo && !d.tpot_slo;
     int K = e->dev_split;
     if (!sliceable || e->dev_streams < 2) K = 1;
     while (K > 1 && b->R / K < 2048) K--;
@@ -1223,9 +1387,11 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
       if (d.prompt_len) q.prompt_len = d.prompt_len + base;
       if (d.model_seed) q.model_seed = d.model_seed + base;
       if (d.adapter_id) q.adapter_id = d.adapter_id + base;
-      q.pick = d.pick + base;
-      q.pick_score = d.pick_score + base;
-      q.tie_count = d.tie_count + base;
+      for (int i = 0; i < n_runs; i++) {
+        q.run[i].pick = d.run[i].pick + base;
+        q.run[i].pick_score = d.run[i].pick_score + base;
+        q.run[i].tie_count = d.run[i].tie_count + base;
+      }
       if (tk) {
         q.topk_m = d.topk_m + (size_t)base * tk;
         q.topk_score = d.topk_score + (size_t)base * tk;
@@ -1255,7 +1421,8 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   const size_t M = (size_t)e->M;
   const size_t mw = (M + 31) / 32;
   const int32_t mb = b->max_blocks > 0 ? b->max_blocks : e->cfg.max_blocks;
-  const bool diag = b->match_blocks || b->scores_out || b->pred_out || b->dense_feat;  // R x M arrays: one chunk at a time is plenty
+  bool diag = b->match_blocks || b->dense_feat;  // R x M arrays: one chunk at a time is plenty
+  for (int i = 0; i < n_runs; i++) diag = diag || runs[i].scores_out || runs[i].pred_out;
   int32_t chunk = e->host_chunk > 0 ? e->host_chunk : b->R;
   if (diag || b->R < 2 * chunk) chunk = b->R;
   const int nstreams = chunk < b->R ? 2 : 1;
@@ -1263,9 +1430,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   // the chunks reuse sc[0] / sc[1], which a device-location batch may still hold
   if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
   if (nstreams == 2 && (rc = pending_wait(e, e->stream2)) != EPPSCORE_OK) return rc;
-  // pinned staging: pick i32 | score f64 | tie i32 | total u16, each [R]; top-k endpoints i32 | scores f64, each [R*k]
-  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk;
-  const size_t o_score = (RR * 4 + 7) & ~(size_t)7, o_tie = o_score + RR * 8, o_total = o_tie + RR * 4;
+  // pinned staging, per run: pick i32 | score f64 | tie i32, each [R]; then total u16 [R]; top-k endpoints i32 | scores f64,
+  // each [R*k]
+  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk, NR = (size_t)n_runs;
+  const size_t o_score = (NR * RR * 4 + 7) & ~(size_t)7, o_tie = o_score + NR * RR * 8, o_total = o_tie + NR * RR * 4;
   const size_t o_tkm = (o_total + RR * 2 + 7) & ~(size_t)7, o_tks = (o_tkm + RK * 4 + 7) & ~(size_t)7, res_bytes = o_tks + RK * 8;
   CK(e, e->h_res.reserve(res_bytes));
   unsigned char* hres = e->h_res.as<unsigned char>();
@@ -1287,6 +1455,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     d.hash_stride = b->hash_stride;
     d.block_chars = b->block_chars;
     d.max_blocks = b->max_blocks;
+    d.n_runs = n_runs;
     if (b->prompt_bytes) {  // the kernels keep using the caller's offsets
       if ((rc = stage_prompts(e, sc.s_prompts, b->prompt_bytes, b->prompt_off, b->prompt_len, r0, r1, st, &d.prompt_bytes)) != EPPSCORE_OK ||
           (rc = h2d(e, sc.s_off, b->prompt_off + r0, R + 1, &d.prompt_off, st)) != EPPSCORE_OK)
@@ -1301,19 +1470,44 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
       H2D(s_nh, n_hashes_in, 1)
     }
     H2D(s_adapter, adapter_id, 1)
-    H2D(s_mask, cand_mask, mw)
     H2D(s_dense, dense_feat, M * 4)
     H2D(s_dtotal, dense_total, 1)
     H2D(s_intok, input_tokens, 1)
     H2D(s_tslo, ttft_slo, 1)
     H2D(s_pslo, tpot_slo, 1)
 #undef H2D
-    CK(e, sc.s_pick.reserve(R * 4));
-    CK(e, sc.s_score.reserve(R * 8));
-    CK(e, sc.s_tie.reserve(R * 4));
-    d.pick = sc.s_pick.as<int32_t>();
-    d.pick_score = sc.s_score.as<double>();
-    d.tie_count = sc.s_tie.as<int32_t>();
+    // per run: slice i of each scratch array
+    size_t n_masks = 0;
+    bool any_scores = false, any_pred = false, any_fmask = false;
+    for (int i = 0; i < n_runs; i++) {
+      n_masks += runs[i].cand_mask ? 1 : 0;
+      any_scores = any_scores || runs[i].scores_out;
+      any_pred = any_pred || runs[i].pred_out;
+      any_fmask = any_fmask || runs[i].filter_mask_out;
+    }
+    if (n_masks) CK(e, sc.s_mask.reserve(NR * R * mw * 4));
+    CK(e, sc.s_pick.reserve(NR * R * 4));
+    CK(e, sc.s_score.reserve(NR * R * 8));
+    CK(e, sc.s_tie.reserve(NR * R * 4));
+    if (any_scores) CK(e, sc.s_scores.reserve(NR * R * M * 8));
+    if (any_pred) CK(e, sc.s_pred.reserve(NR * R * M * 16));
+    if (any_fmask) CK(e, sc.s_fmask.reserve(NR * R * mw * 4));
+    for (int i = 0; i < n_runs; i++) {
+      const eppscore_profile_run& x = runs[i];
+      DevRun& y = d.run[i];
+      y.profile = x.profile;
+      if (x.cand_mask) {
+        uint32_t* dm = sc.s_mask.as<uint32_t>() + (size_t)i * R * mw;
+        CK(e, cudaMemcpyAsync(dm, x.cand_mask + (size_t)r0 * mw, R * mw * 4, cudaMemcpyHostToDevice, st));
+        y.cand_mask = dm;
+      }
+      y.pick = sc.s_pick.as<int32_t>() + (size_t)i * R;
+      y.pick_score = sc.s_score.as<double>() + (size_t)i * R;
+      y.tie_count = sc.s_tie.as<int32_t>() + (size_t)i * R;
+      if (x.scores_out) y.scores_out = sc.s_scores.as<double>() + (size_t)i * R * M;
+      if (x.pred_out) y.pred_out = sc.s_pred.as<double>() + (size_t)i * R * M * 2;
+      if (x.filter_mask_out) y.filter_mask_out = sc.s_fmask.as<uint32_t>() + (size_t)i * R * mw;
+    }
     if (tk) {  // [R*k]: small, like the picks (the chunks keep overlapping)
       CK(e, sc.s_topk_m.reserve(R * tk * 4));
       CK(e, sc.s_topk_s.reserve(R * tk * 8));
@@ -1329,18 +1523,6 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
       CK(e, sc.s_total.reserve(R * 2));
       d.total_blocks = sc.s_total.as<uint16_t>();
     }
-    if (b->scores_out) {
-      CK(e, sc.s_scores.reserve(R * M * 8));
-      d.scores_out = sc.s_scores.as<double>();
-    }
-    if (b->pred_out) {
-      CK(e, sc.s_pred.reserve(R * M * 16));
-      d.pred_out = sc.s_pred.as<double>();
-    }
-    if (b->filter_mask_out) {
-      CK(e, sc.s_fmask.reserve(R * mw * 4));
-      d.filter_mask_out = sc.s_fmask.as<uint32_t>();
-    }
     uint64_t* hashes_dev = nullptr;
     if (b->hashes_out) {
       // reuse the internal hash scratch as the device-side hashes_out; entries past n_hashes[r] are zero
@@ -1351,31 +1533,55 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
     }
     rc = wide ? schedule_wide(e, d, tk, st, sc, ci & 1) : schedule_device(e, d, st, sc);
     if (rc != EPPSCORE_OK) return rc;
-    if (b->pick) CK(e, cudaMemcpyAsync(hp_pick + r0, d.pick, R * 4, cudaMemcpyDeviceToHost, st));
-    if (b->pick_score) CK(e, cudaMemcpyAsync(hp_score + r0, d.pick_score, R * 8, cudaMemcpyDeviceToHost, st));
-    if (b->tie_count) CK(e, cudaMemcpyAsync(hp_tie + r0, d.tie_count, R * 4, cudaMemcpyDeviceToHost, st));
+    for (int i = 0; i < n_runs; i++) {
+      const eppscore_profile_run& x = runs[i];
+      const DevRun& y = d.run[i];
+      if (x.pick) CK(e, cudaMemcpyAsync(hp_pick + i * RR + r0, y.pick, R * 4, cudaMemcpyDeviceToHost, st));
+      if (x.pick_score) CK(e, cudaMemcpyAsync(hp_score + i * RR + r0, y.pick_score, R * 8, cudaMemcpyDeviceToHost, st));
+      if (x.tie_count) CK(e, cudaMemcpyAsync(hp_tie + i * RR + r0, y.tie_count, R * 4, cudaMemcpyDeviceToHost, st));
+      if (x.scores_out) CK(e, cudaMemcpyAsync(x.scores_out + (size_t)r0 * M, y.scores_out, R * M * 8, cudaMemcpyDeviceToHost, st));
+      if (x.pred_out) CK(e, cudaMemcpyAsync(x.pred_out + (size_t)r0 * M * 2, y.pred_out, R * M * 16, cudaMemcpyDeviceToHost, st));
+      if (x.filter_mask_out)
+        CK(e, cudaMemcpyAsync(x.filter_mask_out + (size_t)r0 * mw, y.filter_mask_out, R * mw * 4, cudaMemcpyDeviceToHost, st));
+    }
     if (tk) {
       CK(e, cudaMemcpyAsync(hp_tkm + (size_t)r0 * tk, d.topk_m, R * tk * 4, cudaMemcpyDeviceToHost, st));
       CK(e, cudaMemcpyAsync(hp_tks + (size_t)r0 * tk, d.topk_score, R * tk * 8, cudaMemcpyDeviceToHost, st));
     }
     if (b->match_blocks) CK(e, cudaMemcpyAsync(b->match_blocks + (size_t)r0 * M, d.match_blocks, R * M * 2, cudaMemcpyDeviceToHost, st));
     if (b->total_blocks) CK(e, cudaMemcpyAsync(hp_total + r0, d.total_blocks, R * 2, cudaMemcpyDeviceToHost, st));
-    if (b->scores_out) CK(e, cudaMemcpyAsync(b->scores_out + (size_t)r0 * M, d.scores_out, R * M * 8, cudaMemcpyDeviceToHost, st));
-    if (b->pred_out) CK(e, cudaMemcpyAsync(b->pred_out + (size_t)r0 * M * 2, d.pred_out, R * M * 16, cudaMemcpyDeviceToHost, st));
-    if (b->filter_mask_out) CK(e, cudaMemcpyAsync(b->filter_mask_out + (size_t)r0 * mw, d.filter_mask_out, R * mw * 4, cudaMemcpyDeviceToHost, st));
     if (hashes_dev) CK(e, cudaMemcpyAsync(b->hashes_out + (size_t)r0 * mb, hashes_dev, R * (size_t)mb * 8, cudaMemcpyDeviceToHost, st));
   }
   CK(e, cudaStreamSynchronize(e->stream));
   if (nstreams == 2) CK(e, cudaStreamSynchronize(e->stream2));
-  if (b->pick) memcpy(b->pick, hp_pick, RR * 4);
-  if (b->pick_score) memcpy(b->pick_score, hp_score, RR * 8);
-  if (b->tie_count) memcpy(b->tie_count, hp_tie, RR * 4);
+  for (int i = 0; i < n_runs; i++) {
+    if (runs[i].pick) memcpy(runs[i].pick, hp_pick + i * RR, RR * 4);
+    if (runs[i].pick_score) memcpy(runs[i].pick_score, hp_score + i * RR, RR * 8);
+    if (runs[i].tie_count) memcpy(runs[i].tie_count, hp_tie + i * RR, RR * 4);
+  }
   if (b->total_blocks) memcpy(b->total_blocks, hp_total, RR * 2);
   if (tk) {
     memcpy(t->endpoints, hp_tkm, RK * 4);
     memcpy(t->scores, hp_tks, RK * 8);
   }
   return EPPSCORE_OK;
+}
+
+// eppscore_schedule_batch and its top-k forms: one run of profile 0 from the batch's own filter result and outputs
+int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t, bool wide = false) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  eppscore_profile_run run{};
+  run.struct_size = sizeof(run);
+  run.profile = 0;
+  run.cand_mask = b->cand_mask;
+  run.pick = b->pick;
+  run.pick_score = b->pick_score;
+  run.tie_count = b->tie_count;
+  run.scores_out = b->scores_out;
+  run.pred_out = b->pred_out;
+  run.filter_mask_out = b->filter_mask_out;
+  return schedule_batch(e, b, 1, &run, t, wide);
 }
 
 }  // namespace
@@ -1394,6 +1600,94 @@ int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_bat
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!t) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
   return schedule_batch(e, b, t, true);
+}
+
+int32_t eppscore_add_profile(eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!p || p->struct_size != sizeof(eppscore_profile) || !id_out) return fail(e, EPPSCORE_ERR_INVALID, "profile NULL, struct_size mismatch or id_out NULL");
+  if (e->n_prof >= EPPSCORE_MAX_PROFILES) return fail(e, EPPSCORE_ERR_CAPACITY, "at most EPPSCORE_MAX_PROFILES profiles");
+  CK(e, cudaSetDevice(e->device));
+  if (is_capturing(e->stream)) return fail(e, EPPSCORE_ERR_INVALID, "add_profile under CUDA-graph capture");
+  eppscore_config c = e->cfg;  // engine-wide fields stay the engine's
+  c.n_scorers = p->n_scorers;
+  memcpy(c.scorer_kind, p->scorer_kind, sizeof(c.scorer_kind));
+  memcpy(c.scorer_weight, p->scorer_weight, sizeof(c.scorer_weight));
+  c.pick_mode = p->pick_mode;
+  c.n_filters = p->n_filters;
+  memcpy(c.filter_kind, p->filter_kind, sizeof(c.filter_kind));
+  memcpy(c.filter_param, p->filter_param, sizeof(c.filter_param));
+  if (const char* why = profile_error(c)) return fail(e, EPPSCORE_ERR_INVALID, why);
+  const int32_t id = e->n_prof;
+  c.tie_seed = e->cfg.tie_seed ^ ((uint64_t)id * 0x9E3779B97F4A7C15ull);  // (include/eppscore.h: eppscore_profile)
+  Profile& P = e->prof[id];
+  P.cfg = c;
+  int32_t rc = profile_init(e, e, id);
+  if (rc != EPPSCORE_OK) {
+    P = Profile{};
+    return rc;
+  }
+  e->n_prof = id + 1;
+  if (e->have_snapshot) {  // prepared for the current snapshot at once, behind everything that reads or rewrites the terms
+    if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
+    if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
+    profile_pa(e, id);
+    if ((rc = prepare_snapshot(e, e->stream, 1u << id)) != EPPSCORE_OK) return rc;
+  }
+  CK(e, cudaStreamSynchronize(e->stream));
+  *id_out = id;
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_set_profile_endpoints(eppscore_engine* e, int32_t profile, const uint32_t* mask, int32_t words) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (profile < 0 || profile >= e->n_prof) return fail(e, EPPSCORE_ERR_INVALID, "set_profile_endpoints: unknown profile");
+  if (mask && words < 0) return fail(e, EPPSCORE_ERR_INVALID, "set_profile_endpoints: words < 0");
+  CK(e, cudaSetDevice(e->device));
+  if (is_capturing(e->stream)) return fail(e, EPPSCORE_ERR_INVALID, "set_profile_endpoints under CUDA-graph capture");
+  Profile& P = e->prof[profile];
+  if (!mask) {
+    P.next_subset = false;
+    return EPPSCORE_OK;
+  }
+  // the next rows are copied by set_snapshot on its stream: the last one (on whatever stream) has finished copying them
+  CK(e, cudaEventSynchronize(e->ev_snapshot));
+  const int32_t nw = e->geo.Mpad / 32;
+  std::vector<uint32_t> nat((size_t)nw, 0u), perm((size_t)e->geo.row_words, 0u);
+  for (int32_t w = 0; w < nw && w < words; w++) nat[(size_t)w] = mask[w];
+  const uint32_t max_ep = (uint32_t)e->cfg.max_endpoints;
+  for (uint32_t m = 0; m < (uint32_t)e->geo.Mpad; m++) {
+    const bool in = m < max_ep && ((nat[m >> 5] >> (m & 31)) & 1u);
+    if (!in) {
+      nat[m >> 5] &= ~(1u << (m & 31));
+      continue;
+    }
+    const uint32_t pos = perm_bitpos(m, e->geo.log_epl);
+    perm[pos >> 5] |= 1u << (pos & 31);
+  }
+  // the next rows are only read by the next set_snapshot (stream-ordered after this copy)
+  CK(e, cudaMemcpyAsync(P.next_nat.p, nat.data(), nat.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(e, cudaMemcpyAsync(P.next_perm.p, perm.data(), perm.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  P.next_subset = true;
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_schedule_batch_profiles(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  if (b->pick || b->pick_score || b->tie_count || b->cand_mask || b->scores_out || b->pred_out || b->filter_mask_out)
+    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_profiles: per-profile batch fields belong to the runs (must be NULL)");
+  if (n_runs < 1 || n_runs > EPPSCORE_MAX_PROFILES || !runs) return fail(e, EPPSCORE_ERR_INVALID, "n_runs outside [1, EPPSCORE_MAX_PROFILES]");
+  unsigned seen = 0;
+  for (int32_t i = 0; i < n_runs; i++) {
+    const eppscore_profile_run& x = runs[i];
+    if (x.struct_size != sizeof(eppscore_profile_run)) return fail(e, EPPSCORE_ERR_INVALID, "profile_run struct_size mismatch");
+    if (x.profile < 0 || x.profile >= e->n_prof) return fail(e, EPPSCORE_ERR_INVALID, "profile_run: unknown profile");
+    if (seen & (1u << x.profile)) return fail(e, EPPSCORE_ERR_INVALID, "profile_run: a profile appears in two runs");
+    seen |= 1u << x.profile;
+    if (!x.pick || !x.pick_score || !x.tie_count) return fail(e, EPPSCORE_ERR_INVALID, "profile_run: pick/pick_score/tie_count required");
+  }
+  return schedule_batch(e, b, n_runs, runs, nullptr);
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,
@@ -1502,69 +1796,90 @@ static int32_t index_status(eppscore_engine* e, cudaError_t c, const char* what)
   return cuda_fail(e, c, what);
 }
 
-int32_t eppscore_commit_picks(eppscore_engine* e, int32_t R, const int32_t* pick, const uint64_t* hashes,
-                              const uint16_t* n_hashes, int32_t hash_stride, const int32_t* lru_capacity) {
+// PreRequest for R requests with n_picks picks each (eppscore_commit_picks[_device|_profiles]): host arrays are staged and the
+// call returns when the commit is done; device arrays are committed asynchronously, ordered on `stream`.
+static int32_t commit_calls(eppscore_engine* e, int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes,
+                            const uint16_t* n_hashes, int32_t hash_stride, const int32_t* lru_capacity, bool on_device,
+                            int64_t touch_bound, void* stream, const char* what) {
   if (!e) return EPPSCORE_ERR_INVALID;
-  if (R < 0 || (R > 0 && (!pick || !hashes || !n_hashes))) return fail(e, EPPSCORE_ERR_INVALID, "NULL argument");
+  if (n_picks < 1 || n_picks > EPPSCORE_MAX_PROFILES || (R > 0 && !picks)) return fail(e, EPPSCORE_ERR_INVALID, "n_picks outside [1, EPPSCORE_MAX_PROFILES]");
+  bool null_pick = false;
+  for (int32_t p = 0; R > 0 && p < n_picks; p++) null_pick = null_pick || !picks[p];
+  if (R < 0 || (R > 0 && (null_pick || !hashes || !n_hashes))) return fail(e, EPPSCORE_ERR_INVALID, "NULL argument");
   if (R == 0) return EPPSCORE_OK;
   if (hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "hash_stride must be > 0");
   CK(e, cudaSetDevice(e->device));
-  int32_t lo = e->geo.Mpad, hi = -1;
-  int64_t touches = 0;
-  for (int32_t r = 0; r < R; r++) {
-    const int32_t ep = pick[r];
-    if (ep < 0) continue;  // no target endpoint: nothing to record (plugin.go:173-175)
-    if (ep >= e->geo.Mpad) return fail(e, EPPSCORE_ERR_INVALID, "pick out of range");
-    if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "n_hashes exceeds hash_stride");
-    lo = std::min(lo, ep);
-    hi = std::max(hi, ep);
-    touches += n_hashes[r];
-  }
-  if (hi < 0) return EPPSCORE_OK;  // (a pick with zero hashes still creates the endpoint's LRU, indexer.go:57-68)
   std::vector<int32_t> caps;
   int32_t rc = pad_caps(e, lru_capacity, &caps);
   if (rc != EPPSCORE_OK) return rc;
+  const int32_t* d_picks[EPPSCORE_MAX_PROFILES] = {};
+  if (on_device) {
+    cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
+    if (cs != e->stream) {  // the arrays are produced on the caller's stream
+      CK(e, cudaEventRecord(e->ev_caller, cs));
+      CK(e, cudaStreamWaitEvent(e->stream, e->ev_caller, 0));
+    }
+    if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
+    for (int32_t p = 0; p < n_picks; p++) d_picks[p] = picks[p];
+    const int32_t n_eps = e->M > 0 ? e->M : e->geo.Mpad;
+    rc = index_status(e, e->index->commit(R, n_picks, d_picks, hashes, n_hashes, hash_stride, caps.empty() ? nullptr : caps.data(), 0, 0,
+                                          n_eps, touch_bound, e->stream),
+                      what);
+    if (rc != EPPSCORE_OK) return rc;
+    if ((rc = index_end(e)) != EPPSCORE_OK) return rc;
+    if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));  // stream-ordered for the caller
+    return EPPSCORE_OK;
+  }
+  int32_t lo = e->geo.Mpad, hi = -1;
+  int64_t touches = 0;
+  for (int32_t r = 0; r < R; r++)
+    for (int32_t p = 0; p < n_picks; p++) {
+      const int32_t ep = picks[p][r];
+      if (ep < 0) continue;  // no target endpoint: nothing to record (plugin.go:173-175)
+      if (ep >= e->geo.Mpad) return fail(e, EPPSCORE_ERR_INVALID, "pick out of range");
+      if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "n_hashes exceeds hash_stride");
+      lo = std::min(lo, ep);
+      hi = std::max(hi, ep);
+      touches += n_hashes[r];
+    }
+  if (hi < 0) return EPPSCORE_OK;  // (a pick with zero hashes still creates the endpoint's LRU, indexer.go:57-68)
   if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
-  const int32_t* d_pick;
   const uint64_t* d_hash;
   const uint16_t* d_nh;
-  if ((rc = h2d(e, e->stage[0], pick, (size_t)R, &d_pick)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
+  CK(e, e->stage[0].reserve((size_t)n_picks * R * 4));
+  for (int32_t p = 0; p < n_picks; p++) {
+    int32_t* dst = e->stage[0].as<int32_t>() + (size_t)p * R;
+    CK(e, cudaMemcpyAsync(dst, picks[p], (size_t)R * 4, cudaMemcpyHostToDevice, e->stream));
+    d_picks[p] = dst;
+  }
+  if ((rc = h2d(e, e->stage[1], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
       (rc = h2d(e, e->stage[2], n_hashes, (size_t)R, &d_nh)) != EPPSCORE_OK)
     return rc;
-  rc = index_status(e, e->index->commit(R, d_pick, d_hash, d_nh, hash_stride, caps.empty() ? nullptr : caps.data(), 0, lo, hi - lo + 1,
-                                        std::max<int64_t>(touches, 1), e->stream),
-                    "commit_picks");
+  rc = index_status(e, e->index->commit(R, n_picks, d_picks, d_hash, d_nh, hash_stride, caps.empty() ? nullptr : caps.data(), 0, lo,
+                                        hi - lo + 1, std::max<int64_t>(touches, 1), e->stream),
+                    what);
   if (rc != EPPSCORE_OK) return rc;
   CK(e, cudaStreamSynchronize(e->stream));  // the caller's host arrays (pageable) may be reused
   return index_end(e);
 }
 
+int32_t eppscore_commit_picks(eppscore_engine* e, int32_t R, const int32_t* pick, const uint64_t* hashes,
+                              const uint16_t* n_hashes, int32_t hash_stride, const int32_t* lru_capacity) {
+  return commit_calls(e, R, 1, &pick, hashes, n_hashes, hash_stride, lru_capacity, false, 0, nullptr, "commit_picks");
+}
+
 int32_t eppscore_commit_picks_device(eppscore_engine* e, int32_t R, const int32_t* pick, const uint64_t* hashes,
                                      const uint16_t* n_hashes, int32_t hash_stride, const int32_t* lru_capacity,
                                      int64_t touch_bound, void* stream) {
-  if (!e) return EPPSCORE_ERR_INVALID;
-  if (R < 0 || (R > 0 && (!pick || !hashes || !n_hashes))) return fail(e, EPPSCORE_ERR_INVALID, "NULL argument");
-  if (R == 0) return EPPSCORE_OK;
-  if (hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "hash_stride must be > 0");
-  CK(e, cudaSetDevice(e->device));
-  std::vector<int32_t> caps;
-  int32_t rc = pad_caps(e, lru_capacity, &caps);
-  if (rc != EPPSCORE_OK) return rc;
-  cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
-  if (cs != e->stream) {  // the arrays are produced on the caller's stream
-    CK(e, cudaEventRecord(e->ev_caller, cs));
-    CK(e, cudaStreamWaitEvent(e->stream, e->ev_caller, 0));
-  }
-  if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
-  const int32_t n_eps = e->M > 0 ? e->M : e->geo.Mpad;
-  rc = index_status(e, e->index->commit(R, pick, hashes, n_hashes, hash_stride, caps.empty() ? nullptr : caps.data(), 0, 0, n_eps,
-                                        touch_bound, e->stream),
-                    "commit_picks_device");
-  if (rc != EPPSCORE_OK) return rc;
-  if ((rc = index_end(e)) != EPPSCORE_OK) return rc;
-  if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));  // stream-ordered for the caller
-  return EPPSCORE_OK;
+  return commit_calls(e, R, 1, &pick, hashes, n_hashes, hash_stride, lru_capacity, true, touch_bound, stream, "commit_picks_device");
+}
+
+int32_t eppscore_commit_picks_profiles(eppscore_engine* e, int32_t R, int32_t n_picks, const int32_t* const* picks,
+                                       const uint64_t* hashes, const uint16_t* n_hashes, int32_t hash_stride,
+                                       const int32_t* lru_capacity, int32_t location, int64_t touch_bound, void* stream) {
+  if (e && location != 0 && location != 1) return fail(e, EPPSCORE_ERR_INVALID, "commit_picks_profiles: location must be 0 or 1");
+  return commit_calls(e, R, n_picks, picks, hashes, n_hashes, hash_stride, lru_capacity, location == 1, touch_bound, stream,
+                      "commit_picks_profiles");
 }
 
 int32_t eppscore_prefix_add(eppscore_engine* e, const uint64_t* hashes, int32_t n, int32_t endpoint, int32_t lru_capacity) {
@@ -1583,7 +1898,8 @@ int32_t eppscore_prefix_add(eppscore_engine* e, const uint64_t* hashes, int32_t 
   CK(e, cudaMemcpyAsync(e->stage[0].p, &endpoint, 4, cudaMemcpyHostToDevice, e->stream));
   if (n) CK(e, cudaMemcpyAsync(e->stage[1].p, hashes, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
   CK(e, cudaMemcpyAsync(e->stage[2].p, &nh, 2, cudaMemcpyHostToDevice, e->stream));
-  rc = index_status(e, e->index->commit(1, e->stage[0].as<int32_t>(), e->stage[1].as<uint64_t>(), e->stage[2].as<uint16_t>(), stride,
+  const int32_t* d_ep = e->stage[0].as<int32_t>();
+  rc = index_status(e, e->index->commit(1, 1, &d_ep, e->stage[1].as<uint64_t>(), e->stage[2].as<uint16_t>(), stride,
                                         nullptr, lru_capacity, endpoint, 1, std::max(n, 1), e->stream),
                     "prefix_add");
   if (rc != EPPSCORE_OK) return rc;

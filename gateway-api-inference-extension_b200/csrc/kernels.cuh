@@ -148,7 +148,8 @@ struct ScoreArgs {
   int32_t A;
   const AdapterSummary* summ;   // [A+1]  (sparse path)
   const uint32_t* tiemask;      // [A+1][row_words] permuted bits: G[a][m] == gmax  (sparse path)
-  const double* prefix_lut2d;   // [(kLutMax+1)^2]: lut2d[total*(kLutMax+1)+c] = clamp(c/total)*w_prefix, or null
+  const uint32_t* member;       // [row_words] permuted bits: the profile's endpoint subset (sparse path), or null: all endpoints
+  const double* prefix_lut2d;  // [(kLutMax+1)^2]: lut2d[total*(kLutMax+1)+c] = clamp(c/total)*w_prefix, or null
   const int32_t* adapter_id;    // [R] or null
   const uint32_t* cand_mask;    // [R][mask_words] natural order or null
   int32_t mask_words;
@@ -219,6 +220,7 @@ struct PrepareArgs {
   const int32_t* maxm;
   const double* col[4];
   const int64_t* tokens;        // InFlightLoad.Tokens or null
+  const uint32_t* member;       // [Mpad/32] natural-order bits of the profile's endpoint subset, or null: every endpoint
   double token_threshold;
   int32_t lora_words;
   int32_t A;
@@ -260,6 +262,13 @@ int launch_score_matrix(const ScoreArgs& a, cudaStream_t s, int sm_count);      
 int launch_score_dense_fast(const ScoreArgs& a, cudaStream_t s, int sm_count);         // 0 if no specialisation applies
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count);              // 0 if not applicable
 bool pick_sparse_probes(const ScoreArgs& a);  // launch_pick_sparse takes the batch and probes the index for it (plan, outputs and geometry set; table and hashes are not looked at)
+bool pick_sparse_applies(const ScoreArgs& a);  // launch_pick_sparse takes the batch (same inputs)
+// With a.member set, launch_pick_sparse leaves the requests it deferred (pick == kPickDeferred) to the caller, which scores them
+// with the masked full-matrix kernel on the rows launch_subset_mask writes for them.
+// Candidate rows for the masked kernels on a profile with an endpoint subset: out[r] = member & cand_mask[r] (member alone
+// without cand_mask), [R][mask_words] natural order.  only_pick: only the rows whose pick is kPickDeferred are written.
+int launch_subset_mask(const uint32_t* member, const uint32_t* cand_mask, int R, int mask_words, const int32_t* only_pick,
+                       uint32_t* out, cudaStream_t s, int sm_count);
 
 // top-k lists of any length from weighted score rows (topk_select.cu): row r of `scores` ([R][M], NaN = not a candidate) is
 // request request_base + r; the first k entries of its pick order (device_common.cuh topk_key) go to out_m / out_s [R][k]

@@ -15,6 +15,14 @@
 // So a request costs O(matched blocks + exceptions) instead of O(M) — bit-identical picks, scores and
 // tie counts (tests compare against the oracle and against the generic kernel).
 //
+// On a profile with an endpoint subset (eppscore_set_profile_endpoints) the same argument runs over the member set N instead
+// of all endpoints: G[a][m], gmax, garg, gcnt and the tie mask are taken over N (prepare_adapters_kernel), the base terms'
+// queue / running min/max over N (prepare_endpoints_kernel), and an exception e ∉ N is skipped wherever it comes from (a probe
+// round, the uniform inline set, or a ProbeRec's set).  For e ∈ N, S(r,e) >= G[a][e] still holds, so
+//     max_{m ∈ N} S(r,m) = max( gmax[a], max_{e ∈ N} S(r,e) )
+// with the three cases above unchanged; N empty gives garg = -1 and no exception, i.e. pick -1.  The member bitmap uses the
+// permuted layout of the tie mask, so the word a lane already loads for the tie mask position holds the member bit too.
+//
 // Work split: a group of G = row_words/4 lanes serves one request, so a warp serves 32/G requests at once.  The table is
 // the device-resident index of prefix_table.cuh: a hit brings its endpoint set along in the 32-byte slot (up to 10 members
 // inline), so matchLongestPrefix is: probe -> each hit's lane adds 1 to its members' entries of a small per-request hash
@@ -303,9 +311,9 @@ __global__ void __launch_bounds__(kSparseWarps * 32, EPP_SPARSE_MINBLOCKS) pick_
     Best best = best_none();
     int xg = 0;
     auto consider = [&](int m, int c) {  // one exception: endpoint m matched c blocks
-      if (m < M) {
-        const uint32_t pos = perm_bitpos((uint32_t)m, LOG_EPL);
-        const int wi = (int)(pos >> 5), kb = (int)(pos & 31);
+      const uint32_t pos = perm_bitpos((uint32_t)m, LOG_EPL);
+      const int wi = (int)(pos >> 5), kb = (int)(pos & 31);
+      if (m < M && (!a.member || ((__ldg(a.member + wi) >> kb) & 1u))) {
         const uint32_t clo = __ldg(a.cls_lo + (size_t)ad * RW + wi), chi = __ldg(a.cls_hi + (size_t)ad * RW + wi);
         const uint32_t tmw = __ldg(a.tiemask + (size_t)ad * RW + wi);  // bit kb: G[ad][m] == gmax
         const int cls = (int)((clo >> kb) & 1u) | ((int)((chi >> kb) & 1u) << 1);
@@ -461,22 +469,23 @@ static int launch_sparse_seq(const ScoreArgs& a, cudaStream_t s, int sm_count) {
 }
 
 // Applicable when: unmasked, not dense, no per-pair diagnostics, plan flagged sparse_ok, summaries present.
-// Returns the number of launches: the sparse kernel plus the full-matrix kernel restricted to the requests it deferred.
-static bool sparse_applies(const ScoreArgs& a) {
+// Returns the number of launches: the sparse kernel plus the full-matrix kernel restricted to the requests it deferred (without
+// an endpoint subset; with one, the caller scores those on member rows).
+bool pick_sparse_applies(const ScoreArgs& a) {
   if (a.R <= 0) return false;
   if (!a.plan.sparse_ok || !a.summ || !a.tiemask || a.cand_mask || a.dense || a.match_out || a.scores_out || a.topk > 0) return false;
   return a.geo.Mpad <= 65536;  // inline members are uint16
 }
 
 bool pick_sparse_probes(const ScoreArgs& a) {
-  if (!sparse_applies(a)) return false;
+  if (!pick_sparse_applies(a)) return false;
   for (int s = 0; s < a.plan.n_steps; s++)
     if (a.plan.kind[s] == STEP_PREFIX) return true;
   return false;
 }
 
 int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
-  if (!sparse_applies(a)) return 0;
+  if (!pick_sparse_applies(a)) return 0;
   int launched;
   switch (a.geo.J) {
     case 1: launched = launch_sparse_seq<1>(a, s, sm_count); break;
@@ -484,7 +493,7 @@ int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
     case 4: launched = launch_sparse_seq<4>(a, s, sm_count); break;
     default: launched = launch_sparse_seq<8>(a, s, sm_count); break;
   }
-  if (launched > 0 && a.table && a.hashes) {  // only a request with prefix matches can overflow its exception table
+  if (launched > 0 && a.table && a.hashes && !a.member) {  // only a request with prefix matches can overflow its exception table
     ScoreArgs d = a;
     d.only_deferred = 1;
     const int deferred = launch_score_matrix(d, s, sm_count);
@@ -492,6 +501,33 @@ int launch_pick_sparse(const ScoreArgs& a, cudaStream_t s, int sm_count) {
     launched += deferred;
   }
   return launched;
+}
+
+// one thread per word of a row; with only_pick, one thread per request (deferred requests are rare: only their rows are written)
+__global__ void subset_mask_kernel(const uint32_t* __restrict__ member, const uint32_t* __restrict__ cand, int R, int mw,
+                                   const int32_t* __restrict__ only_pick, uint32_t* __restrict__ out) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  if (only_pick) {
+    for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < R; r += stride)
+      if (__ldg(only_pick + r) == kPickDeferred)
+        for (int w = 0; w < mw; w++) out[r * mw + w] = __ldg(member + w);
+    return;
+  }
+  const long long n = (long long)R * mw;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int r = (int)(i / mw), w = (int)(i - (long long)r * mw);
+    out[i] = __ldg(member + w) & (cand ? __ldg(cand + i) : 0xffffffffu);
+  }
+}
+
+int launch_subset_mask(const uint32_t* member, const uint32_t* cand_mask, int R, int mask_words, const int32_t* only_pick,
+                       uint32_t* out, cudaStream_t s, int sm_count) {
+  const long long n = only_pick ? (long long)R : (long long)R * mask_words;
+  if (n <= 0 || mask_words <= 0) return 0;
+  const long long want = (n + 255) / 256;
+  const int blocks = (int)(want < (long long)sm_count * 8 ? want : (long long)sm_count * 8);
+  subset_mask_kernel<<<blocks, 256, 0, s>>>(member, cand_mask, R, mask_words, only_pick, out);
+  return 1;
 }
 
 }  // namespace eppscore

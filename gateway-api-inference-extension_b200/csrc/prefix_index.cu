@@ -180,11 +180,13 @@ __global__ void table_rehash_kernel(const TSlot* old_slots, uint64_t old_cap, Ta
   }
 }
 
-// Σ n_hashes over the requests that have a pick: the exact number of touches of a commit whose arrays are on the device
-__global__ void sum_touches_kernel(const int32_t* pick, const uint16_t* nh, int32_t R, unsigned long long* out) {
+// Σ n_hashes over the calls that have a pick: the exact number of touches of a commit whose arrays are on the device
+__global__ void sum_touches_kernel(const CommitArgs a, unsigned long long* out) {
   unsigned long long t = 0;
-  for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < R; r += gridDim.x * blockDim.x)
-    if (pick[r] >= 0) t += nh[r];
+  const int32_t np = a.n_picks > 1 ? a.n_picks : 1;
+  for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.R; r += gridDim.x * blockDim.x)
+    for (int32_t s = 0; s < np; s++)
+      if ((s == 0 ? a.pick : a.more_picks[s - 1])[r] >= 0) t += a.n_hashes[r];
 #pragma unroll
   for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
   if ((threadIdx.x & 31) == 0 && t) atomicAdd(out, t);
@@ -365,22 +367,22 @@ int64_t DeviceIndex::lru_bytes() const {
 }
 
 // PreRequest for a batch whose arrays are on the device; async on `s` (which must be the index's stream).
-cudaError_t DeviceIndex::commit(int32_t R, const int32_t* pick, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
-                                const int32_t* cap_req_host, int32_t single_cap, int32_t ep_first, int32_t n_eps,
-                                int64_t max_touches, cudaStream_t s) {
-  if (R <= 0 || n_eps <= 0) return cudaSuccess;
+cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes,
+                                const uint16_t* n_hashes, int32_t stride, const int32_t* cap_req_host, int32_t single_cap,
+                                int32_t ep_first, int32_t n_eps, int64_t max_touches, cudaStream_t s) {
+  if (R <= 0 || n_eps <= 0 || n_picks < 1 || n_picks > 4) return cudaSuccess;
   uint32_t want = (uint32_t)std::max(single_cap, 0);
   if (cap_req_host)
     for (int32_t i = 0; i < n_endpoints_; i++) want = std::max(want, (uint32_t)std::max(cap_req_host[i], 0));
   IX_CK(ensure_lru(want, s));
   if (want > lv_.max_cap) return cudaErrorInvalidValue;  // the LRU regions were sized for a smaller largest capacity
   CommitArgs a{};
-  a.pick = pick;
   a.hashes = hashes;
   a.n_hashes = n_hashes;
   a.stride = stride;
   a.single_cap = single_cap;
   a.ep_first = ep_first;
+  a.n_picks = n_picks;
   if (cap_req_host) {
     IX_CK(cudaMemcpyAsync(d_capreq_, cap_req_host, (size_t)n_endpoints_ * 4, cudaMemcpyHostToDevice, s));
     a.cap_req = d_capreq_;
@@ -389,12 +391,17 @@ cudaError_t DeviceIndex::commit(int32_t R, const int32_t* pick, const uint64_t* 
   const int32_t kSub = 65536;
   for (int32_t r0 = 0; r0 < R; r0 += kSub) {
     const int32_t n = std::min(kSub, R - r0);
-    int64_t touches = std::min<int64_t>(max_touches, (int64_t)n * stride);
+    a.R = n;
+    a.pick = picks[0] + r0;
+    for (int32_t p = 1; p < n_picks; p++) a.more_picks[p - 1] = picks[p] + r0;
+    a.hashes = hashes + (size_t)r0 * stride;
+    a.n_hashes = n_hashes + r0;
+    int64_t touches = std::min<int64_t>(max_touches, (int64_t)n * n_picks * stride);
     if (max_touches <= 0) {  // no bound from the caller: count them (one small synchronous read-back)
       unsigned long long* d_t = reinterpret_cast<unsigned long long*>(d_scratch_);
       unsigned long long t = 0;
       IX_CK(cudaMemsetAsync(d_t, 0, 8, s));
-      sum_touches_kernel<<<64, 256, 0, s>>>(pick + r0, n_hashes + r0, n, d_t);
+      sum_touches_kernel<<<64, 256, 0, s>>>(a, d_t);
       launches_++;
       IX_CK(cudaMemcpyAsync(&t, d_t, 8, cudaMemcpyDeviceToHost, s));
       IX_CK(cudaStreamSynchronize(s));
@@ -402,10 +409,6 @@ cudaError_t DeviceIndex::commit(int32_t R, const int32_t* pick, const uint64_t* 
     }
     if (touches < 1) touches = 1;
     IX_CK(ensure_room(touches, s));
-    a.R = n;
-    a.pick = pick + r0;
-    a.hashes = hashes + (size_t)r0 * stride;
-    a.n_hashes = n_hashes + r0;
     index_commit_kernel<<<n_eps, kCommitThreads, sizeof(CommitSmem), s>>>(d_tv_, d_lv_, a);
     launches_++;
     IX_CK(cudaGetLastError());

@@ -28,9 +28,10 @@ class DeviceIndex {
   cudaError_t init(cudaStream_t s);
   const TableView* view() const { return d_tv_; }  // device pointer, stable for the engine's lifetime
 
-  // PreRequest for R requests (device arrays), endpoints [ep_first, ep_first + n_eps).  max_touches: an upper bound on
-  // Σ n_hashes over the requests (<= 0: R * stride).  cap_req_host: optional [n_endpoints] CacheNumBlocks.
-  cudaError_t commit(int32_t R, const int32_t* pick, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
+  // PreRequest for R requests (device arrays), endpoints [ep_first, ep_first + n_eps): picks[0..n_picks) are [R] each, applied
+  // per request in slot order (CommitArgs).  max_touches: an upper bound on Σ n_hashes over the calls (<= 0: counted on the
+  // device).  cap_req_host: optional [n_endpoints] CacheNumBlocks.
+  cudaError_t commit(int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
                      const int32_t* cap_req_host, int32_t single_cap, int32_t ep_first, int32_t n_eps, int64_t max_touches,
                      cudaStream_t s);
   cudaError_t apply(int64_t n, const uint64_t* hash, const int32_t* endpoint, const uint8_t* op, cudaStream_t s);  // device arrays

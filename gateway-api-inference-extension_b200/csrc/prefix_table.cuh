@@ -339,6 +339,11 @@ struct CommitArgs {
   const int32_t* cap_req;    // [n_endpoints] CacheNumBlocks per endpoint (autotune, plugin.go:207-216) or null
   int32_t single_cap;        // capacity request when cap_req is null (<= 0: default)
   int32_t ep_first;          // CTA b serves endpoint ep_first + b
+  // Several picks per request (the primary profile's, then the "prefill" profile's, plugin.go:177-197): n_picks slots, slot 0
+  // is `pick`, slot s > 0 is more_picks[s - 1].  The calls are (request, slot) in request order, slots ascending within a
+  // request.  0 or 1: `pick` alone.
+  int32_t n_picks;
+  const int32_t* more_picks[3];
 };
 
 template <class X>
@@ -620,12 +625,20 @@ struct IndexProgram {
     bool created = x.ld32(&d->created) != 0;
     const int32_t cap_req = a.cap_req ? a.cap_req[p] : a.single_cap;
     uint32_t fill = 0, cap = 0, chunk_cap = 0;
-    for (int32_t r0 = 0; r0 < a.R; r0 += kPickWindow) {
-      // this endpoint's requests in the window, in request order: thread t looks at picks [r0 + 8t, r0 + 8t + 8)
+    // call i is (request i / np, slot i % np): this endpoint's calls in call order, then each call's request
+    const int32_t np = a.n_picks > 1 ? a.n_picks : 1;
+    const int32_t n_calls = a.R * np;
+    auto call_pick = [&](int32_t i) {
+      if (np == 1) return a.pick[i];
+      const int32_t r = i / np, s = i - r * np;
+      return (s == 0 ? a.pick : a.more_picks[s - 1])[r];
+    };
+    for (int32_t r0 = 0; r0 < n_calls; r0 += kPickWindow) {
+      // this endpoint's calls in the window, in call order: thread t looks at calls [r0 + 8t, r0 + 8t + 8)
       x.par([&](int tid) {
         uint32_t c = 0;
         const int32_t rb = r0 + tid * kPicksPerThread;
-        for (int32_t k = 0; k < kPicksPerThread; k++) c += (rb + k < a.R && a.pick[rb + k] == (int32_t)p) ? 1u : 0u;
+        for (int32_t k = 0; k < kPicksPerThread; k++) c += (rb + k < n_calls && call_pick(rb + k) == (int32_t)p) ? 1u : 0u;
         sm->scan[tid] = c;
       });
       const uint32_t nreq = x.scan(sm->scan, &sm->total);
@@ -634,7 +647,7 @@ struct IndexProgram {
         uint32_t at = sm->scan[tid];
         const int32_t rb = r0 + tid * kPicksPerThread;
         for (int32_t k = 0; k < kPicksPerThread; k++)
-          if (rb + k < a.R && a.pick[rb + k] == (int32_t)p) sm->req[at++] = (uint32_t)(rb + k);
+          if (rb + k < n_calls && call_pick(rb + k) == (int32_t)p) sm->req[at++] = (uint32_t)((rb + k) / np);
       });
       if (!created) {
         ensure_created(cap_req);

@@ -9,18 +9,25 @@
 
 namespace eppscore {
 
+// Whether endpoint m is in the profile's endpoint subset (every endpoint without one).  A subset is the head of the profile's
+// filter chain, so everything computed "over all endpoints" below is computed over the members.
+__device__ __forceinline__ bool is_member(const uint32_t* member, int m) {
+  return !member || ((__ldg(member + (m >> 5)) >> (m & 31)) & 1u);
+}
+
 __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const __grid_constant__ PrepareArgs a) {
   __shared__ long long s_red[2][2][32];  // [queue|running][min|max][warp]
   __shared__ long long s_mm[2][2];
   const int M = a.geo.M, Mpad = a.geo.Mpad;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
-  // min / max of WaitingQueueSize and RunningRequestsSize over ALL endpoints (queue.go:79-91)
+  // min / max of WaitingQueueSize and RunningRequestsSize over the profile's endpoints (queue.go:79-91)
   for (int which = 0; which < 2; which++) {
     const int64_t* q = which == 0 ? a.queue : a.running;
     long long mn = 0x7fffffffffffffffLL, mx = (long long)0x8000000000000000ULL;
     if (q)
       for (int m = tid; m < M; m += blockDim.x) {
+        if (!is_member(a.member, m)) continue;
         const long long v = q[m];
         mn = v < mn ? v : mn;
         mx = v > mx ? v : mx;
@@ -67,6 +74,7 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const __grid_co
     __syncthreads();
     if (ok)
       for (int m = tid; m < M; m += blockDim.x) {
+        if (!is_member(a.member, m)) continue;  // (the masked kernels only see members: their rows carry the subset)
         const int v = (int)(q[m] - mn);
         atomicOr(&tbl[v * MW + (m >> 5)], 1u << (m & 31));
         atomicOr(&hdr->occ[v >> 5], 1u << (v & 31));
@@ -182,14 +190,16 @@ __global__ void __launch_bounds__(kAdapterThreads) prepare_adapters_kernel(const
   if (!a.summ) return;
   __syncthreads();
 
-  // G[ai][m]: the weighted score with zero prefix match, steps in profile order; arg-max over m
+  // G[ai][m]: the weighted score with zero prefix match, steps in profile order; arg-max over the profile's endpoints (the
+  // exactness argument of pick_sparse.cu holds over the member set: non-members are never candidates, exceptions included)
   auto score_of = [&](int m) {
     const uint32_t pos = perm_bitpos((uint32_t)m, log_epl);
     const int cls = (int)((s_lo[pos >> 5] >> (pos & 31)) & 1u) | ((int)((s_hi[pos >> 5] >> (pos & 31)) & 1u) << 1);
     return eval_steps(a.plan_u, a.plan_term, m, 0, 0, cls);
   };
   Best b = best_none();
-  for (int m = tid; m < M; m += blockDim.x) best_update(b, score_of(m), m, 0, 0, 0);
+  for (int m = tid; m < M; m += blockDim.x)
+    if (is_member(a.member, m)) best_update(b, score_of(m), m, 0, 0, 0);
   best_group_reduce<32>(b, 0);
   if (lane == 0) {
     s_bs[warp] = b.score;
@@ -210,7 +220,7 @@ __global__ void __launch_bounds__(kAdapterThreads) prepare_adapters_kernel(const
   __syncthreads();
   const double gmax = s_gmax;
   for (int m = tid; m < M; m += blockDim.x)
-    if (score_of(m) == gmax) {
+    if (is_member(a.member, m) && score_of(m) == gmax) {
       const uint32_t pos = perm_bitpos((uint32_t)m, log_epl);
       atomicOr(&s_tie[pos >> 5], 1u << (pos & 31));
     }

@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 
 from . import _capi as capi
-from ._capi import Batch, Config, EppscoreError, LatencyParams, SCORER, Snapshot, Stats, TopK
+from ._capi import Batch, Config, EppscoreError, LatencyParams, Profile, ProfileRun, SCORER, Snapshot, Stats, TopK
 
 
 def default_config(scorers=None, filters=(), **kw) -> Config:
@@ -240,6 +240,111 @@ class Engine:
             self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
         return res
 
+    # ------------------------------------------------------------------ several scheduler profiles
+    def add_profile(self, scorers, pick_mode=0, filters=()) -> int:
+        """eppscore_add_profile: scorers [(kind name | int, weight)] in profile order, the picker and the device-side
+        filters [(kind, (params...))]; everything else is the engine's.  Returns the profile id."""
+        if len(scorers) > capi.MAX_SCORERS or len(filters) > 4:
+            raise ValueError("too many scorers or filters")
+        p = Profile()
+        p.struct_size = C.sizeof(Profile)
+        p.n_scorers = len(scorers)
+        for i, (k, w) in enumerate(scorers):
+            p.scorer_kind[i] = SCORER[k] if isinstance(k, str) else int(k)
+            p.scorer_weight[i] = float(w)
+        p.pick_mode = pick_mode
+        p.n_filters = len(filters)
+        for i, (k, par) in enumerate(filters):
+            p.filter_kind[i] = int(k)
+            for j, v in enumerate(par):
+                p.filter_param[i][j] = float(v)
+        pid = C.c_int32()
+        self._check(self._lib.eppscore_add_profile(self._h, C.byref(p), C.byref(pid)))
+        return pid.value
+
+    def set_profile_endpoints(self, profile: int, mask=None):
+        """The profile's endpoint subset as a uint32 bitmask over endpoint rows (None: every endpoint); applied by the next
+        set_snapshot."""
+        a = _Args(False)
+        words = 0 if mask is None else int(np.asarray(mask).size)
+        self._check(self._lib.eppscore_set_profile_endpoints(self._h, profile, a.ptr(mask, np.uint32), words))
+
+    def schedule_profiles(self, R, runs, *, prompt_bytes=None, prompt_off=None, prompt_len=None, model_seed=None, hashes_in=None,
+                          n_hashes_in=None, hash_stride=0, adapter_id=None, dense_feat=None, dense_total=None, block_chars=0,
+                          max_blocks=0, request_base=0, want_match=False, want_total=True, want_hashes=False, input_tokens=None,
+                          ttft_slo=None, tpot_slo=None, device=False, stream=None, out=None):
+        """eppscore_schedule_batch_profiles: one hash stage, then one Filter -> Score -> Pick per run.  runs: list of dicts
+        {"profile": id, "cand_mask": optional, "want_scores" / "want_pred" / "want_filter_mask": optional bools (host mode)};
+        in device mode each run dict also holds its preallocated outputs (pick, pick_score, tie_count, optional scores_out,
+        pred_out, filter_mask_out) and `out` the batch's (total_blocks, match_blocks, hashes_out).
+        Host mode returns (batch outputs dict, [per-run outputs dict])."""
+        a = _Args(device)
+        b = Batch()
+        b.struct_size = C.sizeof(Batch)
+        b.R = R
+        b.location = 1 if device else 0
+        b.request_base = request_base
+        b.prompt_bytes = a.ptr(prompt_bytes, np.uint8)
+        b.prompt_off = a.ptr(prompt_off, np.int64)
+        b.prompt_len = a.ptr(prompt_len, np.int32)
+        b.model_seed = a.ptr(model_seed, np.uint64)
+        b.hashes_in = a.ptr(hashes_in, np.uint64)
+        b.n_hashes_in = a.ptr(n_hashes_in, np.uint16)
+        if hashes_in is not None and not hash_stride:
+            hash_stride = int(hashes_in.shape[1])
+        b.hash_stride = hash_stride
+        b.block_chars = block_chars
+        b.max_blocks = max_blocks
+        b.adapter_id = a.ptr(adapter_id, np.int32)
+        b.dense_feat = a.ptr(dense_feat, np.float32)
+        b.dense_total = a.ptr(dense_total, np.uint16)
+        b.input_tokens = a.ptr(input_tokens, np.int32)
+        b.ttft_slo = a.ptr(ttft_slo, np.float64)
+        b.tpot_slo = a.ptr(tpot_slo, np.float64)
+        b.stream = stream
+        arr = (ProfileRun * len(runs))()
+        M = self.M
+        mw = max((M + 31) // 32, 1)
+        res_runs = []
+        for i, run in enumerate(runs):
+            x = arr[i]
+            x.struct_size = C.sizeof(ProfileRun)
+            x.profile = run["profile"]
+            x.cand_mask = a.ptr(run.get("cand_mask"), np.uint32)
+            if device:
+                for k in ("pick", "pick_score", "tie_count", "scores_out", "pred_out", "filter_mask_out"):
+                    setattr(x, k, a.ptr(run.get(k), None))
+                continue
+            o = dict(pick=np.full(R, -2, np.int32), pick_score=np.zeros(R, np.float64), tie_count=np.zeros(R, np.int32))
+            if run.get("want_scores"):
+                o["scores_out"] = np.zeros((R, M), np.float64)
+            if run.get("want_pred"):
+                o["pred_out"] = np.zeros((R, M, 2), np.float64)
+            if run.get("want_filter_mask"):
+                o["filter_mask_out"] = np.zeros((R, mw), np.uint32)
+            for k, v in o.items():
+                setattr(x, k, v.ctypes.data)
+            res_runs.append(o)
+        if device:
+            if out is None:
+                out = {}
+            b.match_blocks = a.ptr(out.get("match_blocks"), None)
+            b.total_blocks = a.ptr(out.get("total_blocks"), None)
+            b.hashes_out = a.ptr(out.get("hashes_out"), None)
+            self._check(self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr))
+            return out, runs
+        res = {}
+        if want_total:
+            res["total_blocks"] = np.zeros(R, np.uint16)
+        if want_match:
+            res["match_blocks"] = np.zeros((R, M), np.uint16)
+        if want_hashes:
+            res["hashes_out"] = np.zeros((R, max_blocks or self.cfg.max_blocks), np.uint64)
+        for k, v in res.items():
+            setattr(b, k, v.ctypes.data)
+        self._check(self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr))
+        return res, res_runs
+
     @staticmethod
     def _topk(k, endpoints, scores) -> TopK:
         t = TopK()
@@ -390,6 +495,27 @@ class Engine:
         stride = int(hashes.shape[1])
         self._check(self._lib.eppscore_commit_picks_device(self._h, R, a.ptr(pick, None), a.ptr(hashes, None), a.ptr(n_hashes, None),
                                                            stride, ah.ptr(lru_capacity, np.int32), int(touch_bound), stream))
+
+    def commit_picks_profiles(self, picks, hashes, n_hashes, lru_capacity=None, device=False, touch_bound=0, stream=None):
+        """PreRequest with several picks per request (eppscore_commit_picks_profiles): picks is a list of [R] arrays (the primary
+        profile's first, then e.g. the "prefill" profile's); Adds run per request in list order.  device=True: CUDA tensors /
+        raw pointers, asynchronous on `stream`; lru_capacity is always a HOST array."""
+        a = _Args(device)
+        ah = _Args(False)
+        if device:
+            R = int(picks[0].shape[0])
+            stride = int(hashes.shape[1])
+            hp, nhp = a.ptr(hashes, None), a.ptr(n_hashes, None)
+            pp = [a.ptr(p, None) for p in picks]
+        else:
+            hashes = np.ascontiguousarray(hashes, np.uint64)
+            R = len(picks[0])
+            stride = hashes.shape[1] if hashes.ndim == 2 else 0
+            hp, nhp = a.ptr(hashes, np.uint64), a.ptr(n_hashes, np.uint16)
+            pp = [a.ptr(p, np.int32) for p in picks]
+        arr = (C.c_void_p * len(pp))(*pp)
+        self._check(self._lib.eppscore_commit_picks_profiles(self._h, R, len(pp), arr, hp, nhp, stride, ah.ptr(lru_capacity, np.int32),
+                                                             1 if device else 0, int(touch_bound), stream))
 
     def prefix_add(self, hashes, endpoint, lru_capacity=0):
         a = _Args(False)

@@ -18,6 +18,7 @@
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <memory>
 #include <stdexcept>
@@ -70,6 +71,21 @@ inline bool EngineHasRunningQueues() {
 }
 inline bool EngineHasTopK() { return &eppscore_schedule_batch_topk != nullptr; }
 inline bool EngineHasTopKWide() { return &eppscore_schedule_batch_topk_wide != nullptr; }
+// Several scheduler profiles (eppscore_add_profile ...) came the same way: bound weakly, EngineHasProfiles() tells.  Without them
+// a config with more than one profile is refused when the Scheduler is built.
+extern "C" int32_t eppscore_add_profile(struct eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) __attribute__((weak));
+extern "C" int32_t eppscore_set_profile_endpoints(struct eppscore_engine* e, int32_t profile, const uint32_t* mask, int32_t words)
+    __attribute__((weak));
+extern "C" int32_t eppscore_schedule_batch_profiles(struct eppscore_engine* e, const eppscore_batch* b, int32_t n_runs,
+                                                    const eppscore_profile_run* runs) __attribute__((weak));
+extern "C" int32_t eppscore_commit_picks_profiles(struct eppscore_engine* e, int32_t R, int32_t n_picks, const int32_t* const* picks,
+                                                  const uint64_t* hashes, const uint16_t* n_hashes, int32_t hash_stride,
+                                                  const int32_t* lru_capacity, int32_t location, int64_t touch_bound, void* stream)
+    __attribute__((weak));
+inline bool EngineHasProfiles() {
+  return &eppscore_add_profile != nullptr && &eppscore_set_profile_endpoints != nullptr && &eppscore_schedule_batch_profiles != nullptr &&
+         &eppscore_commit_picks_profiles != nullptr;
+}
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
          &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
@@ -176,6 +192,11 @@ class SchedulerProfile {
   SchedulerProfile& WithScorers(std::vector<WeightedScorer> s) { scorers_ = std::move(s); return *this; }
   SchedulerProfile& WithPicker(MaxScorePicker p) { picker_ = p; return *this; }
   SchedulerProfile& WithDeviceFilters(std::vector<DeviceFilter> f) { device_filters_ = std::move(f); return *this; }
+  // A request-independent Filter at the head of the profile's filter chain (e.g. a prefill / decode role label): the endpoints
+  // it keeps are the profile's endpoint subset on the engine (eppscore_set_profile_endpoints), packed with every snapshot, so
+  // batches need no per-request mask for it.  Multi-profile configs only.
+  SchedulerProfile& WithEndpointSubset(std::function<bool(const Endpoint&)> keep) { subset_ = std::move(keep); return *this; }
+  const std::function<bool(const Endpoint&)>& endpoint_subset() const { return subset_; }
   const std::vector<DeviceFilter>& device_filters() const { return device_filters_; }
   SchedulerProfile& WithPredictedLatencyProducer(std::shared_ptr<PredictedLatencyProducer> p) { producer_ = std::move(p); return *this; }
   const std::shared_ptr<PredictedLatencyProducer>& producer() const { return producer_; }
@@ -189,6 +210,34 @@ class SchedulerProfile {
   MaxScorePicker picker_;
   std::shared_ptr<PredictedLatencyProducer> producer_;
   std::vector<DeviceFilter> device_filters_;
+  std::function<bool(const Endpoint&)> subset_;
+};
+
+// framework.ProfileHandler (scheduler.go:54-102): Pick names the profiles to run for a request given the results so far (empty
+// on the first round; an empty answer ends the loop), ProcessResults turns every profile's result (nullptr: the profile found
+// no endpoint) into the request's SchedulingResult, or throws SchedulingError with the reference's error.
+struct ProfileHandler {
+  virtual ~ProfileHandler() = default;
+  virtual std::vector<std::string> Pick(const InferenceRequest& request, const std::vector<std::string>& profiles,
+                                        const std::map<std::string, const ProfileRunResult*>& results) = 0;
+  virtual SchedulingResult ProcessResults(const InferenceRequest& request,
+                                          const std::map<std::string, const ProfileRunResult*>& results) = 0;
+};
+// single-profile-handler (single_profile_handler.go): the one profile, once; its result is the primary one.
+struct SingleProfileHandler : ProfileHandler {
+  std::vector<std::string> Pick(const InferenceRequest&, const std::vector<std::string>& profiles,
+                                const std::map<std::string, const ProfileRunResult*>& results) override {
+    if (!results.empty() || profiles.empty()) return {};
+    return {profiles[0]};
+  }
+  SchedulingResult ProcessResults(const InferenceRequest&, const std::map<std::string, const ProfileRunResult*>& results) override {
+    const auto& kv = *results.begin();
+    if (!kv.second) throw SchedulingError("failed to run scheduler profile '" + kv.first + "'");
+    SchedulingResult r;
+    r.ProfileResults[kv.first] = *kv.second;
+    r.PrimaryProfileName = kv.first;
+    return r;
+  }
 };
 
 // approximateprefix config (types.go:77-141)
@@ -218,11 +267,65 @@ struct SchedulerConfig {
   // ResponseComplete releases it, RemovePod drops the endpoint's counters, and a token-load scorer reads the counters
   // (Endpoint::InFlightTokens is then not used).  Batches always take the engine route: the counters live on the device.
   std::shared_ptr<InFlightLoadProducer> InFlightLoad;
+  // Several named profiles, in order (the first is the engine's profile 0), and the handler that picks among them.  Empty: the
+  // single `Profile` above with SingleProfileHandler semantics, on the path that has always served it.  A multi-profile config
+  // needs an engine library with the profile calls and takes MaxNumOfEndpoints 1 on every profile; the latency scorer and
+  // TrackRunningRequests stay single-profile.  The profile named "prefill" gets the second prefix-index Add of PreRequest
+  // (approximateprefix/plugin.go:177-197) and its in-flight load is released at ResponseStarted (inflightload/producer.go:137-160).
+  std::vector<std::pair<std::string, SchedulerProfile>> Profiles;
+  std::shared_ptr<ProfileHandler> Handler;
 };
 
 class Scheduler {
  public:
-  explicit Scheduler(const SchedulerConfig& cfg) : cfg_(cfg) {
+  explicit Scheduler(const SchedulerConfig& cfg) : Scheduler(cfg, 0) {
+    if (cfg.Profiles.empty()) return;
+    for (size_t p = 1; p < cfg.Profiles.size(); p++) {  // profile 0 was created with the engine
+      const SchedulerProfile& sp = cfg.Profiles[p].second;
+      eppscore_profile ep{};
+      ep.struct_size = sizeof(ep);
+      if (sp.scorers().size() > EPPSCORE_MAX_SCORERS || sp.device_filters().size() > EPPSCORE_MAX_FILTERS)
+        throw SchedulingError("too many scorers or device filters in profile '" + cfg.Profiles[p].first + "'");
+      ep.n_scorers = (int32_t)sp.scorers().size();
+      for (size_t i = 0; i < sp.scorers().size(); i++) {
+        ep.scorer_kind[i] = sp.scorers()[i].Scorer_->Kind;
+        ep.scorer_weight[i] = sp.scorers()[i].Weight();
+      }
+      ep.pick_mode = sp.picker().Mode;
+      ep.n_filters = (int32_t)sp.device_filters().size();
+      for (size_t i = 0; i < sp.device_filters().size(); i++) {
+        ep.filter_kind[i] = sp.device_filters()[i].Kind;
+        for (int q = 0; q < 3; q++) ep.filter_param[i][q] = sp.device_filters()[i].Param[q];
+      }
+      int32_t id = -1;
+      if (eppscore_add_profile(eng_, &ep, &id) != EPPSCORE_OK)  // (the destructor frees the engine)
+        throw SchedulingError(std::string("eppscore_add_profile: ") + eppscore_last_error(eng_));
+    }
+  }
+
+ private:
+  static SchedulerConfig SingleOrFirst(const SchedulerConfig& cfg) {  // the engine's profile 0 and the checks of its path
+    if (cfg.Profiles.empty()) return cfg;
+    if (!EngineHasProfiles()) throw SchedulingError("a config with several profiles needs an engine library with eppscore_add_profile");
+    if (!cfg.Handler) throw SchedulingError("a config with several profiles needs a ProfileHandler");
+    if (cfg.Profiles.size() > EPPSCORE_MAX_PROFILES) throw SchedulingError("more profiles than EPPSCORE_MAX_PROFILES");
+    for (const auto& np : cfg.Profiles) {
+      if (np.second.picker().MaxNumOfEndpoints != 1)
+        throw SchedulingError("maxNumOfEndpoints > 1 is not supported with several profiles (profile '" + np.first + "')");
+      if (np.second.producer())
+        throw SchedulingError("the predicted-latency producer is not supported with several profiles (profile '" + np.first + "')");
+      for (const auto& w : np.second.scorers())
+        if (w.Scorer_->Kind == EPPSCORE_SCORER_LATENCY)
+          throw SchedulingError("the latency scorer is not supported with several profiles (profile '" + np.first + "')");
+    }
+    SchedulerConfig c = cfg;
+    c.ProfileName = cfg.Profiles[0].first;
+    c.Profile = cfg.Profiles[0].second;
+    c.CpuBatchThreshold = 0;  // the host route serves one profile
+    return c;
+  }
+  Scheduler(const SchedulerConfig& cfg0, int) : cfg_(SingleOrFirst(cfg0)) {
+    const SchedulerConfig& cfg = cfg_;
     eppscore_config c;
     eppscore_config_default(&c);
     const auto& sc = cfg.Profile.scorers();
@@ -280,6 +383,8 @@ class Scheduler {
     c.tie_seed = cfg.TieSeed;
     if (eppscore_create(cfg.Device, &c, &eng_) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_create: ") + eppscore_last_error(nullptr));
   }
+
+ public:
   ~Scheduler() { eppscore_destroy(eng_); }
   Scheduler(const Scheduler&) = delete;
   Scheduler& operator=(const Scheduler&) = delete;
@@ -298,6 +403,7 @@ class Scheduler {
 
   // R concurrent Schedule() calls against the same candidate slice, as ONE engine batch.
   std::vector<BatchItem> ScheduleBatch(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
+    if (!cfg_.Profiles.empty()) return ScheduleBatchProfiles(requests, endpoints);
     const int R = (int)requests.size(), M = (int)endpoints.size();
     std::vector<BatchItem> out((size_t)R);
     last_hashes_.clear();
@@ -337,25 +443,9 @@ class Scheduler {
     // director candidates.go:98).  An endpoint keeps the id it got when it was first seen; the engine's rows are ids, the
     // list's positions are mapped to and from them.  When the list is exactly ids 0..M-1 in order (the common case, and every
     // single-list use) nothing is remapped; a mask is only needed when some row has no endpoint in this list. ---
-    std::vector<int> ids((size_t)M);
+    std::vector<int> ids;
     int Mx = 0;
-    bool identity = true;
-    {
-      std::vector<int> seen;
-      for (int m = 0; m < M; m++) {
-        ids[m] = IdOf(endpoints[(size_t)m].GetMetadata()->NamespacedName_.String());
-        Mx = std::max(Mx, ids[m] + 1);
-        identity = identity && ids[m] == m;
-      }
-      seen.assign((size_t)Mx, 0);
-      bool dup = false;
-      for (int m = 0; m < M; m++) dup = dup || seen[(size_t)ids[m]]++ > 0;
-      if (dup) {  // the same server twice in one list: positions are the only usable ids for this batch
-        for (int m = 0; m < M; m++) ids[m] = m;
-        Mx = M;
-        identity = true;
-      }
-    }
+    bool identity = MapIds(endpoints, &ids, &Mx);
     identity = identity && Mx == M;
     if (Mx > cfg_.MaxEndpoints) throw SchedulingError("more endpoints than SchedulerConfig.MaxEndpoints");
     if (!identity) remapped_batches_++;
@@ -532,6 +622,7 @@ class Scheduler {
   // (inflightload/producer.go:101-120).
   void PreRequest(const std::vector<BatchItem>& results) {
     if (!last_endpoints_ || (last_hashes_.empty() && !inflight_ && !running_)) return;
+    if (!cfg_.Profiles.empty()) return PreRequestProfiles(results);
     const int R = (int)results.size();
     std::vector<int32_t> pick((size_t)R, -1);
     for (int r = 0; r < R; r++)
@@ -578,6 +669,7 @@ class Scheduler {
   // request's estimate.  Without the producer, or for a server that has left the pool since (its id may already be another
   // server's), nothing happens.
   void ResponseComplete(const InferenceRequest& request, const SchedulingResult& result) {
+    if (!cfg_.Profiles.empty()) return ReleaseProfiles(request, result, false);
     RunningRemove(request, result);  // requestcontrol_hooks.go:219
     if (!inflight_) return;
     auto pr = result.ProfileResults.find(cfg_.ProfileName);
@@ -591,6 +683,12 @@ class Scheduler {
       throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
     if (eppscore_inflight_release(eng_, 1, 0, &id, &est, nullptr) != EPPSCORE_OK)
       throw SchedulingError(std::string("eppscore_inflight_release: ") + eppscore_last_error(eng_));
+  }
+
+  // ResponseBody at start of stream (inflightload/producer.go:137-160): with several profiles, the "prefill" profile's target
+  // gives back the request; its other targets stay counted until ResponseComplete.  Nothing for a single-profile config.
+  void ResponseStarted(const InferenceRequest& request, const SchedulingResult& result) {
+    if (!cfg_.Profiles.empty()) ReleaseProfiles(request, result, true);
   }
 
   // indexer.RemovePod (indexer.go:167-182), called when a model server leaves the pool: its LRU and its memberships go, its
@@ -690,6 +788,268 @@ class Scheduler {
       throw SchedulingError(std::string("eppscore_running_remove: ") + eppscore_last_error(eng_));
     v.erase(std::find(v.begin(), v.end(), id));
     if (v.empty()) running_keys_.erase(k);
+  }
+
+  // The batch route with several profiles: the handler's first Pick per request on the host, then ONE
+  // eppscore_schedule_batch_profiles call per distinct set of picked profiles (one hash pass for all of the set's profiles), then
+  // ProcessResults.  A handler that asks for a second round gets that request's error.
+  std::vector<BatchItem> ScheduleBatchProfiles(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
+    const int R = (int)requests.size(), M = (int)endpoints.size(), P = (int)cfg_.Profiles.size();
+    std::vector<BatchItem> out((size_t)R);
+    last_hashes_.clear();
+    last_nh_.clear();
+    if (R == 0) return out;
+    std::vector<std::string> names;
+    for (const auto& np : cfg_.Profiles) names.push_back(np.first);
+    std::vector<unsigned> sets((size_t)R, 0u);
+    for (int r = 0; r < R; r++)
+      for (const std::string& n : cfg_.Handler->Pick(requests[r], names, {})) {
+        const auto it = std::find(names.begin(), names.end(), n);
+        if (it == names.end()) out[r].error = "profile '" + n + "' is not defined";
+        else sets[r] |= 1u << (it - names.begin());
+      }
+    std::vector<int> ids;
+    int Mx = 0;
+    if (M > 0) {
+      MapIds(endpoints, &ids, &Mx);
+      if (Mx > cfg_.MaxEndpoints) throw SchedulingError("more endpoints than SchedulerConfig.MaxEndpoints");
+    }
+    const int mw = (Mx + 31) / 32;
+    if (M > 0) {
+      for (int p = 0; p < P; p++) {  // the request-independent filters: each profile's endpoint subset, applied with the snapshot
+        const auto& keep = cfg_.Profiles[(size_t)p].second.endpoint_subset();
+        std::vector<uint32_t> row((size_t)std::max(mw, 1), 0u);
+        if (keep)
+          for (int m = 0; m < M; m++)
+            if (keep(endpoints[(size_t)m])) row[(size_t)ids[m] >> 5] |= 1u << (ids[m] & 31);
+        if (eppscore_set_profile_endpoints(eng_, p, keep ? row.data() : nullptr, mw) != EPPSCORE_OK)
+          throw SchedulingError(std::string("eppscore_set_profile_endpoints: ") + eppscore_last_error(eng_));
+      }
+      PackSnapshot(endpoints, ids, Mx);
+    }
+    std::vector<int> pos_of_id((size_t)Mx, -1);
+    for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
+    int block_tokens = cfg_.Prefix.BlockSizeTokens;
+    if (M > 0 && cfg_.Prefix.AutoTune && endpoints[0].GetMetrics()->CacheBlockSize > 0) block_tokens = endpoints[0].GetMetrics()->CacheBlockSize;
+    int max_blocks = cfg_.Prefix.MaxPrefixBlocksToMatch;
+    if (cfg_.Prefix.MaxPrefixTokensToMatch > 0 && block_tokens > 0) max_blocks = cfg_.Prefix.MaxPrefixTokensToMatch / block_tokens;
+    const bool want_prefix = max_blocks > 0 && block_tokens > 0;
+    last_stride_ = want_prefix ? max_blocks : 1;
+    last_nh_.assign((size_t)R, 0);
+    last_hashes_.assign((size_t)R * last_stride_, 0);
+    if (inflight_) {
+      last_size_.resize((size_t)R);
+      last_hint_.resize((size_t)R);
+      last_chars_.resize((size_t)R);
+      for (int r = 0; r < R; r++) EstimateInputs(requests[r], &last_size_[r], &last_hint_[r], &last_chars_[r]);
+    }
+    // every profile's result per request (empty TargetEndpoints: the profile ran and found no endpoint)
+    std::vector<std::map<std::string, ProfileRunResult>> got((size_t)R);
+    std::vector<unsigned> distinct;
+    for (int r = 0; r < R; r++)
+      if (out[r].error.empty() && sets[r] && std::find(distinct.begin(), distinct.end(), sets[r]) == distinct.end()) distinct.push_back(sets[r]);
+    for (unsigned S : distinct) {
+      if (M == 0) break;  // no endpoints: every profile fails (scheduler_profile.go:119-121)
+      std::vector<int> rows;
+      for (int r = 0; r < R; r++)
+        if (out[r].error.empty() && sets[r] == S) rows.push_back(r);
+      const int n = (int)rows.size();
+      std::vector<uint8_t> bytes;
+      std::vector<int64_t> off((size_t)n + 1, 0);
+      std::vector<int32_t> len((size_t)n), adapter((size_t)n);
+      std::vector<uint64_t> seed((size_t)n), hashes((size_t)n * last_stride_, 0);
+      std::vector<uint16_t> nh((size_t)n, 0);
+      for (int i = 0; i < n; i++) {
+        const InferenceRequest& q = requests[(size_t)rows[i]];
+        while (bytes.size() % 16) bytes.push_back(0);  // 16-byte aligned starts: the fast hash path
+        off[i] = (int64_t)bytes.size();
+        len[i] = (int32_t)q.Prompt.size();
+        bytes.insert(bytes.end(), q.Prompt.begin(), q.Prompt.end());
+        seed[i] = eppscore_model_seed(q.TargetModel.data(), q.TargetModel.size(), q.CacheSalt.data(), q.CacheSalt.size());
+        auto it = adapter_ids_.find(q.TargetModel);
+        adapter[i] = it == adapter_ids_.end() ? -1 : it->second;
+      }
+      off[n] = (int64_t)bytes.size();
+      bytes.resize(bytes.size() + 64, 0);
+      std::vector<int> prof;
+      for (int p = 0; p < P; p++)
+        if (S & (1u << p)) prof.push_back(p);
+      const int nr = (int)prof.size();
+      std::vector<std::vector<uint32_t>> masks((size_t)nr);
+      std::vector<std::vector<int32_t>> pick((size_t)nr, std::vector<int32_t>((size_t)n)), ties = pick;
+      std::vector<std::vector<double>> score((size_t)nr, std::vector<double>((size_t)n));
+      std::vector<eppscore_profile_run> runs((size_t)nr);
+      for (int k = 0; k < nr; k++) {
+        const auto& filters = cfg_.Profiles[(size_t)prof[k]].second.filters();
+        eppscore_profile_run& x = runs[(size_t)k];
+        x = eppscore_profile_run{};
+        x.struct_size = sizeof(x);
+        x.profile = prof[k];
+        if (!filters.empty() || Mx != M) {  // host filters and rows without an endpoint in this list
+          masks[k].assign((size_t)n * mw, 0u);
+          std::vector<int> all((size_t)M);
+          for (int m = 0; m < M; m++) all[m] = m;
+          for (int i = 0; i < n; i++) {
+            std::vector<int> cand = all;
+            for (auto& f : filters) {
+              cand = f->Filter_(requests[(size_t)rows[i]], endpoints, cand);
+              if (cand.empty()) break;
+            }
+            for (int m : cand) masks[k][(size_t)i * mw + (ids[m] >> 5)] |= 1u << (ids[m] & 31);
+          }
+          x.cand_mask = masks[k].data();
+        }
+        x.pick = pick[k].data();
+        x.pick_score = score[k].data();
+        x.tie_count = ties[k].data();
+      }
+      eppscore_batch b{};
+      b.struct_size = sizeof(b);
+      b.R = n;
+      b.prompt_bytes = want_prefix ? bytes.data() : nullptr;
+      b.prompt_off = off.data();
+      b.prompt_len = len.data();
+      b.model_seed = seed.data();
+      b.block_chars = block_tokens * 4;
+      b.max_blocks = max_blocks;
+      b.adapter_id = adapter.data();
+      b.total_blocks = nh.data();
+      b.hashes_out = want_prefix ? hashes.data() : nullptr;
+      if (eppscore_schedule_batch_profiles(eng_, &b, nr, runs.data()) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_schedule_batch_profiles: ") + eppscore_last_error(eng_));
+      for (int i = 0; i < n; i++) {
+        const int r = rows[i];
+        last_nh_[(size_t)r] = nh[i];
+        std::copy(hashes.begin() + (size_t)i * last_stride_, hashes.begin() + (size_t)(i + 1) * last_stride_,
+                  last_hashes_.begin() + (size_t)r * last_stride_);
+        for (int k = 0; k < nr; k++) {
+          ProfileRunResult& pr = got[(size_t)r][names[(size_t)prof[k]]];
+          const int32_t id = pick[k][i];
+          if (id < 0) continue;
+          if (id >= Mx || pos_of_id[(size_t)id] < 0) throw SchedulingError("engine picked an endpoint that is not in the candidate list");
+          ScoredEndpoint se;
+          se.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)id]];
+          se.Index = pos_of_id[(size_t)id];
+          se.Score = score[k][i];
+          se.TieCount = ties[k][i];
+          pr.TargetEndpoints.push_back(se);
+        }
+      }
+    }
+    for (int r = 0; r < R; r++) {
+      if (!out[r].error.empty()) continue;
+      std::map<std::string, const ProfileRunResult*> res;
+      for (int p = 0; p < P; p++) {
+        if (!(sets[r] & (1u << p))) continue;
+        auto it = got[(size_t)r].find(names[(size_t)p]);
+        res[names[(size_t)p]] = (it != got[(size_t)r].end() && !it->second.TargetEndpoints.empty()) ? &it->second : nullptr;
+      }
+      if (!cfg_.Handler->Pick(requests[r], names, res).empty()) {
+        out[r].error = "multi-round profile handlers are not supported by the batch route";
+        continue;
+      }
+      try {
+        out[r].result = cfg_.Handler->ProcessResults(requests[r], res);
+      } catch (const SchedulingError& ex) {
+        out[r].error = ex.what();
+      }
+    }
+    last_endpoints_ = &endpoints;
+    last_ids_ = ids;
+    last_rows_ = Mx;
+    return out;
+  }
+
+  // PreRequest with several profiles: the primary profile's target, then the "prefill" profile's, recorded in the prefix index
+  // in one commit per request in that order (approximateprefix/plugin.go:177-197); the inflight-load-producer counts the
+  // request on every profile's target (inflightload/producer.go:101-120).
+  void PreRequestProfiles(const std::vector<BatchItem>& results) {
+    const int R = (int)results.size();
+    const bool has_prefill = std::any_of(cfg_.Profiles.begin(), cfg_.Profiles.end(), [](const auto& np) { return np.first == "prefill"; });
+    std::vector<int32_t> primary((size_t)R, -1), prefill((size_t)R, -1);
+    std::vector<int32_t> load_ep;
+    std::vector<int> load_req;
+    auto id_of = [&](const ProfileRunResult& pr) {
+      return pr.TargetEndpoints.empty() ? -1 : last_ids_[(size_t)pr.TargetEndpoints[0].Index];
+    };
+    for (int r = 0; r < R; r++) {
+      if (!results[r].error.empty()) continue;
+      const SchedulingResult& sr = results[r].result;
+      for (const auto& kv : sr.ProfileResults) {
+        const int32_t id = id_of(kv.second);
+        if (id < 0) continue;
+        if (kv.first == sr.PrimaryProfileName) primary[r] = id;
+        else if (kv.first == "prefill") prefill[r] = id;
+        load_ep.push_back(id);
+        load_req.push_back(r);
+      }
+    }
+    if (!last_hashes_.empty()) {
+      std::vector<int32_t> cap((size_t)last_rows_, 0);
+      for (size_t m = 0; m < last_endpoints_->size(); m++)  // makeserver, plugin.go:207-216
+        cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks > 0) ? (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks : 0;
+      const int32_t* picks[2] = {primary.data(), prefill.data()};
+      if (eppscore_commit_picks_profiles(eng_, R, has_prefill ? 2 : 1, picks, last_hashes_.data(), last_nh_.data(), last_stride_, cap.data(),
+                                         0, 0, nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_commit_picks_profiles: ") + eppscore_last_error(eng_));
+    }
+    if (inflight_ && (int)last_size_.size() == R && !load_ep.empty()) {
+      std::vector<int64_t> est((size_t)R), tok(load_ep.size());
+      if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+      for (size_t i = 0; i < load_ep.size(); i++) tok[i] = est[(size_t)load_req[i]];
+      if (eppscore_inflight_add(eng_, (int32_t)load_ep.size(), 0, load_ep.data(), tok.data(), nullptr) != EPPSCORE_OK)
+        throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
+    }
+  }
+
+  // ResponseBody releases for a multi-profile result: the "prefill" profile's target at start of stream, the others at its end
+  // (inflightload/producer.go:137-160).
+  void ReleaseProfiles(const InferenceRequest& request, const SchedulingResult& result, bool prefill) {
+    if (!inflight_) return;
+    std::vector<int32_t> eps;
+    for (const auto& kv : result.ProfileResults) {
+      if ((kv.first == "prefill") != prefill || kv.second.TargetEndpoints.empty() || !kv.second.TargetEndpoints[0].Endpoint_) continue;
+      const int32_t id = ServerId(kv.second.TargetEndpoints[0].Endpoint_->GetMetadata()->NamespacedName_.String());
+      if (id >= 0) eps.push_back(id);
+    }
+    if (eps.empty()) return;
+    int64_t size = 0, est = 0;
+    int32_t hint = -1, chars = 0;
+    EstimateInputs(request, &size, &hint, &chars);
+    if (eppscore_estimate_tokens(eng_, 1, 0, &size, &hint, &chars, &est, nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+    std::vector<int64_t> tok(eps.size(), est);
+    if (eppscore_inflight_release(eng_, (int32_t)eps.size(), 0, eps.data(), tok.data(), nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_inflight_release: ") + eppscore_last_error(eng_));
+  }
+
+  // Stable endpoint ids of a candidate list (see ScheduleBatch): ids[i] is endpoint i's row, *rows the number of rows; true when
+  // the list is exactly ids 0..M-1 in order.
+  bool MapIds(const std::vector<Endpoint>& endpoints, std::vector<int>* ids_out, int* rows) {
+    const int M = (int)endpoints.size();
+    std::vector<int>& ids = *ids_out;
+    ids.assign((size_t)M, 0);
+    int Mx = 0;
+    bool identity = true;
+    {
+      std::vector<int> seen;
+      for (int m = 0; m < M; m++) {
+        ids[m] = IdOf(endpoints[(size_t)m].GetMetadata()->NamespacedName_.String());
+        Mx = std::max(Mx, ids[m] + 1);
+        identity = identity && ids[m] == m;
+      }
+      seen.assign((size_t)Mx, 0);
+      bool dup = false;
+      for (int m = 0; m < M; m++) dup = dup || seen[(size_t)ids[m]]++ > 0;
+      if (dup) {  // the same server twice in one list: positions are the only usable ids for this batch
+        for (int m = 0; m < M; m++) ids[m] = m;
+        Mx = M;
+        identity = true;
+      }
+    }
+    *rows = Mx;
+    return identity;
   }
 
   // SimpleTokenEstimator's inputs for one request (eppscore_estimate_tokens): the body is always present here

@@ -131,6 +131,40 @@ typedef struct eppscore_config {
   double filter_param[EPPSCORE_MAX_FILTERS][3];
 } eppscore_config;
 
+/* ---- scheduler profiles (scheduler.go:54-102: profileHandler.Pick -> profile.Run per picked profile -> ProcessResults) ----
+ * An engine serves up to EPPSCORE_MAX_PROFILES profiles over ONE snapshot, one prefix index and one set of producer state.
+ * Profile 0 is the one given to eppscore_create; every call that names no profile serves profile 0.  A profile carries the
+ * per-profile fields of eppscore_config, validated by the same rules; everything else stays engine-wide: tie mode, block size,
+ * capacities, token-load threshold, and the latency parameters (the predicted-latency producer is one per engine, so every
+ * profile with a latency scorer reads the same eppscore_set_latency_params).
+ * The stochastic pickers and the seeded-random tie break of profile p draw with tie_seed ^ (p * 0x9E3779B97F4A7C15) (unsigned
+ * 64-bit product), so two profiles do not draw the same numbers; profile 0 draws with tie_seed itself. */
+#define EPPSCORE_MAX_PROFILES 4
+typedef struct eppscore_profile {
+  uint32_t struct_size;
+  int32_t n_scorers;
+  int32_t scorer_kind[EPPSCORE_MAX_SCORERS];
+  double scorer_weight[EPPSCORE_MAX_SCORERS];
+  int32_t pick_mode;
+  int32_t n_filters;
+  int32_t filter_kind[EPPSCORE_MAX_FILTERS];
+  double filter_param[EPPSCORE_MAX_FILTERS][3];
+} eppscore_profile;
+
+/* One profile's share of eppscore_schedule_batch_profiles: its host-side filter result and its outputs, all [R] (or R x M /
+ * R x ceil(M/32) like the eppscore_batch fields of the same name), where the batch's location says. */
+typedef struct eppscore_profile_run {
+  uint32_t struct_size;
+  int32_t profile;             /* id from eppscore_add_profile, 0 = the create profile */
+  const uint32_t *cand_mask;   /* optional [R*ceil(M/32)]: this profile's host Filters; ANDed with its endpoint subset */
+  int32_t *pick;               /* [R], -1 = no candidate */
+  double *pick_score;          /* [R] */
+  int32_t *tie_count;          /* [R] */
+  double *scores_out;          /* optional [R*M] */
+  double *pred_out;            /* optional [R*M*2] */
+  uint32_t *filter_mask_out;   /* optional [R*ceil(M/32)] */
+} eppscore_profile_run;
+
 /* Latency fold-in parameters: the cached Bayesian-ridge coefficients (MetricsResponse.Coefficients,
  * sidecars/latencypredictorasync/prediction.go:164-194), the producer's Config (predictedlatency/plugin.go:118-136)
  * and the latency-scorer's Config (scorer/latency/plugin.go:59-90).  Takes effect at the next eppscore_set_snapshot
@@ -305,6 +339,30 @@ int32_t eppscore_schedule_batch_topk(struct eppscore_engine *e, const eppscore_b
  * ERR_INVALID: k outside [1, max_endpoints], a wrong struct_size or NULL arrays. */
 int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppscore_batch *b, const eppscore_topk *t);
 
+/* ---- several scheduler profiles (see eppscore_profile) ---- */
+/* Adds a profile; *id_out receives its id (1, 2, ...).  With a snapshot present the profile is prepared for it at once, on the
+ * engine stream (a profile with a latency scorer on an engine that had none is usable from the next eppscore_set_snapshot).
+ * ERR_CAPACITY past EPPSCORE_MAX_PROFILES, ERR_INVALID for a bad profile or under CUDA-graph capture. */
+int32_t eppscore_add_profile(struct eppscore_engine *e, const eppscore_profile *p, int32_t *id_out);
+/* A request-independent Filter at the head of the profile's filter chain (e.g. the prefill / decode role label): mask is a host
+ * bitmask over endpoint rows in natural order, `words` 32-bit words (bits past max_endpoints ignored, missing words are 0);
+ * NULL = every endpoint (the default).  Takes effect at the next eppscore_set_snapshot, like eppscore_set_latency_params.  A
+ * request's candidates are then subset ∧ cand_mask ∧ the device filters; the queue / running min/max run over those
+ * candidates (queue.go:79-91); an empty candidate set gives pick -1.  On profile 0 it applies to eppscore_schedule_batch and
+ * its top-k forms as well.  Batches without a cand_mask stay on the sparse path; every other route scores the profile through
+ * the masked kernels on rows subset ∧ cand_mask built on the device.  ERR_INVALID under CUDA-graph capture.  The call first
+ * waits for the last eppscore_set_snapshot's copy of the previous subset.  A set_snapshot captured into a CUDA graph copies the
+ * subset as it stands when the graph is REPLAYED, not when it was captured. */
+int32_t eppscore_set_profile_endpoints(struct eppscore_engine *e, int32_t profile, const uint32_t *mask, int32_t words);
+/* Schedule.Run of several profiles for one batch: the prompts are hashed (and the prefix index probed) ONCE, then each run's
+ * Filter -> Score -> Pick follows on the same stream.  b carries the request inputs and the profile-independent outputs
+ * (total_blocks, match_blocks, hashes_out); its pick / pick_score / tie_count / cand_mask / scores_out / pred_out /
+ * filter_mask_out must be NULL.  1 <= n_runs <= EPPSCORE_MAX_PROFILES, each profile at most once.  Locations, chunking,
+ * request_base shards, device-batch ordering and CUDA-graph capture behave as in eppscore_schedule_batch.  Top-k lists
+ * (maxNumOfEndpoints > 1) are not part of this call.  ERR_INVALID otherwise. */
+int32_t eppscore_schedule_batch_profiles(struct eppscore_engine *e, const eppscore_batch *b, int32_t n_runs,
+                                         const eppscore_profile_run *runs);
+
 /* ---- stand-alone stages (same kernels; for parity tests and hosts that only want one stage) ---- */
 /* hashPrompt for R prompts (hashing.go:34-98). hashes_out [R*max_blocks], n_hashes_out [R]. */
 int32_t eppscore_hash_prompts(struct eppscore_engine *e, int32_t R, int32_t location, const uint8_t *prompt_bytes,
@@ -342,7 +400,16 @@ int32_t eppscore_commit_picks(struct eppscore_engine *e, int32_t R, const int32_
 int32_t eppscore_commit_picks_device(struct eppscore_engine *e, int32_t R, const int32_t *pick, const uint64_t *hashes,
                                      const uint16_t *n_hashes, int32_t hash_stride, const int32_t *lru_capacity,
                                      int64_t touch_bound, void *stream);
-/* indexer.Add for one server (tests, the "prefill" profile's pick plugin.go:180-184). */
+/* PreRequest with several picks per request (plugin.go:177-197: the primary profile's pick, then the "prefill" profile's):
+ * indexer.Add(hashes[r], picks[p][r]) for r ascending and, within r, p ascending, in one commit.  picks: n_picks pointers
+ * (host array of pointers) to [R] arrays where `location` says (0 host, 1 device); pick -1 is skipped, the same endpoint twice
+ * in one request is two Adds.  location 1 is asynchronous on `stream` with eppscore_commit_picks_device's touch_bound
+ * contract (a bound on Σ n_hashes over all picks); location 0 ignores stream and touch_bound.  n_picks = 1 equals
+ * eppscore_commit_picks[_device].  1 <= n_picks <= EPPSCORE_MAX_PROFILES. */
+int32_t eppscore_commit_picks_profiles(struct eppscore_engine *e, int32_t R, int32_t n_picks, const int32_t *const *picks,
+                                       const uint64_t *hashes, const uint16_t *n_hashes, int32_t hash_stride,
+                                       const int32_t *lru_capacity, int32_t location, int64_t touch_bound, void *stream);
+/* indexer.Add for one server (tests). */
 int32_t eppscore_prefix_add(struct eppscore_engine *e, const uint64_t *hashes, int32_t n, int32_t endpoint,
                             int32_t lru_capacity);
 /* Raw deltas for hosts that keep their own LRU: op 0 = insert (hash,endpoint), 1 = evict; applied in order. */
