@@ -60,6 +60,7 @@ struct eppscore_engine {
   Geo geo{};
   int32_t A_cap = 64;
   Event ev_snapshot, ev_table, ev_caller;
+  Event ev_subset;  // behind the last set_snapshot outside a capture: its copies of the profiles' next subset rows are done
   cudaStream_t snapshot_stream = nullptr;        // stream the last snapshot preparation ran on
   unsigned long long snapshot_capture_id = 0;    // != 0: ev_snapshot was recorded inside that CUDA-graph capture
   std::string err;
@@ -1016,6 +1017,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   // every failure below frees what was allocated before it (the engine's members own it)
   CK(nullptr, make(ep->stream));
   CK(nullptr, make(ep->ev_snapshot));
+  CK(nullptr, make(ep->ev_subset));
   CK(nullptr, make(ep->ev_table));
   // endpoint tile buffers
   const size_t mp = (size_t)ep->geo.Mpad;
@@ -1288,6 +1290,8 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
     }
     profile_pa(e, p);
   }
+  // (inside a capture the copies run at each replay, and eppscore_set_profile_endpoints leaves ordering against those to the caller)
+  if (!capturing) CK(e, cudaEventRecord(e->ev_subset, st));
   if ((rc = prepare_snapshot(e, st, (1u << e->n_prof) - 1)) != EPPSCORE_OK) return rc;
   if (!capturing && !on_device) CK(e, cudaStreamSynchronize(st));  // host arrays may be reused by the caller
   e->have_snapshot = true;
@@ -1645,15 +1649,14 @@ int32_t eppscore_set_profile_endpoints(eppscore_engine* e, int32_t profile, cons
   CK(e, cudaSetDevice(e->device));
   if (is_capturing(e->stream)) return fail(e, EPPSCORE_ERR_INVALID, "set_profile_endpoints under CUDA-graph capture");
   Profile& P = e->prof[profile];
-  if (!mask) {
-    P.next_subset = false;
-    return EPPSCORE_OK;
-  }
-  // the next rows are copied by set_snapshot on its stream: the last one (on whatever stream) has finished copying them
-  CK(e, cudaEventSynchronize(e->ev_snapshot));
+  // the next rows are copied by set_snapshot on its stream: the last one outside a capture (on whatever stream) has finished
+  // copying them.  Not ev_snapshot: that may have been recorded inside a capture, and such an event cannot be waited for.
+  CK(e, cudaEventSynchronize(e->ev_subset));
+  // NULL writes rows with every endpoint: a set_snapshot captured while the profile had a subset copies the next rows at each
+  // replay, and then sees every endpoint
   const int32_t nw = e->geo.Mpad / 32;
-  std::vector<uint32_t> nat((size_t)nw, 0u), perm((size_t)e->geo.row_words, 0u);
-  for (int32_t w = 0; w < nw && w < words; w++) nat[(size_t)w] = mask[w];
+  std::vector<uint32_t> nat((size_t)nw, mask ? 0u : ~0u), perm((size_t)e->geo.row_words, 0u);
+  for (int32_t w = 0; mask && w < nw && w < words; w++) nat[(size_t)w] = mask[w];
   const uint32_t max_ep = (uint32_t)e->cfg.max_endpoints;
   for (uint32_t m = 0; m < (uint32_t)e->geo.Mpad; m++) {
     const bool in = m < max_ep && ((nat[m >> 5] >> (m & 31)) & 1u);
@@ -1668,7 +1671,7 @@ int32_t eppscore_set_profile_endpoints(eppscore_engine* e, int32_t profile, cons
   CK(e, cudaMemcpyAsync(P.next_nat.p, nat.data(), nat.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(e, cudaMemcpyAsync(P.next_perm.p, perm.data(), perm.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(e, cudaStreamSynchronize(e->stream));
-  P.next_subset = true;
+  P.next_subset = mask != nullptr;
   return EPPSCORE_OK;
 }
 

@@ -351,8 +351,11 @@ int32_t eppscore_add_profile(struct eppscore_engine *e, const eppscore_profile *
  * candidates (queue.go:79-91); an empty candidate set gives pick -1.  On profile 0 it applies to eppscore_schedule_batch and
  * its top-k forms as well.  Batches without a cand_mask stay on the sparse path; every other route scores the profile through
  * the masked kernels on rows subset ∧ cand_mask built on the device.  ERR_INVALID under CUDA-graph capture.  The call first
- * waits for the last eppscore_set_snapshot's copy of the previous subset.  A set_snapshot captured into a CUDA graph copies the
- * subset as it stands when the graph is REPLAYED, not when it was captured. */
+ * waits for the last eppscore_set_snapshot made outside a capture to finish copying the previous subset.
+ * A set_snapshot captured into a CUDA graph while the profile had a subset copies the subset as it stands when the graph is
+ * REPLAYED, not when it was captured: the call may follow such a capture (it does not wait for the graph), and NULL then makes
+ * the next replay see every endpoint.  A profile captured without a subset stays without one in that graph; a subset set
+ * later applies from the next set_snapshot outside it.  Do not replay such a graph while this call runs. */
 int32_t eppscore_set_profile_endpoints(struct eppscore_engine *e, int32_t profile, const uint32_t *mask, int32_t words);
 /* Schedule.Run of several profiles for one batch: the prompts are hashed (and the prefix index probed) ONCE, then each run's
  * Filter -> Score -> Pick follows on the same stream.  b carries the request inputs and the profile-independent outputs
