@@ -111,6 +111,8 @@ ABI_SYMBOLS = [
     ("eppscore_add_profile", C.c_int32, [_P, C.POINTER(Profile), C.POINTER(C.c_int32)]),
     ("eppscore_set_profile_endpoints", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_schedule_batch_profiles", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun)]),
+    ("eppscore_schedule_batch_profiles_topk", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun),
+                                                          C.POINTER(TopK)]),
     ("eppscore_hash_prompts", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     ("eppscore_count_fields", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
     ("eppscore_hash_prompts_host", C.c_int32, [C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32]),

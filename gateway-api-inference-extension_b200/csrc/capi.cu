@@ -370,6 +370,10 @@ struct DevRun {
   double* scores_out;
   double* pred_out;
   uint32_t* filter_mask_out;
+  int32_t topk;          // > 0: topk_m / topk_score [R*topk] are written
+  int32_t* topk_m;
+  double* topk_score;
+  bool wide;             // the lists come from topk_select_kernel over the run's score rows (schedule_wide)
 };
 
 struct DevBatch {  // all device pointers
@@ -392,9 +396,6 @@ struct DevBatch {  // all device pointers
   uint16_t* match_blocks;   // profile-independent outputs, written by the kernels of run 0
   uint16_t* total_blocks;
   uint64_t* hashes_out;
-  int32_t topk;          // > 0 (single run only): topk_m / topk_score [R*topk] are written
-  int32_t* topk_m;
-  double* topk_score;
   int32_t n_runs;
   DevRun run[EPPSCORE_MAX_PROFILES];
 };
@@ -451,12 +452,12 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
     x.pick_score = run.pick_score;
     x.tie_count = run.tie_count;
     x.scores_out = run.scores_out;
+    x.topk = run.topk;
+    x.topk_m = run.topk_m;
+    x.topk_score = run.topk_score;
     if (i == 0) {
       x.match_out = b.match_blocks;
       x.total_out = b.total_blocks;
-      x.topk = b.topk;
-      x.topk_m = b.topk_m;
-      x.topk_score = b.topk_score;
     }
     if (cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY)) {
       if (dense) return fail(e, EPPSCORE_ERR_INVALID, "the latency scorer is not available on dense feature rows");
@@ -637,7 +638,7 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
 constexpr unsigned long long kWideSliceBytes = EPP_WIDE_SLICE_BYTES;
 
 // Rows [base, base + n) of a device batch (every per-request array offset; prompt_bytes stays, the offsets index into it).
-DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t mw, size_t mb, size_t k) {
+DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t mw, size_t mb) {
   DevBatch q = d;
   q.R = n;
   q.request_base = d.request_base + base;
@@ -664,40 +665,44 @@ DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t
     y.pick_score = off(x.pick_score, 1);
     y.tie_count = off(x.tie_count, 1);
     y.scores_out = off(x.scores_out, M);
+    y.topk_m = off(x.topk_m, (size_t)x.topk);
+    y.topk_score = off(x.topk_score, (size_t)x.topk);
   }
   q.match_blocks = off(d.match_blocks, M);
   q.total_blocks = off(d.total_blocks, 1);
   q.hashes_out = off(d.hashes_out, mb);
-  q.topk_m = off(d.topk_m, k);
-  q.topk_score = off(d.topk_score, k);
   return q;
 }
 
-// eppscore_schedule_batch_topk_wide on device buffers, asynchronous on `s`, in two steps per slice of rows:
-//   1. the batch's scores_out route (the diagnostics variants of the full-matrix and generic dense kernels) writes the slice's
-//      weighted scores, NaN for non-candidates, into wide_scores[slot] (or into the caller's scores_out, which then needs no
-//      slicing), together with pick / pick_score / tie_count;
-//   2. topk_select_kernel turns the rows into the lists d.topk_m / d.topk_score [R][k].
-// The slices run in order on `s` (the scratch holds one slice), whatever the slicing keys 5 / 6 say.
-int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStream_t s, Scratch& sc, int slot) {
+// eppscore_schedule_batch_topk_wide, and a batch of eppscore_schedule_batch_profiles_topk with a run of k > EPPSCORE_MAX_TOPK,
+// on device buffers, asynchronous on `s`, in two steps per slice of rows:
+//   1. one schedule_device over every run: a wide run takes the scores_out route (the diagnostics variants of the full-matrix
+//      and generic dense kernels), which writes the slice's weighted scores, NaN for non-candidates, into the run's part of
+//      wide_scores[slot] (or into the run's own scores_out, which then needs no slicing), together with pick / pick_score /
+//      tie_count; the other runs compute what they compute outside this function, register lists included;
+//   2. per wide run, topk_select_kernel turns its rows into its lists [R][k], with its profile's pick mode and seed.
+// The scratch holds wide_rows rows whatever the runs: with n wide runs on it, a slice is wide_rows / n rows per run, so a graph
+// captured after the first wide call keeps pointing at live memory.  The slices run in order on `s` (the scratch holds one
+// slice), whatever the slicing keys 5 / 6 say.
+int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, int slot) {
   if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch before set_snapshot");
   if (d.R <= 0) return EPPSCORE_OK;
   const size_t M = (size_t)e->M, mw = (M + 31) / 32;
   const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
-  const Profile& P = e->prof[d.run[0].profile];
-  auto select = [&](const DevBatch& q, const double* scores) -> int32_t {
+  auto select = [&](const DevBatch& q, const DevRun& run) -> int32_t {
+    const Profile& P = e->prof[run.profile];
     TopKSelectArgs t{};
-    t.scores = scores;
+    t.scores = run.scores_out;
     t.R = q.R;
     t.M = e->M;
-    t.k = k;
+    t.k = run.topk;
     t.pick_mode = P.cfg.pick_mode;
     t.tie_mode = P.cfg.tie_mode;
     t.seed_lo = (uint32_t)P.cfg.tie_seed;
     t.seed_hi = (uint32_t)(P.cfg.tie_seed >> 32);
     t.request_base = q.request_base;
-    t.out_m = q.topk_m;
-    t.out_s = q.topk_score;
+    t.out_m = run.topk_m;
+    t.out_s = run.topk_score;
     const int launched = launch_topk_select(t, s);
     if (launched < 0) {
       cudaGetLastError();
@@ -707,13 +712,25 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStre
     CK(e, cudaGetLastError());
     return EPPSCORE_OK;
   };
-  int32_t rc;
-  if (d.run[0].scores_out) {
-    DevBatch q = d;
-    q.topk = 0;
-    if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
-    return select(d, d.run[0].scores_out);
+  // step 1 with the wide runs' lists left to step 2, then step 2
+  auto run_slice = [&](const DevBatch& q) -> int32_t {
+    DevBatch x = q;
+    for (int i = 0; i < x.n_runs; i++)
+      if (x.run[i].wide) x.run[i].topk = 0;
+    int32_t rc = schedule_device(e, x, s, sc);
+    for (int i = 0; i < q.n_runs && rc == EPPSCORE_OK; i++)
+      if (q.run[i].wide) rc = select(q, q.run[i]);
+    return rc;
+  };
+  int32_t n_scratch = 0;  // wide runs whose rows go to the scratch
+  bool any_subset = false, any_lat = false;
+  for (int i = 0; i < d.n_runs; i++) {
+    const Profile& P = e->prof[d.run[i].profile];
+    if (d.run[i].wide && !d.run[i].scores_out) n_scratch++;
+    any_subset = any_subset || P.subset;
+    any_lat = any_lat || cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY);
   }
+  if (n_scratch == 0) return run_slice(d);
   DevBuf& buf = e->wide_scores[slot];
   if (!buf.p) {
     if (is_capturing(s))
@@ -728,14 +745,22 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, int32_t k, cudaStre
     CK(e, sc.s_hashes.reserve((size_t)e->wide_rows * mb * 8));
     CK(e, sc.s_nh.reserve((size_t)e->wide_rows * 2));
   }
-  if (d.prompt_bytes && !d.input_tokens && cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY)) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
-  if (P.subset) CK(e, sc.s_subset.reserve((size_t)e->wide_rows * mw * 4));
-  for (int32_t base = 0; base < d.R; base += e->wide_rows) {
-    DevBatch q = slice_rows(d, base, std::min(e->wide_rows, d.R - base), M, mw, (size_t)mb, (size_t)k);
-    q.topk = 0;
-    q.run[0].scores_out = buf.as<double>();
-    if ((rc = schedule_device(e, q, s, sc)) != EPPSCORE_OK) return rc;
-    if ((rc = select(q, q.run[0].scores_out)) != EPPSCORE_OK) return rc;
+  if (d.prompt_bytes && !d.input_tokens && any_lat) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
+  if (any_subset) CK(e, sc.s_subset.reserve((size_t)e->wide_rows * mw * 4));
+  // a run next to the wide ones may take the hash kernel's probe records
+  if (d.n_runs > 1 && d.prompt_bytes && !d.hashes_in && !d.hashes_out)
+    CK(e, sc.s_probe.reserve((size_t)e->wide_rows * sizeof(ProbeRec)));
+  // n_scratch parts of rows * M doubles must fit the wide_rows * Mpad of the scratch: a slice budget (EPP_WIDE_SLICE_BYTES) of
+  // fewer rows than wide runs cannot hold one row per run
+  if (e->wide_rows < n_scratch)
+    return fail(e, EPPSCORE_ERR_CAPACITY, "the wide score scratch holds fewer rows than the call has wide runs (EPP_WIDE_SLICE_BYTES)");
+  const int32_t rows = e->wide_rows / n_scratch;
+  for (int32_t base = 0; base < d.R; base += rows) {
+    DevBatch q = slice_rows(d, base, std::min(rows, d.R - base), M, mw, (size_t)mb);
+    for (int i = 0, j = 0; i < q.n_runs; i++)
+      if (q.run[i].wide && !d.run[i].scores_out) q.run[i].scores_out = buf.as<double>() + (size_t)(j++) * rows * M;
+    int32_t rc = run_slice(q);
+    if (rc != EPPSCORE_OK) return rc;
   }
   return EPPSCORE_OK;
 }
@@ -1302,21 +1327,22 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
 
 namespace {
 
-// eppscore_schedule_batch(_topk, _topk_wide, _profiles): the runs (profile + per-profile filter result and outputs) of one
-// batch; t == nullptr ⇒ no top-k lists (top-k: one run); wide: any k up to max_endpoints (schedule_wide)
+// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk): the runs (profile + per-profile filter result and
+// outputs) of one batch.  topk: [n_runs] validated lists, or nullptr for none; run i's list (k > 0) comes from the register
+// lists of the full-matrix kernels, or from schedule_wide when `wide` is set or k > EPPSCORE_MAX_TOPK.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
-                       const eppscore_topk* t, bool wide = false) {
-  if (t) {
-    if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
-    if (wide && (t->k < 1 || t->k > e->cfg.max_endpoints)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, max_endpoints]");
-    if (!wide && (t->k < 1 || t->k > EPPSCORE_MAX_TOPK)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
-    if (!t->endpoints || !t->scores) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
-  }
+                       const eppscore_topk* topk, bool wide = false) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
   int32_t rc = EPPSCORE_OK;
-  const int32_t tk = t ? t->k : 0;
+  int32_t tk[EPPSCORE_MAX_PROFILES] = {}, tk_sum = 0;  // per run k, and their sum
+  bool any_wide = false;
+  for (int i = 0; i < n_runs && topk; i++) {
+    tk[i] = topk[i].k;
+    tk_sum += tk[i];
+    any_wide = any_wide || (tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK));
+  }
   DevBatch d{};
   d.R = b->R;
   d.request_base = b->request_base;
@@ -1324,7 +1350,11 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   d.block_chars = b->block_chars;
   d.max_blocks = b->max_blocks;
   d.n_runs = n_runs;
-  for (int i = 0; i < n_runs; i++) d.run[i].profile = runs[i].profile;
+  for (int i = 0; i < n_runs; i++) {
+    d.run[i].profile = runs[i].profile;
+    d.run[i].topk = tk[i];
+    d.run[i].wide = tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK);
+  }
   if (b->location == 1) {
     d.prompt_bytes = b->prompt_bytes;
     d.prompt_off = b->prompt_off;
@@ -1341,9 +1371,6 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     d.match_blocks = b->match_blocks;
     d.total_blocks = b->total_blocks;
     d.hashes_out = b->hashes_out;
-    d.topk = tk;
-    d.topk_m = t ? t->endpoints : nullptr;
-    d.topk_score = t ? t->scores : nullptr;
     bool per_pair = false;  // R x M outputs or masks on some run
     for (int i = 0; i < n_runs; i++) {
       const eppscore_profile_run& x = runs[i];
@@ -1355,11 +1382,15 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       y.scores_out = x.scores_out;
       y.pred_out = x.pred_out;
       y.filter_mask_out = x.filter_mask_out;
+      if (tk[i]) {
+        y.topk_m = topk[i].endpoints;
+        y.topk_score = topk[i].scores;
+      }
       per_pair = per_pair || x.cand_mask || x.scores_out || x.pred_out || x.filter_mask_out;
     }
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
-    if (wide) {
-      if ((rc = schedule_wide(e, d, tk, cs, e->sc[0], 0)) != EPPSCORE_OK) return rc;
+    if (any_wide) {
+      if ((rc = schedule_wide(e, d, cs, e->sc[0], 0)) != EPPSCORE_OK) return rc;
       return pending_record(e, cs);
     }
     // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here)
@@ -1395,10 +1426,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
         q.run[i].pick = d.run[i].pick + base;
         q.run[i].pick_score = d.run[i].pick_score + base;
         q.run[i].tie_count = d.run[i].tie_count + base;
-      }
-      if (tk) {
-        q.topk_m = d.topk_m + (size_t)base * tk;
-        q.topk_score = d.topk_score + (size_t)base * tk;
+        if (tk[i]) {
+          q.run[i].topk_m = d.run[i].topk_m + (size_t)base * tk[i];
+          q.run[i].topk_score = d.run[i].topk_score + (size_t)base * tk[i];
+        }
       }
       if (d.total_blocks) q.total_blocks = d.total_blocks + base;
       if (d.hashes_out) q.hashes_out = d.hashes_out + (size_t)base * mbk;
@@ -1435,8 +1466,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
   if (nstreams == 2 && (rc = pending_wait(e, e->stream2)) != EPPSCORE_OK) return rc;
   // pinned staging, per run: pick i32 | score f64 | tie i32, each [R]; then total u16 [R]; top-k endpoints i32 | scores f64,
-  // each [R*k]
-  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk, NR = (size_t)n_runs;
+  // each [R*Σk], run i's lists at R*tko[i]
+  size_t tko[EPPSCORE_MAX_PROFILES] = {};
+  for (int i = 1; i < n_runs; i++) tko[i] = tko[i - 1] + (size_t)tk[i - 1];
+  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk_sum, NR = (size_t)n_runs;
   const size_t o_score = (NR * RR * 4 + 7) & ~(size_t)7, o_tie = o_score + NR * RR * 8, o_total = o_tie + NR * RR * 4;
   const size_t o_tkm = (o_total + RR * 2 + 7) & ~(size_t)7, o_tks = (o_tkm + RK * 4 + 7) & ~(size_t)7, res_bytes = o_tks + RK * 8;
   CK(e, e->h_res.reserve(res_bytes));
@@ -1512,12 +1545,17 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       if (x.pred_out) y.pred_out = sc.s_pred.as<double>() + (size_t)i * R * M * 2;
       if (x.filter_mask_out) y.filter_mask_out = sc.s_fmask.as<uint32_t>() + (size_t)i * R * mw;
     }
-    if (tk) {  // [R*k]: small, like the picks (the chunks keep overlapping)
-      CK(e, sc.s_topk_m.reserve(R * tk * 4));
-      CK(e, sc.s_topk_s.reserve(R * tk * 8));
-      d.topk = tk;
-      d.topk_m = sc.s_topk_m.as<int32_t>();
-      d.topk_score = sc.s_topk_s.as<double>();
+    if (tk_sum) {  // [R*Σk]: small, like the picks (the chunks keep overlapping)
+      CK(e, sc.s_topk_m.reserve(R * tk_sum * 4));
+      CK(e, sc.s_topk_s.reserve(R * tk_sum * 8));
+      for (int i = 0; i < n_runs; i++)
+        if (tk[i]) {
+          DevRun& y = d.run[i];
+          y.topk = tk[i];
+          y.wide = tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK);
+          y.topk_m = sc.s_topk_m.as<int32_t>() + R * tko[i];
+          y.topk_score = sc.s_topk_s.as<double>() + R * tko[i];
+        }
     }
     if (b->match_blocks) {
       CK(e, sc.s_match.reserve(R * M * 2));
@@ -1535,7 +1573,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       hashes_dev = sc.s_hashes.as<uint64_t>();
       d.hashes_out = hashes_dev;
     }
-    rc = wide ? schedule_wide(e, d, tk, st, sc, ci & 1) : schedule_device(e, d, st, sc);
+    rc = any_wide ? schedule_wide(e, d, st, sc, ci & 1) : schedule_device(e, d, st, sc);
     if (rc != EPPSCORE_OK) return rc;
     for (int i = 0; i < n_runs; i++) {
       const eppscore_profile_run& x = runs[i];
@@ -1547,10 +1585,11 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       if (x.pred_out) CK(e, cudaMemcpyAsync(x.pred_out + (size_t)r0 * M * 2, y.pred_out, R * M * 16, cudaMemcpyDeviceToHost, st));
       if (x.filter_mask_out)
         CK(e, cudaMemcpyAsync(x.filter_mask_out + (size_t)r0 * mw, y.filter_mask_out, R * mw * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (tk) {
-      CK(e, cudaMemcpyAsync(hp_tkm + (size_t)r0 * tk, d.topk_m, R * tk * 4, cudaMemcpyDeviceToHost, st));
-      CK(e, cudaMemcpyAsync(hp_tks + (size_t)r0 * tk, d.topk_score, R * tk * 8, cudaMemcpyDeviceToHost, st));
+      if (tk[i]) {
+        const size_t o = RR * tko[i] + (size_t)r0 * tk[i];
+        CK(e, cudaMemcpyAsync(hp_tkm + o, y.topk_m, R * tk[i] * 4, cudaMemcpyDeviceToHost, st));
+        CK(e, cudaMemcpyAsync(hp_tks + o, y.topk_score, R * tk[i] * 8, cudaMemcpyDeviceToHost, st));
+      }
     }
     if (b->match_blocks) CK(e, cudaMemcpyAsync(b->match_blocks + (size_t)r0 * M, d.match_blocks, R * M * 2, cudaMemcpyDeviceToHost, st));
     if (b->total_blocks) CK(e, cudaMemcpyAsync(hp_total + r0, d.total_blocks, R * 2, cudaMemcpyDeviceToHost, st));
@@ -1564,10 +1603,11 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     if (runs[i].tie_count) memcpy(runs[i].tie_count, hp_tie + i * RR, RR * 4);
   }
   if (b->total_blocks) memcpy(b->total_blocks, hp_total, RR * 2);
-  if (tk) {
-    memcpy(t->endpoints, hp_tkm, RK * 4);
-    memcpy(t->scores, hp_tks, RK * 8);
-  }
+  for (int i = 0; i < n_runs; i++)
+    if (tk[i]) {
+      memcpy(topk[i].endpoints, hp_tkm + RR * tko[i], RR * tk[i] * 4);
+      memcpy(topk[i].scores, hp_tks + RR * tko[i], RR * tk[i] * 8);
+    }
   return EPPSCORE_OK;
 }
 
@@ -1575,6 +1615,12 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppscore_topk* t, bool wide = false) {
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  if (t) {
+    if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
+    if (wide && (t->k < 1 || t->k > e->cfg.max_endpoints)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, max_endpoints]");
+    if (!wide && (t->k < 1 || t->k > EPPSCORE_MAX_TOPK)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
+    if (!t->endpoints || !t->scores) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
+  }
   eppscore_profile_run run{};
   run.struct_size = sizeof(run);
   run.profile = 0;
@@ -1675,8 +1721,12 @@ int32_t eppscore_set_profile_endpoints(eppscore_engine* e, int32_t profile, cons
   return EPPSCORE_OK;
 }
 
-int32_t eppscore_schedule_batch_profiles(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs) {
-  if (!e) return EPPSCORE_ERR_INVALID;
+}  // extern "C"
+
+namespace {
+
+// the arguments eppscore_schedule_batch_profiles refuses
+int32_t check_profile_runs(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs) {
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
   if (b->pick || b->pick_score || b->tie_count || b->cand_mask || b->scores_out || b->pred_out || b->filter_mask_out)
     return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_profiles: per-profile batch fields belong to the runs (must be NULL)");
@@ -1690,7 +1740,36 @@ int32_t eppscore_schedule_batch_profiles(eppscore_engine* e, const eppscore_batc
     seen |= 1u << x.profile;
     if (!x.pick || !x.pick_score || !x.tie_count) return fail(e, EPPSCORE_ERR_INVALID, "profile_run: pick/pick_score/tie_count required");
   }
+  return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_schedule_batch_profiles(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  const int32_t rc = check_profile_runs(e, b, n_runs, runs);
+  if (rc != EPPSCORE_OK) return rc;
   return schedule_batch(e, b, n_runs, runs, nullptr);
+}
+
+int32_t eppscore_schedule_batch_profiles_topk(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs,
+                                              const eppscore_profile_run* runs, const eppscore_topk* topk) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  const int32_t rc = check_profile_runs(e, b, n_runs, runs);
+  if (rc != EPPSCORE_OK) return rc;
+  if (!topk) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
+  bool any = false;
+  for (int32_t i = 0; i < n_runs; i++) {
+    const eppscore_topk& t = topk[i];
+    if (t.struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
+    if (t.k < 0 || t.k > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [0, max_endpoints]");
+    if (t.k > 0 && (!t.endpoints || !t.scores)) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required for k > 0");
+    any = any || t.k > 0;
+  }
+  // without a list the call is eppscore_schedule_batch_profiles
+  return schedule_batch(e, b, n_runs, runs, any ? topk : nullptr);
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,

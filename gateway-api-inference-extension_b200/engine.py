@@ -277,6 +277,9 @@ class Engine:
         {"profile": id, "cand_mask": optional, "want_scores" / "want_pred" / "want_filter_mask": optional bools (host mode)};
         in device mode each run dict also holds its preallocated outputs (pick, pick_score, tie_count, optional scores_out,
         pred_out, filter_mask_out) and `out` the batch's (total_blocks, match_blocks, hashes_out).
+        A run's "topk": k (0..max_endpoints) also asks for the first k endpoints of its pick order; any k > 0 makes the call
+        eppscore_schedule_batch_profiles_topk.  Host mode returns them as topk_pick int32[R, k] (-1 padded) and topk_score
+        float64[R, k] in the run's outputs dict; device mode takes them preallocated in the run dict under the same names.
         Host mode returns (batch outputs dict, [per-run outputs dict])."""
         a = _Args(device)
         b = Batch()
@@ -306,16 +309,29 @@ class Engine:
         M = self.M
         mw = max((M + 31) // 32, 1)
         res_runs = []
+        tarr = (TopK * len(runs))()
+        with_lists = any(run.get("topk", 0) for run in runs)
         for i, run in enumerate(runs):
             x = arr[i]
             x.struct_size = C.sizeof(ProfileRun)
             x.profile = run["profile"]
             x.cand_mask = a.ptr(run.get("cand_mask"), np.uint32)
+            tk = int(run.get("topk", 0))
+            tarr[i].struct_size = C.sizeof(TopK)
+            tarr[i].k = tk
             if device:
                 for k in ("pick", "pick_score", "tie_count", "scores_out", "pred_out", "filter_mask_out"):
                     setattr(x, k, a.ptr(run.get(k), None))
+                if tk:
+                    tarr[i].endpoints = a.ptr(run.get("topk_pick"), None)
+                    tarr[i].scores = a.ptr(run.get("topk_score"), None)
                 continue
             o = dict(pick=np.full(R, -2, np.int32), pick_score=np.zeros(R, np.float64), tie_count=np.zeros(R, np.int32))
+            if tk > 0:
+                o["topk_pick"] = np.full((R, tk), -1, np.int32)
+                o["topk_score"] = np.zeros((R, tk), np.float64)
+                tarr[i].endpoints = o["topk_pick"].ctypes.data
+                tarr[i].scores = o["topk_score"].ctypes.data
             if run.get("want_scores"):
                 o["scores_out"] = np.zeros((R, M), np.float64)
             if run.get("want_pred"):
@@ -323,15 +339,22 @@ class Engine:
             if run.get("want_filter_mask"):
                 o["filter_mask_out"] = np.zeros((R, mw), np.uint32)
             for k, v in o.items():
-                setattr(x, k, v.ctypes.data)
+                if not k.startswith("topk_"):
+                    setattr(x, k, v.ctypes.data)
             res_runs.append(o)
+
+        def call():
+            if with_lists:
+                return self._lib.eppscore_schedule_batch_profiles_topk(self._h, C.byref(b), len(runs), arr, tarr)
+            return self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr)
+
         if device:
             if out is None:
                 out = {}
             b.match_blocks = a.ptr(out.get("match_blocks"), None)
             b.total_blocks = a.ptr(out.get("total_blocks"), None)
             b.hashes_out = a.ptr(out.get("hashes_out"), None)
-            self._check(self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr))
+            self._check(call())
             return out, runs
         res = {}
         if want_total:
@@ -342,7 +365,7 @@ class Engine:
             res["hashes_out"] = np.zeros((R, max_blocks or self.cfg.max_blocks), np.uint64)
         for k, v in res.items():
             setattr(b, k, v.ctypes.data)
-        self._check(self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr))
+        self._check(call())
         return res, res_runs
 
     @staticmethod

@@ -86,6 +86,12 @@ inline bool EngineHasProfiles() {
   return &eppscore_add_profile != nullptr && &eppscore_set_profile_endpoints != nullptr && &eppscore_schedule_batch_profiles != nullptr &&
          &eppscore_commit_picks_profiles != nullptr;
 }
+// maxNumOfEndpoints lists per profile (eppscore_schedule_batch_profiles_topk) came the same way: EngineHasProfilesTopK() tells.
+// Without it a multi-profile config with MaxNumOfEndpoints other than 1 is refused when the Scheduler is built.
+extern "C" int32_t eppscore_schedule_batch_profiles_topk(struct eppscore_engine* e, const eppscore_batch* b, int32_t n_runs,
+                                                         const eppscore_profile_run* runs, const eppscore_topk* topk)
+    __attribute__((weak));
+inline bool EngineHasProfilesTopK() { return EngineHasProfiles() && &eppscore_schedule_batch_profiles_topk != nullptr; }
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
          &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
@@ -269,9 +275,14 @@ struct SchedulerConfig {
   std::shared_ptr<InFlightLoadProducer> InFlightLoad;
   // Several named profiles, in order (the first is the engine's profile 0), and the handler that picks among them.  Empty: the
   // single `Profile` above with SingleProfileHandler semantics, on the path that has always served it.  A multi-profile config
-  // needs an engine library with the profile calls and takes MaxNumOfEndpoints 1 on every profile; the latency scorer and
-  // TrackRunningRequests stay single-profile.  The profile named "prefill" gets the second prefix-index Add of PreRequest
-  // (approximateprefix/plugin.go:177-197) and its in-flight load is released at ResponseStarted (inflightload/producer.go:137-160).
+  // needs an engine library with the profile calls; MaxNumOfEndpoints other than 1 on a profile needs
+  // eppscore_schedule_batch_profiles_topk, and TargetEndpoints then carries that profile's whole list.  The latency parameters
+  // are engine-wide, as the reference has one predicted-latency producer: every profile that has a producer must have the same
+  // one (the same object or equal parameters; the first profile's is read), and every latency scorer equal parameters.  With
+  // TrackRunningRequests, PreRequest queues each request on the primary profile's TargetEndpoints[0] only
+  // (requestcontrol_hooks.go:55-95), and ResponseComplete / RequestExpired remove it there.  The profile named "prefill" gets the
+  // second prefix-index Add of PreRequest (approximateprefix/plugin.go:177-197) and its in-flight load is released at
+  // ResponseStarted (inflightload/producer.go:137-160).
   std::vector<std::pair<std::string, SchedulerProfile>> Profiles;
   std::shared_ptr<ProfileHandler> Handler;
 };
@@ -309,20 +320,50 @@ class Scheduler {
     if (!EngineHasProfiles()) throw SchedulingError("a config with several profiles needs an engine library with eppscore_add_profile");
     if (!cfg.Handler) throw SchedulingError("a config with several profiles needs a ProfileHandler");
     if (cfg.Profiles.size() > EPPSCORE_MAX_PROFILES) throw SchedulingError("more profiles than EPPSCORE_MAX_PROFILES");
+    std::shared_ptr<PredictedLatencyProducer> prod;
+    const LatencyScorer* lat = nullptr;
     for (const auto& np : cfg.Profiles) {
-      if (np.second.picker().MaxNumOfEndpoints != 1)
-        throw SchedulingError("maxNumOfEndpoints > 1 is not supported with several profiles (profile '" + np.first + "')");
-      if (np.second.producer())
-        throw SchedulingError("the predicted-latency producer is not supported with several profiles (profile '" + np.first + "')");
+      const int k = np.second.picker().MaxNumOfEndpoints;
+      if (k < 1) throw SchedulingError("maxNumOfEndpoints must be >= 1 (profile '" + np.first + "')");
+      if (k != 1 && !EngineHasProfilesTopK())
+        throw SchedulingError("maxNumOfEndpoints > 1 with several profiles needs an engine library with "
+                              "eppscore_schedule_batch_profiles_topk (profile '" + np.first + "')");
       for (const auto& w : np.second.scorers())
-        if (w.Scorer_->Kind == EPPSCORE_SCORER_LATENCY)
-          throw SchedulingError("the latency scorer is not supported with several profiles (profile '" + np.first + "')");
+        if (const auto* ls = dynamic_cast<const LatencyScorer*>(w.Scorer_.get())) {
+          if (lat && !SameLatencyScorer(*lat, *ls))
+            throw SchedulingError("the latency scorers of several profiles must have equal parameters, the engine has one set (profile '" +
+                                  np.first + "')");
+          lat = ls;
+        }
+      if (const auto& p = np.second.producer()) {
+        if (prod && prod != p && !SameProducer(*prod, *p))
+          throw SchedulingError("the profiles have different predicted-latency producers; the engine has one, so they must share it (profile '" +
+                                np.first + "')");
+        if (!prod) prod = p;
+      }
     }
     SchedulerConfig c = cfg;
     c.ProfileName = cfg.Profiles[0].first;
     c.Profile = cfg.Profiles[0].second;
+    if (prod) c.Profile.WithPredictedLatencyProducer(prod);  // the engine-wide producer, whichever profile names it
     c.CpuBatchThreshold = 0;  // the host route serves one profile
     return c;
+  }
+  static bool SameLatencyScorer(const LatencyScorer& a, const LatencyScorer& b) {
+    return a.TTFTWeight == b.TTFTWeight && a.TPOTWeight == b.TPOTWeight && a.StrategyMost == b.StrategyMost &&
+           a.CompositeKVWeight == b.CompositeKVWeight && a.CompositeQueueWeight == b.CompositeQueueWeight &&
+           a.CompositePrefixWeight == b.CompositePrefixWeight;
+  }
+  static bool SameProducer(const PredictedLatencyProducer& a, const PredictedLatencyProducer& b) {
+    if (a.State.size() != b.State.size()) return false;
+    for (const auto& kv : a.State) {
+      auto it = b.State.find(kv.first);
+      if (it == b.State.end() || it->second.MinTPOTSLO != kv.second.MinTPOTSLO || it->second.RunningRequests != kv.second.RunningRequests)
+        return false;
+    }
+    return a.SLOBufferFactor == b.SLOBufferFactor && a.StreamingMode == b.StreamingMode && a.EndpointRoleLabel == b.EndpointRoleLabel &&
+           a.HavePredictions == b.HavePredictions && a.TTFTIntercept == b.TTFTIntercept && a.TPOTIntercept == b.TPOTIntercept &&
+           a.TTFTCoeffs == b.TTFTCoeffs && a.TPOTCoeffs == b.TPOTCoeffs && a.TrackRunningRequests == b.TrackRunningRequests;
   }
   Scheduler(const SchedulerConfig& cfg0, int) : cfg_(SingleOrFirst(cfg0)) {
     const SchedulerConfig& cfg = cfg_;
@@ -365,6 +406,9 @@ class Scheduler {
       }
       if (auto* ls = dynamic_cast<LatencyScorer*>(sc[i].Scorer_.get())) latency_scorer_ = ls;
     }
+    for (const auto& np : cfg.Profiles)  // the latency parameters are engine-wide: any profile's scorer (they are equal)
+      for (const auto& w : np.second.scorers())
+        if (auto* ls = dynamic_cast<LatencyScorer*>(w.Scorer_.get())) latency_scorer_ = ls;
     if (latency_scorer_ && !cfg.Profile.producer()) throw SchedulingError("latency-scorer needs a predicted-latency-producer");
     c.block_chars = cfg.Prefix.BlockSizeTokens * 4;  // averageCharactersPerToken (types.go:112)
     c.max_blocks = cfg.Prefix.MaxPrefixBlocksToMatch;
@@ -641,7 +685,13 @@ class Scheduler {
       if (eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr) != EPPSCORE_OK)
         throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
     }
-    if (running_ && (int)last_rid_.size() == R) {  // requestcontrol_hooks.go:73-86
+    RunningAdd(pick);
+  }
+
+  // requestcontrol_hooks.go:73-86: (pick[r], request id, tpot) into the running-request queues, for PreRequest
+  void RunningAdd(const std::vector<int32_t>& pick) {
+    const int R = (int)pick.size();
+    if (running_ && (int)last_rid_.size() == R) {
       std::vector<int32_t> ep((size_t)R, -1);
       std::vector<uint64_t> key((size_t)R, 0);
       for (int r = 0; r < R; r++) {
@@ -669,8 +719,8 @@ class Scheduler {
   // request's estimate.  Without the producer, or for a server that has left the pool since (its id may already be another
   // server's), nothing happens.
   void ResponseComplete(const InferenceRequest& request, const SchedulingResult& result) {
-    if (!cfg_.Profiles.empty()) return ReleaseProfiles(request, result, false);
     RunningRemove(request, result);  // requestcontrol_hooks.go:219
+    if (!cfg_.Profiles.empty()) return ReleaseProfiles(request, result, false);
     if (!inflight_) return;
     auto pr = result.ProfileResults.find(cfg_.ProfileName);
     if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
@@ -772,12 +822,13 @@ class Scheduler {
     auto it = running_keys_.find(rid);
     if (it != running_keys_.end() && it->second.endpoints.empty()) running_keys_.erase(it);
   }
-  // removes (TargetEndpoints[0], request id) from the queues; nothing for an untracked id or a server that has left
+  // removes (the primary profile's TargetEndpoints[0], request id) from the queues; nothing for an untracked id or a server that
+  // has left
   void RunningRemove(const InferenceRequest& request, const SchedulingResult& result) {
     if (!running_ || request.RequestId.empty()) return;
     auto k = running_keys_.find(request.RequestId);
     if (k == running_keys_.end()) return;
-    auto pr = result.ProfileResults.find(cfg_.ProfileName);
+    auto pr = result.ProfileResults.find(cfg_.Profiles.empty() ? cfg_.ProfileName : result.PrimaryProfileName);
     if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
     const int32_t id = ServerId(pr->second.TargetEndpoints[0].Endpoint_->GetMetadata()->NamespacedName_.String());
     auto& v = k->second.endpoints;
@@ -843,6 +894,14 @@ class Scheduler {
       last_chars_.resize((size_t)R);
       for (int r = 0; r < R; r++) EstimateInputs(requests[r], &last_size_[r], &last_hint_[r], &last_chars_[r]);
     }
+    if (running_) {  // PreRequest's inputs: the request id and avgTPOTSLO
+      last_rid_.resize((size_t)R);
+      last_tpot_.resize((size_t)R);
+      for (int r = 0; r < R; r++) {
+        last_rid_[r] = requests[r].RequestId;
+        last_tpot_[r] = SloHeader(requests[r], "x-slo-tpot-ms");
+      }
+    }
     // every profile's result per request (empty TargetEndpoints: the profile ran and found no endpoint)
     std::vector<std::map<std::string, ProfileRunResult>> got((size_t)R);
     std::vector<unsigned> distinct;
@@ -856,11 +915,22 @@ class Scheduler {
       const int n = (int)rows.size();
       std::vector<uint8_t> bytes;
       std::vector<int64_t> off((size_t)n + 1, 0);
-      std::vector<int32_t> len((size_t)n), adapter((size_t)n);
+      std::vector<int32_t> len((size_t)n), adapter((size_t)n), in_tokens;
       std::vector<uint64_t> seed((size_t)n), hashes((size_t)n * last_stride_, 0);
       std::vector<uint16_t> nh((size_t)n, 0);
+      std::vector<double> ttft_slo, tpot_slo;
+      if (latency_scorer_) {  // the latency fold-in's per-request inputs, once for every profile (predictedlatency/plugin.go:276-290)
+        in_tokens.resize((size_t)n);
+        ttft_slo.resize((size_t)n);
+        tpot_slo.resize((size_t)n);
+      }
       for (int i = 0; i < n; i++) {
         const InferenceRequest& q = requests[(size_t)rows[i]];
+        if (latency_scorer_) {
+          in_tokens[i] = CountFields(q.Prompt);
+          ttft_slo[i] = SloHeader(q, "x-slo-ttft-ms");
+          tpot_slo[i] = SloHeader(q, "x-slo-tpot-ms");
+        }
         while (bytes.size() % 16) bytes.push_back(0);  // 16-byte aligned starts: the fast hash path
         off[i] = (int64_t)bytes.size();
         len[i] = (int32_t)q.Prompt.size();
@@ -879,6 +949,24 @@ class Scheduler {
       std::vector<std::vector<int32_t>> pick((size_t)nr, std::vector<int32_t>((size_t)n)), ties = pick;
       std::vector<std::vector<double>> score((size_t)nr, std::vector<double>((size_t)n));
       std::vector<eppscore_profile_run> runs((size_t)nr);
+      // maxNumOfEndpoints per profile: entries past max_endpoints would all be -1
+      std::vector<eppscore_topk> topk((size_t)nr);
+      std::vector<std::vector<int32_t>> list_ids((size_t)nr);
+      std::vector<std::vector<double>> list_scores((size_t)nr);
+      bool lists = false;
+      for (int k = 0; k < nr; k++) {
+        const int kl = std::min(cfg_.Profiles[(size_t)prof[k]].second.picker().MaxNumOfEndpoints, cfg_.MaxEndpoints);
+        eppscore_topk& t = topk[(size_t)k];
+        t = eppscore_topk{};
+        t.struct_size = sizeof(t);
+        if (kl <= 1) continue;
+        lists = true;
+        list_ids[k].assign((size_t)n * kl, -1);
+        list_scores[k].assign((size_t)n * kl, 0.0);
+        t.k = kl;
+        t.endpoints = list_ids[k].data();
+        t.scores = list_scores[k].data();
+      }
       for (int k = 0; k < nr; k++) {
         const auto& filters = cfg_.Profiles[(size_t)prof[k]].second.filters();
         eppscore_profile_run& x = runs[(size_t)k];
@@ -915,8 +1003,17 @@ class Scheduler {
       b.adapter_id = adapter.data();
       b.total_blocks = nh.data();
       b.hashes_out = want_prefix ? hashes.data() : nullptr;
-      if (eppscore_schedule_batch_profiles(eng_, &b, nr, runs.data()) != EPPSCORE_OK)
+      if (latency_scorer_) {
+        b.input_tokens = in_tokens.data();
+        b.ttft_slo = ttft_slo.data();
+        b.tpot_slo = tpot_slo.data();
+      }
+      if (lists) {
+        if (eppscore_schedule_batch_profiles_topk(eng_, &b, nr, runs.data(), topk.data()) != EPPSCORE_OK)
+          throw SchedulingError(std::string("eppscore_schedule_batch_profiles_topk: ") + eppscore_last_error(eng_));
+      } else if (eppscore_schedule_batch_profiles(eng_, &b, nr, runs.data()) != EPPSCORE_OK) {
         throw SchedulingError(std::string("eppscore_schedule_batch_profiles: ") + eppscore_last_error(eng_));
+      }
       for (int i = 0; i < n; i++) {
         const int r = rows[i];
         last_nh_[(size_t)r] = nh[i];
@@ -933,6 +1030,17 @@ class Scheduler {
           se.Score = score[k][i];
           se.TieCount = ties[k][i];
           pr.TargetEndpoints.push_back(se);
+          const int kl = topk[(size_t)k].k;
+          for (int j = 1; j < kl; j++) {  // entries 1..k-1 of the picker's order (entry 0 is the pick); -1 past the last candidate
+            const int32_t lid = list_ids[k][(size_t)i * kl + j];
+            if (lid < 0) break;
+            if (lid >= Mx || pos_of_id[(size_t)lid] < 0) throw SchedulingError("engine listed an endpoint that is not in the candidate list");
+            ScoredEndpoint o2;
+            o2.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)lid]];
+            o2.Index = pos_of_id[(size_t)lid];
+            o2.Score = list_scores[k][(size_t)i * kl + j];
+            pr.TargetEndpoints.push_back(o2);
+          }
         }
       }
     }
@@ -1001,6 +1109,7 @@ class Scheduler {
       if (eppscore_inflight_add(eng_, (int32_t)load_ep.size(), 0, load_ep.data(), tok.data(), nullptr) != EPPSCORE_OK)
         throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
     }
+    RunningAdd(primary);  // the primary target only; the prefill target is not queued (requestcontrol_hooks.go:55-95)
   }
 
   // ResponseBody releases for a multi-profile result: the "prefill" profile's target at start of stream, the others at its end

@@ -272,7 +272,8 @@ typedef struct eppscore_batch {
 #define EPPSCORE_MAX_TOPK 8
 typedef struct eppscore_topk {
   uint32_t struct_size;
-  int32_t k;                   /* 1..EPPSCORE_MAX_TOPK (eppscore_schedule_batch_topk_wide: 1..max_endpoints) */
+  int32_t k;                   /* 1..EPPSCORE_MAX_TOPK (eppscore_schedule_batch_topk_wide: 1..max_endpoints;
+                                  eppscore_schedule_batch_profiles_topk: 0..max_endpoints, 0 = no list) */
   int32_t *endpoints;          /* [R*k] */
   double *scores;              /* [R*k] ScoredEndpoint.Score of each entry */
 } eppscore_topk;
@@ -362,9 +363,30 @@ int32_t eppscore_set_profile_endpoints(struct eppscore_engine *e, int32_t profil
  * (total_blocks, match_blocks, hashes_out); its pick / pick_score / tie_count / cand_mask / scores_out / pred_out /
  * filter_mask_out must be NULL.  1 <= n_runs <= EPPSCORE_MAX_PROFILES, each profile at most once.  Locations, chunking,
  * request_base shards, device-batch ordering and CUDA-graph capture behave as in eppscore_schedule_batch.  Top-k lists
- * (maxNumOfEndpoints > 1) are not part of this call.  ERR_INVALID otherwise. */
+ * (maxNumOfEndpoints > 1) come from eppscore_schedule_batch_profiles_topk.  ERR_INVALID otherwise. */
 int32_t eppscore_schedule_batch_profiles(struct eppscore_engine *e, const eppscore_batch *b, int32_t n_runs,
                                          const eppscore_profile_run *runs);
+/* eppscore_schedule_batch_profiles plus, per run, the first topk[i].k endpoints of that run's pick order (maxNumOfEndpoints is
+ * per profile in the reference: picker/common.go:36-42).  topk: [n_runs], one entry per run, in run order; k == 0 (endpoints /
+ * scores may be NULL) = no list for that run.  k in [0, config.max_endpoints].
+ *   - Run i's list equals, bit for bit, the list eppscore_schedule_batch_topk (k <= EPPSCORE_MAX_TOPK) or
+ *     eppscore_schedule_batch_topk_wide (any k) returns on an engine whose profile 0 has that profile's scorers, picker,
+ *     filters and endpoint subset, and tie_seed ^ (p * 0x9E3779B97F4A7C15) as its tie_seed: the order of each pick mode
+ *     documented above eppscore_topk, entry 0 the run's pick, short lists padded with -1 / 0.0.
+ *   - pick, pick_score and tie_count of every run are those of eppscore_schedule_batch_profiles, with or without lists.  A run
+ *     with k <= EPPSCORE_MAX_TOPK takes the full-matrix kernels' register lists; a run with k == 0 keeps its route (a run
+ *     without a list can stay on the sparse path next to a listed run).  A call with k == 0 on every run is
+ *     eppscore_schedule_batch_profiles.
+ *   - Runs with k > EPPSCORE_MAX_TOPK share the score scratch of eppscore_schedule_batch_topk_wide, which keeps its size: with n
+ *     such runs a slice holds 1/n of its rows per run, the prompts are still hashed once per slice, and a run that passes its
+ *     own scores_out uses that instead.  Such a run inside a CUDA-graph capture before any wide call outside one fails with
+ *     ERR_CAPACITY.  Wide batches on device buffers run their slices in order on the batch's stream (keys 5 / 6 do not cut
+ *     them); the other device batches are sliced as eppscore_schedule_batch_profiles slices them.
+ * Locations, chunking, request_base, device-batch ordering and capture behave as in eppscore_schedule_batch_profiles.
+ * ERR_INVALID: what eppscore_schedule_batch_profiles refuses, topk NULL, a wrong struct_size, k < 0 or k > max_endpoints, and
+ * NULL arrays with k > 0. */
+int32_t eppscore_schedule_batch_profiles_topk(struct eppscore_engine *e, const eppscore_batch *b, int32_t n_runs,
+                                              const eppscore_profile_run *runs, const eppscore_topk *topk);
 
 /* ---- stand-alone stages (same kernels; for parity tests and hosts that only want one stage) ---- */
 /* hashPrompt for R prompts (hashing.go:34-98). hashes_out [R*max_blocks], n_hashes_out [R]. */
