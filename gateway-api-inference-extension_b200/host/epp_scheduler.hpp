@@ -24,6 +24,7 @@
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/eppscore.h"
@@ -445,9 +446,119 @@ class Scheduler {
     std::string error;  // non-empty ⇒ the reference would have returned this error for that request
   };
 
-  // R concurrent Schedule() calls against the same candidate slice, as ONE engine batch.
+  // R concurrent Schedule() calls against the same candidate slice, as ONE engine batch.  The engine's LoRA rows are the
+  // batch's own target adapters (PackSnapshot); a batch that targets more adapters than the engine holds (MaxAdapters rounded
+  // up to 64) runs as contiguous pieces of requests, each with its own snapshot, and comes back exactly as one batch would:
+  // results, top-k lists and PreRequest's inputs in batch order, every request drawing with its index in the whole batch.
   std::vector<BatchItem> ScheduleBatch(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
-    if (!cfg_.Profiles.empty()) return ScheduleBatchProfiles(requests, endpoints);
+    const int R = (int)requests.size(), M = (int)endpoints.size();
+    if (cfg_.Profiles.empty() && cpu_route_ok_ && R > 0 && M > 0 && R <= cfg_.CpuBatchThreshold)  // scores by name: no pieces
+      return ScheduleOnHost(requests, endpoints);
+    std::map<unsigned, int64_t> set_base;  // profiles route: requests of each profile set in earlier pieces
+    const std::vector<size_t> starts = PieceStarts(requests, endpoints);
+    if (starts.size() <= 1)
+      return cfg_.Profiles.empty() ? ScheduleBatchSingle(requests, endpoints, 0) : ScheduleBatchProfiles(requests, endpoints, set_base);
+    std::vector<BatchItem> out;
+    std::vector<uint64_t> hashes;
+    std::vector<uint16_t> nh;
+    std::vector<int64_t> size;
+    std::vector<int32_t> hint, chars;
+    std::vector<std::string> rid;
+    std::vector<double> tpot;
+    for (size_t k = 0; k < starts.size(); k++) {
+      const size_t a = starts[k], b = k + 1 < starts.size() ? starts[k + 1] : requests.size();
+      const std::vector<InferenceRequest> piece(requests.begin() + (ptrdiff_t)a, requests.begin() + (ptrdiff_t)b);
+      auto res = cfg_.Profiles.empty() ? ScheduleBatchSingle(piece, endpoints, (int64_t)a) : ScheduleBatchProfiles(piece, endpoints, set_base);
+      for (auto& x : res) out.push_back(std::move(x));
+      hashes.insert(hashes.end(), last_hashes_.begin(), last_hashes_.end());
+      nh.insert(nh.end(), last_nh_.begin(), last_nh_.end());
+      if (inflight_) {
+        size.insert(size.end(), last_size_.begin(), last_size_.end());
+        hint.insert(hint.end(), last_hint_.begin(), last_hint_.end());
+        chars.insert(chars.end(), last_chars_.begin(), last_chars_.end());
+      }
+      if (running_) {
+        rid.insert(rid.end(), last_rid_.begin(), last_rid_.end());
+        tpot.insert(tpot.end(), last_tpot_.begin(), last_tpot_.end());
+      }
+    }
+    last_hashes_ = std::move(hashes);
+    last_nh_ = std::move(nh);
+    if (inflight_) {
+      last_size_ = std::move(size);
+      last_hint_ = std::move(hint);
+      last_chars_ = std::move(chars);
+    }
+    if (running_) {
+      last_rid_ = std::move(rid);
+      last_tpot_ = std::move(tpot);
+    }
+    return out;
+  }
+  uint64_t CpuRoutedRequests() const { return cpu_routed_; }
+
+ private:
+  // The small-batch route: tiny batch, request-independent profile, evaluated on the host (SmallBatchCpu).
+  std::vector<BatchItem> ScheduleOnHost(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
+    const int R = (int)requests.size(), M = (int)endpoints.size();
+    std::vector<BatchItem> out((size_t)R);
+    last_hashes_.clear();
+    last_nh_.clear();
+    std::vector<int> all((size_t)M);
+    for (int m = 0; m < M; m++) all[m] = m;
+    for (int r = 0; r < R; r++) {
+      std::vector<int> cand = all;
+      for (auto& f : cfg_.Profile.filters()) {
+        cand = f->Filter_(requests[r], endpoints, cand);
+        if (cand.empty()) break;
+      }
+      const CpuPick p = cpu_.Schedule(endpoints, requests[r].TargetModel, cfg_.Profile.filters().empty() ? nullptr : &cand);
+      if (p.pick < 0) {
+        out[r].error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
+        continue;
+      }
+      ScoredEndpoint se;
+      se.Endpoint_ = &endpoints[(size_t)p.pick];
+      se.Index = p.pick;
+      se.Score = p.score;
+      se.TieCount = p.tie_count;
+      out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints.push_back(se);
+      out[r].result.PrimaryProfileName = cfg_.ProfileName;
+    }
+    cpu_routed_ += (uint64_t)R;
+    return out;
+  }
+
+  // Where the pieces of a batch start: a new piece begins at the request whose target would be the engine's A_cap + 1st
+  // distinct adapter of its piece.  Only targets some endpoint carries (active or waiting) need a row: any other name is in
+  // neither map of any endpoint, so its class depends on the capacity rule alone, which the "not a known adapter" row
+  // (adapter id -1) scores the same way (lora_affinity.go:84-99).
+  std::vector<size_t> PieceStarts(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) const {
+    const size_t cap = (size_t)std::max((cfg_.MaxAdapters + 63) / 64 * 64, 64);  // (the engine takes max_adapters < 1 as 64)
+    std::vector<size_t> starts{0};
+    std::unordered_set<std::string> targets, carried, piece;
+    for (const auto& q : requests) targets.insert(q.TargetModel);
+    if (targets.size() <= cap) return starts;
+    for (const auto& e : endpoints) {
+      for (const auto& kv : e.GetMetrics()->ActiveModels)
+        if (targets.count(kv.first)) carried.insert(kv.first);
+      for (const auto& kv : e.GetMetrics()->WaitingModels)
+        if (targets.count(kv.first)) carried.insert(kv.first);
+    }
+    for (size_t r = 0; r < requests.size(); r++) {
+      const std::string& t = requests[r].TargetModel;
+      if (!carried.count(t) || piece.count(t)) continue;
+      if (piece.size() == cap) {
+        starts.push_back(r);
+        piece.clear();
+      }
+      piece.insert(t);
+    }
+    return starts;
+  }
+
+  std::vector<BatchItem> ScheduleBatchSingle(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints,
+                                             int64_t request_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size();
     std::vector<BatchItem> out((size_t)R);
     last_hashes_.clear();
@@ -455,31 +566,6 @@ class Scheduler {
     if (R == 0) return out;
     if (M == 0) {  // scheduler_profile.go:119-121 → single_profile_handler.go:89-91
       for (auto& o : out) o.error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
-      return out;
-    }
-    if (cpu_route_ok_ && R <= cfg_.CpuBatchThreshold) {  // tiny batch, request-independent profile: stay on the host
-      std::vector<int> all((size_t)M);
-      for (int m = 0; m < M; m++) all[m] = m;
-      for (int r = 0; r < R; r++) {
-        std::vector<int> cand = all;
-        for (auto& f : cfg_.Profile.filters()) {
-          cand = f->Filter_(requests[r], endpoints, cand);
-          if (cand.empty()) break;
-        }
-        const CpuPick p = cpu_.Schedule(endpoints, requests[r].TargetModel, cfg_.Profile.filters().empty() ? nullptr : &cand);
-        if (p.pick < 0) {
-          out[r].error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
-          continue;
-        }
-        ScoredEndpoint se;
-        se.Endpoint_ = &endpoints[(size_t)p.pick];
-        se.Index = p.pick;
-        se.Score = p.score;
-        se.TieCount = p.tie_count;
-        out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints.push_back(se);
-        out[r].result.PrimaryProfileName = cfg_.ProfileName;
-      }
-      cpu_routed_ += (uint64_t)R;
       return out;
     }
     // --- stable endpoint ids: the prefix index refers to endpoints by id (ServerID = NamespacedName, indexer.go:34-35), and
@@ -495,7 +581,7 @@ class Scheduler {
     if (!identity) remapped_batches_++;
     std::vector<int> pos_of_id((size_t)Mx, -1);
     for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
-    PackSnapshot(endpoints, ids, Mx);
+    PackSnapshot(endpoints, ids, Mx, requests);
     // --- filters → candidate mask (rows are ids; ids without an endpoint in this list are never candidates) ---
     const int mw = (Mx + 31) / 32;
     std::vector<uint32_t> mask;
@@ -569,6 +655,7 @@ class Scheduler {
     eppscore_batch b{};
     b.struct_size = sizeof(b);
     b.R = R;
+    b.request_base = request_base;
     b.prompt_bytes = want_prefix ? bytes.data() : nullptr;
     b.prompt_off = off.data();
     b.prompt_len = len.data();
@@ -659,8 +746,8 @@ class Scheduler {
     }
     return out;
   }
-  uint64_t CpuRoutedRequests() const { return cpu_routed_; }
 
+ public:
   // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index; with the
   // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
   // (inflightload/producer.go:101-120).
@@ -843,8 +930,10 @@ class Scheduler {
 
   // The batch route with several profiles: the handler's first Pick per request on the host, then ONE
   // eppscore_schedule_batch_profiles call per distinct set of picked profiles (one hash pass for all of the set's profiles), then
-  // ProcessResults.  A handler that asks for a second round gets that request's error.
-  std::vector<BatchItem> ScheduleBatchProfiles(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
+  // ProcessResults.  A handler that asks for a second round gets that request's error.  Request i of a set's call draws with
+  // index set_base[set] + i; set_base counts each set's requests in the earlier pieces of a batch, and is advanced here.
+  std::vector<BatchItem> ScheduleBatchProfiles(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints,
+                                               std::map<unsigned, int64_t>& set_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size(), P = (int)cfg_.Profiles.size();
     std::vector<BatchItem> out((size_t)R);
     last_hashes_.clear();
@@ -876,7 +965,7 @@ class Scheduler {
         if (eppscore_set_profile_endpoints(eng_, p, keep ? row.data() : nullptr, mw) != EPPSCORE_OK)
           throw SchedulingError(std::string("eppscore_set_profile_endpoints: ") + eppscore_last_error(eng_));
       }
-      PackSnapshot(endpoints, ids, Mx);
+      PackSnapshot(endpoints, ids, Mx, requests);
     }
     std::vector<int> pos_of_id((size_t)Mx, -1);
     for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
@@ -994,6 +1083,8 @@ class Scheduler {
       eppscore_batch b{};
       b.struct_size = sizeof(b);
       b.R = n;
+      b.request_base = set_base[S];
+      set_base[S] += n;
       b.prompt_bytes = want_prefix ? bytes.data() : nullptr;
       b.prompt_off = off.data();
       b.prompt_len = len.data();
@@ -1168,7 +1259,7 @@ class Scheduler {
     *chars = (int32_t)std::min<size_t>(q.Prompt.size(), 0x7fffffff);
   }
 
-  // Metrics maps → the packed SoA snapshot; adapter names get dictionary ids in first-seen order.
+  // A server's stable endpoint id: the one it got when first seen, or a freed one for a newcomer.
   int IdOf(const std::string& namespaced_name) {
     auto it = server_ids_.find(namespaced_name);
     if (it != server_ids_.end()) return it->second;
@@ -1184,14 +1275,21 @@ class Scheduler {
   }
 
   // rows of the snapshot are endpoint ids: endpoint eps[i] fills row ids[i]; rows without an endpoint stay zero (they are
-  // never candidates: the batch's mask excludes them)
-  void PackSnapshot(const std::vector<Endpoint>& eps, const std::vector<int>& ids, int rows) {
+  // never candidates: the batch's mask excludes them).  The adapter dictionary is the batch's own: the TargetModels of
+  // `requests` that some endpoint carries, in first-seen order over the endpoints.  A request's class on an endpoint reads only
+  // whether its own target is in the endpoint's maps, plus the map sizes against MaxActiveModels (lora_affinity.go:84-99), so
+  // the other names need no bit; nmodels still counts every name.
+  void PackSnapshot(const std::vector<Endpoint>& eps, const std::vector<int>& ids, int rows, const std::vector<InferenceRequest>& requests) {
     const int N = (int)eps.size();
     const int M = rows;
     adapter_ids_.clear();
+    std::unordered_set<std::string> targets;
+    for (const auto& q : requests) targets.insert(q.TargetModel);
     for (auto& e : eps) {
-      for (auto& kv : e.GetMetrics()->ActiveModels) adapter_ids_.emplace(kv.first, (int)adapter_ids_.size());
-      for (auto& kv : e.GetMetrics()->WaitingModels) adapter_ids_.emplace(kv.first, (int)adapter_ids_.size());
+      for (auto& kv : e.GetMetrics()->ActiveModels)
+        if (targets.count(kv.first)) adapter_ids_.emplace(kv.first, (int)adapter_ids_.size());
+      for (auto& kv : e.GetMetrics()->WaitingModels)
+        if (targets.count(kv.first)) adapter_ids_.emplace(kv.first, (int)adapter_ids_.size());
     }
     const int words = (int)((adapter_ids_.size() + 63) / 64) > 0 ? (int)((adapter_ids_.size() + 63) / 64) : 1;
     std::vector<double> kv((size_t)M);
@@ -1258,8 +1356,14 @@ class Scheduler {
       kv[m] = x->KVCacheUsagePercent;
       queue[m] = x->WaitingQueueSize;
       running[m] = x->RunningRequestsSize;
-      for (auto& a : x->ActiveModels) act[(size_t)m * words + (adapter_ids_[a.first] >> 6)] |= 1ULL << (adapter_ids_[a.first] & 63);
-      for (auto& a : x->WaitingModels) wait[(size_t)m * words + (adapter_ids_[a.first] >> 6)] |= 1ULL << (adapter_ids_[a.first] & 63);
+      for (auto& a : x->ActiveModels) {
+        const auto it = adapter_ids_.find(a.first);
+        if (it != adapter_ids_.end()) act[(size_t)m * words + (it->second >> 6)] |= 1ULL << (it->second & 63);
+      }
+      for (auto& a : x->WaitingModels) {
+        const auto it = adapter_ids_.find(a.first);
+        if (it != adapter_ids_.end()) wait[(size_t)m * words + (it->second >> 6)] |= 1ULL << (it->second & 63);
+      }
       nm[m] = (int32_t)(x->ActiveModels.size() + x->WaitingModels.size());  // len()+len() as MAP sizes (lora_affinity.go:90)
       mx[m] = x->MaxActiveModels;
     }
