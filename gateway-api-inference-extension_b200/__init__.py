@@ -10,7 +10,7 @@ loudly without a CUDA device.
 by `_pkg.py` at the repo root.)
 """
 from ._capi import (  # noqa: F401
-    ABI_SYMBOLS, Batch, Config, EppscoreError, LatencyParams, MAX_TOPK, SCORER, Snapshot, Stats, TopK, TIE_LOWEST_INDEX, TIE_SEEDED_RANDOM, PICK_MAX_SCORE, PICK_WEIGHTED_RANDOM, PICK_RANDOM, FILTER_PREFIX_AFFINITY, FILTER_SLO_HEADROOM_TIER,
+    ABI_SYMBOLS, Batch, Config, EppscoreError, LatencyParams, MAX_STREAMS, MAX_TOPK, SCORER, Snapshot, Stats, TopK, TIE_LOWEST_INDEX, TIE_SEEDED_RANDOM, PICK_MAX_SCORE, PICK_WEIGHTED_RANDOM, PICK_RANDOM, FILTER_PREFIX_AFFINITY, FILTER_SLO_HEADROOM_TIER,
     lib, lib_path,
 )
 from .engine import Engine, default_config, latency_params  # noqa: F401

@@ -9,6 +9,7 @@ MAX_SCORERS = 8
 MAX_ENDPOINT_COLS = 4
 MAX_TOPK = 8
 MAX_PROFILES = 4
+MAX_STREAMS = 8
 
 SCORER = {"queue": 0, "kv": 1, "prefix": 2, "lora": 3, "running": 4, "latency": 5, "token_load": 6,
           "col0": 8, "col1": 9, "col2": 10, "col3": 11, "pair0": 16, "pair1": 17}
@@ -138,6 +139,8 @@ ABI_SYMBOLS = [
     ("eppscore_running_remove_endpoint", C.c_int32, [_P, C.c_int32]),
     ("eppscore_running_get", C.c_int32, [_P, _P, _P, C.c_int32]),
     ("eppscore_running_reserve", C.c_int32, [_P, C.c_int64]),
+    ("eppscore_reserve_stream", C.c_int32, [_P, _P, C.c_int32, C.c_int32]),
+    ("eppscore_release_stream", C.c_int32, [_P, _P]),
     ("eppscore_host_alloc", _P, [C.c_size_t]),
     ("eppscore_host_free", None, [_P]),
 ]

@@ -88,7 +88,7 @@ struct eppscore_engine {
 
   // prefix index: hashToPods + the per-endpoint LRUs, both device-resident (prefix_index.hpp); mutated on `stream`
   std::unique_ptr<DeviceIndex> index;
-  // device-location batches on caller streams that may still read the table, the terms or sc[0] (pending_record)
+  // device-location batches on caller streams that may still read the table, the terms or a scratch set (pending_record)
   std::vector<PendingBatch> pending;
   // Staging for the synchronous host-array calls: slot i holds the call's i-th array.  Each of those calls runs on `stream`
   // and synchronises it before it returns, so one set serves them all.
@@ -125,19 +125,31 @@ struct eppscore_engine {
   bool snapshot_has_min_tpot = false, snapshot_has_dispatched = false;
 
   // scratch for host-location batches and internal hashes: two sets, so the chunks of a host batch can alternate
-  // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i)
+  // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i).  sc[0] also serves device-location
+  // batches on streams without a set of their own (eppscore_reserve_stream), sc[1..3] the slices of a sliced one.
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
         s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe,
         s_subset;  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
+    // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide).  Allocated by the first call that
+    // needs them and never reallocated, so a graph captured after that call keeps pointing at live memory.
+    DevBuf wide;
+    int32_t rows = 0;  // > 0: a reserved stream's set, allocated for this many requests and never grown
   } sc[4];
+  // A caller stream's own scratch set (eppscore_reserve_stream): its device-location batches use it instead of sc[0], so
+  // they can run while batches on other streams do, and a graph captured on the stream never sees it move.  The set is
+  // freed only after the work queued on the stream has finished.
+  struct StreamScratch {
+    cudaStream_t stream = nullptr;
+    int32_t max_R = 0, max_blocks = 0;
+    Scratch sc;
+    ~StreamScratch() {
+      if (stream) cudaStreamSynchronize(stream);
+    }
+  };
   // pinned staging for the small per-request results of a host batch: a D2H copy into the caller's (usually pageable)
   // arrays would block the host after every chunk and serialise the pipeline
   PinnedBuf h_res;
-  // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide): slot 0 serves device-location
-  // batches and the engine stream's host chunks, slot 1 the chunks on stream2.  Allocated by the first call that needs one
-  // and never reallocated, so a graph captured after that call keeps pointing at live memory.
-  DevBuf wide_scores[2];
   int32_t wide_rows = 0;
   int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
@@ -151,8 +163,12 @@ struct eppscore_engine {
   Stream stream;           // the engine stream
   Stream stream2;          // second copy/compute stream of the chunked host path
   Stream split_stream[3];  // the internal streams of a sliced device-location batch
+  // After the engine's streams, so destroyed before them: each set waits for its caller stream before it is freed, and so
+  // before anything else the stream's batches read is freed.
+  std::vector<std::unique_ptr<StreamScratch>> reserved;
 };
 using Scratch = eppscore_engine::Scratch;
+using StreamScratch = eppscore_engine::StreamScratch;
 
 namespace {
 
@@ -180,9 +196,9 @@ bool is_capturing(cudaStream_t st, unsigned long long* id = nullptr) {
   return capturing;
 }
 
-// A device-location batch on caller stream `s` may still read the index table, the snapshot terms and the scratch set sc[0]
-// when its call returns.  Outside a capture its stream's event is recorded again behind it, so the set of pending batches
-// holds one event per caller stream.  Whatever rewrites those first waits for all of them (pending_wait).  Inside a capture
+// A device-location batch on caller stream `s` may still read the index table, the snapshot terms and its scratch set (sc[0],
+// or the stream's own) when its call returns.  Outside a capture its stream's event is recorded again behind it, so the set
+// of pending batches holds one event per caller stream.  Whatever rewrites those first waits for all of them (pending_wait).  Inside a capture
 // the graph's edges order this instead, and the engine stream orders itself.
 int32_t pending_record(eppscore_engine* e, cudaStream_t s) {
   if (s == e->stream || is_capturing(s)) return EPPSCORE_OK;
@@ -210,6 +226,20 @@ int32_t pending_wait(eppscore_engine* e, cudaStream_t st) {
     else CK(e, cudaStreamWaitEvent(st, p.done, 0));
   }
   return EPPSCORE_OK;
+}
+
+// The scratch set reserved for caller stream `s`, or nullptr when it has none.
+StreamScratch* reserved_scratch(eppscore_engine* e, cudaStream_t s) {
+  for (const auto& r : e->reserved)
+    if (r->stream == s) return r.get();
+  return nullptr;
+}
+// Whether `s`, the engine stream or a reserved stream is being captured into a CUDA graph.
+bool capture_open(eppscore_engine* e, cudaStream_t s) {
+  if (is_capturing(s) || is_capturing(e->stream)) return true;
+  for (const auto& r : e->reserved)
+    if (is_capturing(r->stream)) return true;
+  return false;
 }
 
 bool is_endpoint_term_kind(int k, bool masked) {
@@ -678,13 +708,13 @@ DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t
 // on device buffers, asynchronous on `s`, in two steps per slice of rows:
 //   1. one schedule_device over every run: a wide run takes the scores_out route (the diagnostics variants of the full-matrix
 //      and generic dense kernels), which writes the slice's weighted scores, NaN for non-candidates, into the run's part of
-//      wide_scores[slot] (or into the run's own scores_out, which then needs no slicing), together with pick / pick_score /
+//      sc.wide (or into the run's own scores_out, which then needs no slicing), together with pick / pick_score /
 //      tie_count; the other runs compute what they compute outside this function, register lists included;
 //   2. per wide run, topk_select_kernel turns its rows into its lists [R][k], with its profile's pick mode and seed.
 // The scratch holds wide_rows rows whatever the runs: with n wide runs on it, a slice is wide_rows / n rows per run, so a graph
 // captured after the first wide call keeps pointing at live memory.  The slices run in order on `s` (the scratch holds one
 // slice), whatever the slicing keys 5 / 6 say.
-int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, int slot) {
+int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
   if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch before set_snapshot");
   if (d.R <= 0) return EPPSCORE_OK;
   const size_t M = (size_t)e->M, mw = (M + 31) / 32;
@@ -731,7 +761,7 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scr
     any_lat = any_lat || cfg_has(P.cfg, EPPSCORE_SCORER_LATENCY);
   }
   if (n_scratch == 0) return run_slice(d);
-  DevBuf& buf = e->wide_scores[slot];
+  DevBuf& buf = sc.wide;
   if (!buf.p) {
     if (is_capturing(s))
       return fail(e, EPPSCORE_ERR_CAPACITY,
@@ -740,16 +770,16 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scr
     CK(e, buf.reserve((size_t)e->wide_rows * e->geo.Mpad * 8));
   }
   // the per-slice hash scratch is sized for a whole slice up front, so a larger wide call later does not move it under a
-  // captured graph
+  // captured graph (a reserved stream's set holds every slice of the batches it takes already: no slice is longer than its batch)
+  const size_t srows = (size_t)(sc.rows > 0 ? std::min(e->wide_rows, sc.rows) : e->wide_rows);
   if (d.prompt_bytes && !d.hashes_in && !d.hashes_out) {
-    CK(e, sc.s_hashes.reserve((size_t)e->wide_rows * mb * 8));
-    CK(e, sc.s_nh.reserve((size_t)e->wide_rows * 2));
+    CK(e, sc.s_hashes.reserve(srows * mb * 8));
+    CK(e, sc.s_nh.reserve(srows * 2));
   }
-  if (d.prompt_bytes && !d.input_tokens && any_lat) CK(e, sc.s_fields.reserve((size_t)e->wide_rows * 4));
-  if (any_subset) CK(e, sc.s_subset.reserve((size_t)e->wide_rows * mw * 4));
+  if (d.prompt_bytes && !d.input_tokens && any_lat) CK(e, sc.s_fields.reserve(srows * 4));
+  if (any_subset) CK(e, sc.s_subset.reserve(srows * mw * 4));
   // a run next to the wide ones may take the hash kernel's probe records
-  if (d.n_runs > 1 && d.prompt_bytes && !d.hashes_in && !d.hashes_out)
-    CK(e, sc.s_probe.reserve((size_t)e->wide_rows * sizeof(ProbeRec)));
+  if (d.n_runs > 1 && d.prompt_bytes && !d.hashes_in && !d.hashes_out) CK(e, sc.s_probe.reserve(srows * sizeof(ProbeRec)));
   // n_scratch parts of rows * M doubles must fit the wide_rows * Mpad of the scratch: a slice budget (EPP_WIDE_SLICE_BYTES) of
   // fewer rows than wide runs cannot hold one row per run
   if (e->wide_rows < n_scratch)
@@ -1389,18 +1419,27 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       per_pair = per_pair || x.cand_mask || x.scores_out || x.pred_out || x.filter_mask_out;
     }
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
+    StreamScratch* own = reserved_scratch(e, cs);
+    if (own) {  // refused before anything is launched: the stream's set is never grown
+      if (b->R > own->max_R) return fail(e, EPPSCORE_ERR_CAPACITY, "R exceeds the max_R the batch's stream was reserved for");
+      const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
+      if (d.prompt_bytes && !d.hashes_in && mb > own->max_blocks)
+        return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks exceeds the max_blocks the batch's stream was reserved for");
+    }
+    Scratch& sc = own ? own->sc : e->sc[0];
     if (any_wide) {
-      if ((rc = schedule_wide(e, d, cs, e->sc[0], 0)) != EPPSCORE_OK) return rc;
+      if ((rc = schedule_wide(e, d, cs, sc)) != EPPSCORE_OK) return rc;
       return pending_record(e, cs);
     }
-    // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here)
+    // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here), and so does a
+    // batch on a reserved stream (the slices share the engine's fork / join events and internal streams)
     const bool sliceable = d.prompt_bytes && !d.hashes_in && !per_pair && !d.dense_feat && !d.match_blocks && !d.input_tokens &&
-                           !d.ttft_slo && !d.tpot_slo;
+                           !d.ttft_slo && !d.tpot_slo && !own;
     int K = e->dev_split;
     if (!sliceable || e->dev_streams < 2) K = 1;
     while (K > 1 && b->R / K < 2048) K--;
     if (K <= 1) {
-      if ((rc = schedule_device(e, d, cs, e->sc[0])) != EPPSCORE_OK) return rc;
+      if ((rc = schedule_device(e, d, cs, sc)) != EPPSCORE_OK) return rc;
       return pending_record(e, cs);
     }
     // fork: the internal streams join the caller's stream (also inside a CUDA-graph capture), slice c goes to stream c mod S
@@ -1573,7 +1612,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
       hashes_dev = sc.s_hashes.as<uint64_t>();
       d.hashes_out = hashes_dev;
     }
-    rc = any_wide ? schedule_wide(e, d, st, sc, ci & 1) : schedule_device(e, d, st, sc);
+    rc = any_wide ? schedule_wide(e, d, st, sc) : schedule_device(e, d, st, sc);
     if (rc != EPPSCORE_OK) return rc;
     for (int i = 0; i < n_runs; i++) {
       const eppscore_profile_run& x = runs[i];
@@ -2362,6 +2401,48 @@ int32_t eppscore_running_reserve(eppscore_engine* e, int64_t live_entries) {
     if ((rc = run_scratch(e, e->stream, live_entries, false)) != EPPSCORE_OK) return rc;
   }
   return (int32_t)(e->run_cap / 2);
+}
+
+int32_t eppscore_reserve_stream(eppscore_engine* e, void* stream, int32_t max_R, int32_t max_blocks) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!stream) return fail(e, EPPSCORE_ERR_INVALID, "reserve_stream: stream is NULL");
+  if (max_R < 1) return fail(e, EPPSCORE_ERR_INVALID, "reserve_stream: max_R < 1");
+  if (max_blocks < 0 || max_blocks > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_INVALID, "reserve_stream: max_blocks outside [0, 65535]");
+  CK(e, cudaSetDevice(e->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (capture_open(e, s)) return fail(e, EPPSCORE_ERR_INVALID, "reserve_stream under CUDA-graph capture");
+  if (reserved_scratch(e, s)) return fail(e, EPPSCORE_ERR_INVALID, "reserve_stream: the stream is already reserved (release it first)");
+  if (e->reserved.size() >= EPPSCORE_MAX_STREAMS) return fail(e, EPPSCORE_ERR_CAPACITY, "reserve_stream: at most EPPSCORE_MAX_STREAMS streams");
+  // everything schedule_device and schedule_wide reserve in a set, for max_R requests; the wide score rows come with the
+  // first wide call, as for sc[0]
+  auto r = std::make_unique<StreamScratch>();
+  const int32_t mb = max_blocks > 0 ? max_blocks : e->cfg.max_blocks;
+  const size_t R = (size_t)max_R, mw = (size_t)e->geo.Mpad / 32;
+  Scratch& sc = r->sc;
+  CK(e, sc.s_hashes.reserve(R * mb * 8));
+  CK(e, sc.s_nh.reserve(R * 2));
+  CK(e, sc.s_fields.reserve(R * 4));
+  CK(e, sc.s_probe.reserve(R * sizeof(ProbeRec)));
+  CK(e, sc.s_subset.reserve(R * mw * 4));  // whatever the profiles: profiles and subsets may come after the reserve
+  sc.rows = max_R;
+  r->max_R = max_R;
+  r->max_blocks = mb;
+  r->stream = s;  // (last: a set that failed above is freed without waiting for the stream)
+  e->reserved.push_back(std::move(r));
+  return EPPSCORE_OK;
+}
+
+int32_t eppscore_release_stream(eppscore_engine* e, void* stream) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!stream) return fail(e, EPPSCORE_ERR_INVALID, "release_stream: stream is NULL");
+  CK(e, cudaSetDevice(e->device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (capture_open(e, s)) return fail(e, EPPSCORE_ERR_INVALID, "release_stream under CUDA-graph capture");
+  auto it = std::find_if(e->reserved.begin(), e->reserved.end(), [s](const auto& r) { return r->stream == s; });
+  if (it == e->reserved.end()) return fail(e, EPPSCORE_ERR_INVALID, "release_stream: the stream is not reserved");
+  CK(e, cudaStreamSynchronize(s));
+  e->reserved.erase(it);
+  return EPPSCORE_OK;
 }
 
 void* eppscore_host_alloc(size_t bytes) {

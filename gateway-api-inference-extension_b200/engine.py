@@ -50,6 +50,11 @@ def _is_torch(x) -> bool:
     return hasattr(x, "data_ptr") and hasattr(x, "is_cuda")
 
 
+def _stream_handle(stream):
+    """the raw cudaStream_t of a torch.cuda.Stream; raw handles and None pass through"""
+    return getattr(stream, "cuda_stream", stream)
+
+
 class _Args:
     """Keeps converted arrays alive for the duration of a call and yields raw pointers."""
 
@@ -492,6 +497,17 @@ class Engine:
         """Room for live_entries entries (and calls of up to that many) before a graph capture; returns the capacity in
         entries (live_entries 0: only the query)."""
         return self._check(self._lib.eppscore_running_reserve(self._h, int(live_entries)))
+
+    # ------------------------------------------------------------------ per-stream batch scratch
+    def reserve_stream(self, stream, max_R, max_blocks=0):
+        """eppscore_reserve_stream: `stream` (a torch.cuda.Stream or a raw cudaStream_t) gets its own batch scratch for
+        device-location batches of up to max_R requests and max_blocks blocks per prompt (0: config.max_blocks), so its
+        batches run concurrently with other streams' and graphs captured on it survive larger calls elsewhere."""
+        self._check(self._lib.eppscore_reserve_stream(self._h, _stream_handle(stream), int(max_R), int(max_blocks)))
+
+    def release_stream(self, stream):
+        """eppscore_release_stream: waits for the stream's work, then frees its scratch."""
+        self._check(self._lib.eppscore_release_stream(self._h, _stream_handle(stream)))
 
     @staticmethod
     def model_seed(model, salt=b"") -> int:

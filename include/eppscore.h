@@ -244,9 +244,10 @@ typedef struct eppscore_batch {
   double *scores_out;          /* optional [R*M]: the whole weightedScorePerEndpoint map (scheduler_profile.go:155-174),
                                   NaN for non-candidates — diagnostics / parity tests; 8*R*M bytes of HBM writes */
   void *stream;                /* cudaStream_t for location==1 (NULL = engine stream); the call is async on it.  Index
-                                * mutations and eppscore_set_snapshot wait for the last device-location batch; the engine's
-                                * hash scratch is shared, so keep device-location batches that do not pass hashes_out on ONE
-                                * stream at a time (or give each its own hashes_out) */
+                                * mutations and eppscore_set_snapshot wait for the last device-location batch of every stream.
+                                * A stream given its own scratch by eppscore_reserve_stream runs its batches concurrently with
+                                * those of other streams, and graphs captured on it stay valid.  Streams without one share
+                                * the engine's scratch: keep their device-location batches on ONE stream at a time */
   /* latency fold-in, per request (optional, NULL ⇒ 0) */
   const int32_t *input_tokens; /* [R] len(strings.Fields(prompt)) (predictedlatency/training.go:51); NULL with prompt_bytes given ⇒
                                 * counted on the device from those bytes (hosts whose PromptText() differs from the hashed
@@ -313,7 +314,8 @@ int32_t eppscore_get_stats(const struct eppscore_engine *e, eppscore_stats *out)
  *   key 4: 0 = ordinary launches, 1 (default) = programmatic dependent launch between the kernels of a batch;
  *   key 5: slices a device-location batch is cut into (default 1), key 6: streams the slices alternate over (default 2;
  *          the caller's stream plus internal ones, joined before the call returns — also inside a CUDA-graph capture).
- *          Each slice's chain and probe kernels are latency bound and pay their full latency per slice. */
+ *          Each slice's chain and probe kernels are latency bound and pay their full latency per slice.  Batches on a
+ *          reserved stream (eppscore_reserve_stream) are never cut. */
 int32_t eppscore_set_debug(struct eppscore_engine *e, int32_t key, int64_t value);
 
 /* ---- snapshot (replaces the per-request deep clone, director.go:342-349) ---- */
@@ -534,6 +536,29 @@ int32_t eppscore_running_get(struct eppscore_engine *e, double *min_tpot_out, in
  * live_entries entries: do this before capturing running calls into a CUDA graph.  Returns that capacity in entries (> 0),
  * or a negative status; live_entries 0 only queries it. */
 int32_t eppscore_running_reserve(struct eppscore_engine *e, int64_t live_entries);
+
+/* ---- per-stream batch scratch ----
+ * Device-location batches keep internal state in device scratch: hashes (when the batch passes no hashes_out), hash counts,
+ * device-counted prompt fields, probe records, subset rows and the wide top-k score rows.  By default every stream shares one
+ * set, which grows with the largest batch.  A reserved stream owns a set of its own, allocated here for batches of up to max_R
+ * requests and max_blocks blocks per prompt and never reallocated (its wide score rows, one fixed byte budget, come with the
+ * first wide call on the stream outside a capture).  So batches on distinct reserved streams run concurrently on the device,
+ * and a graph captured on a reserved stream stays valid whatever larger calls run elsewhere.  Calls on one engine are still
+ * serialised by the caller.
+ * Every device-location call on a reserved stream uses its set (eppscore_schedule_batch, _topk, _topk_wide, _profiles,
+ * _profiles_topk).  A batch with R > max_R, or one that hashes its prompt bytes with more blocks per prompt than max_blocks,
+ * fails with ERR_CAPACITY before anything is launched.  Debug keys 5 / 6 do not cut batches on a reserved stream.  Pending
+ * batches on reserved streams are waited for by index mutations, eppscore_set_snapshot and producer updates as on any stream. */
+#define EPPSCORE_MAX_STREAMS 8
+/* Gives caller stream `stream` its own batch scratch, sized for device-location batches of up to max_R requests and
+ * max_blocks blocks per prompt (0 = config.max_blocks).  ERR_INVALID: stream NULL, max_R < 1, max_blocks outside
+ * [0, EPPSCORE_MAX_BLOCKS], a stream already reserved (release it first), or while `stream`, the engine stream or a reserved
+ * stream is being captured into a CUDA graph.  ERR_CAPACITY past EPPSCORE_MAX_STREAMS reserved streams. */
+int32_t eppscore_reserve_stream(struct eppscore_engine *e, void *stream, int32_t max_R, int32_t max_blocks);
+/* Waits for the work queued on `stream`, then frees its scratch.  Later batches on it use the shared scratch again.  Graphs
+ * captured on the stream must not be replayed after this.  ERR_INVALID: stream NULL or not reserved, or under capture as
+ * above.  eppscore_destroy releases every reserved stream the same way, so those streams must still exist then. */
+int32_t eppscore_release_stream(struct eppscore_engine *e, void *stream);
 
 /* pinned host memory for callers that want the fast copy path (cudaHostAlloc / cudaFreeHost) */
 void *eppscore_host_alloc(size_t bytes);
