@@ -430,6 +430,114 @@ struct DevBatch {  // all device pointers
   DevRun run[EPPSCORE_MAX_PROFILES];
 };
 
+// How a per-request array of a batch flows.
+enum class Rows {
+  in,       // read by the kernels
+  offsets,  // read by the kernels, R + 1 entries
+  out,      // written by the kernels; a host batch copies it straight to the caller
+  small,    // written by the kernels; a host batch brings it back through pinned staging (h_res)
+  result,   // a small output the kernels always write: a host batch gives it scratch even when the caller did not ask for it
+};
+
+// The row layout of a batch: f(p, per, kind, slot) for each per-request array of `d` and its runs, with p a reference to the
+// array's pointer (nullptr when the batch has none), per its elements per request, and slot the Scratch buffer a host batch
+// stages it in (the runs share one per field).  prompt_bytes is not one of them: prompt_off indexes into it, so it is never cut.
+template <typename F>
+void for_each_row_array(DevBatch& d, size_t M, F&& f) {
+  const size_t mw = (M + 31) / 32;
+  f(d.prompt_off, 1, Rows::offsets, &Scratch::s_off);
+  f(d.prompt_len, 1, Rows::in, &Scratch::s_len);
+  f(d.model_seed, 1, Rows::in, &Scratch::s_seed);
+  f(d.hashes_in, (size_t)d.hash_stride, Rows::in, &Scratch::s_hashes);
+  f(d.n_hashes_in, 1, Rows::in, &Scratch::s_nh);
+  f(d.adapter_id, 1, Rows::in, &Scratch::s_adapter);
+  f(d.dense_feat, M * 4, Rows::in, &Scratch::s_dense);
+  f(d.dense_total, 1, Rows::in, &Scratch::s_dtotal);
+  f(d.input_tokens, 1, Rows::in, &Scratch::s_intok);
+  f(d.ttft_slo, 1, Rows::in, &Scratch::s_tslo);
+  f(d.tpot_slo, 1, Rows::in, &Scratch::s_pslo);
+  for (int i = 0; i < d.n_runs; i++) {
+    DevRun& r = d.run[i];
+    f(r.cand_mask, mw, Rows::in, &Scratch::s_mask);
+    f(r.pick, 1, Rows::result, &Scratch::s_pick);
+    f(r.pick_score, 1, Rows::result, &Scratch::s_score);
+    f(r.tie_count, 1, Rows::result, &Scratch::s_tie);
+    f(r.scores_out, M, Rows::out, &Scratch::s_scores);
+    f(r.pred_out, M * 2, Rows::out, &Scratch::s_pred);
+    f(r.filter_mask_out, mw, Rows::out, &Scratch::s_fmask);
+    f(r.topk_m, (size_t)r.topk, Rows::small, &Scratch::s_topk_m);
+    f(r.topk_score, (size_t)r.topk, Rows::small, &Scratch::s_topk_s);
+  }
+  f(d.match_blocks, M, Rows::out, &Scratch::s_match);
+  f(d.total_blocks, 1, Rows::small, &Scratch::s_total);
+  f(d.hashes_out, (size_t)d.max_blocks, Rows::out, &Scratch::s_hashes);  // (a host batch never has hashes_in with it)
+}
+
+// Rows [base, base + n) of a batch.
+DevBatch slice_rows(DevBatch d, int32_t base, int32_t n, size_t M) {
+  for_each_row_array(d, M, [base](auto*& p, size_t per, Rows, auto) {
+    if (p) p += (size_t)base * per;
+  });
+  d.R = n;
+  d.request_base += base;
+  return d;
+}
+
+// The batch's arrays as one DevBatch, host or device pointers as b.location says, with block_chars / max_blocks and each run's
+// list resolved.  runs: [n_runs], or nullptr for the batch's own single run on profile 0.  topk: [n_runs] validated lists, or
+// nullptr for none; run i's list (k > 0) comes from the register lists of the full-matrix kernels, or from schedule_wide when
+// `wide` is set or k > EPPSCORE_MAX_TOPK.
+DevBatch make_batch(const eppscore_engine* e, const eppscore_batch& b, int32_t n_runs, const eppscore_profile_run* runs,
+                    const eppscore_topk* topk, bool wide) {
+  DevBatch d{};
+  d.R = b.R;
+  d.request_base = b.request_base;
+  d.prompt_bytes = b.prompt_bytes;
+  d.prompt_off = b.prompt_bytes ? b.prompt_off : nullptr;  // the offsets and counts are read only with what they describe
+  d.prompt_len = b.prompt_len;
+  d.model_seed = b.model_seed;
+  d.hashes_in = b.hashes_in;
+  d.n_hashes_in = b.hashes_in ? b.n_hashes_in : nullptr;
+  d.hash_stride = b.hash_stride;
+  d.block_chars = b.block_chars > 0 ? b.block_chars : e->cfg.block_chars;
+  d.max_blocks = b.max_blocks > 0 ? b.max_blocks : e->cfg.max_blocks;
+  d.adapter_id = b.adapter_id;
+  d.dense_feat = b.dense_feat;
+  d.dense_total = b.dense_total;
+  d.input_tokens = b.input_tokens;
+  d.ttft_slo = b.ttft_slo;
+  d.tpot_slo = b.tpot_slo;
+  d.match_blocks = b.match_blocks;
+  d.total_blocks = b.total_blocks;
+  d.hashes_out = b.hashes_out;
+  d.n_runs = n_runs;
+  for (int i = 0; i < n_runs; i++) {
+    DevRun& y = d.run[i];
+    auto set = [&y](const auto& x) {  // an eppscore_profile_run, or the batch itself
+      y.cand_mask = x.cand_mask;
+      y.pick = x.pick;
+      y.pick_score = x.pick_score;
+      y.tie_count = x.tie_count;
+      y.scores_out = x.scores_out;
+      y.pred_out = x.pred_out;
+      y.filter_mask_out = x.filter_mask_out;
+    };
+    if (runs) {
+      set(runs[i]);
+      y.profile = runs[i].profile;
+    } else {
+      set(b);
+    }
+    y.topk = topk ? topk[i].k : 0;
+    if (y.topk > 0) {
+      y.topk_m = topk[i].endpoints;
+      y.topk_score = topk[i].scores;
+      y.wide = wide || y.topk > EPPSCORE_MAX_TOPK;
+    }
+  }
+  return d;
+}
+
 // The hot path on device-resident buffers: [hash kernel] + each run's score/pick kernels, asynchronous on `s`.  The hash stage
 // runs once for all runs.
 int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, Scratch& sc) {
@@ -555,8 +663,7 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
       n_hashes = b.n_hashes_in;
       hash_stride = b.hash_stride;
     } else {
-      const int32_t bc = b.block_chars > 0 ? b.block_chars : e->cfg.block_chars;
-      const int32_t mb = b.max_blocks > 0 ? b.max_blocks : e->cfg.max_blocks;
+      const int32_t bc = b.block_chars, mb = b.max_blocks;
       if (mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
       if (!b.prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
       uint64_t* hout = b.hashes_out;
@@ -667,43 +774,6 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
 #endif
 constexpr unsigned long long kWideSliceBytes = EPP_WIDE_SLICE_BYTES;
 
-// Rows [base, base + n) of a device batch (every per-request array offset; prompt_bytes stays, the offsets index into it).
-DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t mw, size_t mb) {
-  DevBatch q = d;
-  q.R = n;
-  q.request_base = d.request_base + base;
-  const size_t b = (size_t)base;
-  auto off = [b](auto* p, size_t per) { return p ? p + b * per : p; };
-  q.prompt_off = off(d.prompt_off, 1);
-  q.prompt_len = off(d.prompt_len, 1);
-  q.model_seed = off(d.model_seed, 1);
-  q.hashes_in = off(d.hashes_in, (size_t)d.hash_stride);
-  q.n_hashes_in = off(d.n_hashes_in, 1);
-  q.adapter_id = off(d.adapter_id, 1);
-  q.dense_feat = off(d.dense_feat, M * 4);
-  q.dense_total = off(d.dense_total, 1);
-  q.input_tokens = off(d.input_tokens, 1);
-  q.ttft_slo = off(d.ttft_slo, 1);
-  q.tpot_slo = off(d.tpot_slo, 1);
-  for (int i = 0; i < d.n_runs; i++) {
-    const DevRun& x = d.run[i];
-    DevRun& y = q.run[i];
-    y.cand_mask = off(x.cand_mask, mw);
-    y.pred_out = off(x.pred_out, M * 2);
-    y.filter_mask_out = off(x.filter_mask_out, mw);
-    y.pick = off(x.pick, 1);
-    y.pick_score = off(x.pick_score, 1);
-    y.tie_count = off(x.tie_count, 1);
-    y.scores_out = off(x.scores_out, M);
-    y.topk_m = off(x.topk_m, (size_t)x.topk);
-    y.topk_score = off(x.topk_score, (size_t)x.topk);
-  }
-  q.match_blocks = off(d.match_blocks, M);
-  q.total_blocks = off(d.total_blocks, 1);
-  q.hashes_out = off(d.hashes_out, mb);
-  return q;
-}
-
 // eppscore_schedule_batch_topk_wide, and a batch of eppscore_schedule_batch_profiles_topk with a run of k > EPPSCORE_MAX_TOPK,
 // on device buffers, asynchronous on `s`, in two steps per slice of rows:
 //   1. one schedule_device over every run: a wide run takes the scores_out route (the diagnostics variants of the full-matrix
@@ -717,8 +787,7 @@ DevBatch slice_rows(const DevBatch& d, int32_t base, int32_t n, size_t M, size_t
 int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
   if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch before set_snapshot");
   if (d.R <= 0) return EPPSCORE_OK;
-  const size_t M = (size_t)e->M, mw = (M + 31) / 32;
-  const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
+  const size_t M = (size_t)e->M, mw = (M + 31) / 32, mb = (size_t)d.max_blocks;
   auto select = [&](const DevBatch& q, const DevRun& run) -> int32_t {
     const Profile& P = e->prof[run.profile];
     TopKSelectArgs t{};
@@ -786,7 +855,7 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scr
     return fail(e, EPPSCORE_ERR_CAPACITY, "the wide score scratch holds fewer rows than the call has wide runs (EPP_WIDE_SLICE_BYTES)");
   const int32_t rows = e->wide_rows / n_scratch;
   for (int32_t base = 0; base < d.R; base += rows) {
-    DevBatch q = slice_rows(d, base, std::min(rows, d.R - base), M, mw, (size_t)mb);
+    DevBatch q = slice_rows(d, base, std::min(rows, d.R - base), M);
     for (int i = 0, j = 0; i < q.n_runs; i++)
       if (q.run[i].wide && !d.run[i].scores_out) q.run[i].scores_out = buf.as<double>() + (size_t)(j++) * rows * M;
     int32_t rc = run_slice(q);
@@ -1358,72 +1427,28 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
 namespace {
 
 // eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk): the runs (profile + per-profile filter result and
-// outputs) of one batch.  topk: [n_runs] validated lists, or nullptr for none; run i's list (k > 0) comes from the register
-// lists of the full-matrix kernels, or from schedule_wide when `wide` is set or k > EPPSCORE_MAX_TOPK.
+// outputs) of one batch, as make_batch takes them.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
                        const eppscore_topk* topk, bool wide = false) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
   int32_t rc = EPPSCORE_OK;
-  int32_t tk[EPPSCORE_MAX_PROFILES] = {}, tk_sum = 0;  // per run k, and their sum
+  const DevBatch d = make_batch(e, *b, n_runs, runs, topk, wide);
+  const size_t M = (size_t)e->M;
   bool any_wide = false;
-  for (int i = 0; i < n_runs && topk; i++) {
-    tk[i] = topk[i].k;
-    tk_sum += tk[i];
-    any_wide = any_wide || (tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK));
-  }
-  DevBatch d{};
-  d.R = b->R;
-  d.request_base = b->request_base;
-  d.hash_stride = b->hash_stride;
-  d.block_chars = b->block_chars;
-  d.max_blocks = b->max_blocks;
-  d.n_runs = n_runs;
-  for (int i = 0; i < n_runs; i++) {
-    d.run[i].profile = runs[i].profile;
-    d.run[i].topk = tk[i];
-    d.run[i].wide = tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK);
-  }
+  for (int i = 0; i < n_runs; i++) any_wide = any_wide || d.run[i].wide;
   if (b->location == 1) {
-    d.prompt_bytes = b->prompt_bytes;
-    d.prompt_off = b->prompt_off;
-    d.prompt_len = b->prompt_len;
-    d.model_seed = b->model_seed;
-    d.hashes_in = b->hashes_in;
-    d.n_hashes_in = b->n_hashes_in;
-    d.adapter_id = b->adapter_id;
-    d.dense_feat = b->dense_feat;
-    d.dense_total = b->dense_total;
-    d.input_tokens = b->input_tokens;
-    d.ttft_slo = b->ttft_slo;
-    d.tpot_slo = b->tpot_slo;
-    d.match_blocks = b->match_blocks;
-    d.total_blocks = b->total_blocks;
-    d.hashes_out = b->hashes_out;
     bool per_pair = false;  // R x M outputs or masks on some run
     for (int i = 0; i < n_runs; i++) {
-      const eppscore_profile_run& x = runs[i];
-      DevRun& y = d.run[i];
-      y.cand_mask = x.cand_mask;
-      y.pick = x.pick;
-      y.pick_score = x.pick_score;
-      y.tie_count = x.tie_count;
-      y.scores_out = x.scores_out;
-      y.pred_out = x.pred_out;
-      y.filter_mask_out = x.filter_mask_out;
-      if (tk[i]) {
-        y.topk_m = topk[i].endpoints;
-        y.topk_score = topk[i].scores;
-      }
+      const DevRun& x = d.run[i];
       per_pair = per_pair || x.cand_mask || x.scores_out || x.pred_out || x.filter_mask_out;
     }
     cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
     StreamScratch* own = reserved_scratch(e, cs);
     if (own) {  // refused before anything is launched: the stream's set is never grown
       if (b->R > own->max_R) return fail(e, EPPSCORE_ERR_CAPACITY, "R exceeds the max_R the batch's stream was reserved for");
-      const int32_t mb = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
-      if (d.prompt_bytes && !d.hashes_in && mb > own->max_blocks)
+      if (d.prompt_bytes && !d.hashes_in && d.max_blocks > own->max_blocks)
         return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks exceeds the max_blocks the batch's stream was reserved for");
     }
     Scratch& sc = own ? own->sc : e->sc[0];
@@ -1451,29 +1476,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     }
     CK(e, cudaEventRecord(e->ev_fork, cs));
     for (int i = 0; i < S - 1; i++) CK(e, cudaStreamWaitEvent(e->split_stream[i], e->ev_fork, 0));
-    const int32_t mbk = d.max_blocks > 0 ? d.max_blocks : e->cfg.max_blocks;
     const int32_t per = ((b->R + K - 1) / K + 63) / 64 * 64;
     for (int c = 0, base = 0; base < b->R; c++, base += per) {
-      DevBatch q = d;
-      q.R = std::min(per, b->R - base);
-      q.request_base = d.request_base + base;
-      q.prompt_off = d.prompt_off + base;
-      if (d.prompt_len) q.prompt_len = d.prompt_len + base;
-      if (d.model_seed) q.model_seed = d.model_seed + base;
-      if (d.adapter_id) q.adapter_id = d.adapter_id + base;
-      for (int i = 0; i < n_runs; i++) {
-        q.run[i].pick = d.run[i].pick + base;
-        q.run[i].pick_score = d.run[i].pick_score + base;
-        q.run[i].tie_count = d.run[i].tie_count + base;
-        if (tk[i]) {
-          q.run[i].topk_m = d.run[i].topk_m + (size_t)base * tk[i];
-          q.run[i].topk_score = d.run[i].topk_score + (size_t)base * tk[i];
-        }
-      }
-      if (d.total_blocks) q.total_blocks = d.total_blocks + base;
-      if (d.hashes_out) q.hashes_out = d.hashes_out + (size_t)base * mbk;
       const int si = c % S;
-      rc = schedule_device(e, q, si == 0 ? cs : e->split_stream[si - 1], e->sc[si]);
+      rc = schedule_device(e, slice_rows(d, base, std::min(per, b->R - base), M), si == 0 ? cs : e->split_stream[si - 1], e->sc[si]);
       if (rc != EPPSCORE_OK) break;
     }
     for (int i = 0; i < S - 1; i++) {  // join, also on the error path (a capture must not be left forked)
@@ -1492,11 +1498,8 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
   if (b->hashes_out && (b->hashes_in || !b->prompt_bytes))
     return fail(e, EPPSCORE_ERR_INVALID, "hashes_out needs prompt_bytes (hashes supplied as hashes_in are already the caller's)");
-  const size_t M = (size_t)e->M;
-  const size_t mw = (M + 31) / 32;
-  const int32_t mb = b->max_blocks > 0 ? b->max_blocks : e->cfg.max_blocks;
-  bool diag = b->match_blocks || b->dense_feat;  // R x M arrays: one chunk at a time is plenty
-  for (int i = 0; i < n_runs; i++) diag = diag || runs[i].scores_out || runs[i].pred_out;
+  bool diag = d.match_blocks || d.dense_feat;  // R x M arrays: one chunk at a time is plenty
+  for (int i = 0; i < n_runs; i++) diag = diag || d.run[i].scores_out || d.run[i].pred_out;
   int32_t chunk = e->host_chunk > 0 ? e->host_chunk : b->R;
   if (diag || b->R < 2 * chunk) chunk = b->R;
   const int nstreams = chunk < b->R ? 2 : 1;
@@ -1504,149 +1507,98 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   // the chunks reuse sc[0] / sc[1], which a device-location batch may still hold
   if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
   if (nstreams == 2 && (rc = pending_wait(e, e->stream2)) != EPPSCORE_OK) return rc;
-  // pinned staging, per run: pick i32 | score f64 | tie i32, each [R]; then total u16 [R]; top-k endpoints i32 | scores f64,
-  // each [R*Σk], run i's lists at R*tko[i]
-  size_t tko[EPPSCORE_MAX_PROFILES] = {};
-  for (int i = 1; i < n_runs; i++) tko[i] = tko[i - 1] + (size_t)tk[i - 1];
-  const size_t RR = (size_t)b->R, RK = RR * (size_t)tk_sum, NR = (size_t)n_runs;
-  const size_t o_score = (NR * RR * 4 + 7) & ~(size_t)7, o_tie = o_score + NR * RR * 8, o_total = o_tie + NR * RR * 4;
-  const size_t o_tkm = (o_total + RR * 2 + 7) & ~(size_t)7, o_tks = (o_tkm + RK * 4 + 7) & ~(size_t)7, res_bytes = o_tks + RK * 8;
-  CK(e, e->h_res.reserve(res_bytes));
-  unsigned char* hres = e->h_res.as<unsigned char>();
-  int32_t* hp_pick = reinterpret_cast<int32_t*>(hres);
-  double* hp_score = reinterpret_cast<double*>(hres + o_score);
-  int32_t* hp_tie = reinterpret_cast<int32_t*>(hres + o_tie);
-  uint16_t* hp_total = reinterpret_cast<uint16_t*>(hres + o_total);
-  int32_t* hp_tkm = reinterpret_cast<int32_t*>(hres + o_tkm);
-  double* hp_tks = reinterpret_cast<double*>(hres + o_tks);
+  struct Copy {
+    void* dst;
+    const void* src;
+    size_t bytes;
+  };
+  auto at = [](auto* p, void* base, size_t off) { return reinterpret_cast<decltype(p)>(static_cast<unsigned char*>(base) + off); };
+  // The small results come back through pinned staging, since a D2H copy into the caller's (usually pageable) arrays would
+  // block the host after every chunk: `pinned` is the batch with those outputs in h_res, the 8-byte arrays first so that each
+  // one is aligned, and `results` lists the copies from there to the caller.
+  DevBatch pinned = d;
+  std::vector<Copy> results, d2h;
+  size_t h_end[9] = {};  // by element size: the end of the 8-byte arrays, then of the 4- and 2-byte ones
+  auto via_pinned = [](auto* p, Rows kind) { return p && (kind == Rows::small || kind == Rows::result); };
+  for_each_row_array(pinned, M, [&](auto*& p, size_t per, Rows kind, auto) {
+    if (via_pinned(p, kind)) h_end[sizeof *p] += (size_t)b->R * per * sizeof *p;
+  });
+  h_end[4] += h_end[8];
+  h_end[2] += h_end[4];
+  CK(e, e->h_res.reserve(h_end[2]));
+  for_each_row_array(pinned, M, [&](auto*& p, size_t per, Rows kind, auto) {
+    if (!via_pinned(p, kind)) return;
+    const size_t bytes = (size_t)b->R * per * sizeof *p;
+    h_end[sizeof *p] -= bytes;  // (each array takes the bytes just below the end of its size's part)
+    auto* h = at(p, e->h_res.p, h_end[sizeof *p]);
+    results.push_back({(void*)p, h, bytes});
+    p = h;
+  });
+  std::vector<std::pair<DevBuf*, size_t>> parts;  // a chunk's scratch buffers and their bytes
+  auto part = [&parts](DevBuf& buf) -> size_t& {
+    for (auto& x : parts)
+      if (x.first == &buf) return x.second;
+    return parts.emplace_back(&buf, 0).second;
+  };
   int ci = 0;
   for (int32_t r0 = 0; r0 < b->R; r0 += chunk, ci++) {
-    const int32_t r1 = std::min(b->R, r0 + chunk);
-    const size_t R = (size_t)(r1 - r0);
+    const int32_t n = std::min(b->R, r0 + chunk) - r0;
     Scratch& sc = e->sc[ci & 1];
     cudaStream_t st = (ci & 1) ? e->stream2 : e->stream;
-    DevBatch d{};
-    d.R = (int32_t)R;
-    d.request_base = b->request_base + r0;
-    d.hash_stride = b->hash_stride;
-    d.block_chars = b->block_chars;
-    d.max_blocks = b->max_blocks;
-    d.n_runs = n_runs;
-    if (b->prompt_bytes) {  // the kernels keep using the caller's offsets
-      if ((rc = stage_prompts(e, sc.s_prompts, b->prompt_bytes, b->prompt_off, b->prompt_len, r0, r1, st, &d.prompt_bytes)) != EPPSCORE_OK ||
-          (rc = h2d(e, sc.s_off, b->prompt_off + r0, R + 1, &d.prompt_off, st)) != EPPSCORE_OK)
-        return rc;
+    // the chunk on the host (`q`: the caller's inputs, its outputs where they come back to), then on the device (`x`): the
+    // prompt bytes its offsets reach, and every other array in a part of its scratch buffer
+    const DevBatch q = slice_rows(pinned, r0, n, M);
+    DevBatch x = q;
+    if (q.prompt_bytes &&
+        (rc = stage_prompts(e, sc.s_prompts, q.prompt_bytes, q.prompt_off, q.prompt_len, 0, n, st, &x.prompt_bytes)) != EPPSCORE_OK)
+      return rc;
+    auto bytes = [n](auto* p, size_t per, Rows kind) -> size_t {
+      return (p || kind == Rows::result) ? (n + (kind == Rows::offsets ? 1 : 0)) * per * sizeof *p : 0;
+    };
+    parts.clear();
+    for_each_row_array(x, M, [&](auto*& p, size_t per, Rows kind, DevBuf Scratch::*slot) {
+      if (const size_t nb = bytes(p, per, kind)) part(sc.*slot) += nb;
+    });
+    for (auto& [buf, size] : parts) {
+      CK(e, buf->reserve(size));
+      size = 0;
     }
-#define H2D(buf, field, per) \
-  if ((rc = h2d(e, sc.buf, b->field ? b->field + (size_t)r0 * (per) : b->field, R * (per), &d.field, st)) != EPPSCORE_OK) return rc;
-    H2D(s_len, prompt_len, 1)
-    H2D(s_seed, model_seed, 1)
-    if (b->hashes_in) {
-      H2D(s_hashes, hashes_in, (size_t)b->hash_stride)
-      H2D(s_nh, n_hashes_in, 1)
-    }
-    H2D(s_adapter, adapter_id, 1)
-    H2D(s_dense, dense_feat, M * 4)
-    H2D(s_dtotal, dense_total, 1)
-    H2D(s_intok, input_tokens, 1)
-    H2D(s_tslo, ttft_slo, 1)
-    H2D(s_pslo, tpot_slo, 1)
-#undef H2D
-    // per run: slice i of each scratch array
-    size_t n_masks = 0;
-    bool any_scores = false, any_pred = false, any_fmask = false;
-    for (int i = 0; i < n_runs; i++) {
-      n_masks += runs[i].cand_mask ? 1 : 0;
-      any_scores = any_scores || runs[i].scores_out;
-      any_pred = any_pred || runs[i].pred_out;
-      any_fmask = any_fmask || runs[i].filter_mask_out;
-    }
-    if (n_masks) CK(e, sc.s_mask.reserve(NR * R * mw * 4));
-    CK(e, sc.s_pick.reserve(NR * R * 4));
-    CK(e, sc.s_score.reserve(NR * R * 8));
-    CK(e, sc.s_tie.reserve(NR * R * 4));
-    if (any_scores) CK(e, sc.s_scores.reserve(NR * R * M * 8));
-    if (any_pred) CK(e, sc.s_pred.reserve(NR * R * M * 16));
-    if (any_fmask) CK(e, sc.s_fmask.reserve(NR * R * mw * 4));
-    for (int i = 0; i < n_runs; i++) {
-      const eppscore_profile_run& x = runs[i];
-      DevRun& y = d.run[i];
-      y.profile = x.profile;
-      if (x.cand_mask) {
-        uint32_t* dm = sc.s_mask.as<uint32_t>() + (size_t)i * R * mw;
-        CK(e, cudaMemcpyAsync(dm, x.cand_mask + (size_t)r0 * mw, R * mw * 4, cudaMemcpyHostToDevice, st));
-        y.cand_mask = dm;
+    d2h.clear();
+    cudaError_t c = cudaSuccess;
+    for_each_row_array(x, M, [&](auto*& p, size_t per, Rows kind, DevBuf Scratch::*slot) {
+      const size_t nb = bytes(p, per, kind);
+      if (nb == 0) {
+        p = nullptr;
+        return;
       }
-      y.pick = sc.s_pick.as<int32_t>() + (size_t)i * R;
-      y.pick_score = sc.s_score.as<double>() + (size_t)i * R;
-      y.tie_count = sc.s_tie.as<int32_t>() + (size_t)i * R;
-      if (x.scores_out) y.scores_out = sc.s_scores.as<double>() + (size_t)i * R * M;
-      if (x.pred_out) y.pred_out = sc.s_pred.as<double>() + (size_t)i * R * M * 2;
-      if (x.filter_mask_out) y.filter_mask_out = sc.s_fmask.as<uint32_t>() + (size_t)i * R * mw;
-    }
-    if (tk_sum) {  // [R*Σk]: small, like the picks (the chunks keep overlapping)
-      CK(e, sc.s_topk_m.reserve(R * tk_sum * 4));
-      CK(e, sc.s_topk_s.reserve(R * tk_sum * 8));
-      for (int i = 0; i < n_runs; i++)
-        if (tk[i]) {
-          DevRun& y = d.run[i];
-          y.topk = tk[i];
-          y.wide = tk[i] > 0 && (wide || tk[i] > EPPSCORE_MAX_TOPK);
-          y.topk_m = sc.s_topk_m.as<int32_t>() + R * tko[i];
-          y.topk_score = sc.s_topk_s.as<double>() + R * tko[i];
-        }
-    }
-    if (b->match_blocks) {
-      CK(e, sc.s_match.reserve(R * M * 2));
-      d.match_blocks = sc.s_match.as<uint16_t>();
-    }
-    if (b->total_blocks) {
-      CK(e, sc.s_total.reserve(R * 2));
-      d.total_blocks = sc.s_total.as<uint16_t>();
-    }
-    uint64_t* hashes_dev = nullptr;
-    if (b->hashes_out) {
-      // reuse the internal hash scratch as the device-side hashes_out; entries past n_hashes[r] are zero
-      CK(e, sc.s_hashes.reserve(R * (size_t)mb * 8));
-      CK(e, cudaMemsetAsync(sc.s_hashes.p, 0, R * (size_t)mb * 8, st));
-      hashes_dev = sc.s_hashes.as<uint64_t>();
-      d.hashes_out = hashes_dev;
-    }
-    rc = any_wide ? schedule_wide(e, d, st, sc) : schedule_device(e, d, st, sc);
+      size_t& off = part(sc.*slot);
+      auto* dev = at(p, (sc.*slot).p, off);
+      off += nb;
+      if (kind == Rows::in || kind == Rows::offsets) {
+        if (c == cudaSuccess) c = cudaMemcpyAsync((void*)dev, p, nb, cudaMemcpyHostToDevice, st);
+      } else if (p) {
+        d2h.push_back({(void*)p, dev, nb});
+      }
+      p = dev;
+    });
+    CK(e, c);
+    // hashes_out from the device: entries past n_hashes[r] are zero
+    if (x.hashes_out) CK(e, cudaMemsetAsync(x.hashes_out, 0, (size_t)n * x.max_blocks * 8, st));
+    rc = any_wide ? schedule_wide(e, x, st, sc) : schedule_device(e, x, st, sc);
     if (rc != EPPSCORE_OK) return rc;
-    for (int i = 0; i < n_runs; i++) {
-      const eppscore_profile_run& x = runs[i];
-      const DevRun& y = d.run[i];
-      if (x.pick) CK(e, cudaMemcpyAsync(hp_pick + i * RR + r0, y.pick, R * 4, cudaMemcpyDeviceToHost, st));
-      if (x.pick_score) CK(e, cudaMemcpyAsync(hp_score + i * RR + r0, y.pick_score, R * 8, cudaMemcpyDeviceToHost, st));
-      if (x.tie_count) CK(e, cudaMemcpyAsync(hp_tie + i * RR + r0, y.tie_count, R * 4, cudaMemcpyDeviceToHost, st));
-      if (x.scores_out) CK(e, cudaMemcpyAsync(x.scores_out + (size_t)r0 * M, y.scores_out, R * M * 8, cudaMemcpyDeviceToHost, st));
-      if (x.pred_out) CK(e, cudaMemcpyAsync(x.pred_out + (size_t)r0 * M * 2, y.pred_out, R * M * 16, cudaMemcpyDeviceToHost, st));
-      if (x.filter_mask_out)
-        CK(e, cudaMemcpyAsync(x.filter_mask_out + (size_t)r0 * mw, y.filter_mask_out, R * mw * 4, cudaMemcpyDeviceToHost, st));
-      if (tk[i]) {
-        const size_t o = RR * tko[i] + (size_t)r0 * tk[i];
-        CK(e, cudaMemcpyAsync(hp_tkm + o, y.topk_m, R * tk[i] * 4, cudaMemcpyDeviceToHost, st));
-        CK(e, cudaMemcpyAsync(hp_tks + o, y.topk_score, R * tk[i] * 8, cudaMemcpyDeviceToHost, st));
-      }
-    }
-    if (b->match_blocks) CK(e, cudaMemcpyAsync(b->match_blocks + (size_t)r0 * M, d.match_blocks, R * M * 2, cudaMemcpyDeviceToHost, st));
-    if (b->total_blocks) CK(e, cudaMemcpyAsync(hp_total + r0, d.total_blocks, R * 2, cudaMemcpyDeviceToHost, st));
-    if (hashes_dev) CK(e, cudaMemcpyAsync(b->hashes_out + (size_t)r0 * mb, hashes_dev, R * (size_t)mb * 8, cudaMemcpyDeviceToHost, st));
+    for (const Copy& y : d2h) CK(e, cudaMemcpyAsync(y.dst, y.src, y.bytes, cudaMemcpyDeviceToHost, st));
   }
   CK(e, cudaStreamSynchronize(e->stream));
   if (nstreams == 2) CK(e, cudaStreamSynchronize(e->stream2));
-  for (int i = 0; i < n_runs; i++) {
-    if (runs[i].pick) memcpy(runs[i].pick, hp_pick + i * RR, RR * 4);
-    if (runs[i].pick_score) memcpy(runs[i].pick_score, hp_score + i * RR, RR * 8);
-    if (runs[i].tie_count) memcpy(runs[i].tie_count, hp_tie + i * RR, RR * 4);
-  }
-  if (b->total_blocks) memcpy(b->total_blocks, hp_total, RR * 2);
-  for (int i = 0; i < n_runs; i++)
-    if (tk[i]) {
-      memcpy(topk[i].endpoints, hp_tkm + RR * tko[i], RR * tk[i] * 4);
-      memcpy(topk[i].scores, hp_tks + RR * tko[i], RR * tk[i] * 8);
-    }
+  for (const Copy& y : results) memcpy(y.dst, y.src, y.bytes);
+  return EPPSCORE_OK;
+}
+
+// One eppscore_topk with k in [k_min, k_max] (`range` says which in the message).
+int32_t check_topk(eppscore_engine* e, const eppscore_topk& t, int32_t k_min, int32_t k_max, const char* range) {
+  if (t.struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
+  if (t.k < k_min || t.k > k_max) return fail(e, EPPSCORE_ERR_INVALID, std::string("topk k must be in ") + range);
+  if (t.k > 0 && (!t.endpoints || !t.scores)) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
   return EPPSCORE_OK;
 }
 
@@ -1655,22 +1607,11 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
   if (t) {
-    if (t->struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
-    if (wide && (t->k < 1 || t->k > e->cfg.max_endpoints)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, max_endpoints]");
-    if (!wide && (t->k < 1 || t->k > EPPSCORE_MAX_TOPK)) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [1, EPPSCORE_MAX_TOPK]");
-    if (!t->endpoints || !t->scores) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required");
+    const int32_t rc = wide ? check_topk(e, *t, 1, e->cfg.max_endpoints, "[1, max_endpoints]")
+                            : check_topk(e, *t, 1, EPPSCORE_MAX_TOPK, "[1, EPPSCORE_MAX_TOPK]");
+    if (rc != EPPSCORE_OK) return rc;
   }
-  eppscore_profile_run run{};
-  run.struct_size = sizeof(run);
-  run.profile = 0;
-  run.cand_mask = b->cand_mask;
-  run.pick = b->pick;
-  run.pick_score = b->pick_score;
-  run.tie_count = b->tie_count;
-  run.scores_out = b->scores_out;
-  run.pred_out = b->pred_out;
-  run.filter_mask_out = b->filter_mask_out;
-  return schedule_batch(e, b, 1, &run, t, wide);
+  return schedule_batch(e, b, 1, nullptr, t, wide);
 }
 
 }  // namespace
@@ -1796,19 +1737,12 @@ int32_t eppscore_schedule_batch_profiles(eppscore_engine* e, const eppscore_batc
 int32_t eppscore_schedule_batch_profiles_topk(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs,
                                               const eppscore_profile_run* runs, const eppscore_topk* topk) {
   if (!e) return EPPSCORE_ERR_INVALID;
-  const int32_t rc = check_profile_runs(e, b, n_runs, runs);
+  int32_t rc = check_profile_runs(e, b, n_runs, runs);
   if (rc != EPPSCORE_OK) return rc;
   if (!topk) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
-  bool any = false;
-  for (int32_t i = 0; i < n_runs; i++) {
-    const eppscore_topk& t = topk[i];
-    if (t.struct_size != sizeof(eppscore_topk)) return fail(e, EPPSCORE_ERR_INVALID, "topk struct_size mismatch");
-    if (t.k < 0 || t.k > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "topk k must be in [0, max_endpoints]");
-    if (t.k > 0 && (!t.endpoints || !t.scores)) return fail(e, EPPSCORE_ERR_INVALID, "topk endpoints/scores required for k > 0");
-    any = any || t.k > 0;
-  }
-  // without a list the call is eppscore_schedule_batch_profiles
-  return schedule_batch(e, b, n_runs, runs, any ? topk : nullptr);
+  for (int32_t i = 0; i < n_runs; i++)
+    if ((rc = check_topk(e, topk[i], 0, e->cfg.max_endpoints, "[0, max_endpoints]")) != EPPSCORE_OK) return rc;
+  return schedule_batch(e, b, n_runs, runs, topk);
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,
