@@ -122,6 +122,7 @@ ABI_SYMBOLS = [
     ("eppscore_commit_picks", C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P]),
     ("eppscore_commit_picks_profiles", C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), _P, _P, C.c_int32, _P,
                                                    C.c_int32, C.c_int64, _P]),
+    ("eppscore_prefix_reserve", C.c_int32, [_P, C.c_int64, C.c_int64, C.c_int64]),
     ("eppscore_prefix_add", C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32]),
     ("eppscore_prefix_apply", C.c_int32, [_P, C.c_int64, _P, _P, _P]),
     ("eppscore_prefix_remove_endpoint", C.c_int32, [_P, C.c_int32]),

@@ -60,6 +60,7 @@ struct eppscore_engine {
   Geo geo{};
   int32_t A_cap = 64;
   Event ev_snapshot, ev_table, ev_caller;
+  Event ev_index_join;  // behind a commit captured on the engine stream: the caller's stream joins on it inside the capture
   Event ev_subset;  // behind the last set_snapshot outside a capture: its copies of the profiles' next subset rows are done
   cudaStream_t snapshot_stream = nullptr;        // stream the last snapshot preparation ran on
   unsigned long long snapshot_capture_id = 0;    // != 0: ev_snapshot was recorded inside that CUDA-graph capture
@@ -1203,6 +1204,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   if (int32_t rc = profile_init(ep, nullptr, 0)) return rc;
   // prefix index (device-resident: slot table + per-endpoint LRUs; the LRU regions are allocated by the first Add)
   CK(nullptr, make(ep->ev_caller));
+  CK(nullptr, make(ep->ev_index_join));
   ep->index = std::make_unique<DeviceIndex>(ep->geo.Mpad, ep->geo.Mpad / 32, ep->cfg.prefix_capacity, ep->cfg.lru_capacity_default,
                                             ep->cfg.lru_capacity_max);
   CK(nullptr, ep->index->init(ep->stream));
@@ -1844,6 +1846,15 @@ static int32_t pad_caps(eppscore_engine* e, const int32_t* lru_capacity, std::ve
   for (int32_t i = 0; i < n; i++) (*out)[i] = lru_capacity[i] > 0 ? lru_capacity[i] : 0;
   return EPPSCORE_OK;
 }
+// A reserved index reports a mutation it skipped for lack of room to the next index call outside a capture, which is refused.
+static int32_t index_skips(eppscore_engine* e, bool exact, const char* what) {
+  if (!e->index->reserved()) return EPPSCORE_OK;
+  bool skipped = false;
+  CK(e, e->index->new_skips(exact, e->stream, &skipped));
+  if (!skipped) return EPPSCORE_OK;
+  return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + ": an earlier index mutation found no room within eppscore_prefix_reserve's "
+                                        "sizes and was skipped whole (stats.index_error bit 4); this call was not run");
+}
 static int32_t index_status(eppscore_engine* e, cudaError_t c, const char* what) {
   if (c == cudaSuccess) return EPPSCORE_OK;
   if (c == cudaErrorInvalidValue)
@@ -1870,17 +1881,35 @@ static int32_t commit_calls(eppscore_engine* e, int32_t R, int32_t n_picks, cons
   const int32_t* d_picks[EPPSCORE_MAX_PROFILES] = {};
   if (on_device) {
     cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
+    // Under CUDA-graph capture only a reserved index can commit: room is then decided on the device at each replay.  Refused
+    // before anything is enqueued, so the capture stays valid.
+    const bool capturing = is_capturing(cs);
+    if (capturing && !e->index->reserved())
+      return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + " under CUDA-graph capture: reserve the prefix index before capturing "
+                                            "commits (eppscore_prefix_reserve)");
+    if (capturing && lru_capacity)
+      return fail(e, EPPSCORE_ERR_INVALID, std::string(what) + " under CUDA-graph capture: lru_capacity must be NULL (create the "
+                                           "endpoints' LRUs outside the capture, e.g. eppscore_prefix_add with n = 0)");
+    if (!capturing && (rc = index_skips(e, false, what)) != EPPSCORE_OK) return rc;
     if (cs != e->stream) {  // the arrays are produced on the caller's stream
       CK(e, cudaEventRecord(e->ev_caller, cs));
       CK(e, cudaStreamWaitEvent(e->stream, e->ev_caller, 0));
     }
-    if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
+    if (!capturing && (rc = index_begin(e)) != EPPSCORE_OK) return rc;  // (inside a capture the graph's edges order this)
     for (int32_t p = 0; p < n_picks; p++) d_picks[p] = picks[p];
-    const int32_t n_eps = e->M > 0 ? e->M : e->geo.Mpad;
+    // a graph covers every endpoint row: a replay after set_snapshot raised M still commits the new endpoints' picks
+    const int32_t n_eps = (e->M > 0 && !capturing) ? e->M : e->geo.Mpad;
     rc = index_status(e, e->index->commit(R, n_picks, d_picks, hashes, n_hashes, hash_stride, caps.empty() ? nullptr : caps.data(), 0, 0,
-                                          n_eps, touch_bound, e->stream),
+                                          n_eps, touch_bound, e->stream, capturing),
                       what);
     if (rc != EPPSCORE_OK) return rc;
+    if (capturing) {  // the engine stream joins the caller's capture again through an event recorded inside it
+      if (cs != e->stream) {
+        CK(e, cudaEventRecord(e->ev_index_join, e->stream));
+        CK(e, cudaStreamWaitEvent(cs, e->ev_index_join, 0));
+      }
+      return EPPSCORE_OK;
+    }
     if ((rc = index_end(e)) != EPPSCORE_OK) return rc;
     if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));  // stream-ordered for the caller
     return EPPSCORE_OK;
@@ -1943,7 +1972,8 @@ int32_t eppscore_prefix_add(eppscore_engine* e, const uint64_t* hashes, int32_t 
   if (n > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "more than 65535 hashes in one Add");
   if (endpoint < 0 || endpoint >= e->geo.Mpad) return fail(e, EPPSCORE_ERR_INVALID, "endpoint out of range");
   CK(e, cudaSetDevice(e->device));
-  int32_t rc = index_begin(e);
+  int32_t rc = index_skips(e, true, "prefix_add");
+  if (rc == EPPSCORE_OK) rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
   const int32_t stride = n > 0 ? n : 1;
   const uint16_t nh = (uint16_t)n;
@@ -1969,7 +1999,8 @@ int32_t eppscore_prefix_apply(eppscore_engine* e, int64_t n, const uint64_t* has
   for (int64_t i = 0; i < n; i++)
     if (endpoint[i] < 0 || endpoint[i] >= e->geo.Mpad) return fail(e, EPPSCORE_ERR_CAPACITY, "prefix_apply: endpoint out of range");
   CK(e, cudaSetDevice(e->device));
-  int32_t rc = index_begin(e);
+  int32_t rc = index_skips(e, true, "prefix_apply");
+  if (rc == EPPSCORE_OK) rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
   const uint64_t* d_hash;
   const int32_t* d_ep;
@@ -1986,7 +2017,8 @@ int32_t eppscore_prefix_apply(eppscore_engine* e, int64_t n, const uint64_t* has
 int32_t eppscore_prefix_remove_endpoint(eppscore_engine* e, int32_t endpoint) {
   if (!e) return EPPSCORE_ERR_INVALID;
   CK(e, cudaSetDevice(e->device));
-  int32_t rc = index_begin(e);
+  int32_t rc = index_skips(e, true, "prefix_remove_endpoint");
+  if (rc == EPPSCORE_OK) rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
   rc = index_status(e, e->index->remove_endpoint(endpoint, e->stream), "prefix_remove_endpoint");
   if (rc != EPPSCORE_OK) return rc;
@@ -2335,6 +2367,22 @@ int32_t eppscore_running_reserve(eppscore_engine* e, int64_t live_entries) {
     if ((rc = run_scratch(e, e->stream, live_entries, false)) != EPPSCORE_OK) return rc;
   }
   return (int32_t)(e->run_cap / 2);
+}
+
+int32_t eppscore_prefix_reserve(eppscore_engine* e, int64_t live_hashes, int64_t touches_per_call, int64_t overflow_rows) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  const int64_t lim = (int64_t)1 << 34;
+  if (live_hashes < 0 || touches_per_call < 0 || overflow_rows < 0 || live_hashes > lim || touches_per_call > lim || overflow_rows >= 0xFFFFFFF0LL)
+    return fail(e, EPPSCORE_ERR_INVALID, "prefix_reserve: an argument is negative or too large");
+  CK(e, cudaSetDevice(e->device));
+  if (capture_open(e, e->stream)) return fail(e, EPPSCORE_ERR_INVALID, "prefix_reserve under CUDA-graph capture");
+  if (live_hashes == 0) live_hashes = e->cfg.prefix_capacity;
+  if (touches_per_call == 0) touches_per_call = 65536;
+  if (overflow_rows == 0) overflow_rows = 2 * touches_per_call;
+  int32_t rc = index_begin(e);
+  if (rc != EPPSCORE_OK) return rc;
+  CK(e, e->index->reserve(live_hashes, touches_per_call, overflow_rows, e->stream));
+  return index_end(e);
 }
 
 int32_t eppscore_reserve_stream(eppscore_engine* e, void* stream, int32_t max_R, int32_t max_blocks) {

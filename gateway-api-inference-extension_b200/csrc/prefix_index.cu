@@ -6,6 +6,9 @@
 //     used slots + touches of this call  <= capacity / 2      else the table is rebuilt (dead slots dropped) or doubled,
 //     overflow rows in use + touches     <= overflow capacity else the pool is grown,
 // so no kernel can ever run out of room and nothing is retried.
+// A RESERVED index (reserve()) has a fixed table, a spare table of the same size and a fixed overflow pool; every mutation
+// first runs the room kernels (RoomOps in prefix_table.cuh), which take the same decision on the device — proceed, rebuild
+// into the spare, or skip the mutation whole — so no host wait is needed and the sequence can be captured into a CUDA graph.
 #include "prefix_index.hpp"
 
 #include <algorithm>
@@ -140,7 +143,7 @@ __global__ void index_apply_kernel(TableView* tv, int64_t n, const uint64_t* has
                                    uint32_t n_endpoints) {
   DevX x;
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n_endpoints) return;
+  if (p >= n_endpoints || x.ld32(&tv->room) == kRoomSkip) return;
   for (int64_t i = 0; i < n; i++) {
     if ((uint32_t)endpoint[i] != p) continue;
     if (op[i] == 0) TableOps<DevX>::set_member(x, tv, hash[i], p);
@@ -157,39 +160,76 @@ __global__ void table_get_kernel(const TableView* tv, uint64_t h, uint32_t* out,
 
 // Rebuild: re-insert every slot with a non-empty set into a fresh table (dead slots are dropped).
 __global__ void table_rehash_kernel(const TSlot* old_slots, uint64_t old_cap, TableView* nv) {
-  TSlot* ns = nv->slots;
-  const uint64_t mask = nv->mask;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint4 lo = __ldcg(reinterpret_cast<const uint4*>(old_slots + i));
-    const uint32_t cnt = lo.z;
-    if (cnt == kCntFree || (cnt & kCntMask) == 0) continue;
-    const uint4 hi = __ldcg(reinterpret_cast<const uint4*>(old_slots + i) + 1);
-    const uint64_t key = ((uint64_t)lo.y << 32) | lo.x;
-    for (uint64_t j = key & mask;; j = (j + 1) & mask) {
-      if (atomicCAS(&ns[j].cnt, kCntFree, kCntLock) == kCntFree) {  // keys are unique: claim, fill, publish
-        ns[j].key = key;
-        *slot_row_id(&ns[j]) = lo.w;  // ep[0..1] (or the row id)
-        *(reinterpret_cast<uint4*>(&ns[j]) + 1) = hi;
-        __threadfence();
-        atomicExch(&ns[j].cnt, cnt);
-        atomicAdd(&nv->used, 1ULL);
-        atomicAdd(&nv->live, 1ULL);
-        break;
-      }
-    }
+  DevX x;
+  unsigned long long moved = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < old_cap; i += (uint64_t)gridDim.x * blockDim.x)
+    moved += RoomOps<DevX>::rehash_slot(x, old_slots + i, nv->slots, nv->mask) ? 1 : 0;
+  if (moved) {
+    atomicAdd(&nv->used, moved);
+    atomicAdd(&nv->live, moved);
   }
 }
 
 // Σ n_hashes over the calls that have a pick: the exact number of touches of a commit whose arrays are on the device
 __global__ void sum_touches_kernel(const CommitArgs a, unsigned long long* out) {
   unsigned long long t = 0;
-  const int32_t np = a.n_picks > 1 ? a.n_picks : 1;
-  for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.R; r += gridDim.x * blockDim.x)
-    for (int32_t s = 0; s < np; s++)
-      if ((s == 0 ? a.pick : a.more_picks[s - 1])[r] >= 0) t += a.n_hashes[r];
+  for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.R; r += gridDim.x * blockDim.x) t += request_touches(a, r);
 #pragma unroll
   for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
   if ((threadIdx.x & 31) == 0 && t) atomicAdd(out, t);
+}
+
+// ---- a reserved index: room decided on the device (RoomOps), so a mutation never waits on the host ----
+// Every reserved mutation runs room -> clear spare -> rebuild -> the mutation, with launch shapes that depend only on the
+// reservation; the kernels with nothing to do exit at once.
+constexpr int kRoomThreads = 1024;
+constexpr int kRebuildCtas = 264, kRebuildThreads = 512;
+
+// The decision for one mutation: its touches are host_touches (>= 0), or summed here over a commit's calls.
+__global__ void __launch_bounds__(kRoomThreads) index_room_kernel(TableView* tv, const CommitArgs a, long long host_touches) {
+  __shared__ unsigned long long part[kRoomThreads / 32];
+  unsigned long long t = 0;
+  if (host_touches < 0)
+    for (int32_t r = threadIdx.x; r < a.R; r += kRoomThreads) t += request_touches(a, r);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long total = host_touches < 0 ? 0ULL : (unsigned long long)host_touches;
+    for (int w = 0; w < kRoomThreads / 32; w++) total += part[w];
+    DevX x;
+    RoomOps<DevX>::decide(x, tv, total);
+  }
+}
+
+__global__ void __launch_bounds__(kRebuildThreads) table_clear_spare_kernel(TableView* tv) {
+  DevX x;
+  if (x.ld32(&tv->room) != kRoomRebuild) return;
+  const uint64_t words = (tv->mask + 1) * (sizeof(TSlot) / 4);
+  uint32_t* w = reinterpret_cast<uint32_t*>(tv->spare);
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < words; i += (uint64_t)gridDim.x * blockDim.x)
+    RoomOps<DevX>::clear_spare_word(x, w, i);
+}
+
+// Rehashes the live slots into the (cleared) spare; the last CTA to finish swaps the two tables in the descriptor.
+__global__ void __launch_bounds__(kRebuildThreads) table_rebuild_kernel(TableView* tv) {
+  DevX x;
+  if (x.ld32(&tv->room) != kRoomRebuild) return;
+  const TSlot* old = tv->slots;
+  TSlot* ns = tv->spare;
+  const uint64_t mask = tv->mask;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= mask; i += (uint64_t)gridDim.x * blockDim.x)
+    RoomOps<DevX>::rehash_slot(x, old + i, ns, mask);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&tv->rebuild_done, 1u) == gridDim.x - 1) {
+      __threadfence();
+      RoomOps<DevX>::swap(tv);
+      tv->rebuild_done = 0;
+    }
+  }
 }
 
 // Σ lru.Len() over the endpoints (prefix_indexer_size metric, metrics.go:349)
@@ -218,6 +258,7 @@ DeviceIndex::DeviceIndex(int32_t n_endpoints, int32_t row_words, int64_t capacit
 
 DeviceIndex::~DeviceIndex() {
   if (d_slots_) cudaFree(d_slots_);
+  if (d_spare_) cudaFree(d_spare_);
   if (d_ovf_rows_) cudaFree(d_ovf_rows_);
   if (d_ovf_free_) cudaFree(d_ovf_free_);
   if (d_tv_) cudaFree(d_tv_);
@@ -262,7 +303,19 @@ cudaError_t DeviceIndex::refresh() {
     tv_.ovf_next = h->ovf_next;
     tv_.ovf_free_top = h->ovf_free_top;
     tv_.error = h->error;
+    tv_.rebuilds = h->rebuilds;
+    tv_.skips = h->skips;
   }
+  return cudaSuccess;
+}
+// the whole descriptor as of every mutation enqueued on `s` (synchronous): after graph replays, and before a reservation
+cudaError_t DeviceIndex::read_exact(cudaStream_t s) {
+  IX_CK(cudaStreamSynchronize(s));
+  IX_CK(cudaMemcpy(&tv_, d_tv_, sizeof(tv_), cudaMemcpyDeviceToHost));
+  d_slots_ = tv_.slots;  // the device may have swapped the table with its spare
+  d_spare_ = tv_.spare;
+  snap_pending_ = false;
+  captured_ = false;
   return cudaSuccess;
 }
 cudaError_t DeviceIndex::snapshot_after(cudaStream_t s) {
@@ -272,65 +325,106 @@ cudaError_t DeviceIndex::snapshot_after(cudaStream_t s) {
   return cudaSuccess;
 }
 
+// Moves the live slots into a new table of ncap slots (dead slots dropped) and points the descriptor at it; synchronous.
+cudaError_t DeviceIndex::rehash_into(uint64_t ncap, cudaStream_t s) {
+  const uint64_t cap = tv_.mask + 1;
+  TSlot* ns = nullptr;
+  IX_CK(cudaMalloc(&ns, ncap * sizeof(TSlot)));
+  IX_CK(cudaMemsetAsync(ns, 0xFF, ncap * sizeof(TSlot), s));
+  TableView nv = tv_;
+  nv.slots = ns;
+  nv.mask = ncap - 1;
+  nv.used = 0;
+  nv.live = 0;
+  IX_CK(cudaMemcpyAsync(d_tv_, &nv, sizeof(nv), cudaMemcpyHostToDevice, s));  // pageable source: staged before return
+  table_rehash_kernel<<<1184, 256, 0, s>>>(d_slots_, cap, d_tv_);
+  launches_++;
+  IX_CK(cudaGetLastError());
+  IX_CK(cudaStreamSynchronize(s));  // rare (amortised over >= cap/4 touches); lets the old array go right away
+  cudaFree(d_slots_);
+  d_slots_ = ns;
+  tv_.slots = ns;
+  tv_.mask = ncap - 1;
+  tv_.used = tv_.live;  // d_tv_ already holds the new view (counters were rebuilt by the kernel)
+  rebuilds_++;
+  return cudaSuccess;
+}
+
+// Replaces the overflow pool with one of ncap rows holding the same rows and free list; synchronous.
+cudaError_t DeviceIndex::grow_pool(uint64_t ncap, cudaStream_t s) {
+  if (ncap >= 0xFFFFFFF0ULL) return cudaErrorMemoryAllocation;
+  uint32_t* nr = nullptr;
+  uint32_t* nf = nullptr;
+  IX_CK(cudaMalloc(&nr, ncap * (size_t)row_words_ * 4));
+  IX_CK(cudaMalloc(&nf, ncap * 4));
+  if (tv_.ovf_next) IX_CK(cudaMemcpyAsync(nr, d_ovf_rows_, (size_t)tv_.ovf_next * row_words_ * 4, cudaMemcpyDeviceToDevice, s));
+  if (tv_.ovf_free_top) IX_CK(cudaMemcpyAsync(nf, d_ovf_free_, (size_t)tv_.ovf_free_top * 4, cudaMemcpyDeviceToDevice, s));
+  IX_CK(cudaStreamSynchronize(s));
+  if (d_ovf_rows_) cudaFree(d_ovf_rows_);
+  if (d_ovf_free_) cudaFree(d_ovf_free_);
+  d_ovf_rows_ = nr;
+  d_ovf_free_ = nf;
+  tv_.ovf_rows = nr;
+  tv_.ovf_free = nf;
+  tv_.ovf_cap = (uint32_t)ncap;
+  // only the pointer/capacity fields change; the counters on the device are current (no launch in flight: the caller waited)
+  IX_CK(cudaMemcpyAsync(&d_tv_->ovf_rows, &tv_.ovf_rows, sizeof(tv_.ovf_rows), cudaMemcpyHostToDevice, s));
+  IX_CK(cudaMemcpyAsync(&d_tv_->ovf_cap, &tv_.ovf_cap, sizeof(tv_.ovf_cap), cudaMemcpyHostToDevice, s));
+  IX_CK(cudaMemcpyAsync(&d_tv_->ovf_free, &tv_.ovf_free, sizeof(tv_.ovf_free), cudaMemcpyHostToDevice, s));
+  IX_CK(cudaStreamSynchronize(s));
+  return cudaSuccess;
+}
+
 // Make room for `touches` more set_member calls: each may claim one slot and one overflow row.
 cudaError_t DeviceIndex::ensure_room(int64_t touches, cudaStream_t s) {
   IX_CK(refresh());
   const uint64_t cap = tv_.mask + 1;
-  bool view_changed = false;
   if ((tv_.used + (uint64_t)touches) * 2 > cap) {
     // rebuild: same size when dropping the dead slots is enough (live + touches <= cap/4), else the next power of two
     uint64_t ncap = cap;
     while ((tv_.live + (uint64_t)touches) * 4 > ncap) ncap <<= 1;
-    TSlot* ns = nullptr;
-    IX_CK(cudaMalloc(&ns, ncap * sizeof(TSlot)));
-    IX_CK(cudaMemsetAsync(ns, 0xFF, ncap * sizeof(TSlot), s));
-    TSlot* old = d_slots_;
-    TableView nv = tv_;
-    nv.slots = ns;
-    nv.mask = ncap - 1;
-    nv.used = 0;
-    nv.live = 0;
-    IX_CK(cudaMemcpyAsync(d_tv_, &nv, sizeof(nv), cudaMemcpyHostToDevice, s));  // pageable source: staged before return
-    table_rehash_kernel<<<1184, 256, 0, s>>>(old, cap, d_tv_);
-    launches_++;
-    IX_CK(cudaGetLastError());
-    IX_CK(cudaStreamSynchronize(s));  // rare (amortised over >= cap/4 touches); lets the old array go right away
-    cudaFree(old);
-    d_slots_ = ns;
-    tv_.slots = ns;
-    tv_.mask = ncap - 1;
-    tv_.used = tv_.live;
-    rebuilds_++;
-    view_changed = false;  // d_tv_ already holds the new view (counters were rebuilt by the kernel)
+    IX_CK(rehash_into(ncap, s));
   }
   const uint64_t in_use = (uint64_t)tv_.ovf_next - tv_.ovf_free_top;
-  if (in_use + (uint64_t)touches > tv_.ovf_cap) {
-    uint64_t ncap = std::max<uint64_t>((in_use + (uint64_t)touches) * 5 / 4, 1024);
-    if (ncap >= 0xFFFFFFF0ULL) return cudaErrorMemoryAllocation;
-    uint32_t* nr = nullptr;
-    uint32_t* nf = nullptr;
-    IX_CK(cudaMalloc(&nr, ncap * (size_t)row_words_ * 4));
-    IX_CK(cudaMalloc(&nf, ncap * 4));
-    if (tv_.ovf_next) IX_CK(cudaMemcpyAsync(nr, d_ovf_rows_, (size_t)tv_.ovf_next * row_words_ * 4, cudaMemcpyDeviceToDevice, s));
-    if (tv_.ovf_free_top) IX_CK(cudaMemcpyAsync(nf, d_ovf_free_, (size_t)tv_.ovf_free_top * 4, cudaMemcpyDeviceToDevice, s));
-    IX_CK(cudaStreamSynchronize(s));
-    if (d_ovf_rows_) cudaFree(d_ovf_rows_);
-    if (d_ovf_free_) cudaFree(d_ovf_free_);
-    d_ovf_rows_ = nr;
-    d_ovf_free_ = nf;
-    tv_.ovf_rows = nr;
-    tv_.ovf_free = nf;
-    tv_.ovf_cap = (uint32_t)ncap;
-    view_changed = true;
-  }
-  if (view_changed) {
-    // only the pointer/capacity fields change; the counters on the device are current (no launch in flight: refresh() waited)
-    IX_CK(cudaMemcpyAsync(&d_tv_->ovf_rows, &tv_.ovf_rows, sizeof(tv_.ovf_rows), cudaMemcpyHostToDevice, s));
-    IX_CK(cudaMemcpyAsync(&d_tv_->ovf_cap, &tv_.ovf_cap, sizeof(tv_.ovf_cap), cudaMemcpyHostToDevice, s));
-    IX_CK(cudaMemcpyAsync(&d_tv_->ovf_free, &tv_.ovf_free, sizeof(tv_.ovf_free), cudaMemcpyHostToDevice, s));
-    IX_CK(cudaStreamSynchronize(s));
-  }
+  if (in_use + (uint64_t)touches > tv_.ovf_cap) IX_CK(grow_pool(std::max<uint64_t>((in_use + (uint64_t)touches) * 5 / 4, 1024), s));
   return cudaSuccess;
+}
+
+cudaError_t DeviceIndex::reserve(int64_t live_hashes, int64_t touches_per_call, int64_t overflow_rows, cudaStream_t s) {
+  IX_CK(read_exact(s));
+  uint64_t want = 32;
+  while (want < 4 * (uint64_t)(live_hashes + touches_per_call)) want <<= 1;
+  const bool grow = want > tv_.mask + 1;
+  if (grow) IX_CK(rehash_into(want, s));
+  if (grow || !d_spare_) {  // the spare needs no contents: every rebuild clears it first
+    if (d_spare_) cudaFree(d_spare_);
+    d_spare_ = nullptr;
+    IX_CK(cudaMalloc(&d_spare_, (tv_.mask + 1) * sizeof(TSlot)));
+    tv_.spare = d_spare_;
+  }
+  if ((uint64_t)overflow_rows > tv_.ovf_cap) IX_CK(grow_pool((uint64_t)overflow_rows, s));
+  IX_CK(ensure_lru(0, s));
+  tv_.room = kRoomProceed;
+  tv_.rebuild_done = 0;
+  IX_CK(cudaMemcpyAsync(d_tv_, &tv_, sizeof(tv_), cudaMemcpyHostToDevice, s));
+  IX_CK(cudaStreamSynchronize(s));
+  reserved_ = true;
+  return cudaSuccess;
+}
+
+cudaError_t DeviceIndex::new_skips(bool exact, cudaStream_t s, bool* out) {
+  if (exact || captured_) IX_CK(read_exact(s));
+  else if (snap_pending_ && cudaEventQuery(ev_snap_) == cudaSuccess) IX_CK(refresh());
+  *out = tv_.skips > skips_seen_;
+  skips_seen_ = tv_.skips;
+  return cudaSuccess;
+}
+
+void DeviceIndex::launch_room(const CommitArgs& a, long long host_touches, cudaStream_t s) {
+  index_room_kernel<<<1, kRoomThreads, 0, s>>>(d_tv_, a, host_touches);
+  table_clear_spare_kernel<<<kRebuildCtas, kRebuildThreads, 0, s>>>(d_tv_);
+  table_rebuild_kernel<<<kRebuildCtas, kRebuildThreads, 0, s>>>(d_tv_);
+  launches_ += 3;
 }
 
 cudaError_t DeviceIndex::ensure_lru(uint32_t want_cap, cudaStream_t s) {
@@ -369,7 +463,7 @@ int64_t DeviceIndex::lru_bytes() const {
 // PreRequest for a batch whose arrays are on the device; async on `s` (which must be the index's stream).
 cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes,
                                 const uint16_t* n_hashes, int32_t stride, const int32_t* cap_req_host, int32_t single_cap,
-                                int32_t ep_first, int32_t n_eps, int64_t max_touches, cudaStream_t s) {
+                                int32_t ep_first, int32_t n_eps, int64_t max_touches, cudaStream_t s, bool capturing) {
   if (R <= 0 || n_eps <= 0 || n_picks < 1 || n_picks > 4) return cudaSuccess;
   uint32_t want = (uint32_t)std::max(single_cap, 0);
   if (cap_req_host)
@@ -396,6 +490,15 @@ cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const
     for (int32_t p = 1; p < n_picks; p++) a.more_picks[p - 1] = picks[p] + r0;
     a.hashes = hashes + (size_t)r0 * stride;
     a.n_hashes = n_hashes + r0;
+    if (reserved_) {  // room decided on the device: nothing here waits on the host
+      launch_room(a, -1, s);
+      index_commit_kernel<<<n_eps, kCommitThreads, sizeof(CommitSmem), s>>>(d_tv_, d_lv_, a);
+      launches_++;
+      IX_CK(cudaGetLastError());
+      if (capturing) captured_ = true;
+      else IX_CK(snapshot_after(s));
+      continue;
+    }
     int64_t touches = std::min<int64_t>(max_touches, (int64_t)n * n_picks * stride);
     if (max_touches <= 0) {  // no bound from the caller: count them (one small synchronous read-back)
       unsigned long long* d_t = reinterpret_cast<unsigned long long*>(d_scratch_);
@@ -419,7 +522,8 @@ cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const
 
 cudaError_t DeviceIndex::apply(int64_t n, const uint64_t* hash, const int32_t* endpoint, const uint8_t* op, cudaStream_t s) {
   if (n <= 0) return cudaSuccess;
-  IX_CK(ensure_room(n, s));
+  if (reserved_) launch_room(CommitArgs{}, n, s);
+  else IX_CK(ensure_room(n, s));
   index_apply_kernel<<<(n_endpoints_ + 127) / 128, 128, 0, s>>>(d_tv_, n, hash, endpoint, op, (uint32_t)n_endpoints_);
   launches_++;
   IX_CK(cudaGetLastError());
@@ -428,7 +532,7 @@ cudaError_t DeviceIndex::apply(int64_t n, const uint64_t* hash, const int32_t* e
 
 cudaError_t DeviceIndex::remove_endpoint(int32_t p, cudaStream_t s) {
   if (!d_lv_ || p < 0 || p >= n_endpoints_) return cudaSuccess;
-  IX_CK(refresh());
+  if (!reserved_) IX_CK(refresh());  // (frees slots and rows only: no room to check)
   index_remove_kernel<<<1, kCommitThreads, sizeof(CommitSmem), s>>>(d_tv_, d_lv_, (uint32_t)p);
   launches_++;
   IX_CK(cudaGetLastError());
@@ -485,10 +589,10 @@ cudaError_t DeviceIndex::stats(IndexStats* out, cudaStream_t s) {
   out->live = (int64_t)h.live;
   out->capacity = (int64_t)((h.mask + 1) / 2);
   out->ovf_rows = (int64_t)h.ovf_next - (int64_t)h.ovf_free_top;
-  out->table_bytes = (int64_t)((h.mask + 1) * sizeof(TSlot)) + (int64_t)h.ovf_cap * row_words_ * 4;
+  out->table_bytes = (int64_t)((h.mask + 1) * sizeof(TSlot)) * (h.spare ? 2 : 1) + (int64_t)h.ovf_cap * row_words_ * 4;
   out->lru_bytes = lru_bytes();
   out->error = h.error;
-  out->rebuilds = rebuilds_;
+  out->rebuilds = rebuilds_ + (int64_t)h.rebuilds;
   out->lru_entries = 0;
   if (d_lv_) {
     unsigned long long* d_t = reinterpret_cast<unsigned long long*>(d_scratch_);

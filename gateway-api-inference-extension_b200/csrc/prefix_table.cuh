@@ -70,8 +70,15 @@ struct TableView {
   uint32_t ovf_free_top;    // free-list stack of released rows
   uint32_t* ovf_free;       // [ovf_cap]
   uint32_t ovf_lock;
-  uint32_t error;           // sticky: 1 = overflow pool exhausted (host sizing bug), 2 = table full
+  uint32_t error;           // sticky: 1 = overflow pool exhausted (host sizing bug), 2 = table full, kErrSkipped
+  // A reserved index (DeviceIndex::reserve) decides room on the device (RoomOps below): these fields stay zero otherwise.
+  TSlot* spare;             // a second table of the same capacity: the target of a same-size rebuild, then swapped in
+  uint64_t rebuilds;        // device-side rebuilds
+  uint64_t skips;           // mutations skipped for lack of room
+  uint32_t room;            // kRoomProceed / kRoomRebuild / kRoomSkip: the decision for the mutation being run
+  uint32_t rebuild_done;    // CTAs of the rebuild kernel that have finished (the last one swaps the tables)
 };
+constexpr uint32_t kErrSkipped = 4u;  // sticky: a reserved mutation was skipped whole, the index is as it was before it
 
 constexpr uint64_t kSeqFree = ~0ULL;
 constexpr uint64_t kSeqTomb = ~0ULL - 1;
@@ -344,6 +351,80 @@ struct CommitArgs {
   // request.  0 or 1: `pick` alone.
   int32_t n_picks;
   const int32_t* more_picks[3];
+};
+
+// Σ n_hashes over request r's calls that have a pick: the set_member calls request r can make
+PT_HD uint64_t request_touches(const CommitArgs& a, int32_t r) {
+  const int32_t np = a.n_picks > 1 ? a.n_picks : 1;
+  uint64_t t = 0;
+  for (int32_t s = 0; s < np; s++)
+    if ((s == 0 ? a.pick : a.more_picks[s - 1])[r] >= 0) t += a.n_hashes[r];
+  return t;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Room on the device (a reserved index: table + spare of a fixed capacity, a fixed overflow pool).  Before every mutation
+// that may claim `touches` slots and overflow rows (one each per set_member at most):
+//     rows in use + touches > pool                    -> skip: the mutation does not run at all
+//     used + touches <= cap / 2                       -> proceed
+//     live + touches <= cap / 4                       -> rebuild into the spare (dead slots dropped, same size), proceed
+//     otherwise                                       -> skip
+// A skipped mutation leaves the index bit-identical and sets kErrSkipped; the table never changes size.
+// ------------------------------------------------------------------------------------------------------------------
+enum : uint32_t { kRoomProceed = 0, kRoomRebuild = 1, kRoomSkip = 2 };
+
+PT_HD uint32_t room_decision(uint64_t used, uint64_t live, uint64_t cap, uint64_t ovf_in_use, uint64_t ovf_cap,
+                             uint64_t touches) {
+  if (ovf_in_use + touches > ovf_cap) return kRoomSkip;
+  if ((used + touches) * 2 <= cap) return kRoomProceed;
+  if ((live + touches) * 4 <= cap) return kRoomRebuild;
+  return kRoomSkip;
+}
+
+template <class X>
+struct RoomOps {
+  // One thread, after every earlier mutation: publishes the decision in tv->room.  A rebuild keeps exactly the live slots.
+  static PT_HD uint32_t decide(X& x, TableView* tv, uint64_t touches) {
+    uint64_t* live_p = reinterpret_cast<uint64_t*>(&tv->live);
+    uint64_t* used_p = reinterpret_cast<uint64_t*>(&tv->used);
+    const uint64_t used = x.ld64(used_p), live = x.ld64(live_p);
+    const uint64_t in_use = (uint64_t)x.ld32(&tv->ovf_next) - x.ld32(&tv->ovf_free_top);
+    const uint32_t d = room_decision(used, live, tv->mask + 1, in_use, tv->ovf_cap, touches);
+    if (d == kRoomRebuild) {
+      x.st64(used_p, live);
+      x.st64(&tv->rebuilds, x.ld64(&tv->rebuilds) + 1);
+    } else if (d == kRoomSkip) {
+      x.st64(&tv->skips, x.ld64(&tv->skips) + 1);
+      x.st32(&tv->error, x.ld32(&tv->error) | kErrSkipped);
+    }
+    x.st32(&tv->room, d);
+    return d;
+  }
+  // Rebuild, pass 1 (every 32-bit word i of the spare): empty
+  static PT_HD void clear_spare_word(X& x, uint32_t* spare_words, uint64_t i) { x.st32(&spare_words[i], 0xFFFFFFFFu); }
+  // Rebuild, pass 2 (every slot of the table): a slot with a non-empty set moves to table `ns` unchanged (members, filler and
+  // row id: a canonical slot stays canonical); dead slots are dropped.  Keys are unique, so a claimed slot is never compared:
+  // claim, fill, publish.  Returns whether the slot moved.
+  static PT_HD bool rehash_slot(X& x, const TSlot* old, TSlot* ns, uint64_t mask) {
+    const uint32_t cnt = x.ld32(&old->cnt);
+    if (cnt == kCntFree || (cnt & kCntMask) == 0) return false;
+    const uint64_t key = x.ld64(&old->key);
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(old);
+    for (uint64_t j = key & mask;; j = (j + 1) & mask) {
+      if (x.cas32(&ns[j].cnt, kCntFree, kCntLock) != kCntFree) continue;
+      x.st64(&ns[j].key, key);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(ns + j);
+      for (int k = 3; k < (int)(sizeof(TSlot) / 4); k++) x.st32(&dst[k], x.ld32(&src[k]));  // ep[0..10)
+      x.st_release32(&ns[j].cnt, cnt);
+      return true;
+    }
+  }
+  // Rebuild, last: the spare becomes the table (the old table is the next rebuild's spare)
+  static PT_HD void swap(TableView* tv) {
+    TSlot* t = tv->slots;
+    tv->slots = tv->spare;
+    tv->spare = t;
+  }
 };
 
 template <class X>
@@ -622,6 +703,7 @@ struct IndexProgram {
   // `fill` (touches waiting in sm->tkey) and every branch below are CTA-uniform: all threads compute them identically
   // from values that were published by a completed parallel section.
   PT_HD void commit(const CommitArgs& a) {
+    if (x.ld32(&tv->room) == kRoomSkip) return;  // all or nothing: no room was guaranteed for this call (RoomOps)
     bool created = x.ld32(&d->created) != 0;
     const int32_t cap_req = a.cap_req ? a.cap_req[p] : a.single_cap;
     uint32_t fill = 0, cap = 0, chunk_cap = 0;

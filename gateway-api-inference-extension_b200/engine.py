@@ -556,6 +556,11 @@ class Engine:
         self._check(self._lib.eppscore_commit_picks_profiles(self._h, R, len(pp), arr, hp, nhp, stride, ah.ptr(lru_capacity, np.int32),
                                                              1 if device else 0, int(touch_bound), stream))
 
+    def prefix_reserve(self, live_hashes=0, touches_per_call=0, overflow_rows=0):
+        """Sizes the prefix index up front (eppscore_prefix_reserve): from then on commits decide their room on the device,
+        never wait on the host and may be captured into CUDA graphs.  0 picks the documented default of each size."""
+        self._check(self._lib.eppscore_prefix_reserve(self._h, int(live_hashes), int(touches_per_call), int(overflow_rows)))
+
     def prefix_add(self, hashes, endpoint, lru_capacity=0):
         a = _Args(False)
         h = np.ascontiguousarray(hashes, np.uint64)

@@ -292,7 +292,8 @@ typedef struct eppscore_stats {
   int64_t lru_bytes;            /* device bytes of the per-endpoint LRU regions (maps + logs) */
   int64_t prefix_overflow_rows; /* sets of more than 10 endpoints (bitset rows in use) */
   int64_t prefix_rebuilds;      /* table rebuilds so far */
-  uint32_t index_error;         /* sticky device-side error flags of the index (0 = healthy) */
+  uint32_t index_error;         /* sticky device-side error flags of the index (0 = healthy; bit 4: a mutation was skipped
+                                   for lack of room, see eppscore_prefix_reserve) */
   uint32_t probe_resolved;      /* requests whose prefix match the hashing kernel settled itself, so the pick kernel skipped
                                    their index probe; since creation, modulo 2^32 (diagnostics: read after the batches finished) */
 } eppscore_stats;
@@ -423,7 +424,10 @@ int32_t eppscore_commit_picks(struct eppscore_engine *e, int32_t R, const int32_
                               const uint16_t *n_hashes, int32_t hash_stride, const int32_t *lru_capacity);
 /* The same with DEVICE arrays (e.g. the pick / hashes_out buffers of a device-location eppscore_schedule_batch): nothing
  * crosses PCIe, the call is asynchronous and ordered on `stream` (NULL = engine stream).  touch_bound: an upper bound on
- * Σ n_hashes (room is guaranteed up front); <= 0 ⇒ the engine sums n_hashes itself (one small synchronous read-back). */
+ * Σ n_hashes (room is guaranteed up front); <= 0 ⇒ the engine sums n_hashes itself (one small synchronous read-back).
+ * After eppscore_prefix_reserve the call never waits on the host (touch_bound is ignored: the device counts the touches and
+ * decides the room) and may be captured into a CUDA graph; without the reserve a call on a stream under capture fails with
+ * ERR_CAPACITY before anything is enqueued (the capture stays valid).  See eppscore_prefix_reserve. */
 int32_t eppscore_commit_picks_device(struct eppscore_engine *e, int32_t R, const int32_t *pick, const uint64_t *hashes,
                                      const uint16_t *n_hashes, int32_t hash_stride, const int32_t *lru_capacity,
                                      int64_t touch_bound, void *stream);
@@ -436,6 +440,27 @@ int32_t eppscore_commit_picks_device(struct eppscore_engine *e, int32_t R, const
 int32_t eppscore_commit_picks_profiles(struct eppscore_engine *e, int32_t R, int32_t n_picks, const int32_t *const *picks,
                                        const uint64_t *hashes, const uint16_t *n_hashes, int32_t hash_stride,
                                        const int32_t *lru_capacity, int32_t location, int64_t touch_bound, void *stream);
+/* Reserves the prefix index up front, so that commits decide their room on the device and can run inside CUDA graphs.
+ * Allocates, synchronously and outside any capture (ERR_INVALID under one): a slot table and a spare table of at least
+ * 4 * (live_hashes + touches_per_call) slots each (a power of two; 32 bytes per slot), an overflow pool of at least
+ * overflow_rows rows (max_endpoints / 8 bytes each), and the per-endpoint LRU regions for config.lru_capacity_max.  0 picks a
+ * default: live_hashes = config.prefix_capacity, touches_per_call = 65536, overflow_rows = 2 * touches_per_call.  A later
+ * reserve with larger sizes grows the table, the spare and the pool (never shrinks them, never the LRU regions); graphs
+ * captured earlier stay valid, as every kernel reads the index through its device descriptor.
+ * From then on every index mutation (commits, eppscore_prefix_add, eppscore_prefix_apply) runs a fixed kernel sequence that
+ * counts the call's touches on the device and, with `used` slots ever claimed and `live` non-empty sets of `cap` slots:
+ *   - proceeds when used + touches <= cap / 2;
+ *   - else rebuilds the table into the spare (dead slots dropped, same size) and proceeds when live + touches <= cap / 4;
+ *   - else, or when overflow rows in use + touches exceed the pool, skips the call whole: the index stays as it was,
+ *     stats.index_error gets bit 4, and the next index mutation outside a capture fails with ERR_CAPACITY (a device commit
+ *     sees it once the counters copied back behind the skipped call have landed, a host-array call at once).
+ * The table never changes size behind a captured graph.  Inside a capture a commit's lru_capacity must be NULL (ERR_INVALID):
+ * an LRU's size is fixed by the endpoint's first Add, so create the LRUs that need another size outside the capture (e.g.
+ * eppscore_prefix_add with n = 0).  A captured commit covers every endpoint row up to max_endpoints, so a replay after
+ * eppscore_set_snapshot raised M still records picks on the new endpoints.  After a captured commit, the next host-side index
+ * call reads the device counters once, synchronously.  Returns EPPSCORE_OK or a negative status. */
+int32_t eppscore_prefix_reserve(struct eppscore_engine *e, int64_t live_hashes, int64_t touches_per_call,
+                                int64_t overflow_rows);
 /* indexer.Add for one server (tests). */
 int32_t eppscore_prefix_add(struct eppscore_engine *e, const uint64_t *hashes, int32_t n, int32_t endpoint,
                             int32_t lru_capacity);
