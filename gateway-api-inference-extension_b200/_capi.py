@@ -127,6 +127,7 @@ ABI_SYMBOLS = [
     ("eppscore_prefix_apply", C.c_int32, [_P, C.c_int64, _P, _P, _P]),
     ("eppscore_prefix_remove_endpoint", C.c_int32, [_P, C.c_int32]),
     ("eppscore_prefix_get", C.c_int32, [_P, C.c_uint64, _P, C.c_int32]),
+    ("eppscore_prefix_match", C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P]),
     ("eppscore_prefix_lru_len", C.c_int32, [_P, C.c_int32]),
     ("eppscore_prefix_lru_keys", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_commit_picks_device", C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int64, _P]),

@@ -2050,6 +2050,43 @@ int32_t eppscore_prefix_get(eppscore_engine* e, uint64_t hash, uint32_t* bitset_
   return count;
 }
 
+int32_t eppscore_prefix_match(eppscore_engine* e, int32_t R, int32_t k, int32_t location, const uint64_t* hashes,
+                              const uint16_t* n_hashes, int32_t hash_stride, const int32_t* endpoints, uint16_t* match_out,
+                              void* stream) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (location != 0 && location != 1) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: location must be 0 or 1");
+  if (k < 1 || k > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: k must be in [1, max_endpoints]");
+  if (R < 0 || (R > 0 && (!hashes || !n_hashes || !endpoints || !match_out))) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: NULL argument");
+  if (R == 0) return EPPSCORE_OK;
+  if (hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: hash_stride must be > 0");
+  CK(e, cudaSetDevice(e->device));
+  if (location == 1) {
+    // Ordered like a device-location batch: after the index mutations issued before it (ev_table), and registered as pending so
+    // that later mutations wait for it.  Inside a capture the graph's edges order it.
+    cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
+    if (!is_capturing(cs) && cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
+    e->index->match(R, k, e->cfg.max_endpoints, hashes, n_hashes, hash_stride, endpoints, match_out, cs);
+    CK(e, cudaGetLastError());
+    return pending_record(e, cs);
+  }
+  for (int32_t r = 0; r < R; r++)
+    if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: n_hashes exceeds hash_stride");
+  const uint64_t* d_hash;
+  const uint16_t* d_nh;
+  const int32_t* d_ep;
+  int32_t rc;
+  if ((rc = h2d(e, e->stage[0], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], n_hashes, (size_t)R, &d_nh)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], endpoints, (size_t)R * k, &d_ep)) != EPPSCORE_OK)
+    return rc;
+  CK(e, e->stage[3].reserve((size_t)R * k * 2));
+  e->index->match(R, k, e->cfg.max_endpoints, d_hash, d_nh, hash_stride, d_ep, e->stage[3].as<uint16_t>(), e->stream);
+  CK(e, cudaGetLastError());
+  CK(e, cudaMemcpyAsync(match_out, e->stage[3].p, (size_t)R * k * 2, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  return EPPSCORE_OK;
+}
+
 // ---------------- in-flight load producer ----------------
 int32_t eppscore_estimate_tokens(eppscore_engine* e, int32_t R, int32_t location, const int64_t* request_size_bytes,
                                  const int32_t* token_hint, const int32_t* prompt_chars, int64_t* out, void* stream) {

@@ -158,6 +158,56 @@ __global__ void table_get_kernel(const TableView* tv, uint64_t h, uint32_t* out,
   out[0] = table_get(x, tv, h, out + 1, words);
 }
 
+// Loads for a kernel that only reads the index while no mutation runs (stream order and the pending-batch rules order it
+// against them): through the read-only cache, so the member loads of a probe hit the line its first load brought in.
+struct ReadX {
+  __device__ __forceinline__ uint32_t ld32(const uint32_t* p) { return __ldg(p); }
+  __device__ __forceinline__ uint64_t ld64(const uint64_t* p) { return __ldg(reinterpret_cast<const unsigned long long*>(p)); }
+  __device__ __forceinline__ uint32_t ld16(const uint16_t* p) { return __ldg(p); }
+};
+
+// matchLongestPrefix (approximateprefix/plugin.go:219-235) read at k endpoints per request: one warp per request.  Lane b probes
+// block base + b (32 probes in flight), the ballot of misses gives the first one, and each listed endpoint's count of the hits
+// before it is a ballot of the lanes whose set holds the endpoint.  Lane j keeps endpoint j's count (j < 32); the counts of
+// endpoints past 32 accumulate in the request's out row.
+constexpr int kMatchThreads = 256;
+__global__ void __launch_bounds__(kMatchThreads) prefix_match_kernel(const TableView* tv, int32_t R, int32_t k, uint32_t limit,
+                                                                     const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
+                                                                     const int32_t* endpoints, uint16_t* out) {
+  ReadX x;
+  const uint32_t lane = threadIdx.x & 31;
+  const int32_t warps = gridDim.x * (kMatchThreads / 32);
+  for (int32_t r = blockIdx.x * (kMatchThreads / 32) + (threadIdx.x >> 5); r < R; r += warps) {
+    const uint32_t n = n_hashes[r];
+    const uint64_t* h = hashes + (size_t)r * stride;
+    const int32_t* eps = endpoints + (size_t)r * k;
+    uint16_t* o = out + (size_t)r * k;
+    const int32_t k0 = k < 32 ? k : 32;
+    const uint32_t e0 = (int32_t)lane < k0 ? (uint32_t)eps[lane] : 0xFFFFFFFFu;  // (-1 and >= limit never match)
+    uint32_t c0 = 0;
+    for (uint32_t base = 0;; base += 32) {  // at least one round: it writes the row's entries past 32
+      uint32_t raw = 0;
+      TSlot* s = base + lane < n ? table_find(x, tv, h[base + lane], &raw) : nullptr;
+      const uint32_t miss = __ballot_sync(0xffffffffu, base + lane < n && !s);
+      const uint32_t left = n > base ? n - base : 0;
+      const uint32_t hits = miss ? (uint32_t)__ffs(miss) - 1 : (left < 32 ? left : 32);
+      const bool hit = lane < hits;
+      for (int32_t j = 0; j < k0; j++) {
+        const uint32_t e = __shfl_sync(0xffffffffu, e0, j);
+        const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
+        if ((int32_t)lane == j) c0 += c;
+      }
+      for (int32_t j = 32; j < k; j++) {
+        const uint32_t e = (uint32_t)__ldg(&eps[j]);
+        const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
+        if (lane == (uint32_t)(j & 31)) o[j] = (uint16_t)((base == 0 ? 0u : o[j]) + c);
+      }
+      if (miss || base + 32 >= n) break;
+    }
+    if ((int32_t)lane < k0) o[lane] = (uint16_t)c0;
+  }
+}
+
 // Rebuild: re-insert every slot with a non-empty set into a fresh table (dead slots are dropped).
 __global__ void table_rehash_kernel(const TSlot* old_slots, uint64_t old_cap, TableView* nv) {
   DevX x;
@@ -518,6 +568,13 @@ cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const
     IX_CK(snapshot_after(s));
   }
   return cudaSuccess;
+}
+
+void DeviceIndex::match(int32_t R, int32_t k, int32_t limit, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
+                        const int32_t* endpoints, uint16_t* out, cudaStream_t s) {
+  const int32_t ctas = std::min((R + kMatchThreads / 32 - 1) / (kMatchThreads / 32), 8192);
+  prefix_match_kernel<<<ctas, kMatchThreads, 0, s>>>(d_tv_, R, k, (uint32_t)limit, hashes, n_hashes, stride, endpoints, out);
+  launches_++;
 }
 
 cudaError_t DeviceIndex::apply(int64_t n, const uint64_t* hash, const int32_t* endpoint, const uint8_t* op, cudaStream_t s) {

@@ -46,6 +46,11 @@ class DeviceIndex {
   cudaError_t commit(int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
                      const int32_t* cap_req_host, int32_t single_cap, int32_t ep_first, int32_t n_eps, int64_t max_touches,
                      cudaStream_t s, bool capturing = false);
+  // matchLongestPrefix of R requests (device arrays, R >= 1) read at k endpoints each: out[r*k + j] = the hit blocks before
+  // request r's first miss whose set holds endpoints[r*k + j]; 0 for entries outside [0, limit).  One launch of a fixed shape,
+  // async on `s`; reads the index through its descriptor.
+  void match(int32_t R, int32_t k, int32_t limit, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
+             const int32_t* endpoints, uint16_t* out, cudaStream_t s);
   cudaError_t apply(int64_t n, const uint64_t* hash, const int32_t* endpoint, const uint8_t* op, cudaStream_t s);  // device arrays
   cudaError_t remove_endpoint(int32_t p, cudaStream_t s);
   cudaError_t lru_keys(int32_t p, uint64_t* out_host, int32_t cap, int32_t* len, cudaStream_t s);

@@ -828,17 +828,52 @@ struct IndexProgram {
   }
 };
 
-// indexer.Get (indexer.go:86-102) for one hash, read-only: writes the set as a natural-order bitset, returns its size.
-template <class X>
-PT_HD uint32_t table_get(X& x, const TableView* tv, uint64_t h, uint32_t* bits, uint32_t words) {
-  for (uint32_t w = 0; w < words; w++) bits[w] = 0;
+// indexer.Get's lookup (indexer.go:86-102), read-only: found(slot, cnt word) when `h` has a non-empty set, else 0 (absent, or an
+// emptied set, which the reference has deleted).
+template <class X, class F>
+PT_HD uint32_t table_probe(X& x, const TableView* tv, uint64_t h, F found) {
   for (uint64_t i = h & tv->mask, n = 0; n <= tv->mask; i = (i + 1) & tv->mask, n++) {
     TSlot* s = &tv->slots[i];
     const uint32_t raw = x.ld32(&s->cnt);
     if (raw == kCntFree) return 0;
     if (x.ld64(&s->key) != h) continue;
+    if ((raw & kCntMask) == 0) return 0;
+    return found(s, raw);
+  }
+  return 0;
+}
+// The slot of `h` when its set is non-empty, else nullptr; *raw receives the slot's cnt word.
+template <class X>
+PT_HD TSlot* table_find(X& x, const TableView* tv, uint64_t h, uint32_t* raw) {
+  TSlot* hit = nullptr;
+  table_probe(x, tv, h, [&](TSlot* s, uint32_t c) {
+    hit = s;
+    *raw = c;
+    return 1u;
+  });
+  return hit;
+}
+
+// Whether endpoint p is in the set of a slot table_find returned: a compare against the inline members, or bit p of the row.
+template <class X>
+PT_HD bool slot_holds(X& x, const TableView* tv, TSlot* s, uint32_t raw, uint32_t p) {
+  if (raw & kCntRow) {
+    if ((p >> 5) >= tv->row_words) return false;
+    const uint32_t r = x.ld32(slot_row_id(s));
+    return (x.ld32(&tv->ovf_rows[(size_t)r * tv->row_words + (p >> 5)]) >> (p & 31)) & 1u;
+  }
+  const uint32_t c = raw & kCntMask;
+  for (uint32_t k = 0; k < c; k++)
+    if (x.ld16(&s->ep[k]) == p) return true;
+  return false;
+}
+
+// indexer.Get (indexer.go:86-102) for one hash, read-only: writes the set as a natural-order bitset, returns its size.
+template <class X>
+PT_HD uint32_t table_get(X& x, const TableView* tv, uint64_t h, uint32_t* bits, uint32_t words) {
+  for (uint32_t w = 0; w < words; w++) bits[w] = 0;
+  return table_probe(x, tv, h, [&](TSlot* s, uint32_t raw) {
     const uint32_t c = raw & kCntMask;
-    if (c == 0) return 0;
     if (raw & kCntRow) {
       const uint32_t r = x.ld32(slot_row_id(s));
       for (uint32_t w = 0; w < words && w < tv->row_words; w++) bits[w] = x.ld32(&tv->ovf_rows[(size_t)r * tv->row_words + w]);
@@ -849,8 +884,7 @@ PT_HD uint32_t table_get(X& x, const TableView* tv, uint64_t h, uint32_t* bits, 
       }
     }
     return c;
-  }
-  return 0;
+  });
 }
 
 }  // namespace eppscore

@@ -584,6 +584,29 @@ class Engine:
         assert len(s) == n, (s, n)
         return s
 
+    def prefix_match(self, hashes, n_hashes, endpoints, device=False, stream=None, out=None):
+        """PrefixCacheMatchInfo.matchBlocks at chosen endpoints (eppscore_prefix_match): endpoints is [R, k] (int32, -1 and
+        entries >= max_endpoints give 0), hashes [R, stride] and n_hashes [R] as for the commit calls.  Host mode returns a
+        uint16 array [R, k].  device=True: CUDA tensors / raw pointers, asynchronous on `stream`; `out` is a preallocated
+        uint16 (torch.int16 / torch.uint16) tensor [R, k] that the call fills, and is returned."""
+        a = _Args(device)
+        if device:
+            R, k = int(endpoints.shape[0]), int(endpoints.shape[1])
+            stride = int(hashes.shape[1])
+            if out is None:
+                raise ValueError("device mode fills a preallocated `out` tensor")
+            self._check(self._lib.eppscore_prefix_match(self._h, R, k, 1, a.ptr(hashes, None), a.ptr(n_hashes, None), stride,
+                                                        a.ptr(endpoints, None), a.ptr(out, None), _stream_handle(stream)))
+            return out
+        endpoints = np.ascontiguousarray(endpoints, np.int32)
+        hashes = np.ascontiguousarray(hashes, np.uint64)
+        R, k = endpoints.shape
+        stride = hashes.shape[1] if hashes.ndim == 2 else 0
+        res = np.zeros((R, k), np.uint16)
+        self._check(self._lib.eppscore_prefix_match(self._h, R, k, 0, a.ptr(hashes, np.uint64), a.ptr(n_hashes, np.uint16), stride,
+                                                    a.ptr(endpoints, np.int32), res.ctypes.data, None))
+        return res
+
     def prefix_lru_len(self, endpoint) -> int:
         return self._lib.eppscore_prefix_lru_len(self._h, endpoint)
 

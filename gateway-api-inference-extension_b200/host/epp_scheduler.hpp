@@ -17,6 +17,7 @@
 // become the per-request candidate mask.  One Scheduler owns one engine (one GPU).
 #pragma once
 #include <algorithm>
+#include <array>
 #include <cstdint>
 #include <functional>
 #include <map>
@@ -93,6 +94,33 @@ extern "C" int32_t eppscore_schedule_batch_profiles_topk(struct eppscore_engine*
                                                          const eppscore_profile_run* runs, const eppscore_topk* topk)
     __attribute__((weak));
 inline bool EngineHasProfilesTopK() { return EngineHasProfiles() && &eppscore_schedule_batch_profiles_topk != nullptr; }
+// eppscore_prefix_match (PrefixCacheMatchInfo at chosen endpoints) came the same way: EngineHasPrefixMatch() tells.  Without it a
+// config with SchedulerConfig::PrefixMatchInfo is refused when the Scheduler is built.
+extern "C" int32_t eppscore_prefix_match(struct eppscore_engine* e, int32_t R, int32_t k, int32_t location, const uint64_t* hashes,
+                                         const uint16_t* n_hashes, int32_t hash_stride, const int32_t* endpoints, uint16_t* match_out,
+                                         void* stream) __attribute__((weak));
+inline bool EngineHasPrefixMatch() { return &eppscore_prefix_match != nullptr; }
+
+// A prometheus histogram as client_golang keeps it: an observation lands in the first bucket whose upper bound is >= it
+// (sort.SearchFloat64s over the bounds), past the last bound in +Inf; Count and Sum accumulate in observation order.
+template <size_t N>
+struct Histogram {
+  std::array<double, N> UpperBounds;
+  std::array<uint64_t, N + 1> Counts{};  // per bucket, not cumulative: Counts[i] for UpperBounds[i], Counts[N] for +Inf
+  uint64_t Count = 0;
+  double Sum = 0.0;
+  void Observe(double v) {
+    Counts[(size_t)(std::lower_bound(UpperBounds.begin(), UpperBounds.end(), v) - UpperBounds.begin())]++;
+    Count++;
+    Sum += v;
+  }
+};
+// The approximate-prefix producer's two PreRequest histograms (metrics.go:358-377), fed by RecordPrefixCacheMatch (:830-841).
+struct PrefixIndexerHistograms {
+  Histogram<11> HitRatio{{0.0, 0.1, 0.2, 0.3, 0.4, 0.5, 0.6, 0.7, 0.8, 0.9, 1.0}};  // prefix_indexer_hit_ratio
+  Histogram<14> HitBytes{{0, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536}};  // prefix_indexer_hit_bytes
+};
+
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
          &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
@@ -286,6 +314,13 @@ struct SchedulerConfig {
   // ResponseStarted (inflightload/producer.go:137-160).
   std::vector<std::pair<std::string, SchedulerProfile>> Profiles;
   std::shared_ptr<ProfileHandler> Handler;
+  // Opt-in (off by default): after each engine batch that hashed its prompts, one eppscore_prefix_match call gives every
+  // TargetEndpoints entry of every profile (lists and the "prefill" profile included) its PrefixCacheMatchInfo, as
+  // PrepareRequestData puts it on every endpoint (approximateprefix/plugin.go:140-153), and PreRequest records the
+  // prefix-indexer histograms for the primary target (plugin.go:199-204; Scheduler::PrefixIndexerMetrics).  Batches the engine
+  // did not hash (the small-batch host route, a config without prefix hashing) leave it empty.  Needs an engine library with
+  // eppscore_prefix_match.
+  bool PrefixMatchInfo = false;
 };
 
 class Scheduler {
@@ -380,6 +415,8 @@ class Scheduler {
       throw SchedulingError("maxNumOfEndpoints > 1 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk");
     if (cfg.InFlightLoad && !EngineHasInFlightLoad())
       throw SchedulingError("the inflight-load-producer needs an engine library with eppscore_inflight_add");
+    if (cfg.PrefixMatchInfo && !EngineHasPrefixMatch())
+      throw SchedulingError("SchedulerConfig::PrefixMatchInfo needs an engine library with eppscore_prefix_match");
     inflight_ = cfg.InFlightLoad != nullptr;
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
@@ -744,6 +781,13 @@ class Scheduler {
         }
       }
     }
+    if (cfg_.PrefixMatchInfo && want_prefix) {
+      std::vector<std::vector<ScoredEndpoint*>> targets((size_t)R);
+      for (int r = 0; r < R; r++)
+        if (out[r].error.empty())
+          for (ScoredEndpoint& t : out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints) targets[(size_t)r].push_back(&t);
+      FillPrefixMatch(targets, last_hashes_.data(), last_nh_.data(), last_stride_, ids, block_tokens);
+    }
     return out;
   }
 
@@ -752,6 +796,7 @@ class Scheduler {
   // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
   // (inflightload/producer.go:101-120).
   void PreRequest(const std::vector<BatchItem>& results) {
+    RecordPrefixCacheMatch(results);
     if (!last_endpoints_ || (last_hashes_.empty() && !inflight_ && !running_)) return;
     if (!cfg_.Profiles.empty()) return PreRequestProfiles(results);
     const int R = (int)results.size();
@@ -880,9 +925,60 @@ class Scheduler {
   uint64_t RemappedBatches() const { return remapped_batches_; }  // batches whose list was not ids 0..M-1 in order
 
   const std::vector<uint16_t>& LastTotalBlocks() const { return last_nh_; }
+  // The prefix-indexer histograms PreRequest records with SchedulerConfig::PrefixMatchInfo (empty without it).
+  const PrefixIndexerHistograms& PrefixIndexerMetrics() const { return prefix_metrics_; }
   eppscore_engine* engine() { return eng_; }
 
  private:
+  // One eppscore_prefix_match call for an engine batch that hashed its prompts: targets[i] are request i's TargetEndpoints
+  // entries (every profile's), hashes / nh / stride the batch's hashes_out, ids the list position -> endpoint id map.  Each
+  // entry gets {matchBlocks at its endpoint, totalBlocks, the batch's block size} (plugin.go:140-153).  A request's endpoints
+  // are listed once each, so k never passes the number of endpoint rows.
+  void FillPrefixMatch(const std::vector<std::vector<ScoredEndpoint*>>& targets, const uint64_t* hashes, const uint16_t* nh,
+                       int32_t stride, const std::vector<int>& ids, int block_tokens) {
+    const int n = (int)targets.size();
+    std::vector<std::vector<int32_t>> cols((size_t)n);
+    size_t k = 0;
+    for (int i = 0; i < n; i++) {
+      for (const ScoredEndpoint* t : targets[(size_t)i]) {
+        const int32_t id = ids[(size_t)t->Index];
+        if (std::find(cols[(size_t)i].begin(), cols[(size_t)i].end(), id) == cols[(size_t)i].end()) cols[(size_t)i].push_back(id);
+      }
+      k = std::max(k, cols[(size_t)i].size());
+    }
+    if (n == 0 || k == 0) return;
+    if (block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+    std::vector<int32_t> eps((size_t)n * k, -1);
+    for (int i = 0; i < n; i++) std::copy(cols[(size_t)i].begin(), cols[(size_t)i].end(), eps.begin() + (ptrdiff_t)((size_t)i * k));
+    std::vector<uint16_t> match((size_t)n * k, 0);
+    if (eppscore_prefix_match(eng_, n, (int32_t)k, 0, hashes, nh, stride, eps.data(), match.data(), nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_prefix_match: ") + eppscore_last_error(eng_));
+    for (int i = 0; i < n; i++)
+      for (ScoredEndpoint* t : targets[(size_t)i]) {
+        const auto& c = cols[(size_t)i];
+        const size_t j = (size_t)(std::find(c.begin(), c.end(), ids[(size_t)t->Index]) - c.begin());
+        t->PrefixMatch = PrefixCacheMatchInfo{match[(size_t)i * k + j], nh[i], (uint16_t)block_tokens};
+      }
+  }
+
+  // PreRequest's metrics (approximateprefix/plugin.go:199-204): per request with a primary target that carries its match, in
+  // request order, RecordPrefixCacheMatch(matchLen * blockSize * 4, total * blockSize * 4) with GetBlockSize of the primary
+  // profile's TargetEndpoints (the target's CacheBlockSize when autotuning); the ratio only when the total is > 0.
+  void RecordPrefixCacheMatch(const std::vector<BatchItem>& results) {
+    for (const BatchItem& it : results) {
+      if (!it.error.empty()) continue;
+      auto pr = it.result.ProfileResults.find(it.result.PrimaryProfileName);
+      if (pr == it.result.ProfileResults.end() || pr->second.TargetEndpoints.empty()) continue;
+      const ScoredEndpoint& t = pr->second.TargetEndpoints[0];
+      if (!t.PrefixMatch || !t.Endpoint_) continue;
+      int64_t bs = cfg_.Prefix.BlockSizeTokens;
+      if (cfg_.Prefix.AutoTune && t.Endpoint_->GetMetrics()->CacheBlockSize > 0) bs = t.Endpoint_->GetMetrics()->CacheBlockSize;
+      const int64_t matched = (int64_t)t.PrefixMatch->MatchBlocks * bs * 4, total = (int64_t)t.PrefixMatch->TotalBlocks * bs * 4;
+      prefix_metrics_.HitBytes.Observe((double)matched);
+      if (total > 0) prefix_metrics_.HitRatio.Observe((double)matched / (double)total);
+    }
+  }
+
   // x-slo-ttft-ms / x-slo-tpot-ms (predictedlatency/plugin.go:276-290): a parse error gives 0 (logged only)
   static double SloHeader(const InferenceRequest& q, const char* key) {
     auto it = q.Headers.find(key);
@@ -1133,6 +1229,16 @@ class Scheduler {
             pr.TargetEndpoints.push_back(o2);
           }
         }
+      }
+      if (cfg_.PrefixMatchInfo && want_prefix) {  // every run's entries of this call's requests, against the call's hashes
+        std::vector<std::vector<ScoredEndpoint*>> targets((size_t)n);
+        for (int i = 0; i < n; i++)
+          for (int k = 0; k < nr; k++) {
+            auto it = got[(size_t)rows[i]].find(names[(size_t)prof[k]]);
+            if (it != got[(size_t)rows[i]].end())
+              for (ScoredEndpoint& t : it->second.TargetEndpoints) targets[(size_t)i].push_back(&t);
+          }
+        FillPrefixMatch(targets, hashes.data(), nh.data(), last_stride_, ids, block_tokens);
       }
     }
     for (int r = 0; r < R; r++) {
@@ -1416,6 +1522,7 @@ class Scheduler {
   std::vector<double> last_tpot_;
   std::unordered_map<std::string, KeyUse> running_keys_;
   uint64_t next_key_ = 1;
+  PrefixIndexerHistograms prefix_metrics_;
 };
 
 inline Scheduler* NewSchedulerWithConfig(const SchedulerConfig& c) { return new Scheduler(c); }

@@ -4,6 +4,7 @@
 #pragma once
 #include <cstdint>
 #include <map>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -92,12 +93,27 @@ inline int CountFields(const std::string& str) {
   return count;
 }
 
+// attrprefix.PrefixCacheMatchInfo (datalayer/attribute/prefix/data_types.go): what PrepareRequestData puts on every endpoint
+// (approximateprefix/plugin.go:150-153).  Block counts, and the block length in tokens the prompt was hashed with.  All three
+// fit 16 bits: the engine hashes at most EPPSCORE_MAX_BLOCKS = 65535 blocks, and the Scheduler refuses block sizes past 65535
+// tokens for the info, so a ScoredEndpoint keeps its size.
+struct PrefixCacheMatchInfo {
+  uint16_t MatchBlocks = 0;
+  uint16_t TotalBlocks = 0;
+  uint16_t BlockSizeTokens = 0;
+};
+
 struct ScoredEndpoint {
   const Endpoint* Endpoint_ = nullptr;
-  int Index = -1;  // position in the candidate slice given to Schedule
   double Score = 0.0;
+  int Index = -1;  // position in the candidate slice given to Schedule
   int TieCount = 0;  // size of the arg-max set the reference would shuffle over (picker/maxscore/picker.go:91-102)
+  // The endpoint's PrefixCacheMatchInfo attribute; set only with SchedulerConfig::PrefixMatchInfo on a batch whose prompts the
+  // engine hashed.
+  std::optional<PrefixCacheMatchInfo> PrefixMatch;
 };
+static_assert(sizeof(ScoredEndpoint) == 32, "the match info lives in the struct's tail");
+
 struct ProfileRunResult {
   std::vector<ScoredEndpoint> TargetEndpoints;
 };

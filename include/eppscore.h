@@ -470,6 +470,26 @@ int32_t eppscore_prefix_apply(struct eppscore_engine *e, int64_t n, const uint64
 int32_t eppscore_prefix_remove_endpoint(struct eppscore_engine *e, int32_t endpoint); /* indexer.RemovePod :167-182 */
 /* indexer.Get (reads the DEVICE table): bitset_out[ceil(M/32)] words, natural order; returns set size or <0. */
 int32_t eppscore_prefix_get(struct eppscore_engine *e, uint64_t hash, uint32_t *bitset_out, int32_t words);
+/* PrefixCacheMatchInfo.matchBlocks (approximateprefix/plugin.go:140-153,219-235) for chosen endpoints:
+ * match_out[r*k + j] = number of blocks among request r's leading blocks that are all in the index (the walk stops at the
+ * first block whose endpoint set is empty or absent, as matchLongestPrefix does) whose set holds endpoints[r*k + j].  Hits need
+ * not be contiguous for an endpoint: every hit block before the first miss that holds it counts.  Entries outside
+ * [0, max_endpoints) give 0, so -1 list padding needs no special case.  1 <= k <= config.max_endpoints: a pick (k = 1), a
+ * top-k list, or one list per profile run.  hashes [R*hash_stride] / n_hashes [R] have the layout of eppscore_batch.hashes_out
+ * and of the commit calls: pass the arrays given to eppscore_commit_picks*.
+ *   location 0 (host arrays): staged through the engine's staging buffers; the call returns when match_out is filled.
+ *     n_hashes[r] > hash_stride is ERR_INVALID.
+ *   location 1 (device arrays): asynchronous on `stream` (NULL = engine stream); it needs no scratch, so it behaves the same on
+ *     reserved and unreserved streams.  It reads the index under the ordering of a device-location batch: after the index
+ *     mutations issued before it, and later mutations wait for it (it is registered like a pending device batch).  It may be
+ *     captured into a CUDA graph wherever a batch may; the kernel reads the index through its device descriptor, so replays
+ *     stay valid across device rebuilds and later reserves.
+ * Documented use: schedule (with hashes_out) -> eppscore_prefix_match -> commit, in that order (the reference computes the match
+ * before indexer.Add).  One kernel launch (counted in eppscore_stats.kernel_launches).  ERR_INVALID: k outside its range, R < 0,
+ * NULL arrays with R > 0, hash_stride <= 0, a location other than 0 / 1. */
+int32_t eppscore_prefix_match(struct eppscore_engine *e, int32_t R, int32_t k, int32_t location, const uint64_t *hashes,
+                              const uint16_t *n_hashes, int32_t hash_stride, const int32_t *endpoints /* [R*k] */,
+                              uint16_t *match_out /* [R*k] */, void *stream);
 int32_t eppscore_prefix_lru_len(const struct eppscore_engine *e, int32_t endpoint); /* -1: endpoint has no LRU */
 int32_t eppscore_prefix_lru_keys(const struct eppscore_engine *e, int32_t endpoint, uint64_t *out, int32_t cap); /* oldest first */
 /* Replication across GPUs: the index is a deterministic function of the ordered commit stream, so every rank applies the
