@@ -93,6 +93,12 @@ class Stats(C.Structure):
                 ("probe_resolved", C.c_uint32)]
 
 
+class LatencyInfo(C.Structure):
+    _fields_ = [("ttft", C.c_double), ("tpot", C.c_double), ("ttft_headroom", C.c_double), ("tpot_headroom", C.c_double),
+                ("prefix_cache_score", C.c_double), ("dispatched", C.c_int32), ("present", C.c_uint8),
+                ("ttft_valid", C.c_uint8), ("tpot_valid", C.c_uint8), ("reserved", C.c_uint8)]
+
+
 # every symbol include/eppscore.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 ABI_SYMBOLS = [
@@ -128,6 +134,8 @@ ABI_SYMBOLS = [
     ("eppscore_prefix_remove_endpoint", C.c_int32, [_P, C.c_int32]),
     ("eppscore_prefix_get", C.c_int32, [_P, C.c_uint64, _P, C.c_int32]),
     ("eppscore_prefix_match", C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P]),
+    ("eppscore_predict_latency", C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, _P, _P, _P, _P, _P,
+                                             _P]),
     ("eppscore_prefix_lru_len", C.c_int32, [_P, C.c_int32]),
     ("eppscore_prefix_lru_keys", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_commit_picks_device", C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int64, _P]),

@@ -93,7 +93,7 @@ struct eppscore_engine {
   std::vector<PendingBatch> pending;
   // Staging for the synchronous host-array calls: slot i holds the call's i-th array.  Each of those calls runs on `stream`
   // and synchronises it before it returns, so one set serves them all.
-  DevBuf stage[6];
+  DevBuf stage[8];
 
   // Producer state the scorers read: mutations of either producer below prepare the terms of the profiles that read the state
   // again (with their Profile::pa).  Mutations outside a CUDA-graph capture are ordered through ev_producer, recorded after
@@ -124,6 +124,12 @@ struct eppscore_engine {
   bool run_copy_issued = false;
   bool run_captured = false;  // a mutation was captured since the last exact read: its replays are invisible to the bound
   bool snapshot_has_min_tpot = false, snapshot_has_dispatched = false;
+  // Device-location eppscore_predict_latency calls read the running-request counts in place, so a running-request update must
+  // not rewrite them before those reads are done (count_reads_wait).  count_readers: a call on a caller stream may still be
+  // pending (it is in the pending set); cleared once that set has drained.  ev_count_read: recorded behind the last call on the
+  // engine stream (count_read_engine until it has completed).
+  bool count_readers = false, count_read_engine = false;
+  Event ev_count_read;
 
   // scratch for host-location batches and internal hashes: two sets, so the chunks of a host batch can alternate
   // between two streams (H2D of chunk i+1 under the kernels and the D2H of chunk i).  sc[0] also serves device-location
@@ -1164,6 +1170,7 @@ int32_t eppscore_create(int32_t device, const eppscore_config* cfg, eppscore_eng
   CK(nullptr, ep->probe_resolved.reserve(8));
   CK(nullptr, cudaMemsetAsync(ep->probe_resolved.p, 0, 8, ep->stream));
   CK(nullptr, make(ep->ev_producer));
+  CK(nullptr, make(ep->ev_count_read));
   CK(nullptr, init_inflight_update());
   {  // running-request queues: every endpoint empty, a small table (grown by the first calls that need room)
     CK(nullptr, ep->run_count.reserve(mp * 4));
@@ -2087,6 +2094,91 @@ int32_t eppscore_prefix_match(eppscore_engine* e, int32_t R, int32_t k, int32_t 
   return EPPSCORE_OK;
 }
 
+int32_t eppscore_predict_latency(eppscore_engine* e, int32_t R, int32_t k, int32_t location, const uint64_t* hashes,
+                                 const uint16_t* n_hashes, int32_t hash_stride, const int32_t* input_tokens, const double* ttft_slo,
+                                 const double* tpot_slo, const int32_t* endpoints, eppscore_latency_info* info_out,
+                                 uint16_t* match_out, void* stream) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (location != 0 && location != 1) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: location must be 0 or 1");
+  if (k < 1 || k > e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: k must be in [1, max_endpoints]");
+  if (R < 0 || (R > 0 && (!hashes || !n_hashes || !endpoints || !info_out)))
+    return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: NULL argument");
+  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency before set_snapshot");
+  if (!e->lat_ep.p || !e->lat_args.enabled)
+    return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: the snapshot was prepared without a profile with a latency scorer");
+  if (R == 0) return EPPSCORE_OK;
+  if (hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: hash_stride must be > 0");
+  CK(e, cudaSetDevice(e->device));
+  const LatArgs& L = e->lat_args;
+  LatInfoArgs a{};
+  a.R = R;
+  a.k = k;
+  a.M = e->M;
+  a.has_predictions = L.has_predictions;
+  a.stride = hash_stride;
+  a.ep = L.ep;
+  a.dispatched = e->base_pa.dispatched;  // the snapshot's array, else the running-request counts (eppscore_set_snapshot)
+  a.ttft_input = L.ttft_input;
+  a.ttft_prefix = L.ttft_prefix;
+  a.tpot_input = L.tpot_input;
+  a.tpot_generated = L.tpot_generated;
+  a.buffer = L.buffer;
+  if (location == 1) {
+    // Ordered like a device-location batch: after the index mutations, snapshot preparations and producer updates issued before
+    // it, and registered as pending so that later ones wait for it.  Inside a capture the graph's edges order it.
+    cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
+    unsigned long long cap_id = 0;
+    const bool capturing = is_capturing(cs, &cap_id);
+    if (!capturing && cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
+    if (!capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(cs, e->ev_producer, 0));
+    if (capturing ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
+                  : (e->snapshot_capture_id == 0 && cs != e->snapshot_stream))
+      CK(e, cudaStreamWaitEvent(cs, e->ev_snapshot, 0));
+    a.hashes = hashes;
+    a.n_hashes = n_hashes;
+    a.endpoints = endpoints;
+    a.input_tokens = input_tokens;
+    a.ttft_slo = ttft_slo;
+    a.tpot_slo = tpot_slo;
+    a.match_out = match_out;
+    a.out = info_out;
+    e->index->latency_info(a, e->cfg.max_endpoints, cs);
+    CK(e, cudaGetLastError());
+    if (!capturing && !e->snapshot_has_dispatched) {  // it reads the running-request counts in place (count_reads_wait)
+      if (cs == e->stream) {
+        CK(e, cudaEventRecord(e->ev_count_read, cs));
+        e->count_read_engine = true;
+      } else {
+        e->count_readers = true;
+      }
+    }
+    return pending_record(e, cs);
+  }
+  for (int32_t r = 0; r < R; r++)
+    if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: n_hashes exceeds hash_stride");
+  if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
+  int32_t rc;
+  if ((rc = h2d(e, e->stage[0], hashes, (size_t)R * hash_stride, &a.hashes)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[1], n_hashes, (size_t)R, &a.n_hashes)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[2], endpoints, (size_t)R * k, &a.endpoints)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[3], input_tokens, (size_t)R, &a.input_tokens)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[4], ttft_slo, (size_t)R, &a.ttft_slo)) != EPPSCORE_OK ||
+      (rc = h2d(e, e->stage[5], tpot_slo, (size_t)R, &a.tpot_slo)) != EPPSCORE_OK)
+    return rc;
+  CK(e, e->stage[6].reserve((size_t)R * k * sizeof(eppscore_latency_info)));
+  a.out = e->stage[6].p;
+  if (match_out) {
+    CK(e, e->stage[7].reserve((size_t)R * k * 2));
+    a.match_out = e->stage[7].as<uint16_t>();
+  }
+  e->index->latency_info(a, e->cfg.max_endpoints, e->stream);
+  CK(e, cudaGetLastError());
+  CK(e, cudaMemcpyAsync(info_out, e->stage[6].p, (size_t)R * k * sizeof(eppscore_latency_info), cudaMemcpyDeviceToHost, e->stream));
+  if (match_out) CK(e, cudaMemcpyAsync(match_out, e->stage[7].p, (size_t)R * k * 2, cudaMemcpyDeviceToHost, e->stream));
+  CK(e, cudaStreamSynchronize(e->stream));
+  return EPPSCORE_OK;
+}
+
 // ---------------- in-flight load producer ----------------
 int32_t eppscore_estimate_tokens(eppscore_engine* e, int32_t R, int32_t location, const int64_t* request_size_bytes,
                                  const int32_t* token_hint, const int32_t* prompt_chars, int64_t* out, void* stream) {
@@ -2299,6 +2391,24 @@ int32_t run_copy_back(eppscore_engine* e, cudaStream_t st, bool capturing) {
   return EPPSCORE_OK;
 }
 
+// Before a running-request update's kernel on `st` (outside a capture): every device-location eppscore_predict_latency issued
+// earlier that reads the counts in place has finished reading them.  The flags clear once those reads are known to be done, so
+// the extra waits last only while such a call may be in flight.
+int32_t count_reads_wait(eppscore_engine* e, cudaStream_t st) {
+  if (e->count_readers) {
+    int32_t rc = pending_wait(e, st);
+    if (rc != EPPSCORE_OK) return rc;
+    bool armed = false;
+    for (const PendingBatch& p : e->pending) armed = armed || p.armed;
+    if (!armed) e->count_readers = false;
+  }
+  if (e->count_read_engine) {
+    if (cudaEventQuery(e->ev_count_read) == cudaSuccess) e->count_read_engine = false;
+    else if (st != e->stream) CK(e, cudaStreamWaitEvent(st, e->ev_count_read, 0));
+  }
+  return EPPSCORE_OK;
+}
+
 int32_t running_update(eppscore_engine* e, int op, int32_t R, int32_t location, const int32_t* endpoint, const uint64_t* key,
                        const double* tpot, uint8_t* out, void* stream) {
   if (!e) return EPPSCORE_ERR_INVALID;
@@ -2316,6 +2426,7 @@ int32_t running_update(eppscore_engine* e, int op, int32_t R, int32_t location, 
   bool capturing = false;
   int32_t rc = producer_begin(e, st, &capturing);
   if (rc != EPPSCORE_OK) return rc;
+  if (!capturing && (rc = count_reads_wait(e, st)) != EPPSCORE_OK) return rc;
   if (op == 0 && (rc = run_make_room(e, st, R, capturing)) != EPPSCORE_OK) return rc;
   if ((rc = run_scratch(e, st, R, capturing)) != EPPSCORE_OK) return rc;
   const int32_t* d_ep = endpoint;
@@ -2358,6 +2469,7 @@ int32_t eppscore_running_remove_endpoint(eppscore_engine* e, int32_t endpoint) {
   CK(e, cudaSetDevice(e->device));
   bool capturing = false;
   int32_t rc = producer_begin(e, e->stream, &capturing);
+  if (rc == EPPSCORE_OK && !capturing) rc = count_reads_wait(e, e->stream);
   if (rc != EPPSCORE_OK) return rc;
   e->launches += launch_running_drop_endpoint(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, endpoint,
                                               e->cfg.max_endpoints, e->sm_count, e->stream);

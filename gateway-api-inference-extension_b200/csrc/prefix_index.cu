@@ -15,6 +15,8 @@
 #include <cstring>
 #include <vector>
 
+#include "../../include/eppscore.h"
+
 namespace eppscore {
 
 // ---------------------------------------------------------------------------------------------
@@ -170,7 +172,37 @@ struct ReadX {
 // block base + b (32 probes in flight), the ballot of misses gives the first one, and each listed endpoint's count of the hits
 // before it is a ballot of the lanes whose set holds the endpoint.  Lane j keeps endpoint j's count (j < 32); the counts of
 // endpoints past 32 accumulate in the request's out row.
+// One request's walk, by its whole warp: returns lane j's count for endpoint j < min(k, 32); the counts of entries j >= 32
+// accumulate in o[j * os] (written by lane j & 31, which alone reads them back).
 constexpr int kMatchThreads = 256;
+template <class X>
+__device__ __forceinline__ uint32_t match_walk(X& x, const TableView* tv, uint32_t lane, int32_t k, uint32_t limit, uint32_t n,
+                                               const uint64_t* h, const int32_t* eps, uint16_t* o, int32_t os) {
+  const int32_t k0 = k < 32 ? k : 32;
+  const uint32_t e0 = (int32_t)lane < k0 ? (uint32_t)eps[lane] : 0xFFFFFFFFu;  // (-1 and >= limit never match)
+  uint32_t c0 = 0;
+  for (uint32_t base = 0;; base += 32) {  // at least one round: it writes the row's entries past 32
+    uint32_t raw = 0;
+    TSlot* s = base + lane < n ? table_find(x, tv, h[base + lane], &raw) : nullptr;
+    const uint32_t miss = __ballot_sync(0xffffffffu, base + lane < n && !s);
+    const uint32_t left = n > base ? n - base : 0;
+    const uint32_t hits = miss ? (uint32_t)__ffs(miss) - 1 : (left < 32 ? left : 32);
+    const bool hit = lane < hits;
+    for (int32_t j = 0; j < k0; j++) {
+      const uint32_t e = __shfl_sync(0xffffffffu, e0, j);
+      const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
+      if ((int32_t)lane == j) c0 += c;
+    }
+    for (int32_t j = 32; j < k; j++) {
+      const uint32_t e = (uint32_t)__ldg(&eps[j]);
+      const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
+      if (lane == (uint32_t)(j & 31)) o[(size_t)j * os] = (uint16_t)((base == 0 ? 0u : o[(size_t)j * os]) + c);
+    }
+    if (miss || base + 32 >= n) break;
+  }
+  return c0;
+}
+
 __global__ void __launch_bounds__(kMatchThreads) prefix_match_kernel(const TableView* tv, int32_t R, int32_t k, uint32_t limit,
                                                                      const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
                                                                      const int32_t* endpoints, uint16_t* out) {
@@ -178,33 +210,57 @@ __global__ void __launch_bounds__(kMatchThreads) prefix_match_kernel(const Table
   const uint32_t lane = threadIdx.x & 31;
   const int32_t warps = gridDim.x * (kMatchThreads / 32);
   for (int32_t r = blockIdx.x * (kMatchThreads / 32) + (threadIdx.x >> 5); r < R; r += warps) {
-    const uint32_t n = n_hashes[r];
-    const uint64_t* h = hashes + (size_t)r * stride;
-    const int32_t* eps = endpoints + (size_t)r * k;
     uint16_t* o = out + (size_t)r * k;
-    const int32_t k0 = k < 32 ? k : 32;
-    const uint32_t e0 = (int32_t)lane < k0 ? (uint32_t)eps[lane] : 0xFFFFFFFFu;  // (-1 and >= limit never match)
-    uint32_t c0 = 0;
-    for (uint32_t base = 0;; base += 32) {  // at least one round: it writes the row's entries past 32
-      uint32_t raw = 0;
-      TSlot* s = base + lane < n ? table_find(x, tv, h[base + lane], &raw) : nullptr;
-      const uint32_t miss = __ballot_sync(0xffffffffu, base + lane < n && !s);
-      const uint32_t left = n > base ? n - base : 0;
-      const uint32_t hits = miss ? (uint32_t)__ffs(miss) - 1 : (left < 32 ? left : 32);
-      const bool hit = lane < hits;
-      for (int32_t j = 0; j < k0; j++) {
-        const uint32_t e = __shfl_sync(0xffffffffu, e0, j);
-        const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
-        if ((int32_t)lane == j) c0 += c;
+    const uint32_t c0 = match_walk(x, tv, lane, k, limit, n_hashes[r], hashes + (size_t)r * stride, endpoints + (size_t)r * k, o, 1);
+    if ((int32_t)lane < (k < 32 ? k : 32)) o[lane] = (uint16_t)c0;
+  }
+}
+
+// PrepareRequestData of the predicted-latency producer (predictedlatency/preparedata_hooks.go:36-106, prediction.go:44-166) at
+// k listed endpoints per request: the walk of prefix_match_kernel gives each entry's match count c, then lane j owns entries
+// j, j + 32, ...: it gathers the endpoint's tile column and evaluates lat_pair with the prefix term pcoef * (c/total) exactly
+// as score_matrix_kernel forms it, and writes the entry's 48-byte record.  Without match_out the counts of entries past 32
+// accumulate in their own record's `dispatched` field until the record is written.
+__global__ void __launch_bounds__(kMatchThreads) latency_info_kernel(const TableView* tv, uint32_t limit, const LatInfoArgs a) {
+  ReadX x;
+  const uint32_t lane = threadIdx.x & 31;
+  const int32_t warps = gridDim.x * (kMatchThreads / 32), k = a.k;
+  eppscore_latency_info* const out = static_cast<eppscore_latency_info*>(a.out);
+  for (int32_t r = blockIdx.x * (kMatchThreads / 32) + (threadIdx.x >> 5); r < a.R; r += warps) {
+    const uint32_t n = a.n_hashes[r];
+    const int32_t* eps = a.endpoints + (size_t)r * k;
+    eppscore_latency_info* rec = out + (size_t)r * k;
+    uint16_t* o = a.match_out ? a.match_out + (size_t)r * k : reinterpret_cast<uint16_t*>(&rec->dispatched);
+    const int32_t os = a.match_out ? 1 : (int32_t)(sizeof(eppscore_latency_info) / 2);
+    const uint32_t c0 = match_walk(x, tv, lane, k, limit, n, a.hashes + (size_t)r * a.stride, eps, o, os);
+    const double in_tok = (double)(a.input_tokens ? a.input_tokens[r] : 0);  // len(strings.Fields(prompt)), training.go:51
+    const double x_in = __dmul_rn(a.ttft_input, in_tok), y_in = __dmul_rn(a.tpot_input, in_tok);
+    const double tslo = a.ttft_slo ? a.ttft_slo[r] : 0.0;
+    const double buf = __dmul_rn(a.tpot_slo ? a.tpot_slo[r] : 0.0, a.buffer);  // prediction.go:150
+    for (int32_t j = (int32_t)lane; j < k; j += 32) {
+      const uint32_t c = j < 32 ? c0 : o[(size_t)j * os];
+      if (a.match_out) o[j] = (uint16_t)c;
+      const int32_t m = __ldg(&eps[j]);
+      double v[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+      int32_t disp = 0;
+      uint32_t flags = 0;  // present | ttft_valid << 8 | tpot_valid << 16 (little-endian bytes of the record)
+      if (a.has_predictions && m >= 0 && m < a.M) {
+        const double frac = n ? __ddiv_rn((double)c, (double)n) : 0.0;  // match/total, NaN (0/0) => 0
+        const LatPair lp = lat_pair(a.ep + (size_t)(m >> 5) * 256 + (m & 31), a.tpot_generated, __dmul_rn(a.ttft_prefix, frac),
+                                    x_in, y_in, tslo, buf);
+        const bool neutral = (__ldg(reinterpret_cast<const int*>(a.ep + (size_t)(m >> 5) * 256 + (m & 31) + 224)) & 2) != 0;
+        v[0] = lp.ttft;
+        v[1] = lp.tpot;
+        v[2] = lp.hT;
+        v[3] = lp.hP;
+        v[4] = frac;
+        disp = __ldg(&a.dispatched[m]);
+        flags = 1u | (lp.ttft < tslo ? 1u << 8 : 0u) | ((neutral || lp.tpot < lp.buffered) ? 1u << 16 : 0u);
       }
-      for (int32_t j = 32; j < k; j++) {
-        const uint32_t e = (uint32_t)__ldg(&eps[j]);
-        const uint32_t c = __popc(__ballot_sync(0xffffffffu, hit && e < limit && slot_holds(x, tv, s, raw, e)));
-        if (lane == (uint32_t)(j & 31)) o[j] = (uint16_t)((base == 0 ? 0u : o[j]) + c);
-      }
-      if (miss || base + 32 >= n) break;
+      double* d = reinterpret_cast<double*>(rec + j);
+      for (int i = 0; i < 5; i++) d[i] = v[i];
+      reinterpret_cast<int2*>(d + 5)[0] = make_int2(disp, (int32_t)flags);
     }
-    if ((int32_t)lane < k0) o[lane] = (uint16_t)c0;
   }
 }
 
@@ -574,6 +630,12 @@ void DeviceIndex::match(int32_t R, int32_t k, int32_t limit, const uint64_t* has
                         const int32_t* endpoints, uint16_t* out, cudaStream_t s) {
   const int32_t ctas = std::min((R + kMatchThreads / 32 - 1) / (kMatchThreads / 32), 8192);
   prefix_match_kernel<<<ctas, kMatchThreads, 0, s>>>(d_tv_, R, k, (uint32_t)limit, hashes, n_hashes, stride, endpoints, out);
+  launches_++;
+}
+
+void DeviceIndex::latency_info(const LatInfoArgs& a, int32_t limit, cudaStream_t s) {
+  const int32_t ctas = std::min((a.R + kMatchThreads / 32 - 1) / (kMatchThreads / 32), 8192);
+  latency_info_kernel<<<ctas, kMatchThreads, 0, s>>>(d_tv_, (uint32_t)limit, a);
   launches_++;
 }
 

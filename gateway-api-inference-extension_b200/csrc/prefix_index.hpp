@@ -6,6 +6,7 @@
 
 #include <cstdint>
 
+#include "lat_pair.cuh"
 #include "prefix_table.cuh"
 
 namespace eppscore {
@@ -51,6 +52,9 @@ class DeviceIndex {
   // async on `s`; reads the index through its descriptor.
   void match(int32_t R, int32_t k, int32_t limit, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
              const int32_t* endpoints, uint16_t* out, cudaStream_t s);
+  // The same walk, then the predicted-latency producer's record at each listed endpoint (lat_pair.cuh: LatInfoArgs; a.R >= 1,
+  // device arrays).  match_out, when set, receives what match() writes.  One launch of a fixed shape, async on `s`.
+  void latency_info(const LatInfoArgs& a, int32_t limit, cudaStream_t s);
   cudaError_t apply(int64_t n, const uint64_t* hash, const int32_t* endpoint, const uint8_t* op, cudaStream_t s);  // device arrays
   cudaError_t remove_endpoint(int32_t p, cudaStream_t s);
   cudaError_t lru_keys(int32_t p, uint64_t* out_host, int32_t cap, int32_t* len, cudaStream_t s);

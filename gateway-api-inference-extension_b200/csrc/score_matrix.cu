@@ -15,6 +15,7 @@
 //                                                             candidates in one pass, then the normalised score
 // The scorer sequence is a template parameter (SEQ packs kind+1 per step, 4 bits each; 0 = runtime loop).
 #include "device_common.cuh"
+#include "lat_pair.cuh"
 #include "prefix_table.cuh"
 
 namespace eppscore {
@@ -23,32 +24,6 @@ constexpr int kMatrixWarps = 8;
 constexpr int kMaxJ = 8;
 
 constexpr int kLatW = 128;  // latency-scorer weights w/100 are tabulated for w in [0, 128) (plugin.go:301-306: w in [1,101])
-
-// One (request, endpoint) pair of the predicted-latency producer: TTFT/TPOT (prediction.go:171-185, left to right),
-// headrooms (predictedlatency/prediction.go:143-161, :100-104) and the endpoint's tier:
-//   0 positive, 1 negative & idle, 2 only TPOT negative, 3 only TTFT negative, 4 both negative
-// (plugin.go:177-238: the scorer scores the lowest non-empty tier only).
-struct LatPair {
-  double ttft, tpot, hT, hP;
-  int rank;
-};
-// tile layout of the per-endpoint arrays: slot i of endpoint (t*32 + lane) lives at ((t*8 + i)*32 + lane), so one
-// address per pair and seven coalesced 8-byte loads at immediate offsets (kernels.cuh: LatArgs)
-__device__ __forceinline__ LatPair lat_pair(const double* tp, double tpot_generated, double pref_term, double x_in,
-                                            double y_in, double ttft_slo, double buf_tpot) {
-  LatPair o;
-  o.ttft = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(__ldg(tp), x_in), __ldg(tp + 32)), __ldg(tp + 64)), pref_term);
-  o.tpot = __dadd_rn(__dadd_rn(__dadd_rn(__dadd_rn(__ldg(tp + 96), y_in), __ldg(tp + 128)), __ldg(tp + 160)),
-                     tpot_generated);                        // NumTokensGenerated = 1 (prediction.go:69)
-  o.hT = __dsub_rn(ttft_slo, o.ttft);
-  const int fl = __ldg(reinterpret_cast<const int*>(tp + 224));
-  const double lim = __ldg(tp + 192);
-  const double buffered = lim < buf_tpot ? lim : buf_tpot;   // min(bufferedTPOT, podMinTPOTSLO*factor)
-  o.hP = (fl & 2) ? 0.0 : __dsub_rn(buffered, o.tpot);
-  const bool tn = o.hT < 0.0, pn = o.hP < 0.0;
-  o.rank = !(tn || pn) ? 0 : ((fl & 1) ? 1 : (tn && pn ? 4 : (tn ? 3 : 2)));
-  return o;
-}
 
 __host__ __device__ constexpr bool seq_has_minmax(uint32_t seq) {
   return seq != 0 && ((int)(seq & 15u) - 1 == STEP_MINMAX || seq_has_minmax(seq >> 4));

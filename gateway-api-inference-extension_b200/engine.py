@@ -46,6 +46,13 @@ def latency_params(**kw) -> LatencyParams:
     return p
 
 
+# eppscore_latency_info as a numpy structured dtype (48 bytes, the C layout)
+LATENCY_INFO_DTYPE = np.dtype([("ttft", "<f8"), ("tpot", "<f8"), ("ttft_headroom", "<f8"), ("tpot_headroom", "<f8"),
+                               ("prefix_cache_score", "<f8"), ("dispatched", "<i4"), ("present", "u1"), ("ttft_valid", "u1"),
+                               ("tpot_valid", "u1"), ("reserved", "u1")])
+assert LATENCY_INFO_DTYPE.itemsize == C.sizeof(capi.LatencyInfo) == 48
+
+
 def _is_torch(x) -> bool:
     return hasattr(x, "data_ptr") and hasattr(x, "is_cuda")
 
@@ -606,6 +613,38 @@ class Engine:
         self._check(self._lib.eppscore_prefix_match(self._h, R, k, 0, a.ptr(hashes, np.uint64), a.ptr(n_hashes, np.uint16), stride,
                                                     a.ptr(endpoints, np.int32), res.ctypes.data, None))
         return res
+
+    def predict_latency(self, hashes, n_hashes, endpoints, input_tokens=None, ttft_slo=None, tpot_slo=None, device=False,
+                        stream=None, out=None, match_out=None):
+        """The predicted-latency producer's LatencyPredictionInfo and prefix cache score at chosen endpoints
+        (eppscore_predict_latency), from the current snapshot: endpoints is [R, k] (int32; -1 and entries outside [0, M) give
+        present = 0), hashes [R, stride] and n_hashes [R] as for prefix_match, input_tokens / ttft_slo / tpot_slo [R] or None (0).
+        Host mode returns a LATENCY_INFO_DTYPE array [R, k]; with match_out=True it returns (info, match), match the uint16
+        array prefix_match gives.  device=True: CUDA tensors / raw pointers, asynchronous on `stream`; `out` is a preallocated
+        tensor of R*k*48 bytes (e.g. torch.uint8 [R, k, 48]) that the call fills and returns, `match_out` an optional uint16 [R, k]
+        tensor filled as prefix_match fills it."""
+        a = _Args(device)
+        if device:
+            R, k = int(endpoints.shape[0]), int(endpoints.shape[1])
+            stride = int(hashes.shape[1])
+            if out is None:
+                raise ValueError("device mode fills a preallocated `out` tensor")
+            self._check(self._lib.eppscore_predict_latency(
+                self._h, R, k, 1, a.ptr(hashes, None), a.ptr(n_hashes, None), stride, a.ptr(input_tokens, None),
+                a.ptr(ttft_slo, None), a.ptr(tpot_slo, None), a.ptr(endpoints, None), a.ptr(out, None), a.ptr(match_out, None),
+                _stream_handle(stream)))
+            return out
+        endpoints = np.ascontiguousarray(endpoints, np.int32)
+        hashes = np.ascontiguousarray(hashes, np.uint64)
+        R, k = endpoints.shape
+        stride = hashes.shape[1] if hashes.ndim == 2 else 0
+        info = np.zeros((R, k), LATENCY_INFO_DTYPE)
+        match = np.zeros((R, k), np.uint16) if match_out else None
+        self._check(self._lib.eppscore_predict_latency(
+            self._h, R, k, 0, a.ptr(hashes, np.uint64), a.ptr(n_hashes, np.uint16), stride, a.ptr(input_tokens, np.int32),
+            a.ptr(ttft_slo, np.float64), a.ptr(tpot_slo, np.float64), a.ptr(endpoints, np.int32), info.ctypes.data,
+            None if match is None else match.ctypes.data, None))
+        return (info, match) if match_out else info
 
     def prefix_lru_len(self, endpoint) -> int:
         return self._lib.eppscore_prefix_lru_len(self._h, endpoint)

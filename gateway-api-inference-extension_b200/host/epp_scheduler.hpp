@@ -100,6 +100,25 @@ extern "C" int32_t eppscore_prefix_match(struct eppscore_engine* e, int32_t R, i
                                          const uint16_t* n_hashes, int32_t hash_stride, const int32_t* endpoints, uint16_t* match_out,
                                          void* stream) __attribute__((weak));
 inline bool EngineHasPrefixMatch() { return &eppscore_prefix_match != nullptr; }
+// eppscore_predict_latency (LatencyPredictionInfo at chosen endpoints) likewise: EngineHasPredictLatency() tells.  Without it a
+// config with SchedulerConfig::LatencyPredictionInfo is refused when the Scheduler is built.
+extern "C" int32_t eppscore_predict_latency(struct eppscore_engine* e, int32_t R, int32_t k, int32_t location, const uint64_t* hashes,
+                                            const uint16_t* n_hashes, int32_t hash_stride, const int32_t* input_tokens,
+                                            const double* ttft_slo, const double* tpot_slo, const int32_t* endpoints,
+                                            eppscore_latency_info* info_out, uint16_t* match_out, void* stream) __attribute__((weak));
+inline bool EngineHasPredictLatency() { return &eppscore_predict_latency != nullptr; }
+
+// What PreRequest keeps per request id with SchedulerConfig::LatencyPredictionInfo, as predictedLatencyCtx holds it after
+// processPreRequestForLatencyPrediction (requestcontrol_hooks.go:236-251) and predictFirstTPOT (:309-321): the predicted TTFT and
+// the prefix cache score at the "prefill" profile's target when there is one, else at the primary target; the stored TPOT at
+// the primary target; the request's SLOs.  0 where no prediction was stored.
+struct PredictedLatencyAtDispatch {
+  double PredictedTTFT = 0.0;
+  double PrefixCacheScore = 0.0;
+  double FirstPredictedTPOT = 0.0;
+  double TTFTSLO = 0.0;
+  double AvgTPOTSLO = 0.0;
+};
 
 // A prometheus histogram as client_golang keeps it: an observation lands in the first bucket whose upper bound is >= it
 // (sort.SearchFloat64s over the bounds), past the last bound in +Inf; Count and Sum accumulate in observation order.
@@ -321,6 +340,13 @@ struct SchedulerConfig {
   // did not hash (the small-batch host route, a config without prefix hashing) leave it empty.  Needs an engine library with
   // eppscore_prefix_match.
   bool PrefixMatchInfo = false;
+  // Opt-in (off by default): after each engine batch piece, one eppscore_predict_latency call gives every TargetEndpoints entry
+  // of every profile (lists and the "prefill" profile included) its LatencyPredictionInfo (SchedulingResult::TargetLatency), as the
+  // predicted-latency producer's PrepareRequestData stores it on every endpoint; with PrefixMatchInfo as well, the same call
+  // fills the PrefixCacheMatchInfo.  PreRequest then keeps the dispatch record of each request with an id
+  // (Scheduler::PredictedLatencyAtDispatch) until ResponseComplete / RequestExpired.  Batches of the small-batch host route leave
+  // it empty.  Needs a profile with a latency scorer and an engine library with eppscore_predict_latency.
+  bool LatencyPredictionInfo = false;
 };
 
 class Scheduler {
@@ -417,6 +443,8 @@ class Scheduler {
       throw SchedulingError("the inflight-load-producer needs an engine library with eppscore_inflight_add");
     if (cfg.PrefixMatchInfo && !EngineHasPrefixMatch())
       throw SchedulingError("SchedulerConfig::PrefixMatchInfo needs an engine library with eppscore_prefix_match");
+    if (cfg.LatencyPredictionInfo && !EngineHasPredictLatency())
+      throw SchedulingError("SchedulerConfig::LatencyPredictionInfo needs an engine library with eppscore_predict_latency");
     inflight_ = cfg.InFlightLoad != nullptr;
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
@@ -448,6 +476,8 @@ class Scheduler {
       for (const auto& w : np.second.scorers())
         if (auto* ls = dynamic_cast<LatencyScorer*>(w.Scorer_.get())) latency_scorer_ = ls;
     if (latency_scorer_ && !cfg.Profile.producer()) throw SchedulingError("latency-scorer needs a predicted-latency-producer");
+    if (cfg.LatencyPredictionInfo && !latency_scorer_)
+      throw SchedulingError("SchedulerConfig::LatencyPredictionInfo needs a profile with a latency-scorer");
     c.block_chars = cfg.Prefix.BlockSizeTokens * 4;  // averageCharactersPerToken (types.go:112)
     c.max_blocks = cfg.Prefix.MaxPrefixBlocksToMatch;
     c.lru_capacity_default = cfg.Prefix.LRUCapacityPerServer;
@@ -502,6 +532,7 @@ class Scheduler {
     std::vector<int32_t> hint, chars;
     std::vector<std::string> rid;
     std::vector<double> tpot;
+    std::vector<LatencyCtx> lat;
     for (size_t k = 0; k < starts.size(); k++) {
       const size_t a = starts[k], b = k + 1 < starts.size() ? starts[k + 1] : requests.size();
       const std::vector<InferenceRequest> piece(requests.begin() + (ptrdiff_t)a, requests.begin() + (ptrdiff_t)b);
@@ -518,7 +549,9 @@ class Scheduler {
         rid.insert(rid.end(), last_rid_.begin(), last_rid_.end());
         tpot.insert(tpot.end(), last_tpot_.begin(), last_tpot_.end());
       }
+      for (auto& c : lat_ctx_) lat.push_back(std::move(c));
     }
+    lat_ctx_ = std::move(lat);
     last_hashes_ = std::move(hashes);
     last_nh_ = std::move(nh);
     if (inflight_) {
@@ -541,6 +574,7 @@ class Scheduler {
     std::vector<BatchItem> out((size_t)R);
     last_hashes_.clear();
     last_nh_.clear();
+    lat_ctx_.clear();
     std::vector<int> all((size_t)M);
     for (int m = 0; m < M; m++) all[m] = m;
     for (int r = 0; r < R; r++) {
@@ -598,6 +632,7 @@ class Scheduler {
                                              int64_t request_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size();
     std::vector<BatchItem> out((size_t)R);
+    lat_ctx_.assign(cfg_.LatencyPredictionInfo ? (size_t)R : 0, LatencyCtx{});
     last_hashes_.clear();
     last_nh_.clear();
     if (R == 0) return out;
@@ -781,7 +816,17 @@ class Scheduler {
         }
       }
     }
-    if (cfg_.PrefixMatchInfo && want_prefix) {
+    if (cfg_.LatencyPredictionInfo) {
+      std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>> runs((size_t)R);
+      std::vector<int> rows((size_t)R);
+      for (int r = 0; r < R; r++) {
+        rows[(size_t)r] = r;
+        if (out[r].error.empty()) runs[(size_t)r].emplace_back(cfg_.ProfileName, &out[r].result.ProfileResults[cfg_.ProfileName]);
+      }
+      FillLatency(runs, rows, requests, endpoints, ids, last_hashes_.data(), last_nh_.data(), last_stride_, in_tokens.data(),
+                  ttft_slo.data(), tpot_slo.data(), cfg_.PrefixMatchInfo && want_prefix, block_tokens);
+      for (int r = 0; r < R; r++) AttachLatency(out[r], lat_ctx_[(size_t)r], endpoints, ids);
+    } else if (cfg_.PrefixMatchInfo && want_prefix) {
       std::vector<std::vector<ScoredEndpoint*>> targets((size_t)R);
       for (int r = 0; r < R; r++)
         if (out[r].error.empty())
@@ -797,6 +842,7 @@ class Scheduler {
   // (inflightload/producer.go:101-120).
   void PreRequest(const std::vector<BatchItem>& results) {
     RecordPrefixCacheMatch(results);
+    RecordDispatch(results);
     if (!last_endpoints_ || (last_hashes_.empty() && !inflight_ && !running_)) return;
     if (!cfg_.Profiles.empty()) return PreRequestProfiles(results);
     const int R = (int)results.size();
@@ -844,13 +890,17 @@ class Scheduler {
 
   // Context TTL expiry (predictedlatency/plugin.go:190-196) for a request PreRequest added: removed from its endpoint's
   // running-request queue, as at the end of the stream.  The caller owns the TTL clock.
-  void RequestExpired(const InferenceRequest& request, const SchedulingResult& result) { RunningRemove(request, result); }
+  void RequestExpired(const InferenceRequest& request, const SchedulingResult& result) {
+    dispatch_.erase(request.RequestId);
+    RunningRemove(request, result);
+  }
 
   // ResponseBody at end of stream (inflightload/producer.go:122-169) for a request PreRequest counted, given the result it was
   // scheduled with (the reference reads it from request.SchedulingResult): its TargetEndpoints[0] gives back one request and the
   // request's estimate.  Without the producer, or for a server that has left the pool since (its id may already be another
   // server's), nothing happens.
   void ResponseComplete(const InferenceRequest& request, const SchedulingResult& result) {
+    dispatch_.erase(request.RequestId);
     RunningRemove(request, result);  // requestcontrol_hooks.go:219
     if (!cfg_.Profiles.empty()) return ReleaseProfiles(request, result, false);
     if (!inflight_) return;
@@ -927,6 +977,14 @@ class Scheduler {
   const std::vector<uint16_t>& LastTotalBlocks() const { return last_nh_; }
   // The prefix-indexer histograms PreRequest records with SchedulerConfig::PrefixMatchInfo (empty without it).
   const PrefixIndexerHistograms& PrefixIndexerMetrics() const { return prefix_metrics_; }
+  // The dispatch record PreRequest kept for a request id with SchedulerConfig::LatencyPredictionInfo, or nullptr (none kept, or
+  // dropped at ResponseComplete / RequestExpired).
+  const epp::PredictedLatencyAtDispatch* PredictedLatencyAtDispatch(const std::string& request_id) const {
+    auto it = dispatch_.find(request_id);
+    return it == dispatch_.end() ? nullptr : &it->second;
+  }
+  size_t TrackedDispatches() const { return dispatch_.size(); }
+
   eppscore_engine* engine() { return eng_; }
 
  private:
@@ -959,6 +1017,145 @@ class Scheduler {
         const size_t j = (size_t)(std::find(c.begin(), c.end(), ids[(size_t)t->Index]) - c.begin());
         t->PrefixMatch = PrefixCacheMatchInfo{match[(size_t)i * k + j], nh[i], (uint16_t)block_tokens};
       }
+  }
+
+  // A batch row's share of the predicted-latency producer's request context: the request id and SLOs, the info of every endpoint
+  // a profile chose for it (by endpoint id), and the values predictionsForScheduling / prefixCacheScoresForEndpoints hold.
+  // Those are keyed by NamespacedName.Name (predictedlatency/preparedata_hooks.go:36-106), so of two candidates with one name
+  // the later one's values stand for both.  The prefix cache score is match / total whether or not a prediction was stored:
+  // PrepareRequestData fills it before, and independently of, the prediction branch (preparedata_hooks.go:42-58).
+  struct LatencyCtx {
+    bool set = false;
+    std::string rid;
+    double ttft_slo = 0.0, tpot_slo = 0.0;
+    std::map<int32_t, std::optional<LatencyPredictionInfo>> by_id;  // endpoint id -> its info
+    std::map<std::string, std::pair<std::optional<LatencyPredictionInfo>, double>> by_name;  // Name -> (info, prefix score)
+  };
+
+  // The final result's SchedulingResult::TargetLatency from the row's LatencyCtx: every profile's TargetEndpoints, in the order
+  // the result holds them (after ProcessResults), looked up by endpoint id.
+  void AttachLatency(BatchItem& it, const LatencyCtx& ctx, const std::vector<Endpoint>& endpoints, const std::vector<int>& ids) const {
+    if (!ctx.set || !it.error.empty()) return;
+    for (const auto& kv : it.result.ProfileResults) {
+      auto& tl = it.result.TargetLatency[kv.first];
+      tl.clear();
+      for (const ScoredEndpoint& t : kv.second.TargetEndpoints) {
+        const bool in_list = t.Index >= 0 && (size_t)t.Index < endpoints.size() && t.Endpoint_ == &endpoints[(size_t)t.Index];
+        const auto f = in_list ? ctx.by_id.find(ids[(size_t)t.Index]) : ctx.by_id.end();
+        tl.push_back(f == ctx.by_id.end() ? std::nullopt : f->second);
+      }
+    }
+  }
+
+  // One eppscore_predict_latency call for an engine batch piece: runs[i] are piece row i's (profile name, result) pairs (rows[i]
+  // its index in `requests`), hashes / nh / stride the piece's hashes_out (all zero when the engine did not hash), ids the list
+  // position -> endpoint id map.  Every TargetEndpoints entry's LatencyPredictionInfo goes into the row's LatencyCtx (AttachLatency
+  // puts it on the final result); with fill_match the entry also gets its PrefixMatch (as FillPrefixMatch gives it).  The row's
+  // LatencyCtx also gets each target name's values at the last candidate of that name.
+  void FillLatency(const std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>>& runs, const std::vector<int>& rows,
+                   const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints, const std::vector<int>& ids,
+                   const uint64_t* hashes, const uint16_t* nh, int32_t stride, const int32_t* in_tokens, const double* ttft_slo,
+                   const double* tpot_slo, bool fill_match, int block_tokens) {
+    const int n = (int)runs.size();
+    std::map<std::string, int> last_of_name;  // Name -> the last candidate position with it
+    for (size_t m = 0; m < endpoints.size(); m++) last_of_name[endpoints[m].GetMetadata()->NamespacedName_.Name] = (int)m;
+    std::vector<std::vector<int32_t>> cols((size_t)n);
+    auto col_of = [&](int i, int32_t id) {
+      auto& c = cols[(size_t)i];
+      const auto it = std::find(c.begin(), c.end(), id);
+      if (it != c.end()) return (size_t)(it - c.begin());
+      c.push_back(id);
+      return c.size() - 1;
+    };
+    size_t k = 0;
+    for (int i = 0; i < n; i++) {
+      for (const auto& run : runs[(size_t)i])
+        for (const ScoredEndpoint& t : run.second->TargetEndpoints) {
+          col_of(i, ids[(size_t)t.Index]);
+          col_of(i, ids[(size_t)last_of_name[endpoints[(size_t)t.Index].GetMetadata()->NamespacedName_.Name]]);
+        }
+      k = std::max(k, cols[(size_t)i].size());
+    }
+    if (n == 0 || k == 0) return;
+    if (fill_match && block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+    std::vector<int32_t> eps((size_t)n * k, -1), tok((size_t)n);
+    std::vector<double> tslo((size_t)n), pslo((size_t)n);
+    for (int i = 0; i < n; i++) {
+      std::copy(cols[(size_t)i].begin(), cols[(size_t)i].end(), eps.begin() + (ptrdiff_t)((size_t)i * k));
+      tok[(size_t)i] = in_tokens[i];
+      tslo[(size_t)i] = ttft_slo[i];
+      pslo[(size_t)i] = tpot_slo[i];
+    }
+    std::vector<eppscore_latency_info> info((size_t)n * k);
+    std::vector<uint16_t> match((size_t)n * k);  // (also the prefix cache score when no prediction was stored)
+    if (eppscore_predict_latency(eng_, n, (int32_t)k, 0, hashes, nh, stride, tok.data(), tslo.data(), pslo.data(), eps.data(), info.data(),
+                                 match.data(), nullptr) != EPPSCORE_OK)
+      throw SchedulingError(std::string("eppscore_predict_latency: ") + eppscore_last_error(eng_));
+    auto as_info = [](const eppscore_latency_info& x) -> std::optional<LatencyPredictionInfo> {
+      if (!x.present) return std::nullopt;
+      LatencyPredictionInfo v;
+      v.TTFTValid = x.ttft_valid != 0;
+      v.TPOTValid = x.tpot_valid != 0;
+      v.TTFTHeadroom = x.ttft_headroom;
+      v.TPOTHeadroom = x.tpot_headroom;
+      v.TTFT = x.ttft;
+      v.TPOT = x.tpot;
+      v.DispatchedRequestCount = x.dispatched;
+      return v;
+    };
+    for (int i = 0; i < n; i++) {
+      const InferenceRequest& q = requests[(size_t)rows[(size_t)i]];
+      LatencyCtx& ctx = lat_ctx_[(size_t)rows[(size_t)i]];
+      ctx.set = true;
+      ctx.rid = q.RequestId;
+      ctx.ttft_slo = ttft_slo[i];
+      ctx.tpot_slo = tpot_slo[i];
+      for (const auto& run : runs[(size_t)i]) {
+        for (ScoredEndpoint& t : run.second->TargetEndpoints) {
+          const int32_t id = ids[(size_t)t.Index];
+          const size_t j = (size_t)i * k + col_of(i, id);
+          ctx.by_id[id] = as_info(info[j]);
+          if (fill_match) t.PrefixMatch = PrefixCacheMatchInfo{match[j], nh[i], (uint16_t)block_tokens};
+          const std::string& name = endpoints[(size_t)t.Index].GetMetadata()->NamespacedName_.Name;
+          const size_t a = (size_t)i * k + col_of(i, ids[(size_t)last_of_name[name]]);
+          const double score = nh[i] ? (double)match[a] / (double)nh[i] : 0.0;  // match/total, NaN (0/0) => 0
+          ctx.by_name[name] = {as_info(info[a]), score};
+        }
+      }
+    }
+  }
+
+  // PreRequest's dispatch record (requestcontrol_hooks.go:236-251, :309-321), per request with an id, from the batch's LatencyCtx:
+  // TTFT and prefix score at the "prefill" profile's target when it has one, else at the primary target; TPOT at the primary.
+  void RecordDispatch(const std::vector<BatchItem>& results) {
+    if (!cfg_.LatencyPredictionInfo) return;
+    for (size_t r = 0; r < results.size() && r < lat_ctx_.size(); r++) {
+      const LatencyCtx& ctx = lat_ctx_[r];
+      const BatchItem& it = results[r];
+      if (!ctx.set || ctx.rid.empty() || !it.error.empty()) continue;
+      auto target = [&](const std::string& profile) -> const Endpoint* {
+        auto pr = it.result.ProfileResults.find(profile);
+        if (pr == it.result.ProfileResults.end() || pr->second.TargetEndpoints.empty()) return nullptr;
+        return pr->second.TargetEndpoints[0].Endpoint_;
+      };
+      auto values = [&](const Endpoint* ep) -> const std::pair<std::optional<LatencyPredictionInfo>, double>* {
+        if (!ep) return nullptr;
+        auto v = ctx.by_name.find(ep->GetMetadata()->NamespacedName_.Name);
+        return v == ctx.by_name.end() ? nullptr : &v->second;
+      };
+      const Endpoint* primary = target(it.result.PrimaryProfileName);
+      const Endpoint* prefill = target("prefill");
+      epp::PredictedLatencyAtDispatch d;
+      d.TTFTSLO = ctx.ttft_slo;
+      d.AvgTPOTSLO = ctx.tpot_slo;
+      if (const auto* v = values(prefill ? prefill : primary)) {
+        if (v->first) d.PredictedTTFT = v->first->TTFT;
+        d.PrefixCacheScore = v->second;
+      }
+      if (const auto* v = values(primary))
+        if (v->first) d.FirstPredictedTPOT = v->first->TPOT;
+      dispatch_[ctx.rid] = d;
+    }
   }
 
   // PreRequest's metrics (approximateprefix/plugin.go:199-204): per request with a primary target that carries its match, in
@@ -1032,6 +1229,7 @@ class Scheduler {
                                                std::map<unsigned, int64_t>& set_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size(), P = (int)cfg_.Profiles.size();
     std::vector<BatchItem> out((size_t)R);
+    lat_ctx_.assign(cfg_.LatencyPredictionInfo ? (size_t)R : 0, LatencyCtx{});
     last_hashes_.clear();
     last_nh_.clear();
     if (R == 0) return out;
@@ -1230,7 +1428,16 @@ class Scheduler {
           }
         }
       }
-      if (cfg_.PrefixMatchInfo && want_prefix) {  // every run's entries of this call's requests, against the call's hashes
+      if (cfg_.LatencyPredictionInfo) {  // every run's entries of this call's requests, before the next piece's snapshot
+        std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>> lruns((size_t)n);
+        for (int i = 0; i < n; i++)
+          for (int k = 0; k < nr; k++) {
+            auto it = got[(size_t)rows[i]].find(names[(size_t)prof[k]]);
+            if (it != got[(size_t)rows[i]].end()) lruns[(size_t)i].emplace_back(it->first, &it->second);
+          }
+        FillLatency(lruns, rows, requests, endpoints, ids, hashes.data(), nh.data(), last_stride_, in_tokens.data(), ttft_slo.data(),
+                    tpot_slo.data(), cfg_.PrefixMatchInfo && want_prefix, block_tokens);
+      } else if (cfg_.PrefixMatchInfo && want_prefix) {  // every run's entries of this call's requests, against the call's hashes
         std::vector<std::vector<ScoredEndpoint*>> targets((size_t)n);
         for (int i = 0; i < n; i++)
           for (int k = 0; k < nr; k++) {
@@ -1258,6 +1465,7 @@ class Scheduler {
       } catch (const SchedulingError& ex) {
         out[r].error = ex.what();
       }
+      if (cfg_.LatencyPredictionInfo) AttachLatency(out[r], lat_ctx_[(size_t)r], endpoints, ids);
     }
     last_endpoints_ = &endpoints;
     last_ids_ = ids;
@@ -1523,6 +1731,8 @@ class Scheduler {
   std::unordered_map<std::string, KeyUse> running_keys_;
   uint64_t next_key_ = 1;
   PrefixIndexerHistograms prefix_metrics_;
+  std::vector<LatencyCtx> lat_ctx_;  // the last batch's rows (SchedulerConfig::LatencyPredictionInfo)
+  std::unordered_map<std::string, epp::PredictedLatencyAtDispatch> dispatch_;
 };
 
 inline Scheduler* NewSchedulerWithConfig(const SchedulerConfig& c) { return new Scheduler(c); }

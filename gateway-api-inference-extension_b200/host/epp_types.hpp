@@ -114,12 +114,26 @@ struct ScoredEndpoint {
 };
 static_assert(sizeof(ScoredEndpoint) == 32, "the match info lives in the struct's tail");
 
+// attrlatency.LatencyPredictionInfo (datalayer/attribute/latency/data_types.go): what the predicted-latency producer's
+// PrepareRequestData stores on an endpoint for a request (predictedlatency/preparedata_hooks.go:36-106).
+struct LatencyPredictionInfo {
+  bool TTFTValid = false, TPOTValid = false;
+  double TTFTHeadroom = 0.0, TPOTHeadroom = 0.0;
+  double TTFT = 0.0, TPOT = 0.0;
+  int DispatchedRequestCount = 0;
+};
+
 struct ProfileRunResult {
   std::vector<ScoredEndpoint> TargetEndpoints;
 };
 struct SchedulingResult {
   std::map<std::string, ProfileRunResult> ProfileResults;
   std::string PrimaryProfileName;
+  // With SchedulerConfig::LatencyPredictionInfo, per profile name: each TargetEndpoints entry's LatencyPredictionInfo attribute,
+  // parallel to ProfileResults[name].TargetEndpoints of this result (an entry is empty when no prediction was stored).  Filled
+  // from the final result, after the profile handler's ProcessResults, so it follows whatever order and entries the handler
+  // returned.  Empty without the option and for batches of the small-batch host route.
+  std::map<std::string, std::vector<std::optional<LatencyPredictionInfo>>> TargetLatency;
 };
 
 // errcommon.Error{Code: Internal, ...} / fmt.Errorf of the reference, as an exception with the same text

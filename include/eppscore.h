@@ -490,6 +490,43 @@ int32_t eppscore_prefix_get(struct eppscore_engine *e, uint64_t hash, uint32_t *
 int32_t eppscore_prefix_match(struct eppscore_engine *e, int32_t R, int32_t k, int32_t location, const uint64_t *hashes,
                               const uint16_t *n_hashes, int32_t hash_stride, const int32_t *endpoints /* [R*k] */,
                               uint16_t *match_out /* [R*k] */, void *stream);
+/* What the predicted-latency producer's PrepareRequestData stores on one endpoint for one request
+ * (predictedlatency/preparedata_hooks.go:36-106, prediction.go:44-166): attrlatency.LatencyPredictionInfo
+ * (datalayer/attribute/latency/data_types.go) plus the prefix cache score it also keeps. */
+typedef struct eppscore_latency_info {
+  double ttft, tpot;                  /* prediction.go:171-185, NumTokensGenerated = 1 */
+  double ttft_headroom, tpot_headroom;/* ttft_slo - ttft; buffered - tpot, 0 when neutralised (prediction.go:99-103,143-161) */
+  double prefix_cache_score;          /* match / total blocks, NaN (0/0) -> 0 (preparedata_hooks.go:44-56) */
+  int32_t dispatched;                 /* getEndpointRunningRequestCount (plugin.go:357-363) */
+  uint8_t present;                    /* 0: no prediction stored, every other field 0 */
+  uint8_t ttft_valid;                 /* ttft < ttft_slo (strict: equality is not valid) */
+  uint8_t tpot_valid;                 /* tpot < buffered; 1 when neutralised (!streaming_mode or a prefill-role endpoint) */
+  uint8_t reserved;
+} eppscore_latency_info;              /* 48 bytes */
+/* The predicted-latency producer's values at chosen endpoints: info_out[r*k + j] is what PrepareRequestData would store on
+ * endpoint endpoints[r*k + j] for request r, from the engine's current prepared snapshot, its latency parameters and its
+ * running-request view (the inputs the last batch's latency fold-in read).  The prefix term is
+ * ttft_prefix * prefix_cache_score with the match of eppscore_prefix_match; input_tokens / ttft_slo / tpot_slo [R] as
+ * the eppscore_batch fields of the same names, NULL => 0.  buffered = tpot_slo * slo_buffer_factor, lowered to
+ * podMinTPOTSLO * slo_buffer_factor when the endpoint's podMinTPOTSLO > 0.  dispatched comes from the snapshot's array
+ * when it carries one, else from the running-request queues.  present = 0 (all fields 0) for entries outside [0, snapshot M), -1 padding included, and for every
+ * entry while the snapshot was prepared with has_predictions = 0 (no attribute is stored).
+ * match_out: optional [R*k], filled with what eppscore_prefix_match returns for the same arguments.
+ * location, hashes / n_hashes / hash_stride, k and the stream semantics are those of eppscore_prefix_match; a device-location
+ * call also waits for the snapshot preparations and producer updates issued before it, and later ones (set_snapshot,
+ * running_add / running_remove / running_remove_endpoint, index commits) wait for it.  Running-request updates wait for it only
+ * while a device call that reads the queue counts (a snapshot without `dispatched`) may still be in flight.
+ * One known difference from the reference: each entry's TTFT uses that endpoint's own match count.  The reference keys the
+ * prefix cache score it feeds the prediction by NamespacedName.Name (prediction.go:59-60), so where two candidates in different
+ * namespaces share a Name, it predicts the earlier one's TTFT with the later one's score.  running_add and set_snapshot change the view, so the documented order is
+ * schedule -> eppscore_predict_latency (and/or eppscore_prefix_match) -> commit / running_add / inflight_add.
+ * One kernel launch.  ERR_INVALID: k outside [1, max_endpoints], a bad location, R < 0, NULL required arrays, hash_stride <= 0,
+ * n_hashes > hash_stride (host location), no snapshot yet, or no profile with a latency scorer. */
+int32_t eppscore_predict_latency(struct eppscore_engine *e, int32_t R, int32_t k, int32_t location, const uint64_t *hashes,
+                                 const uint16_t *n_hashes, int32_t hash_stride, const int32_t *input_tokens,
+                                 const double *ttft_slo, const double *tpot_slo, const int32_t *endpoints /* [R*k] */,
+                                 eppscore_latency_info *info_out /* [R*k] */, uint16_t *match_out /* optional [R*k] */,
+                                 void *stream);
 int32_t eppscore_prefix_lru_len(const struct eppscore_engine *e, int32_t endpoint); /* -1: endpoint has no LRU */
 int32_t eppscore_prefix_lru_keys(const struct eppscore_engine *e, int32_t endpoint, uint64_t *out, int32_t cap); /* oldest first */
 /* Replication across GPUs: the index is a deterministic function of the ordered commit stream, so every rank applies the
