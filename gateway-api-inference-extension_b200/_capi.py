@@ -115,6 +115,7 @@ ABI_SYMBOLS = [
     ("eppscore_schedule_batch", C.c_int32, [_P, C.POINTER(Batch)]),
     ("eppscore_schedule_batch_topk", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
     ("eppscore_schedule_batch_topk_wide", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
+    ("eppscore_schedule_batch_inorder", C.c_int32, [_P, C.POINTER(Batch), _P]),
     ("eppscore_add_profile", C.c_int32, [_P, C.POINTER(Profile), C.POINTER(C.c_int32)]),
     ("eppscore_set_profile_endpoints", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_schedule_batch_profiles", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun)]),

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libeppscore.so")
 SOURCES = ["capi.cu", "hash_kernel.cu", "prepare_kernel.cu", "score_generic.cu", "score_dense.cu", "pick_sparse.cu",
-           "prefix_index.cu", "fields_kernel.cu", "host_path.cu", "inflight_kernel.cu", "running_kernel.cu", "topk_select.cu"]
+           "prefix_index.cu", "fields_kernel.cu", "host_path.cu", "inflight_kernel.cu", "running_kernel.cu", "topk_select.cu", "inorder_kernel.cu"]
 # score_matrix.cu holds 64 instantiations of one kernel template: compiled as eight objects (one (MASKED, DIAG) combination each,
 # with and without top-k lists, -DEPP_MATRIX_PART=k) so that they build in parallel
 PART_SOURCES = [("score_matrix.cu", f"score_matrix_p{k}.o", [f"-DEPP_MATRIX_PART={k}"]) for k in range(8)]

@@ -137,7 +137,11 @@ struct eppscore_engine {
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
         s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe,
-        s_subset;  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
+        s_subset,  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
+        // an in-order batch's slice (schedule_inorder): match rows, totals and candidate min / max.  Allocated by the first call
+        // outside a capture for a fixed number of rows and never reallocated, like `wide`.
+        s_io_match, s_io_total, s_io_minmax;
+    int32_t io_rows = 0;
     // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide).  Allocated by the first call that
     // needs them and never reallocated, so a graph captured after that call keeps pointing at live memory.
     DevBuf wide;
@@ -158,6 +162,7 @@ struct eppscore_engine {
   // arrays would block the host after every chunk and serialise the pipeline
   PinnedBuf h_res;
   int32_t wide_rows = 0;
+  int32_t io_cluster = 0;          // CTAs per cluster of inorder_pick_kernel (0: not decided yet)
   int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
@@ -1639,6 +1644,171 @@ int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_bat
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!t) return fail(e, EPPSCORE_ERR_INVALID, "topk NULL");
   return schedule_batch(e, b, t, true);
+}
+
+}  // extern "C"
+
+namespace {
+
+// Rows per slice of an in-order batch: a fixed byte budget of match rows (uint16 per endpoint), so the scratch depends on
+// max_endpoints only and a captured graph never sees it move.
+constexpr size_t kInOrderSliceBytes = 32ull << 20;
+
+// eppscore_schedule_batch_inorder on device buffers, asynchronous on `s`.  Per slice of rows: the batch kernels of
+// schedule_device with their match_out route (the prefix match counts and totals, which depend on no load; their provisional
+// picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
+// inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
+// so the next slice continues from them.
+int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, const int64_t* tokens, cudaStream_t s, Scratch& sc) {
+  const Profile& P = e->prof[0];
+  const eppscore_config& c = P.cfg;
+  if (!sc.s_io_match.p) {
+    if (is_capturing(s))
+      return fail(e, EPPSCORE_ERR_CAPACITY,
+                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
+                  "CUDA-graph capture first");
+    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
+    if (sc.rows > 0) rows = std::min(rows, sc.rows);
+    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
+    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
+    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
+    sc.io_rows = rows;
+  }
+  InOrderArgs a{};
+  a.M = e->M;
+  a.Mpad = e->geo.Mpad;
+  a.log_epl = e->geo.log_epl;
+  a.RW = e->geo.row_words;
+  a.A = e->A;
+  a.mask_words = (e->M + 31) / 32;
+  a.n_scorers = c.n_scorers;
+  bool minmax = false;
+  static const double cls_score[4] = {0.0, 0.6, 0.8, 1.0};  // lora_affinity.go:84-99
+  for (int i = 0; i < c.n_scorers; i++) {
+    const int k = c.scorer_kind[i];
+    a.kind[i] = k;
+    a.weight[i] = c.scorer_weight[i];
+    const bool static_term = k == EPPSCORE_SCORER_KV_CACHE || (k >= EPPSCORE_SCORER_ENDPOINT_COL0 && k < EPPSCORE_SCORER_ENDPOINT_COL0 + 4);
+    a.term[i] = static_term ? P.term[i].as<double>() : nullptr;
+    for (int q = 0; q < 4; q++) a.lora_term[i][q] = clamp01_host(cls_score[q]) * c.scorer_weight[i];
+    minmax = minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
+  }
+  a.pick_mode = c.pick_mode;
+  a.tie_mode = c.tie_mode;
+  a.seed_lo = (uint32_t)c.tie_seed;
+  a.seed_hi = (uint32_t)(c.tie_seed >> 32);
+  a.token_threshold = e->base_pa.token_threshold;
+  a.member = P.subset ? P.member_nat.as<uint32_t>() : nullptr;
+  a.queue = e->cur_queue;
+  a.running = e->cur_running;
+  a.cls_lo = e->cls_lo.as<uint32_t>();
+  a.cls_hi = e->cls_hi.as<uint32_t>();
+  a.inflight_req = e->inflight_req.as<int64_t>();
+  a.inflight_tok = e->inflight_tok.as<int64_t>();
+  for (int32_t base = 0; base < d.R; base += sc.io_rows) {
+    DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
+    q.match_blocks = sc.s_io_match.as<uint16_t>();
+    if (!q.total_blocks) q.total_blocks = sc.s_io_total.as<uint16_t>();
+    int32_t rc = schedule_device(e, q, s, sc);
+    if (rc != EPPSCORE_OK) return rc;
+    a.R = q.R;
+    a.request_base = q.request_base;
+    a.match = q.match_blocks;
+    a.total = q.total_blocks;
+    a.adapter_id = q.adapter_id;
+    a.cand_mask = q.run[0].cand_mask;
+    a.tokens = tokens ? tokens + base : nullptr;
+    a.pick = q.run[0].pick;
+    a.pick_score = q.run[0].pick_score;
+    a.tie_count = q.run[0].tie_count;
+    a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
+    if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
+    const int launched = launch_inorder_pick(a, e->io_cluster, s);
+    if (launched < 0) {
+      cudaGetLastError();
+      return cuda_fail(e, (cudaError_t)-launched, "inorder_pick_kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
+  }
+  return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
+  if (cfg_has(e->prof[0].cfg, EPPSCORE_SCORER_LATENCY))
+    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: the latency scorer's inputs are PreRequest state the call does not order");
+  if (e->have_snapshot && e->snapshot_has_tokens)
+    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: the snapshot supplies inflight_tokens; the in-order view needs the engine's counters");
+  if (b->dense_feat || b->scores_out || b->match_blocks || b->pred_out || b->filter_mask_out)
+    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: dense_feat, scores_out, match_blocks, pred_out and filter_mask_out are not available");
+  if (!b->pick || !b->pick_score || !b->tie_count) return fail(e, EPPSCORE_ERR_INVALID, "pick/pick_score/tie_count required");
+  if (b->location != 0 && b->location != 1) return fail(e, EPPSCORE_ERR_INVALID, "location must be 0 or 1");
+  if (b->R == 0) return EPPSCORE_OK;
+  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch_inorder before set_snapshot");
+  if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
+  CK(e, cudaSetDevice(e->device));
+  if (e->io_cluster == 0) {  // the cluster shape, decided once per engine and before the first call launches anything
+    const int C = inorder_cluster_size(e->geo.Mpad);
+    if (C < 0) return cuda_fail(e, (cudaError_t)-C, "inorder_pick_kernel cluster attributes");
+    if (C == 0)
+      return fail(e, EPPSCORE_ERR_CAPACITY, "schedule_batch_inorder: no thread-block cluster of this device holds max_endpoints "
+                                            "endpoints (8192 needs the non-portable cluster size 16)");
+    e->io_cluster = C;
+  }
+  const DevBatch d = make_batch(e, *b, 1, nullptr, nullptr, false);
+  bool capturing = false;
+  int32_t rc;
+  if (b->location == 1) {
+    cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
+    StreamScratch* own = reserved_scratch(e, cs);
+    if (own) {  // refused before anything is launched: the stream's set is never grown
+      if (b->R > own->max_R) return fail(e, EPPSCORE_ERR_CAPACITY, "R exceeds the max_R the batch's stream was reserved for");
+      if (d.prompt_bytes && !d.hashes_in && d.max_blocks > own->max_blocks)
+        return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks exceeds the max_blocks the batch's stream was reserved for");
+    }
+    if ((rc = producer_begin(e, cs, &capturing)) != EPPSCORE_OK) return rc;
+    if ((rc = schedule_inorder(e, d, tokens, cs, own ? own->sc : e->sc[0])) != EPPSCORE_OK) return rc;
+    if ((rc = producer_end(e, cs, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
+    return pending_record(e, cs);
+  }
+  // host arrays: staged whole into sc[0] on the engine stream, scheduled there, copied back
+  if (b->hashes_out && (b->hashes_in || !b->prompt_bytes))
+    return fail(e, EPPSCORE_ERR_INVALID, "hashes_out needs prompt_bytes (hashes supplied as hashes_in are already the caller's)");
+  cudaStream_t st = e->stream;
+  Scratch& sc = e->sc[0];
+  if ((rc = pending_wait(e, st)) != EPPSCORE_OK) return rc;  // a device-location batch may still hold sc[0]
+  DevBatch x = d;
+  if (b->prompt_bytes &&
+      (rc = stage_prompts(e, sc.s_prompts, b->prompt_bytes, b->prompt_off, b->prompt_len, 0, b->R, st, &x.prompt_bytes)) != EPPSCORE_OK)
+    return rc;
+  std::vector<std::pair<void*, std::pair<const void*, size_t>>> d2h;
+  cudaError_t c = cudaSuccess;
+  for_each_row_array(x, (size_t)e->M, [&](auto*& p, size_t per, Rows kind, DevBuf Scratch::*slot) {
+    if (!p || c != cudaSuccess) return;
+    const size_t nb = ((size_t)b->R + (kind == Rows::offsets ? 1 : 0)) * per * sizeof *p;
+    if ((c = (sc.*slot).reserve(nb)) != cudaSuccess) return;
+    auto* dev = reinterpret_cast<std::remove_reference_t<decltype(p)>>((sc.*slot).p);
+    if (kind == Rows::in || kind == Rows::offsets) c = cudaMemcpyAsync((void*)dev, p, nb, cudaMemcpyHostToDevice, st);
+    else d2h.push_back({(void*)p, {(const void*)dev, nb}});
+    p = dev;
+  });
+  CK(e, c);
+  if (x.hashes_out) CK(e, cudaMemsetAsync(x.hashes_out, 0, (size_t)b->R * x.max_blocks * 8, st));
+  const int64_t* d_tok = nullptr;
+  if ((rc = h2d(e, e->stage[0], tokens, (size_t)b->R, &d_tok, st)) != EPPSCORE_OK) return rc;
+  if ((rc = producer_begin(e, st, &capturing)) != EPPSCORE_OK) return rc;
+  if ((rc = schedule_inorder(e, x, d_tok, st, sc)) != EPPSCORE_OK) return rc;
+  if ((rc = producer_end(e, st, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
+  for (const auto& [dst, src] : d2h) CK(e, cudaMemcpyAsync(dst, src.first, src.second, cudaMemcpyDeviceToHost, st));
+  CK(e, cudaStreamSynchronize(st));
+  return EPPSCORE_OK;
 }
 
 int32_t eppscore_add_profile(eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) {

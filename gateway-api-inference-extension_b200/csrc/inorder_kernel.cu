@@ -1,0 +1,289 @@
+// inorder_kernel.cu — a batch scheduled in arrival order against the in-flight load (eppscore_schedule_batch_inorder): request r
+// is scored with the token-load terms left by requests 0..r-1's picks, as R consecutive Scheduler.Schedule + PreRequest calls
+// see them (inflightload/producer.go:101-120 feeding scorer/tokenload/token_load.go:83-111).
+//   inorder_minmax_kernel  per request, in parallel: min / max of WaitingQueueSize and RunningRequestsSize over its candidates
+//                          (queue.go:79-91 over the FILTERED endpoints)
+//   inorder_pick_kernel    one thread-block cluster walks the requests in order.  Thread t of CTA c owns endpoint c*T + t: its
+//                          in-flight counters live in its registers, its request-independent terms in shared memory.  Per
+//                          request every thread scores its endpoint in profile order (the float64 operations of
+//                          score_matrix_kernel, and of prepare_endpoints_kernel's token-load branch for the moving term), the
+//                          CTA reduces to a winner, the cluster merges the CTA winners through distributed shared memory behind
+//                          barrier.cluster, and the owner of the pick adds the request's tokens.
+// The prefix match counts and totals come from the ordinary batch kernels (their match_out route), which depend on no load.
+#include <cooperative_groups.h>
+
+#include "device_common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace eppscore {
+
+constexpr int kInOrderMaxThreads = 512;  // 128 registers per thread: the next request's inputs are prefetched
+constexpr int kInOrderWarps = kInOrderMaxThreads / 32;
+
+__global__ void __launch_bounds__(256) inorder_minmax_kernel(const __grid_constant__ InOrderArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+  for (int r = gw; r < a.R; r += nw) {
+    long long mn[2] = {0x7fffffffffffffffLL, 0x7fffffffffffffffLL};
+    long long mx[2] = {(long long)0x8000000000000000ULL, (long long)0x8000000000000000ULL};
+    const uint32_t* mrow = a.cand_mask ? a.cand_mask + (size_t)r * a.mask_words : nullptr;
+    for (int m = lane; m < a.M; m += 32) {
+      if (mrow && !((__ldg(mrow + (m >> 5)) >> (m & 31)) & 1u)) continue;
+      if (a.member && !((__ldg(a.member + (m >> 5)) >> (m & 31)) & 1u)) continue;
+#pragma unroll
+      for (int which = 0; which < 2; which++) {
+        const int64_t* q = which == 0 ? a.queue : a.running;
+        const long long v = q ? __ldg(reinterpret_cast<const long long*>(q) + m) : 0LL;
+        mn[which] = v < mn[which] ? v : mn[which];
+        mx[which] = v > mx[which] ? v : mx[which];
+      }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+#pragma unroll
+      for (int which = 0; which < 2; which++) {
+        const long long omn = shfl_xor_i64(mn[which], o), omx = shfl_xor_i64(mx[which], o);
+        mn[which] = omn < mn[which] ? omn : mn[which];
+        mx[which] = omx > mx[which] ? omx : mx[which];
+      }
+    if (lane < 4) a.minmax[(size_t)r * 4 + lane] = lane == 0 ? mn[0] : (lane == 1 ? mx[0] : (lane == 2 ? mn[1] : mx[1]));
+  }
+}
+
+// clamp(score) of the token-load scorer for an endpoint with `tokens` in flight (prepare_kernel.cu, token_load.go:96-106)
+__device__ __forceinline__ double token_load_score(long long tokens, double threshold) {
+  double load = __ll2double_rn(tokens);
+  if (load <= 0.0) return 1.0;
+  if (load > threshold) load = threshold;
+  return clamp01(__dsub_rn(1.0, __ddiv_rn(load, threshold)));
+}
+
+// One CTA's (or warp's) partial result: the max-score state, or the two stochastic-picker states.
+struct InOrderBest {
+  Best b;
+  RBest pos, all;
+};
+
+template <bool RND>
+__device__ __forceinline__ void inorder_warp_reduce(InOrderBest& x, int tie_mode) {
+  if (RND) {
+    rbest_warp_reduce(x.pos);
+    rbest_warp_reduce(x.all);
+  } else {
+    best_group_reduce<32>(x.b, tie_mode);
+  }
+}
+__device__ __forceinline__ InOrderBest inorder_none() {
+  InOrderBest x;
+  x.b = best_none();
+  x.pos = rbest_none();
+  x.all = rbest_none();
+  return x;
+}
+
+// Per-request inputs of one thread's endpoint: loaded one request ahead, while the previous request is reduced.
+struct InOrderReq {
+  long long mn0, mx0, mn1, mx1;  // queue, running
+  int32_t c, total, cls;
+  bool cand;
+  long long tokens;
+};
+
+template <bool RND>
+__global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(const __grid_constant__ InOrderArgs a) {
+  extern __shared__ __align__(16) double s_term[];  // [n_scorers][blockDim.x]: the request-independent terms of each thread's endpoint
+  __shared__ InOrderBest s_warp[kInOrderWarps];
+  __shared__ InOrderBest s_cta[2];  // the CTA's winner of the last two requests (read by the other CTAs of the cluster)
+  cg::cluster_group cluster = cg::this_cluster();
+  const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = T >> 5;
+  const int C = (int)cluster.num_blocks();
+  const int m = (int)cluster.block_rank() * T + tid;
+  const bool real = m < a.M;
+  const int tie_mode = a.tie_mode;
+
+  for (int s = 0; s < a.n_scorers; s++) s_term[(size_t)s * T + tid] = (real && a.term[s]) ? a.term[s][m] : 0.0;
+  const long long q0 = (real && a.queue) ? a.queue[m] : 0LL, q1 = (real && a.running) ? a.running[m] : 0LL;
+  const bool member = real && (!a.member || ((__ldg(a.member + (m >> 5)) >> (m & 31)) & 1u));
+  long long tok = m < a.Mpad ? a.inflight_tok[m] : 0, req = m < a.Mpad ? a.inflight_req[m] : 0;
+  double tl = real ? token_load_score(tok, a.token_threshold) : 0.0;
+  const uint32_t pos = perm_bitpos((uint32_t)(m < a.Mpad ? m : 0), a.log_epl);
+
+  auto load = [&](int r) {
+    InOrderReq x;
+    x.cand = member && r < a.R;
+    x.c = x.total = x.cls = 0;
+    x.tokens = 0;
+    x.mn0 = x.mx0 = x.mn1 = x.mx1 = 0;
+    if (r >= a.R) return x;
+    if (a.cand_mask) x.cand = x.cand && ((__ldg(a.cand_mask + (size_t)r * a.mask_words + (m >> 5)) >> (m & 31)) & 1u);
+    if (a.match && real) x.c = __ldg(a.match + (size_t)r * a.M + m);
+    if (a.total) x.total = __ldg(a.total + r);
+    if (a.minmax) {
+      const long long* mm = reinterpret_cast<const long long*>(a.minmax) + (size_t)r * 4;
+      x.mn0 = __ldg(mm);
+      x.mx0 = __ldg(mm + 1);
+      x.mn1 = __ldg(mm + 2);
+      x.mx1 = __ldg(mm + 3);
+    }
+    if (a.cls_lo && real) {
+      int ad = a.adapter_id ? __ldg(a.adapter_id + r) : -1;
+      if (ad < 0 || ad >= a.A) ad = a.A;
+      const size_t word = (size_t)ad * a.RW + (pos >> 5);
+      x.cls = (int)((__ldg(a.cls_lo + word) >> (pos & 31)) & 1u) | ((int)((__ldg(a.cls_hi + word) >> (pos & 31)) & 1u) << 1);
+    }
+    if (a.tokens) x.tokens = __ldg(reinterpret_cast<const long long*>(a.tokens) + r);
+    return x;
+  };
+
+  cluster.sync();  // every CTA of the cluster is running before any reads another's shared memory
+  InOrderReq cur = load(0);
+  for (int r = 0; r < a.R; r++) {
+    const InOrderReq nxt = load(r + 1);
+    // ---- Score (scheduler_profile.go:151-174): profile order from 0.0, the operations of score_matrix_kernel ----
+    double acc = 0.0;
+    for (int s = 0; s < a.n_scorers; s++) {
+      const int kind = a.kind[s];
+      const double w = a.weight[s];
+      double term;
+      if (kind == 6) {
+        term = __dmul_rn(tl, w);                                                       // the moving term
+      } else if (kind == 0 || kind == 4) {
+        const bool queue = kind == 0;
+        const long long mn = queue ? cur.mn0 : cur.mn1, mx = queue ? cur.mx0 : cur.mx1, qv = queue ? q0 : q1;
+        term = mx == mn ? __dmul_rn(1.0, w)                                            // queue.go:95-98
+                        : __dmul_rn(clamp01(__ddiv_rn(__ll2double_rn(mx - qv), __ll2double_rn(mx - mn))), w);
+      } else if (kind == 2) {
+        term = prefix_term_direct(cur.c, cur.total, w);                                // prefix/plugin.go:108-110
+      } else if (kind == 3) {
+        term = a.lora_term[s][cur.cls];
+      } else if (kind >= 16) {
+        term = __dmul_rn(0.0, w);                                                      // pair columns absent
+      } else {
+        term = s_term[(size_t)s * T + tid];                                            // kv-cache, endpoint columns
+      }
+      acc = __dadd_rn(acc, term);
+    }
+    // ---- Pick: this thread's candidate, then warp, CTA and cluster merges (all commutative and associative) ----
+    const uint32_t areq = tie_areq(a.request_base + r, a.seed_lo);
+    InOrderBest x = inorder_none();
+    if (cur.cand) {
+      const uint32_t pr = tie_prio(areq, m, a.seed_hi);
+      if (RND) {
+        rbest_update(x.all, (double)pr, acc, m);
+        if (a.pick_mode == 1 && acc > 0.0) rbest_update(x.pos, ares_key(pr, m, acc), acc, m);
+      } else {
+        best_update(x.b, acc, m, tie_mode, areq, a.seed_hi);
+      }
+    }
+    inorder_warp_reduce<RND>(x, tie_mode);
+    if (lane == 0) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      x = lane < nwarps ? s_warp[lane] : inorder_none();
+      inorder_warp_reduce<RND>(x, tie_mode);
+      if (lane == 0) s_cta[r & 1] = x;
+    }
+    cluster.sync();  // barrier.cluster: the CTA winners of request r are visible cluster-wide
+    x = lane < C ? *cluster.map_shared_rank(&s_cta[r & 1], lane) : inorder_none();
+    inorder_warp_reduce<RND>(x, tie_mode);
+    int pick;
+    double score;
+    int cnt;
+    if (RND) {
+      const RBest& wb = x.pos.m >= 0 ? x.pos : x.all;  // no positive score: the random picker (weightedrandom/picker.go:113-116)
+      pick = wb.m;
+      score = wb.score;
+      cnt = wb.n;
+    } else {
+      pick = x.b.m;
+      score = x.b.score;
+      cnt = x.b.cnt;
+    }
+    // ---- PreRequest: requests += 1, tokens += tokens[r] on the pick (producer.go:101-120) ----
+    if (pick == m) {
+      tok += cur.tokens;
+      req += 1;
+      tl = token_load_score(tok, a.token_threshold);
+    }
+    if (m == 0) {
+      a.pick[r] = pick;
+      a.pick_score[r] = pick >= 0 ? score : 0.0;
+      a.tie_count[r] = cnt;
+    }
+    cur = nxt;
+  }
+  if (m < a.Mpad) {
+    a.inflight_tok[m] = tok;
+    a.inflight_req[m] = req;
+  }
+  cluster.sync();  // no CTA leaves while another may still read its winners
+}
+
+int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count) {
+  if (a.R <= 0) return 0;
+  int blocks = (a.R + 7) / 8;
+  if (blocks > sm_count * 8) blocks = sm_count * 8;
+  inorder_minmax_kernel<<<blocks, 256, 0, s>>>(a);
+  return 1;
+}
+
+// The cluster: C CTAs of T = Mpad / C threads, one endpoint per thread.  Up to 16 CTAs when the device grants the non-portable
+// size, else 8 (then max_endpoints 8192 does not fit); fewer at small Mpad, so that a CTA keeps at least 256 endpoints (each
+// CTA is one more arrival at every barrier).  The dynamic shared memory (8 bytes per scorer per thread, at most 32 KiB) needs no
+// opt-in.
+template <bool RND>
+static cudaLaunchConfig_t pick_config(int Mpad, int C, cudaStream_t s, cudaLaunchAttribute* at) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(C);
+  cfg.blockDim = dim3(Mpad / C);
+  cfg.dynamicSmemBytes = (size_t)kMaxSteps * 8 * (Mpad / C);
+  cfg.stream = s;
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = C;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+template <bool RND>
+static int cluster_size(int Mpad) {
+  auto kernel = inorder_pick_kernel<RND>;
+  cudaError_t c = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  if (c != cudaSuccess) return -(int)c;
+  for (int cmax = 16; cmax >= 8; cmax /= 2) {
+    int C = Mpad / 256;
+    if (C < 1) C = 1;
+    if (C > cmax) C = cmax;
+    if (Mpad / C > kInOrderMaxThreads) continue;
+    cudaLaunchAttribute at[1];
+    const cudaLaunchConfig_t cfg = pick_config<RND>(Mpad, C, nullptr, at);
+    int clusters = 0;
+    c = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
+    if (c == cudaSuccess && clusters >= 1) return C;
+    cudaGetLastError();
+  }
+  return 0;
+}
+
+int inorder_cluster_size(int Mpad) {
+  const int a = cluster_size<false>(Mpad);
+  if (a <= 0) return a;
+  const int b = cluster_size<true>(Mpad);
+  return b <= 0 ? b : (a < b ? a : b);
+}
+
+int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s) {
+  if (a.R <= 0) return 0;
+  cudaLaunchAttribute at[1];
+  if (a.pick_mode != 0) {
+    const cudaLaunchConfig_t cfg = pick_config<true>(a.Mpad, C, s, at);
+    return launched_one(cudaLaunchKernelEx(&cfg, inorder_pick_kernel<true>, a));
+  }
+  const cudaLaunchConfig_t cfg = pick_config<false>(a.Mpad, C, s, at);
+  return launched_one(cudaLaunchKernelEx(&cfg, inorder_pick_kernel<false>, a));
+}
+
+}  // namespace eppscore

@@ -290,6 +290,43 @@ int launch_inflight_update(const int32_t* endpoint, const int64_t* tokens, int R
                            int64_t* token_sum, uint32_t* err, cudaStream_t s);
 int launch_estimate_tokens(const int64_t* size, const int32_t* hint, const int32_t* chars, int R, int64_t* out, cudaStream_t s);
 
+// a batch in arrival order against the in-flight counters (inorder_kernel.cu, eppscore_schedule_batch_inorder): profile 0's
+// scorers in profile order, one request at a time; the owner of each pick adds the request's tokens to the counters
+struct InOrderArgs {
+  int32_t M, Mpad, log_epl, RW, A, mask_words;
+  int32_t n_scorers;
+  int32_t kind[kMaxSteps];             // eppscore_scorer_kind (no latency scorer)
+  double weight[kMaxSteps];
+  double lora_term[kMaxSteps][4];      // per LoRA scorer: clamp({0,0.6,0.8,1.0})*w, as Plan::lora_term
+  const double* term[kMaxSteps];       // the prepared [Mpad] terms of the kv-cache and endpoint-column scorers, else null
+  int32_t pick_mode, tie_mode;
+  uint32_t seed_lo, seed_hi;
+  int64_t request_base;
+  double token_threshold;
+  int32_t R;
+  const uint16_t* match;               // [R][M] match counts (the batch kernels' match_out) or null
+  const uint16_t* total;               // [R] or null
+  long long* minmax;                   // [R][4]: queue min, max, running min, max over the candidates (or null: no such scorer)
+  const int32_t* adapter_id;           // [R] or null
+  const uint32_t* cand_mask;           // [R][mask_words] natural order or null
+  const uint32_t* member;              // [Mpad/32] natural-order bits of profile 0's endpoint subset, or null
+  const int64_t* queue;
+  const int64_t* running;
+  const uint32_t* cls_lo;              // LoRA class planes, permuted, [A+1][RW]
+  const uint32_t* cls_hi;
+  const int64_t* tokens;               // [R] or null (0 tokens)
+  int64_t* inflight_req;               // [Mpad] counters, read at the start and written back at the end
+  int64_t* inflight_tok;
+  int32_t* pick;
+  double* pick_score;
+  int32_t* tie_count;
+};
+int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count);  // fills a.minmax
+// CTAs per cluster of inorder_pick_kernel at this Mpad on the current device (sets the kernels' cluster attribute): > 0, 0 when no
+// cluster shape fits, or -(cudaError_t)
+int inorder_cluster_size(int Mpad);
+int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s);            // one cluster of C CTAs
+
 // predicted-latency producer's running-request queues (running_kernel.cu).  Table slot: {key, meta}, meta = endpoint + 1
 // (| kRunTomb once removed), {0, 0} empty; tpot[] holds the entry's tpot bits, owner[] / rm[] the (gen << 32 | r) bids of
 // an add / remove call (~0 when none).  Per endpoint: count, min_bits (kRunMinNone when empty), min_cnt = live entries

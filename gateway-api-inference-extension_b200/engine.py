@@ -171,7 +171,7 @@ class Engine:
                  n_hashes_in=None, hash_stride=0, adapter_id=None, cand_mask=None, dense_feat=None, dense_total=None,
                  block_chars=0, max_blocks=0, request_base=0, want_match=False, want_total=True, want_hashes=False,
                  want_scores=False, input_tokens=None, ttft_slo=None, tpot_slo=None, want_pred=False, want_filter_mask=False,
-                 topk=0, topk_wide=0, device=False, stream=None, out=None):
+                 topk=0, topk_wide=0, device=False, stream=None, out=None, _inorder=None):
         """Host mode (device=False): numpy in, returns dict of numpy outputs (copies inside the call).
         Device mode: CUDA tensors / raw pointers in; `out` must hold preallocated CUDA tensors
         (pick int32[R], pick_score float64[R], tie_count int32[R], optional match_blocks/total_blocks/hashes_out);
@@ -184,6 +184,11 @@ class Engine:
         call, topk = ((self._lib.eppscore_schedule_batch_topk_wide, topk_wide) if topk_wide else
                       (self._lib.eppscore_schedule_batch_topk, topk))
         a = _Args(device)
+        if _inorder is not None:  # schedule_inorder: (tokens,)
+            tok = a.ptr(_inorder[0], np.int64)
+            call = lambda h, bp: self._lib.eppscore_schedule_batch_inorder(h, bp, tok)
+        else:
+            call = self._lib.eppscore_schedule_batch if not topk else call
         b = Batch()
         b.struct_size = C.sizeof(Batch)
         b.R = R
@@ -224,7 +229,7 @@ class Engine:
                 t = self._topk(topk, a.ptr(out["topk_pick"], None), a.ptr(out["topk_score"], None))
                 self._check(call(self._h, C.byref(b), C.byref(t)))
             else:
-                self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
+                self._check(call(self._h, C.byref(b)))
             return out
         M = self.M
         mb = max_blocks or self.cfg.max_blocks
@@ -249,8 +254,18 @@ class Engine:
             t = self._topk(topk, res["topk_pick"].ctypes.data, res["topk_score"].ctypes.data)
             self._check(call(self._h, C.byref(b), C.byref(t)))
         else:
-            self._check(self._lib.eppscore_schedule_batch(self._h, C.byref(b)))
+            self._check(call(self._h, C.byref(b)))
         return res
+
+    def schedule_inorder(self, R, tokens=None, **kw):
+        """eppscore_schedule_batch_inorder: `schedule` for profile 0 with request r scored against the in-flight load that
+        requests 0..r-1 were sent with, and each pick's tokens (int64[R], None = 0) added to the counters in order.  Takes the
+        arguments of `schedule` except the R x M outputs, dense rows and top-k lists; host mode returns the same dict, device
+        mode fills `out` asynchronously on `stream` (tokens then a CUDA tensor)."""
+        for k in ("want_match", "want_scores", "want_pred", "want_filter_mask", "topk", "topk_wide"):
+            if kw.get(k):
+                raise ValueError(f"schedule_inorder does not take {k}")
+        return self.schedule(R, _inorder=(tokens,), **kw)
 
     # ------------------------------------------------------------------ several scheduler profiles
     def add_profile(self, scorers, pick_mode=0, filters=()) -> int:

@@ -140,6 +140,12 @@ struct PrefixIndexerHistograms {
   Histogram<14> HitBytes{{0, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384, 32768, 65536}};  // prefix_indexer_hit_bytes
 };
 
+// eppscore_schedule_batch_inorder (a batch in arrival order against the in-flight load) came the same way: EngineHasInOrderLoad()
+// tells.  Without it a config with SchedulerConfig::InOrderInFlightLoad is refused when the Scheduler is built.
+extern "C" int32_t eppscore_schedule_batch_inorder(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens)
+    __attribute__((weak));
+inline bool EngineHasInOrderLoad() { return &eppscore_schedule_batch_inorder != nullptr; }
+
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
          &eppscore_inflight_remove_endpoint != nullptr && &eppscore_inflight_get != nullptr;
@@ -347,6 +353,14 @@ struct SchedulerConfig {
   // (Scheduler::PredictedLatencyAtDispatch) until ResponseComplete / RequestExpired.  Batches of the small-batch host route leave
   // it empty.  Needs a profile with a latency scorer and an engine library with eppscore_predict_latency.
   bool LatencyPredictionInfo = false;
+  // Opt-in (off by default), with InFlightLoad: every engine batch goes through eppscore_schedule_batch_inorder, so request r of
+  // a batch is scored against the load requests 0..r-1 were sent with, as the reference's per-request Schedule + PreRequest
+  // sequence does (inflightload/producer.go:101-120 before token_load.go:83-111), instead of one load view per batch.  The
+  // call adds each request's estimate to its TargetEndpoints[0] while it schedules, so PreRequest does not add it again;
+  // ResponseComplete releases it as before.  The counters after ScheduleBatch + PreRequest are those of the per-request
+  // sequence.  Refused with a latency scorer, with the Profiles list, with MaxNumOfEndpoints > 1, without InFlightLoad and with
+  // an engine library without the call.
+  bool InOrderInFlightLoad = false;
 };
 
 class Scheduler {
@@ -446,6 +460,17 @@ class Scheduler {
     if (cfg.LatencyPredictionInfo && !EngineHasPredictLatency())
       throw SchedulingError("SchedulerConfig::LatencyPredictionInfo needs an engine library with eppscore_predict_latency");
     inflight_ = cfg.InFlightLoad != nullptr;
+    if (cfg0.InOrderInFlightLoad) {
+      if (!inflight_) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs the inflight-load-producer (InFlightLoad)");
+      if (!cfg0.Profiles.empty()) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad serves the single-profile config, not the Profiles list");
+      if (cfg.Profile.picker().MaxNumOfEndpoints > 1) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs maxNumOfEndpoints == 1");
+      for (const auto& w : sc)
+        if (dynamic_cast<const LatencyScorer*>(w.Scorer_.get()))
+          throw SchedulingError("SchedulerConfig::InOrderInFlightLoad cannot order the latency scorer's inputs");
+      if (!EngineHasInOrderLoad())
+        throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs an engine library with eppscore_schedule_batch_inorder");
+      inorder_ = true;
+    }
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
       throw SchedulingError("TrackRunningRequests needs an engine library with eppscore_running_add");
@@ -772,7 +797,15 @@ class Scheduler {
         all_scores.resize((size_t)R * Mx);
         b.scores_out = all_scores.data();
       }
-      if (eppscore_schedule_batch(eng_, &b) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_schedule_batch: ") + eppscore_last_error(eng_));
+      if (inorder_) {  // the estimates go in with the batch: the call adds each pick's load in request order
+        std::vector<int64_t> est((size_t)R);
+        if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
+          throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+        if (eppscore_schedule_batch_inorder(eng_, &b, est.data()) != EPPSCORE_OK)
+          throw SchedulingError(std::string("eppscore_schedule_batch_inorder: ") + eppscore_last_error(eng_));
+      } else if (eppscore_schedule_batch(eng_, &b) != EPPSCORE_OK) {
+        throw SchedulingError(std::string("eppscore_schedule_batch: ") + eppscore_last_error(eng_));
+      }
     }
     last_endpoints_ = &endpoints;
     last_ids_ = ids;
@@ -839,7 +872,7 @@ class Scheduler {
  public:
   // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index; with the
   // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
-  // (inflightload/producer.go:101-120).
+  // (inflightload/producer.go:101-120), unless InOrderInFlightLoad counted it while scheduling.
   void PreRequest(const std::vector<BatchItem>& results) {
     RecordPrefixCacheMatch(results);
     RecordDispatch(results);
@@ -856,7 +889,7 @@ class Scheduler {
       if (eppscore_commit_picks(eng_, R, pick.data(), last_hashes_.data(), last_nh_.data(), last_stride_, cap.data()) != EPPSCORE_OK)
         throw SchedulingError(std::string("eppscore_commit_picks: ") + eppscore_last_error(eng_));
     }
-    if (inflight_ && (int)last_size_.size() == R) {
+    if (inflight_ && !inorder_ && (int)last_size_.size() == R) {  // (in order: ScheduleBatch added the load already)
       std::vector<int64_t> est((size_t)R);
       if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
         throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
@@ -1693,7 +1726,7 @@ class Scheduler {
     s.lora_nmodels = nm.data();
     s.lora_max = mx.data();
     // with the producer, a token-load scorer reads the engine's in-flight counters (a snapshot array would take precedence)
-    s.inflight_tokens = (have_tokens && !(inflight_ && token_load_)) ? tokens.data() : nullptr;
+    s.inflight_tokens = (have_tokens && !(inflight_ && (token_load_ || inorder_))) ? tokens.data() : nullptr;
     if (prod) {
       // with TrackRunningRequests the engine's queues feed the latency fold-in: the arrays stay NULL
       s.min_tpot_slo = running_ ? nullptr : min_tpot.data();
@@ -1723,6 +1756,7 @@ class Scheduler {
   uint64_t remapped_batches_ = 0;
   bool inflight_ = false;    // SchedulerConfig::InFlightLoad
   bool token_load_ = false;  // the profile has a token-load scorer
+  bool inorder_ = false;     // SchedulerConfig::InOrderInFlightLoad
   std::vector<int64_t> last_size_;  // estimator inputs of the last engine batch, per request
   std::vector<int32_t> last_hint_, last_chars_;
   bool running_ = false;  // PredictedLatencyProducer::TrackRunningRequests

@@ -343,6 +343,36 @@ int32_t eppscore_schedule_batch_topk(struct eppscore_engine *e, const eppscore_b
  * ERR_INVALID: k outside [1, max_endpoints], a wrong struct_size or NULL arrays. */
 int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppscore_batch *b, const eppscore_topk *t);
 
+/* A batch in arrival order against the in-flight load: the outputs (pick, pick_score, tie_count, total_blocks, hashes_out) and
+ * the in-flight counters afterwards equal, bit for bit, what this loop gives:
+ *     for r in 0 .. R-1:
+ *         eppscore_schedule_batch(request r alone, request_base = b->request_base + r)
+ *         eppscore_inflight_add(1, &pick[r], &tokens[r])
+ * so request r's token-load scorer sees the load requests 0..r-1 were sent with, as R consecutive Schedule + PreRequest calls
+ * of the reference do (inflightload/producer.go:101-120, token_load.go:83-111), instead of one load view for the whole batch.
+ * tokens: [R] where b->location says (usually eppscore_estimate_tokens' output); NULL = 0 tokens.  A request with pick -1 adds
+ * nothing; both the requests and the tokens counters are updated.  Only the token-load terms move from one request to the next:
+ * the queue / running min / max are over each request's own candidates, as in eppscore_schedule_batch.
+ * Scope: profile 0, any scorer set without the latency scorer, cand_mask, hashes_in or prompt bytes, every pick and tie mode.
+ * Locations and ordering: host arrays are staged and the call returns when done; device arrays run asynchronously on b->stream
+ * (reserved streams use their own scratch).  The call is a batch and a producer update: it waits for pending device batches
+ * and earlier producer updates as eppscore_inflight_add does, is registered as a pending batch, and ends by preparing the
+ * snapshot terms again from the new counters, so a following eppscore_schedule_batch sees what it would see after the loop.
+ * It can be captured into a CUDA graph once one call on the same stream (the engine stream for host arrays) has run outside a
+ * capture: that call allocates a fixed slice scratch, and a first call under capture fails with ERR_CAPACITY.
+ * Per slice of rows the batch kernels compute the prefix match (what does not depend on the load), then one thread-block
+ * cluster walks the requests in order with the counters in its registers and reduces each request's pick across its CTAs.
+ * Known cost: that pre-pass is the ordinary batch with its R x M match_blocks route (2 bytes per pair written and read back;
+ * its provisional picks are overwritten), which a match-only pre-pass could avoid; today the in-order walk dominates.  The
+ * cluster shape is decided by the engine's first call, before anything is launched: ERR_CAPACITY when no cluster of the device
+ * holds max_endpoints endpoints (8192 needs the non-portable cluster size 16).
+ * Not ordered: the prefix index (request r+1 does not see the blocks request r adds; commit after the call), the latency
+ * scorer's running queues, top-k lists, several profiles, and requests on other GPU shards (each engine orders its own batch).
+ * ERR_INVALID before anything is launched: a profile 0 with the latency scorer, a current snapshot that supplies
+ * inflight_tokens, dense_feat / scores_out / match_blocks / pred_out / filter_mask_out set, and what eppscore_schedule_batch
+ * refuses.  ERR_NO_SNAPSHOT before eppscore_set_snapshot. */
+int32_t eppscore_schedule_batch_inorder(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens);
+
 /* ---- several scheduler profiles (see eppscore_profile) ---- */
 /* Adds a profile; *id_out receives its id (1, 2, ...).  With a snapshot present the profile is prepared for it at once, on the
  * engine stream (a profile with a latency scorer on an engine that had none is usable from the next eppscore_set_snapshot).
