@@ -5,10 +5,12 @@
 
 #include <algorithm>
 #include <array>
+#include <cassert>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
 #include <memory>
 #include <string>
 #include <utility>
@@ -91,8 +93,8 @@ struct eppscore_engine {
   std::unique_ptr<DeviceIndex> index;
   // device-location batches on caller streams that may still read the table, the terms or a scratch set (pending_record)
   std::vector<PendingBatch> pending;
-  // Staging for the synchronous host-array calls: slot i holds the call's i-th array.  Each of those calls runs on `stream`
-  // and synchronises it before it returns, so one set serves them all.
+  // Staging for the synchronous host-array calls (HostStage): slot i holds the call's i-th array.  Each of those calls runs on
+  // `stream` and synchronises it before it returns, so one set serves them all.
   DevBuf stage[8];
 
   // Producer state the scorers read: mutations of either producer below prepare the terms of the profiles that read the state
@@ -136,7 +138,7 @@ struct eppscore_engine {
   // batches on streams without a set of their own (eppscore_reserve_stream), sc[1..3] the slices of a sliced one.
   struct Scratch {
     DevBuf s_prompts, s_off, s_len, s_seed, s_hashes, s_nh, s_adapter, s_mask, s_dense, s_dtotal, s_pick, s_score,
-        s_tie, s_match, s_total, s_scores, s_intok, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe,
+        s_tie, s_match, s_total, s_scores, s_intok, s_tokens, s_tslo, s_pslo, s_pred, s_fields, s_fmask, s_topk_m, s_topk_s, s_probe,
         s_subset,  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
         // an in-order batch's slice (schedule_inorder): match rows, totals and candidate min / max.  Allocated by the first call
         // outside a capture for a fixed number of rows and never reallocated, like `wide`.
@@ -237,6 +239,22 @@ int32_t pending_wait(eppscore_engine* e, cudaStream_t st) {
     if (cudaEventQuery(p.done) == cudaSuccess) p.armed = false;
     else CK(e, cudaStreamWaitEvent(st, p.done, 0));
   }
+  return EPPSCORE_OK;
+}
+
+// Orders a device-location reader on caller stream `s` after the index mutations issued before it (ev_table; the engine stream
+// orders itself, and inside a capture the graph's edges do).  *wait_snapshot (when given) says whether `s` must also wait for
+// ev_snapshot before it reads the snapshot terms: outside a capture when the last preparation ran outside one on another
+// stream, inside one when it was recorded in this same capture (a captured stream may only wait on events of its own
+// capture).  *capturing (when given) receives whether `s` is being captured.
+int32_t reader_begin(eppscore_engine* e, cudaStream_t s, bool* capturing, bool* wait_snapshot) {
+  unsigned long long cap_id = 0;
+  const bool cap = is_capturing(s, &cap_id);
+  if (!cap && s != e->stream) CK(e, cudaStreamWaitEvent(s, e->ev_table, 0));
+  if (capturing) *capturing = cap;
+  if (wait_snapshot)
+    *wait_snapshot = cap ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
+                         : (e->snapshot_capture_id == 0 && s != e->snapshot_stream);
   return EPPSCORE_OK;
 }
 
@@ -435,6 +453,7 @@ struct DevBatch {  // all device pointers
   const int32_t* input_tokens;
   const double* ttft_slo;
   const double* tpot_slo;
+  const int64_t* tokens;    // an in-order batch's per-request token estimates (schedule_inorder)
   uint16_t* match_blocks;   // profile-independent outputs, written by the kernels of run 0
   uint16_t* total_blocks;
   uint64_t* hashes_out;
@@ -468,6 +487,7 @@ void for_each_row_array(DevBatch& d, size_t M, F&& f) {
   f(d.input_tokens, 1, Rows::in, &Scratch::s_intok);
   f(d.ttft_slo, 1, Rows::in, &Scratch::s_tslo);
   f(d.tpot_slo, 1, Rows::in, &Scratch::s_pslo);
+  f(d.tokens, 1, Rows::in, &Scratch::s_tokens);
   for (int i = 0; i < d.n_runs; i++) {
     DevRun& r = d.run[i];
     f(r.cand_mask, mw, Rows::in, &Scratch::s_mask);
@@ -557,15 +577,10 @@ int32_t schedule_device(eppscore_engine* e, const DevBatch& b, cudaStream_t s, S
   if (b.R <= 0) return EPPSCORE_OK;
   const bool dense = b.dense_feat != nullptr;
 
-  // Ordering against the snapshot preparation and the table flush, which may have run on other streams.
-  // The hash kernels depend on neither, so the snapshot wait is issued only before the pick kernel: a caller
+  // The hash kernels do not read the snapshot terms, so the snapshot wait is issued only before the pick kernel: a caller
   // may prepare the snapshot on a second stream concurrently with the hashing of the batch.
-  // Under CUDA-graph capture a stream may only wait on events recorded inside the SAME capture.
-  unsigned long long cap_id = 0;
-  const bool capturing = is_capturing(s, &cap_id);
-  if (!capturing && s != e->stream) CK(e, cudaStreamWaitEvent(s, e->ev_table, 0));
-  const bool wait_snapshot = capturing ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
-                                       : (e->snapshot_capture_id == 0 && s != e->snapshot_stream);
+  bool wait_snapshot = false;
+  if (int32_t rc = reader_begin(e, s, nullptr, &wait_snapshot); rc != EPPSCORE_OK) return rc;
 
   // Per run: its profile's arguments.  A run on a profile with an endpoint subset and no cand_mask stays on the sparse path with
   // the member bitmap when that path takes it; every other run on such a profile is scored by the masked kernels on rows
@@ -876,16 +891,6 @@ int32_t schedule_wide(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scr
   return EPPSCORE_OK;
 }
 
-template <typename T>
-int32_t h2d(eppscore_engine* e, DevBuf& buf, const T* src, size_t count, const T** out, cudaStream_t st = nullptr) {
-  *out = nullptr;
-  if (!src || count == 0) return EPPSCORE_OK;
-  CK(e, buf.reserve(count * sizeof(T)));
-  CK(e, cudaMemcpyAsync(buf.p, src, count * sizeof(T), cudaMemcpyHostToDevice, st ? st : e->stream));
-  *out = buf.as<T>();
-  return EPPSCORE_OK;
-}
-
 // Copies the bytes of prompts [r0, r1) from the host to `buf` on `st`; *out is the device base that the caller's offsets
 // index into.  The extent comes from prompt_off (and prompt_len when given).  The copy starts at a 16-byte aligned source
 // offset so every prompt keeps its alignment (the fast hash path needs 16-byte aligned starts), and is padded by 64 B so
@@ -908,6 +913,78 @@ int32_t stage_prompts(eppscore_engine* e, DevBuf& buf, const uint8_t* bytes, con
   *out = buf.as<uint8_t>() - start;
   return EPPSCORE_OK;
 }
+
+// One copy of a host-array call's results (HostStage, schedule_batch).
+struct Copy {
+  void* dst;
+  const void* src;
+  size_t bytes;
+};
+
+// The staging of one host-array call: its inputs, prompt bytes and outputs each take the next of e->stage's slots, in call
+// order, and are copied on the engine stream.  finish() runs the call's device form, copies the outputs back and synchronises
+// the engine stream, after which the caller's arrays may be reused and the slots serve the next call.  The first failure is
+// kept: finish() returns it without running anything.
+class HostStage {
+ public:
+  explicit HostStage(eppscore_engine* e) : e_(e) {}
+  // The next slot, holding n elements of T.
+  template <typename T>
+  T* slot(size_t n) {
+    DevBuf& b = next();
+    return check(b.reserve(n * sizeof(T)), "staging allocation") ? b.as<T>() : nullptr;
+  }
+  // rows[0..n_rows) of n elements each, one after the other in one slot; nullptr when there are none.
+  template <typename T>
+  const T* in(const T* const* rows, int n_rows, size_t n) {
+    if (!rows[0] || n == 0) return nullptr;
+    T* d = slot<T>(n_rows * n);
+    for (int i = 0; i < n_rows && d; i++)
+      check(cudaMemcpyAsync(d + i * n, rows[i], n * sizeof(T), cudaMemcpyHostToDevice, e_->stream), "staging copy");
+    return d;
+  }
+  template <typename T>
+  const T* in(const T* src, size_t n) { return in(&src, 1, n); }
+  // The bytes prompts [0, R) reach (stage_prompts).
+  const uint8_t* prompts(const uint8_t* bytes, const int64_t* off, const int32_t* len, int32_t R) {
+    const uint8_t* d = nullptr;
+    DevBuf& b = next();
+    if (rc_ == EPPSCORE_OK) rc_ = stage_prompts(e_, b, bytes, off, len, 0, R, e_->stream, &d);
+    return d;
+  }
+  // A slot for n elements the device form writes, copied back to dst by finish(); zeroed first when `zero` is set.  nullptr
+  // when dst is.
+  template <typename T>
+  T* out(T* dst, size_t n, bool zero = false) {
+    if (!dst) return nullptr;
+    T* d = slot<T>(n);
+    if (d && zero) check(cudaMemsetAsync(d, 0, n * sizeof(T), e_->stream), "staging memset");
+    if (d) back_.push_back({dst, d, n * sizeof(T)});
+    return d;
+  }
+  template <typename F>
+  int32_t finish(F&& call) {
+    int32_t rc = rc_ == EPPSCORE_OK ? call() : rc_;
+    if (rc != EPPSCORE_OK) return rc;
+    for (const Copy& b : back_) CK(e_, cudaMemcpyAsync(b.dst, b.src, b.bytes, cudaMemcpyDeviceToHost, e_->stream));
+    CK(e_, cudaStreamSynchronize(e_->stream));
+    return EPPSCORE_OK;
+  }
+
+ private:
+  DevBuf& next() {
+    assert(next_ < (int)std::size(e_->stage) && "HostStage: more arrays than e->stage has slots");
+    return e_->stage[next_++];
+  }
+  bool check(cudaError_t c, const char* what) {
+    if (c != cudaSuccess && rc_ == EPPSCORE_OK) rc_ = cuda_fail(e_, c, what);
+    return rc_ == EPPSCORE_OK;
+  }
+  eppscore_engine* e_;
+  int next_ = 0;
+  int32_t rc_ = EPPSCORE_OK;
+  std::vector<Copy> back_;
+};
 
 constexpr int64_t kRunInitialSlots = 4096;
 
@@ -1440,18 +1517,114 @@ int32_t eppscore_set_snapshot(eppscore_engine* e, const eppscore_snapshot* s) {
 
 namespace {
 
-// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk): the runs (profile + per-profile filter result and
-// outputs) of one batch, as make_batch takes them.
+// Rows per slice of an in-order batch: a fixed byte budget of match rows (uint16 per endpoint), so the scratch depends on
+// max_endpoints only and a captured graph never sees it move.
+constexpr size_t kInOrderSliceBytes = 32ull << 20;
+
+// eppscore_schedule_batch_inorder on device buffers, asynchronous on `s`.  Per slice of rows: the batch kernels of
+// schedule_device with their match_out route (the prefix match counts and totals, which depend on no load; their provisional
+// picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
+// inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
+// so the next slice continues from them.
+int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
+  const Profile& P = e->prof[0];
+  const eppscore_config& c = P.cfg;
+  if (!sc.s_io_match.p) {
+    if (is_capturing(s))
+      return fail(e, EPPSCORE_ERR_CAPACITY,
+                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
+                  "CUDA-graph capture first");
+    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
+    if (sc.rows > 0) rows = std::min(rows, sc.rows);
+    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
+    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
+    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
+    sc.io_rows = rows;
+  }
+  InOrderArgs a{};
+  a.M = e->M;
+  a.Mpad = e->geo.Mpad;
+  a.log_epl = e->geo.log_epl;
+  a.RW = e->geo.row_words;
+  a.A = e->A;
+  a.mask_words = (e->M + 31) / 32;
+  a.n_scorers = c.n_scorers;
+  bool minmax = false;
+  static const double cls_score[4] = {0.0, 0.6, 0.8, 1.0};  // lora_affinity.go:84-99
+  for (int i = 0; i < c.n_scorers; i++) {
+    const int k = c.scorer_kind[i];
+    a.kind[i] = k;
+    a.weight[i] = c.scorer_weight[i];
+    const bool static_term = k == EPPSCORE_SCORER_KV_CACHE || (k >= EPPSCORE_SCORER_ENDPOINT_COL0 && k < EPPSCORE_SCORER_ENDPOINT_COL0 + 4);
+    a.term[i] = static_term ? P.term[i].as<double>() : nullptr;
+    for (int q = 0; q < 4; q++) a.lora_term[i][q] = clamp01_host(cls_score[q]) * c.scorer_weight[i];
+    minmax = minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
+  }
+  a.pick_mode = c.pick_mode;
+  a.tie_mode = c.tie_mode;
+  a.seed_lo = (uint32_t)c.tie_seed;
+  a.seed_hi = (uint32_t)(c.tie_seed >> 32);
+  a.token_threshold = e->base_pa.token_threshold;
+  a.member = P.subset ? P.member_nat.as<uint32_t>() : nullptr;
+  a.queue = e->cur_queue;
+  a.running = e->cur_running;
+  a.cls_lo = e->cls_lo.as<uint32_t>();
+  a.cls_hi = e->cls_hi.as<uint32_t>();
+  a.inflight_req = e->inflight_req.as<int64_t>();
+  a.inflight_tok = e->inflight_tok.as<int64_t>();
+  for (int32_t base = 0; base < d.R; base += sc.io_rows) {
+    DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
+    q.match_blocks = sc.s_io_match.as<uint16_t>();
+    if (!q.total_blocks) q.total_blocks = sc.s_io_total.as<uint16_t>();
+    int32_t rc = schedule_device(e, q, s, sc);
+    if (rc != EPPSCORE_OK) return rc;
+    a.R = q.R;
+    a.request_base = q.request_base;
+    a.match = q.match_blocks;
+    a.total = q.total_blocks;
+    a.adapter_id = q.adapter_id;
+    a.cand_mask = q.run[0].cand_mask;
+    a.tokens = q.tokens;
+    a.pick = q.run[0].pick;
+    a.pick_score = q.run[0].pick_score;
+    a.tie_count = q.run[0].tie_count;
+    a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
+    if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
+    const int launched = launch_inorder_pick(a, e->io_cluster, s);
+    if (launched < 0) {
+      cudaGetLastError();
+      return cuda_fail(e, (cudaError_t)-launched, "inorder_pick_kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
+  }
+  return EPPSCORE_OK;
+}
+
+// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk, _inorder): the runs (profile + per-profile filter
+// result and outputs) of one batch, as make_batch takes them.  `inorder`: the batch's single run is scheduled in arrival order
+// against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
-                       const eppscore_topk* topk, bool wide = false) {
+                       const eppscore_topk* topk, bool wide = false, bool inorder = false, const int64_t* tokens = nullptr) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
   int32_t rc = EPPSCORE_OK;
-  const DevBatch d = make_batch(e, *b, n_runs, runs, topk, wide);
+  DevBatch d = make_batch(e, *b, n_runs, runs, topk, wide);
+  d.tokens = tokens;
   const size_t M = (size_t)e->M;
   bool any_wide = false;
   for (int i = 0; i < n_runs; i++) any_wide = any_wide || d.run[i].wide;
+  // What one piece of the batch runs on `st` with scratch set `sc`.  The in-order step reads and writes the in-flight counters,
+  // so it is ordered as a producer mutation.
+  auto step = [&](const DevBatch& x, cudaStream_t st, Scratch& sc) -> int32_t {
+    if (!inorder) return any_wide ? schedule_wide(e, x, st, sc) : schedule_device(e, x, st, sc);
+    bool capturing = false;
+    int32_t rc = producer_begin(e, st, &capturing);
+    if (rc == EPPSCORE_OK) rc = schedule_inorder(e, x, st, sc);
+    if (rc == EPPSCORE_OK) rc = producer_end(e, st, capturing, counters_feed_scorer(e));
+    return rc;
+  };
   if (b->location == 1) {
     bool per_pair = false;  // R x M outputs or masks on some run
     for (int i = 0; i < n_runs; i++) {
@@ -1466,19 +1639,16 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
         return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks exceeds the max_blocks the batch's stream was reserved for");
     }
     Scratch& sc = own ? own->sc : e->sc[0];
-    if (any_wide) {
-      if ((rc = schedule_wide(e, d, cs, sc)) != EPPSCORE_OK) return rc;
-      return pending_record(e, cs);
-    }
     // R x M outputs, masks, supplied hashes and dense rows go as one slice (their layouts are not sliced here), and so does a
-    // batch on a reserved stream (the slices share the engine's fork / join events and internal streams)
+    // batch on a reserved stream (the slices share the engine's fork / join events and internal streams), a wide batch
+    // (schedule_wide slices it in order on `cs`) and an in-order one (its requests run in order against one set of counters)
     const bool sliceable = d.prompt_bytes && !d.hashes_in && !per_pair && !d.dense_feat && !d.match_blocks && !d.input_tokens &&
-                           !d.ttft_slo && !d.tpot_slo && !own;
+                           !d.ttft_slo && !d.tpot_slo && !own && !any_wide && !inorder;
     int K = e->dev_split;
     if (!sliceable || e->dev_streams < 2) K = 1;
     while (K > 1 && b->R / K < 2048) K--;
     if (K <= 1) {
-      if ((rc = schedule_device(e, d, cs, sc)) != EPPSCORE_OK) return rc;
+      if ((rc = step(d, cs, sc)) != EPPSCORE_OK) return rc;
       return pending_record(e, cs);
     }
     // fork: the internal streams join the caller's stream (also inside a CUDA-graph capture), slice c goes to stream c mod S
@@ -1515,17 +1685,12 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   bool diag = d.match_blocks || d.dense_feat;  // R x M arrays: one chunk at a time is plenty
   for (int i = 0; i < n_runs; i++) diag = diag || d.run[i].scores_out || d.run[i].pred_out;
   int32_t chunk = e->host_chunk > 0 ? e->host_chunk : b->R;
-  if (diag || b->R < 2 * chunk) chunk = b->R;
+  if (diag || inorder || b->R < 2 * chunk) chunk = b->R;  // (an in-order batch: its requests run in order on one stream)
   const int nstreams = chunk < b->R ? 2 : 1;
   if (nstreams == 2 && !e->stream2) CK(e, make(e->stream2));
   // the chunks reuse sc[0] / sc[1], which a device-location batch may still hold
   if ((rc = pending_wait(e, e->stream)) != EPPSCORE_OK) return rc;
   if (nstreams == 2 && (rc = pending_wait(e, e->stream2)) != EPPSCORE_OK) return rc;
-  struct Copy {
-    void* dst;
-    const void* src;
-    size_t bytes;
-  };
   auto at = [](auto* p, void* base, size_t off) { return reinterpret_cast<decltype(p)>(static_cast<unsigned char*>(base) + off); };
   // The small results come back through pinned staging, since a D2H copy into the caller's (usually pageable) arrays would
   // block the host after every chunk: `pinned` is the batch with those outputs in h_res, the 8-byte arrays first so that each
@@ -1598,8 +1763,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     CK(e, c);
     // hashes_out from the device: entries past n_hashes[r] are zero
     if (x.hashes_out) CK(e, cudaMemsetAsync(x.hashes_out, 0, (size_t)n * x.max_blocks * 8, st));
-    rc = any_wide ? schedule_wide(e, x, st, sc) : schedule_device(e, x, st, sc);
-    if (rc != EPPSCORE_OK) return rc;
+    if ((rc = step(x, st, sc)) != EPPSCORE_OK) return rc;
     for (const Copy& y : d2h) CK(e, cudaMemcpyAsync(y.dst, y.src, y.bytes, cudaMemcpyDeviceToHost, st));
   }
   CK(e, cudaStreamSynchronize(e->stream));
@@ -1646,98 +1810,6 @@ int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_bat
   return schedule_batch(e, b, t, true);
 }
 
-}  // extern "C"
-
-namespace {
-
-// Rows per slice of an in-order batch: a fixed byte budget of match rows (uint16 per endpoint), so the scratch depends on
-// max_endpoints only and a captured graph never sees it move.
-constexpr size_t kInOrderSliceBytes = 32ull << 20;
-
-// eppscore_schedule_batch_inorder on device buffers, asynchronous on `s`.  Per slice of rows: the batch kernels of
-// schedule_device with their match_out route (the prefix match counts and totals, which depend on no load; their provisional
-// picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
-// inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
-// so the next slice continues from them.
-int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, const int64_t* tokens, cudaStream_t s, Scratch& sc) {
-  const Profile& P = e->prof[0];
-  const eppscore_config& c = P.cfg;
-  if (!sc.s_io_match.p) {
-    if (is_capturing(s))
-      return fail(e, EPPSCORE_ERR_CAPACITY,
-                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
-                  "CUDA-graph capture first");
-    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
-    if (sc.rows > 0) rows = std::min(rows, sc.rows);
-    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
-    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
-    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
-    sc.io_rows = rows;
-  }
-  InOrderArgs a{};
-  a.M = e->M;
-  a.Mpad = e->geo.Mpad;
-  a.log_epl = e->geo.log_epl;
-  a.RW = e->geo.row_words;
-  a.A = e->A;
-  a.mask_words = (e->M + 31) / 32;
-  a.n_scorers = c.n_scorers;
-  bool minmax = false;
-  static const double cls_score[4] = {0.0, 0.6, 0.8, 1.0};  // lora_affinity.go:84-99
-  for (int i = 0; i < c.n_scorers; i++) {
-    const int k = c.scorer_kind[i];
-    a.kind[i] = k;
-    a.weight[i] = c.scorer_weight[i];
-    const bool static_term = k == EPPSCORE_SCORER_KV_CACHE || (k >= EPPSCORE_SCORER_ENDPOINT_COL0 && k < EPPSCORE_SCORER_ENDPOINT_COL0 + 4);
-    a.term[i] = static_term ? P.term[i].as<double>() : nullptr;
-    for (int q = 0; q < 4; q++) a.lora_term[i][q] = clamp01_host(cls_score[q]) * c.scorer_weight[i];
-    minmax = minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
-  }
-  a.pick_mode = c.pick_mode;
-  a.tie_mode = c.tie_mode;
-  a.seed_lo = (uint32_t)c.tie_seed;
-  a.seed_hi = (uint32_t)(c.tie_seed >> 32);
-  a.token_threshold = e->base_pa.token_threshold;
-  a.member = P.subset ? P.member_nat.as<uint32_t>() : nullptr;
-  a.queue = e->cur_queue;
-  a.running = e->cur_running;
-  a.cls_lo = e->cls_lo.as<uint32_t>();
-  a.cls_hi = e->cls_hi.as<uint32_t>();
-  a.inflight_req = e->inflight_req.as<int64_t>();
-  a.inflight_tok = e->inflight_tok.as<int64_t>();
-  for (int32_t base = 0; base < d.R; base += sc.io_rows) {
-    DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
-    q.match_blocks = sc.s_io_match.as<uint16_t>();
-    if (!q.total_blocks) q.total_blocks = sc.s_io_total.as<uint16_t>();
-    int32_t rc = schedule_device(e, q, s, sc);
-    if (rc != EPPSCORE_OK) return rc;
-    a.R = q.R;
-    a.request_base = q.request_base;
-    a.match = q.match_blocks;
-    a.total = q.total_blocks;
-    a.adapter_id = q.adapter_id;
-    a.cand_mask = q.run[0].cand_mask;
-    a.tokens = tokens ? tokens + base : nullptr;
-    a.pick = q.run[0].pick;
-    a.pick_score = q.run[0].pick_score;
-    a.tie_count = q.run[0].tie_count;
-    a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
-    if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
-    const int launched = launch_inorder_pick(a, e->io_cluster, s);
-    if (launched < 0) {
-      cudaGetLastError();
-      return cuda_fail(e, (cudaError_t)-launched, "inorder_pick_kernel launch");
-    }
-    e->launches += launched;
-    CK(e, cudaGetLastError());
-  }
-  return EPPSCORE_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
 int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens) {
   if (!e) return EPPSCORE_ERR_INVALID;
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
@@ -1762,53 +1834,7 @@ int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch
                                             "endpoints (8192 needs the non-portable cluster size 16)");
     e->io_cluster = C;
   }
-  const DevBatch d = make_batch(e, *b, 1, nullptr, nullptr, false);
-  bool capturing = false;
-  int32_t rc;
-  if (b->location == 1) {
-    cudaStream_t cs = b->stream ? (cudaStream_t)b->stream : e->stream;
-    StreamScratch* own = reserved_scratch(e, cs);
-    if (own) {  // refused before anything is launched: the stream's set is never grown
-      if (b->R > own->max_R) return fail(e, EPPSCORE_ERR_CAPACITY, "R exceeds the max_R the batch's stream was reserved for");
-      if (d.prompt_bytes && !d.hashes_in && d.max_blocks > own->max_blocks)
-        return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks exceeds the max_blocks the batch's stream was reserved for");
-    }
-    if ((rc = producer_begin(e, cs, &capturing)) != EPPSCORE_OK) return rc;
-    if ((rc = schedule_inorder(e, d, tokens, cs, own ? own->sc : e->sc[0])) != EPPSCORE_OK) return rc;
-    if ((rc = producer_end(e, cs, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
-    return pending_record(e, cs);
-  }
-  // host arrays: staged whole into sc[0] on the engine stream, scheduled there, copied back
-  if (b->hashes_out && (b->hashes_in || !b->prompt_bytes))
-    return fail(e, EPPSCORE_ERR_INVALID, "hashes_out needs prompt_bytes (hashes supplied as hashes_in are already the caller's)");
-  cudaStream_t st = e->stream;
-  Scratch& sc = e->sc[0];
-  if ((rc = pending_wait(e, st)) != EPPSCORE_OK) return rc;  // a device-location batch may still hold sc[0]
-  DevBatch x = d;
-  if (b->prompt_bytes &&
-      (rc = stage_prompts(e, sc.s_prompts, b->prompt_bytes, b->prompt_off, b->prompt_len, 0, b->R, st, &x.prompt_bytes)) != EPPSCORE_OK)
-    return rc;
-  std::vector<std::pair<void*, std::pair<const void*, size_t>>> d2h;
-  cudaError_t c = cudaSuccess;
-  for_each_row_array(x, (size_t)e->M, [&](auto*& p, size_t per, Rows kind, DevBuf Scratch::*slot) {
-    if (!p || c != cudaSuccess) return;
-    const size_t nb = ((size_t)b->R + (kind == Rows::offsets ? 1 : 0)) * per * sizeof *p;
-    if ((c = (sc.*slot).reserve(nb)) != cudaSuccess) return;
-    auto* dev = reinterpret_cast<std::remove_reference_t<decltype(p)>>((sc.*slot).p);
-    if (kind == Rows::in || kind == Rows::offsets) c = cudaMemcpyAsync((void*)dev, p, nb, cudaMemcpyHostToDevice, st);
-    else d2h.push_back({(void*)p, {(const void*)dev, nb}});
-    p = dev;
-  });
-  CK(e, c);
-  if (x.hashes_out) CK(e, cudaMemsetAsync(x.hashes_out, 0, (size_t)b->R * x.max_blocks * 8, st));
-  const int64_t* d_tok = nullptr;
-  if ((rc = h2d(e, e->stage[0], tokens, (size_t)b->R, &d_tok, st)) != EPPSCORE_OK) return rc;
-  if ((rc = producer_begin(e, st, &capturing)) != EPPSCORE_OK) return rc;
-  if ((rc = schedule_inorder(e, x, d_tok, st, sc)) != EPPSCORE_OK) return rc;
-  if ((rc = producer_end(e, st, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
-  for (const auto& [dst, src] : d2h) CK(e, cudaMemcpyAsync(dst, src.first, src.second, cudaMemcpyDeviceToHost, st));
-  CK(e, cudaStreamSynchronize(st));
-  return EPPSCORE_OK;
+  return schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens);
 }
 
 int32_t eppscore_add_profile(eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) {
@@ -1953,26 +1979,14 @@ int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, c
     return EPPSCORE_OK;
   }
   // host arrays: staged, hashed by the device form on the engine stream, copied back
-  const uint8_t* d_bytes;
-  const int64_t* d_off;
-  const int32_t* d_len;
-  const uint64_t* d_seed;
-  int32_t rc;
-  if ((rc = stage_prompts(e, e->stage[0], prompt_bytes, prompt_off, prompt_len, 0, R, e->stream, &d_bytes)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], prompt_off, (size_t)R + 1, &d_off)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], prompt_len, (size_t)R, &d_len)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[3], model_seed, (size_t)R, &d_seed)) != EPPSCORE_OK)
-    return rc;
-  CK(e, e->stage[4].reserve((size_t)R * mb * 8));
-  CK(e, e->stage[5].reserve((size_t)R * 2));
-  CK(e, cudaMemsetAsync(e->stage[4].p, 0, (size_t)R * mb * 8, e->stream));  // entries past n_hashes[r] are zero
-  rc = eppscore_hash_prompts(e, R, 1, d_bytes, d_off, d_len, d_seed, bc, mb, e->stage[4].as<uint64_t>(), e->stage[5].as<uint16_t>(),
-                             e->stream);
-  if (rc != EPPSCORE_OK) return rc;
-  CK(e, cudaMemcpyAsync(hashes_out, e->stage[4].p, (size_t)R * mb * 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaMemcpyAsync(n_hashes_out, e->stage[5].p, (size_t)R * 2, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
-  return EPPSCORE_OK;
+  HostStage st(e);
+  const uint8_t* d_bytes = st.prompts(prompt_bytes, prompt_off, prompt_len, R);
+  const int64_t* d_off = st.in(prompt_off, (size_t)R + 1);
+  const int32_t* d_len = st.in(prompt_len, R);
+  const uint64_t* d_seed = st.in(model_seed, R);
+  uint64_t* d_hashes = st.out(hashes_out, (size_t)R * mb, true);  // entries past n_hashes[r] are zero
+  uint16_t* d_nh = st.out(n_hashes_out, R);
+  return st.finish([&] { return eppscore_hash_prompts(e, R, 1, d_bytes, d_off, d_len, d_seed, bc, mb, d_hashes, d_nh, e->stream); });
 }
 
 uint64_t eppscore_xxh64(const void* data, size_t len, uint64_t seed) { return xxh64_host(data, len, seed); }
@@ -1999,19 +2013,12 @@ int32_t eppscore_count_fields(eppscore_engine* e, int32_t R, int32_t location, c
     return EPPSCORE_OK;
   }
   // host arrays: staged, counted by the device form on the engine stream, copied back
-  const uint8_t* d_bytes;
-  const int64_t* d_off;
-  const int32_t* d_len;
-  int32_t rc;
-  if ((rc = stage_prompts(e, e->stage[0], prompt_bytes, prompt_off, prompt_len, 0, R, e->stream, &d_bytes)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], prompt_off, (size_t)R + 1, &d_off)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], prompt_len, (size_t)R, &d_len)) != EPPSCORE_OK)
-    return rc;
-  CK(e, e->stage[3].reserve((size_t)R * 4));
-  if ((rc = eppscore_count_fields(e, R, 1, d_bytes, d_off, d_len, e->stage[3].as<int32_t>(), e->stream)) != EPPSCORE_OK) return rc;
-  CK(e, cudaMemcpyAsync(out, e->stage[3].p, (size_t)R * 4, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
-  return EPPSCORE_OK;
+  HostStage st(e);
+  const uint8_t* d_bytes = st.prompts(prompt_bytes, prompt_off, prompt_len, R);
+  const int64_t* d_off = st.in(prompt_off, (size_t)R + 1);
+  const int32_t* d_len = st.in(prompt_len, R);
+  int32_t* d_out = st.out(out, R);
+  return st.finish([&] { return eppscore_count_fields(e, R, 1, d_bytes, d_off, d_len, d_out, e->stream); });
 }
 
 // lru_capacity (host, [M] or NULL) -> a padded host vector the index can copy; validates the values
@@ -2105,22 +2112,17 @@ static int32_t commit_calls(eppscore_engine* e, int32_t R, int32_t n_picks, cons
     }
   if (hi < 0) return EPPSCORE_OK;  // (a pick with zero hashes still creates the endpoint's LRU, indexer.go:57-68)
   if ((rc = index_begin(e)) != EPPSCORE_OK) return rc;
-  const uint64_t* d_hash;
-  const uint16_t* d_nh;
-  CK(e, e->stage[0].reserve((size_t)n_picks * R * 4));
-  for (int32_t p = 0; p < n_picks; p++) {
-    int32_t* dst = e->stage[0].as<int32_t>() + (size_t)p * R;
-    CK(e, cudaMemcpyAsync(dst, picks[p], (size_t)R * 4, cudaMemcpyHostToDevice, e->stream));
-    d_picks[p] = dst;
-  }
-  if ((rc = h2d(e, e->stage[1], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], n_hashes, (size_t)R, &d_nh)) != EPPSCORE_OK)
-    return rc;
-  rc = index_status(e, e->index->commit(R, n_picks, d_picks, d_hash, d_nh, hash_stride, caps.empty() ? nullptr : caps.data(), 0, lo,
-                                        hi - lo + 1, std::max<int64_t>(touches, 1), e->stream),
-                    what);
+  HostStage st(e);
+  const int32_t* d_pk = st.in(picks, n_picks, R);  // pick array p at row p
+  const uint64_t* d_hash = st.in(hashes, (size_t)R * hash_stride);
+  const uint16_t* d_nh = st.in(n_hashes, R);
+  rc = st.finish([&] {
+    for (int32_t p = 0; p < n_picks; p++) d_picks[p] = d_pk + (size_t)p * R;
+    return index_status(e, e->index->commit(R, n_picks, d_picks, d_hash, d_nh, hash_stride, caps.empty() ? nullptr : caps.data(), 0,
+                                            lo, hi - lo + 1, std::max<int64_t>(touches, 1), e->stream),
+                        what);
+  });
   if (rc != EPPSCORE_OK) return rc;
-  CK(e, cudaStreamSynchronize(e->stream));  // the caller's host arrays (pageable) may be reused
   return index_end(e);
 }
 
@@ -2152,20 +2154,17 @@ int32_t eppscore_prefix_add(eppscore_engine* e, const uint64_t* hashes, int32_t 
   int32_t rc = index_skips(e, true, "prefix_add");
   if (rc == EPPSCORE_OK) rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
-  const int32_t stride = n > 0 ? n : 1;
   const uint16_t nh = (uint16_t)n;
-  CK(e, e->stage[0].reserve(4));
-  CK(e, e->stage[1].reserve((size_t)stride * 8));
-  CK(e, e->stage[2].reserve(2));
-  CK(e, cudaMemcpyAsync(e->stage[0].p, &endpoint, 4, cudaMemcpyHostToDevice, e->stream));
-  if (n) CK(e, cudaMemcpyAsync(e->stage[1].p, hashes, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(e, cudaMemcpyAsync(e->stage[2].p, &nh, 2, cudaMemcpyHostToDevice, e->stream));
-  const int32_t* d_ep = e->stage[0].as<int32_t>();
-  rc = index_status(e, e->index->commit(1, 1, &d_ep, e->stage[1].as<uint64_t>(), e->stage[2].as<uint16_t>(), stride,
-                                        nullptr, lru_capacity, endpoint, 1, std::max(n, 1), e->stream),
-                    "prefix_add");
+  HostStage st(e);
+  const int32_t* d_ep = st.in(&endpoint, 1);
+  const uint64_t* d_hash = st.in(hashes, n);  // (nullptr for n = 0: the commit reads n hashes)
+  const uint16_t* d_nh = st.in(&nh, 1);
+  rc = st.finish([&] {
+    return index_status(e, e->index->commit(1, 1, &d_ep, d_hash, d_nh, std::max(n, 1), nullptr, lru_capacity, endpoint, 1,
+                                            std::max(n, 1), e->stream),
+                        "prefix_add");
+  });
   if (rc != EPPSCORE_OK) return rc;
-  CK(e, cudaStreamSynchronize(e->stream));
   return index_end(e);
 }
 
@@ -2179,15 +2178,12 @@ int32_t eppscore_prefix_apply(eppscore_engine* e, int64_t n, const uint64_t* has
   int32_t rc = index_skips(e, true, "prefix_apply");
   if (rc == EPPSCORE_OK) rc = index_begin(e);
   if (rc != EPPSCORE_OK) return rc;
-  const uint64_t* d_hash;
-  const int32_t* d_ep;
-  const uint8_t* d_op;
-  if ((rc = h2d(e, e->stage[0], hash, (size_t)n, &d_hash)) != EPPSCORE_OK || (rc = h2d(e, e->stage[1], endpoint, (size_t)n, &d_ep)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], op, (size_t)n, &d_op)) != EPPSCORE_OK)
-    return rc;
-  rc = index_status(e, e->index->apply(n, d_hash, d_ep, d_op, e->stream), "prefix_apply");
+  HostStage st(e);
+  const uint64_t* d_hash = st.in(hash, n);
+  const int32_t* d_ep = st.in(endpoint, n);
+  const uint8_t* d_op = st.in(op, n);
+  rc = st.finish([&] { return index_status(e, e->index->apply(n, d_hash, d_ep, d_op, e->stream), "prefix_apply"); });
   if (rc != EPPSCORE_OK) return rc;
-  CK(e, cudaStreamSynchronize(e->stream));
   return index_end(e);
 }
 
@@ -2240,28 +2236,22 @@ int32_t eppscore_prefix_match(eppscore_engine* e, int32_t R, int32_t k, int32_t 
   if (location == 1) {
     // Ordered like a device-location batch: after the index mutations issued before it (ev_table), and registered as pending so
     // that later mutations wait for it.  Inside a capture the graph's edges order it.
+    // It reads no snapshot term, so it does not wait for the snapshot preparation.
     cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
-    if (!is_capturing(cs) && cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
+    if (int32_t rc = reader_begin(e, cs, nullptr, nullptr); rc != EPPSCORE_OK) return rc;
     e->index->match(R, k, e->cfg.max_endpoints, hashes, n_hashes, hash_stride, endpoints, match_out, cs);
     CK(e, cudaGetLastError());
     return pending_record(e, cs);
   }
   for (int32_t r = 0; r < R; r++)
     if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "prefix_match: n_hashes exceeds hash_stride");
-  const uint64_t* d_hash;
-  const uint16_t* d_nh;
-  const int32_t* d_ep;
-  int32_t rc;
-  if ((rc = h2d(e, e->stage[0], hashes, (size_t)R * hash_stride, &d_hash)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], n_hashes, (size_t)R, &d_nh)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], endpoints, (size_t)R * k, &d_ep)) != EPPSCORE_OK)
-    return rc;
-  CK(e, e->stage[3].reserve((size_t)R * k * 2));
-  e->index->match(R, k, e->cfg.max_endpoints, d_hash, d_nh, hash_stride, d_ep, e->stage[3].as<uint16_t>(), e->stream);
-  CK(e, cudaGetLastError());
-  CK(e, cudaMemcpyAsync(match_out, e->stage[3].p, (size_t)R * k * 2, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
-  return EPPSCORE_OK;
+  // host arrays: staged, matched by the device form on the engine stream, copied back
+  HostStage st(e);
+  const uint64_t* d_hash = st.in(hashes, (size_t)R * hash_stride);
+  const uint16_t* d_nh = st.in(n_hashes, R);
+  const int32_t* d_ep = st.in(endpoints, (size_t)R * k);
+  uint16_t* d_out = st.out(match_out, (size_t)R * k);
+  return st.finish([&] { return eppscore_prefix_match(e, R, k, 1, d_hash, d_nh, hash_stride, d_ep, d_out, e->stream); });
 }
 
 int32_t eppscore_predict_latency(eppscore_engine* e, int32_t R, int32_t k, int32_t location, const uint64_t* hashes,
@@ -2279,6 +2269,30 @@ int32_t eppscore_predict_latency(eppscore_engine* e, int32_t R, int32_t k, int32
   if (R == 0) return EPPSCORE_OK;
   if (hash_stride <= 0) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: hash_stride must be > 0");
   CK(e, cudaSetDevice(e->device));
+  if (location == 0) {
+    for (int32_t r = 0; r < R; r++)
+      if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: n_hashes exceeds hash_stride");
+    // host arrays: staged, predicted by the device form on the engine stream, copied back
+    HostStage st(e);
+    const uint64_t* d_hash = st.in(hashes, (size_t)R * hash_stride);
+    const uint16_t* d_nh = st.in(n_hashes, R);
+    const int32_t* d_ep = st.in(endpoints, (size_t)R * k);
+    const int32_t* d_tok = st.in(input_tokens, R);
+    const double* d_ttft = st.in(ttft_slo, R);
+    const double* d_tpot = st.in(tpot_slo, R);
+    eppscore_latency_info* d_info = st.out(info_out, (size_t)R * k);
+    uint16_t* d_match = st.out(match_out, (size_t)R * k);
+    return st.finish([&] {
+      return eppscore_predict_latency(e, R, k, 1, d_hash, d_nh, hash_stride, d_tok, d_ttft, d_tpot, d_ep, d_info, d_match, e->stream);
+    });
+  }
+  // Ordered like a device-location batch: after the index mutations, snapshot preparations and producer updates issued before
+  // it, and registered as pending so that later ones wait for it.  Inside a capture the graph's edges order it.
+  cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
+  bool capturing = false, wait_snapshot = false;
+  if (int32_t rc = reader_begin(e, cs, &capturing, &wait_snapshot); rc != EPPSCORE_OK) return rc;
+  if (!capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(cs, e->ev_producer, 0));
+  if (wait_snapshot) CK(e, cudaStreamWaitEvent(cs, e->ev_snapshot, 0));
   const LatArgs& L = e->lat_args;
   LatInfoArgs a{};
   a.R = R;
@@ -2293,60 +2307,25 @@ int32_t eppscore_predict_latency(eppscore_engine* e, int32_t R, int32_t k, int32
   a.tpot_input = L.tpot_input;
   a.tpot_generated = L.tpot_generated;
   a.buffer = L.buffer;
-  if (location == 1) {
-    // Ordered like a device-location batch: after the index mutations, snapshot preparations and producer updates issued before
-    // it, and registered as pending so that later ones wait for it.  Inside a capture the graph's edges order it.
-    cudaStream_t cs = stream ? (cudaStream_t)stream : e->stream;
-    unsigned long long cap_id = 0;
-    const bool capturing = is_capturing(cs, &cap_id);
-    if (!capturing && cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
-    if (!capturing && e->producer_pending) CK(e, cudaStreamWaitEvent(cs, e->ev_producer, 0));
-    if (capturing ? (e->snapshot_capture_id != 0 && e->snapshot_capture_id == cap_id)
-                  : (e->snapshot_capture_id == 0 && cs != e->snapshot_stream))
-      CK(e, cudaStreamWaitEvent(cs, e->ev_snapshot, 0));
-    a.hashes = hashes;
-    a.n_hashes = n_hashes;
-    a.endpoints = endpoints;
-    a.input_tokens = input_tokens;
-    a.ttft_slo = ttft_slo;
-    a.tpot_slo = tpot_slo;
-    a.match_out = match_out;
-    a.out = info_out;
-    e->index->latency_info(a, e->cfg.max_endpoints, cs);
-    CK(e, cudaGetLastError());
-    if (!capturing && !e->snapshot_has_dispatched) {  // it reads the running-request counts in place (count_reads_wait)
-      if (cs == e->stream) {
-        CK(e, cudaEventRecord(e->ev_count_read, cs));
-        e->count_read_engine = true;
-      } else {
-        e->count_readers = true;
-      }
-    }
-    return pending_record(e, cs);
-  }
-  for (int32_t r = 0; r < R; r++)
-    if (n_hashes[r] > hash_stride) return fail(e, EPPSCORE_ERR_INVALID, "predict_latency: n_hashes exceeds hash_stride");
-  if (e->producer_pending) CK(e, cudaStreamWaitEvent(e->stream, e->ev_producer, 0));
-  int32_t rc;
-  if ((rc = h2d(e, e->stage[0], hashes, (size_t)R * hash_stride, &a.hashes)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], n_hashes, (size_t)R, &a.n_hashes)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], endpoints, (size_t)R * k, &a.endpoints)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[3], input_tokens, (size_t)R, &a.input_tokens)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[4], ttft_slo, (size_t)R, &a.ttft_slo)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[5], tpot_slo, (size_t)R, &a.tpot_slo)) != EPPSCORE_OK)
-    return rc;
-  CK(e, e->stage[6].reserve((size_t)R * k * sizeof(eppscore_latency_info)));
-  a.out = e->stage[6].p;
-  if (match_out) {
-    CK(e, e->stage[7].reserve((size_t)R * k * 2));
-    a.match_out = e->stage[7].as<uint16_t>();
-  }
-  e->index->latency_info(a, e->cfg.max_endpoints, e->stream);
+  a.hashes = hashes;
+  a.n_hashes = n_hashes;
+  a.endpoints = endpoints;
+  a.input_tokens = input_tokens;
+  a.ttft_slo = ttft_slo;
+  a.tpot_slo = tpot_slo;
+  a.match_out = match_out;
+  a.out = info_out;
+  e->index->latency_info(a, e->cfg.max_endpoints, cs);
   CK(e, cudaGetLastError());
-  CK(e, cudaMemcpyAsync(info_out, e->stage[6].p, (size_t)R * k * sizeof(eppscore_latency_info), cudaMemcpyDeviceToHost, e->stream));
-  if (match_out) CK(e, cudaMemcpyAsync(match_out, e->stage[7].p, (size_t)R * k * 2, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
-  return EPPSCORE_OK;
+  if (!capturing && !e->snapshot_has_dispatched) {  // it reads the running-request counts in place (count_reads_wait)
+    if (cs == e->stream) {
+      CK(e, cudaEventRecord(e->ev_count_read, cs));
+      e->count_read_engine = true;
+    } else {
+      e->count_readers = true;
+    }
+  }
+  return pending_record(e, cs);
 }
 
 // ---------------- in-flight load producer ----------------
@@ -2362,18 +2341,12 @@ int32_t eppscore_estimate_tokens(eppscore_engine* e, int32_t R, int32_t location
     return EPPSCORE_OK;
   }
   // host arrays: staged, estimated by the device form on the engine stream, copied back
-  const int64_t* d_size;
-  const int32_t *d_hint, *d_chars;
-  int32_t rc;
-  if ((rc = h2d(e, e->stage[0], request_size_bytes, (size_t)R, &d_size)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[1], token_hint, (size_t)R, &d_hint)) != EPPSCORE_OK ||
-      (rc = h2d(e, e->stage[2], prompt_chars, (size_t)R, &d_chars)) != EPPSCORE_OK)
-    return rc;
-  CK(e, e->stage[3].reserve((size_t)R * 8));
-  if ((rc = eppscore_estimate_tokens(e, R, 1, d_size, d_hint, d_chars, e->stage[3].as<int64_t>(), e->stream)) != EPPSCORE_OK) return rc;
-  CK(e, cudaMemcpyAsync(out, e->stage[3].p, (size_t)R * 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(e, cudaStreamSynchronize(e->stream));
-  return EPPSCORE_OK;
+  HostStage st(e);
+  const int64_t* d_size = st.in(request_size_bytes, R);
+  const int32_t* d_hint = st.in(token_hint, R);
+  const int32_t* d_chars = st.in(prompt_chars, R);
+  int64_t* d_out = st.out(out, R);
+  return st.finish([&] { return eppscore_estimate_tokens(e, R, 1, d_size, d_hint, d_chars, d_out, e->stream); });
 }
 
 static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const int64_t* tokens,
@@ -2386,23 +2359,23 @@ static int32_t inflight_update(eppscore_engine* e, int32_t R, int32_t location, 
   cudaStream_t st = (on_device && stream) ? (cudaStream_t)stream : e->stream;
   const int32_t* d_ep = endpoint;
   const int64_t* d_tok = tokens;
+  HostStage staged(e);
   if (!on_device) {
     for (int32_t r = 0; r < R; r++)
       if (endpoint[r] >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "inflight update: endpoint >= max_endpoints");
+    d_ep = staged.in(endpoint, R);
+    d_tok = staged.in(tokens, R);
   }
-  bool capturing = false;
-  int32_t rc = producer_begin(e, st, &capturing);
-  if (rc != EPPSCORE_OK) return rc;
-  if (!on_device) {
-    if ((rc = h2d(e, e->stage[0], endpoint, (size_t)R, &d_ep)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->stage[1], tokens, (size_t)R, &d_tok)) != EPPSCORE_OK) return rc;
-  }
-  e->launches += launch_inflight_update(d_ep, d_tok, R, e->cfg.max_endpoints, sign, e->inflight_req.as<int64_t>(),
-                                        e->inflight_tok.as<int64_t>(), e->inflight_err.as<uint32_t>(), st);
-  CK(e, cudaGetLastError());
-  if ((rc = producer_end(e, st, capturing, counters_feed_scorer(e))) != EPPSCORE_OK) return rc;
-  if (!on_device) CK(e, cudaStreamSynchronize(st));  // the caller's host arrays may be reused
-  return EPPSCORE_OK;
+  auto update = [&]() -> int32_t {
+    bool capturing = false;
+    int32_t rc = producer_begin(e, st, &capturing);
+    if (rc != EPPSCORE_OK) return rc;
+    e->launches += launch_inflight_update(d_ep, d_tok, R, e->cfg.max_endpoints, sign, e->inflight_req.as<int64_t>(),
+                                          e->inflight_tok.as<int64_t>(), e->inflight_err.as<uint32_t>(), st);
+    CK(e, cudaGetLastError());
+    return producer_end(e, st, capturing, counters_feed_scorer(e));
+  };
+  return on_device ? update() : staged.finish(update);
 }
 
 int32_t eppscore_inflight_add(eppscore_engine* e, int32_t R, int32_t location, const int32_t* endpoint, const int64_t* tokens,
@@ -2587,36 +2560,36 @@ int32_t running_update(eppscore_engine* e, int op, int32_t R, int32_t location, 
   CK(e, cudaSetDevice(e->device));
   const bool on_device = location == 1;
   cudaStream_t st = (on_device && stream) ? (cudaStream_t)stream : e->stream;
+  const int32_t* d_ep = endpoint;
+  const uint64_t* d_key = key;
+  const double* d_tpot = tpot;
+  HostStage staged(e);
   if (!on_device) {
     for (int32_t r = 0; r < R; r++) {
       if (endpoint[r] >= e->cfg.max_endpoints) return fail(e, EPPSCORE_ERR_INVALID, "running update: endpoint >= max_endpoints");
       if (tpot && std::isnan(tpot[r])) return fail(e, EPPSCORE_ERR_INVALID, "running_add: tpot_slo is NaN");
     }
+    d_ep = staged.in(endpoint, R);
+    d_key = staged.in(key, R);
+    d_tpot = staged.in(tpot, R);
   }
-  bool capturing = false;
-  int32_t rc = producer_begin(e, st, &capturing);
-  if (rc != EPPSCORE_OK) return rc;
-  if (!capturing && (rc = count_reads_wait(e, st)) != EPPSCORE_OK) return rc;
-  if (op == 0 && (rc = run_make_room(e, st, R, capturing)) != EPPSCORE_OK) return rc;
-  if ((rc = run_scratch(e, st, R, capturing)) != EPPSCORE_OK) return rc;
-  const int32_t* d_ep = endpoint;
-  const uint64_t* d_key = key;
-  const double* d_tpot = tpot;
-  if (!on_device) {
-    if ((rc = h2d(e, e->stage[0], endpoint, (size_t)R, &d_ep, st)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->stage[1], key, (size_t)R, &d_key, st)) != EPPSCORE_OK) return rc;
-    if ((rc = h2d(e, e->stage[2], tpot, (size_t)R, &d_tpot, st)) != EPPSCORE_OK) return rc;
-  }
-  e->launches += launch_running_update(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, op, d_ep, d_key,
-                                        op == 0 ? d_tpot : nullptr, R, e->cfg.max_endpoints, on_device ? out : nullptr,
-                                        e->sm_count, st);
-  CK(e, cudaGetLastError());
-  if (!on_device && out) CK(e, cudaMemcpyAsync(out, e->c_rwon.p, (size_t)R, cudaMemcpyDeviceToHost, st));
-  if (op == 0) e->run_bound_live += R;
-  if ((rc = run_copy_back(e, st, capturing)) != EPPSCORE_OK) return rc;
-  if ((rc = producer_end(e, st, capturing, running_feeds_scorer(e))) != EPPSCORE_OK) return rc;
-  if (!on_device) CK(e, cudaStreamSynchronize(st));  // the caller's host arrays may be reused
-  return EPPSCORE_OK;
+  auto update = [&]() -> int32_t {
+    bool capturing = false;
+    int32_t rc = producer_begin(e, st, &capturing);
+    if (rc != EPPSCORE_OK) return rc;
+    if (!capturing && (rc = count_reads_wait(e, st)) != EPPSCORE_OK) return rc;
+    if (op == 0 && (rc = run_make_room(e, st, R, capturing)) != EPPSCORE_OK) return rc;
+    if ((rc = run_scratch(e, st, R, capturing)) != EPPSCORE_OK) return rc;
+    e->launches += launch_running_update(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, op, d_ep, d_key,
+                                          op == 0 ? d_tpot : nullptr, R, e->cfg.max_endpoints, on_device ? out : nullptr,
+                                          e->sm_count, st);
+    CK(e, cudaGetLastError());
+    if (!on_device && out) CK(e, cudaMemcpyAsync(out, e->c_rwon.p, (size_t)R, cudaMemcpyDeviceToHost, st));
+    if (op == 0) e->run_bound_live += R;
+    if ((rc = run_copy_back(e, st, capturing)) != EPPSCORE_OK) return rc;
+    return producer_end(e, st, capturing, running_feeds_scorer(e));
+  };
+  return on_device ? update() : staged.finish(update);
 }
 
 }  // namespace
