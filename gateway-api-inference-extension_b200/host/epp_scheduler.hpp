@@ -22,6 +22,7 @@
 #include <functional>
 #include <map>
 #include <memory>
+#include <numeric>
 #include <stdexcept>
 #include <string>
 #include <unordered_map>
@@ -373,24 +374,32 @@ class Scheduler {
       ep.struct_size = sizeof(ep);
       if (sp.scorers().size() > EPPSCORE_MAX_SCORERS || sp.device_filters().size() > EPPSCORE_MAX_FILTERS)
         throw SchedulingError("too many scorers or device filters in profile '" + cfg.Profiles[p].first + "'");
-      ep.n_scorers = (int32_t)sp.scorers().size();
-      for (size_t i = 0; i < sp.scorers().size(); i++) {
-        ep.scorer_kind[i] = sp.scorers()[i].Scorer_->Kind;
-        ep.scorer_weight[i] = sp.scorers()[i].Weight();
-      }
-      ep.pick_mode = sp.picker().Mode;
-      ep.n_filters = (int32_t)sp.device_filters().size();
-      for (size_t i = 0; i < sp.device_filters().size(); i++) {
-        ep.filter_kind[i] = sp.device_filters()[i].Kind;
-        for (int q = 0; q < 3; q++) ep.filter_param[i][q] = sp.device_filters()[i].Param[q];
-      }
+      CopyProfile(sp, &ep);
       int32_t id = -1;
-      if (eppscore_add_profile(eng_, &ep, &id) != EPPSCORE_OK)  // (the destructor frees the engine)
-        throw SchedulingError(std::string("eppscore_add_profile: ") + eppscore_last_error(eng_));
+      Check(eppscore_add_profile(eng_, &ep, &id), "eppscore_add_profile");  // (the destructor frees the engine)
     }
   }
 
  private:
+  // A profile's scorers, picker and device filters into eppscore_config or eppscore_profile, which name these fields alike.
+  template <class EngineProfile>
+  static void CopyProfile(const SchedulerProfile& sp, EngineProfile* c) {
+    c->n_scorers = (int32_t)sp.scorers().size();
+    for (size_t i = 0; i < sp.scorers().size(); i++) {
+      c->scorer_kind[i] = sp.scorers()[i].Scorer_->Kind;
+      c->scorer_weight[i] = sp.scorers()[i].Weight();
+    }
+    c->pick_mode = sp.picker().Mode;
+    c->n_filters = (int32_t)sp.device_filters().size();
+    for (size_t i = 0; i < sp.device_filters().size(); i++) {
+      c->filter_kind[i] = sp.device_filters()[i].Kind;
+      for (int q = 0; q < 3; q++) c->filter_param[i][q] = sp.device_filters()[i].Param[q];
+    }
+  }
+  void Check(int32_t rc, const char* call) const {
+    if (rc != EPPSCORE_OK) throw SchedulingError(std::string(call) + ": " + eppscore_last_error(eng_));
+  }
+
   static SchedulerConfig SingleOrFirst(const SchedulerConfig& cfg) {  // the engine's profile 0 and the checks of its path
     if (cfg.Profiles.empty()) return cfg;
     if (!EngineHasProfiles()) throw SchedulingError("a config with several profiles needs an engine library with eppscore_add_profile");
@@ -474,7 +483,6 @@ class Scheduler {
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
       throw SchedulingError("TrackRunningRequests needs an engine library with eppscore_running_add");
-    c.n_scorers = (int32_t)sc.size();
     {  // the small-batch CPU route applies to request-independent profiles only
       std::vector<int32_t> kinds;
       std::vector<double> weights;
@@ -488,14 +496,12 @@ class Scheduler {
       cpu_route_ok_ = cfg.CpuBatchThreshold > 0 && !inflight_ && !running_ && cfg.Profile.device_filters().empty() && cfg.Profile.picker().Mode == EPPSCORE_PICK_MAX_SCORE &&
                       cfg.Profile.picker().MaxNumOfEndpoints == 1 && cfg.TieMode == EPPSCORE_TIE_LOWEST_INDEX && cpu_.Configure(kinds, weights, thr);
     }
-    for (size_t i = 0; i < sc.size(); i++) {
-      c.scorer_kind[i] = sc[i].Scorer_->Kind;
-      c.scorer_weight[i] = sc[i].Weight();
-      if (auto* tl = dynamic_cast<TokenLoadScorer*>(sc[i].Scorer_.get())) {
+    for (const auto& w : sc) {
+      if (auto* tl = dynamic_cast<TokenLoadScorer*>(w.Scorer_.get())) {
         c.token_load_threshold = (double)tl->QueueThresholdTokens;
         token_load_ = true;
       }
-      if (auto* ls = dynamic_cast<LatencyScorer*>(sc[i].Scorer_.get())) latency_scorer_ = ls;
+      if (auto* ls = dynamic_cast<LatencyScorer*>(w.Scorer_.get())) latency_scorer_ = ls;
     }
     for (const auto& np : cfg.Profiles)  // the latency parameters are engine-wide: any profile's scorer (they are equal)
       for (const auto& w : np.second.scorers())
@@ -509,13 +515,8 @@ class Scheduler {
     c.max_endpoints = cfg.MaxEndpoints;
     c.max_adapters = cfg.MaxAdapters;
     c.prefix_capacity = cfg.PrefixCapacity;
-    c.pick_mode = cfg.Profile.picker().Mode;
     if (cfg.Profile.device_filters().size() > EPPSCORE_MAX_FILTERS) throw SchedulingError("too many device filters");
-    c.n_filters = (int32_t)cfg.Profile.device_filters().size();
-    for (size_t i = 0; i < cfg.Profile.device_filters().size(); i++) {
-      c.filter_kind[i] = cfg.Profile.device_filters()[i].Kind;
-      for (int q = 0; q < 3; q++) c.filter_param[i][q] = cfg.Profile.device_filters()[i].Param[q];
-    }
+    CopyProfile(cfg.Profile, &c);
     c.tie_mode = cfg.TieMode;
     c.tie_seed = cfg.TieSeed;
     if (eppscore_create(cfg.Device, &c, &eng_) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_create: ") + eppscore_last_error(nullptr));
@@ -551,43 +552,15 @@ class Scheduler {
     if (starts.size() <= 1)
       return cfg_.Profiles.empty() ? ScheduleBatchSingle(requests, endpoints, 0) : ScheduleBatchProfiles(requests, endpoints, set_base);
     std::vector<BatchItem> out;
-    std::vector<uint64_t> hashes;
-    std::vector<uint16_t> nh;
-    std::vector<int64_t> size;
-    std::vector<int32_t> hint, chars;
-    std::vector<std::string> rid;
-    std::vector<double> tpot;
-    std::vector<LatencyCtx> lat;
+    BatchRecord whole;
     for (size_t k = 0; k < starts.size(); k++) {
       const size_t a = starts[k], b = k + 1 < starts.size() ? starts[k + 1] : requests.size();
       const std::vector<InferenceRequest> piece(requests.begin() + (ptrdiff_t)a, requests.begin() + (ptrdiff_t)b);
       auto res = cfg_.Profiles.empty() ? ScheduleBatchSingle(piece, endpoints, (int64_t)a) : ScheduleBatchProfiles(piece, endpoints, set_base);
       for (auto& x : res) out.push_back(std::move(x));
-      hashes.insert(hashes.end(), last_hashes_.begin(), last_hashes_.end());
-      nh.insert(nh.end(), last_nh_.begin(), last_nh_.end());
-      if (inflight_) {
-        size.insert(size.end(), last_size_.begin(), last_size_.end());
-        hint.insert(hint.end(), last_hint_.begin(), last_hint_.end());
-        chars.insert(chars.end(), last_chars_.begin(), last_chars_.end());
-      }
-      if (running_) {
-        rid.insert(rid.end(), last_rid_.begin(), last_rid_.end());
-        tpot.insert(tpot.end(), last_tpot_.begin(), last_tpot_.end());
-      }
-      for (auto& c : lat_ctx_) lat.push_back(std::move(c));
+      whole.Append(last_);
     }
-    lat_ctx_ = std::move(lat);
-    last_hashes_ = std::move(hashes);
-    last_nh_ = std::move(nh);
-    if (inflight_) {
-      last_size_ = std::move(size);
-      last_hint_ = std::move(hint);
-      last_chars_ = std::move(chars);
-    }
-    if (running_) {
-      last_rid_ = std::move(rid);
-      last_tpot_ = std::move(tpot);
-    }
+    last_ = std::move(whole);
     return out;
   }
   uint64_t CpuRoutedRequests() const { return cpu_routed_; }
@@ -595,19 +568,11 @@ class Scheduler {
  private:
   // The small-batch route: tiny batch, request-independent profile, evaluated on the host (SmallBatchCpu).
   std::vector<BatchItem> ScheduleOnHost(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints) {
-    const int R = (int)requests.size(), M = (int)endpoints.size();
+    const int R = (int)requests.size();
     std::vector<BatchItem> out((size_t)R);
-    last_hashes_.clear();
-    last_nh_.clear();
-    lat_ctx_.clear();
-    std::vector<int> all((size_t)M);
-    for (int m = 0; m < M; m++) all[m] = m;
+    last_.Clear(0);
     for (int r = 0; r < R; r++) {
-      std::vector<int> cand = all;
-      for (auto& f : cfg_.Profile.filters()) {
-        cand = f->Filter_(requests[r], endpoints, cand);
-        if (cand.empty()) break;
-      }
+      const std::vector<int> cand = Candidates(cfg_.Profile.filters(), requests[r], endpoints);
       const CpuPick p = cpu_.Schedule(endpoints, requests[r].TargetModel, cfg_.Profile.filters().empty() ? nullptr : &cand);
       if (p.pick < 0) {
         out[r].error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
@@ -653,13 +618,140 @@ class Scheduler {
     return starts;
   }
 
+  // GetBlockSize (endpoints[0]'s CacheBlockSize when autotuning, else the config's) and the prefix blocks a prompt is hashed to
+  // (approximateprefix/plugin.go:140-165); stride is the length of a request's row of hashes_out.
+  struct PrefixGeometry {
+    int block_tokens, max_blocks;
+    bool want_prefix;
+    int32_t stride;
+  };
+  PrefixGeometry Geometry(const std::vector<Endpoint>& endpoints) const {
+    PrefixGeometry g;
+    g.block_tokens = cfg_.Prefix.BlockSizeTokens;
+    if (!endpoints.empty() && cfg_.Prefix.AutoTune && endpoints[0].GetMetrics()->CacheBlockSize > 0)
+      g.block_tokens = endpoints[0].GetMetrics()->CacheBlockSize;
+    g.max_blocks = cfg_.Prefix.MaxPrefixBlocksToMatch;
+    if (cfg_.Prefix.MaxPrefixTokensToMatch > 0 && g.block_tokens > 0) g.max_blocks = cfg_.Prefix.MaxPrefixTokensToMatch / g.block_tokens;
+    g.want_prefix = g.max_blocks > 0 && g.block_tokens > 0;
+    g.stride = g.want_prefix ? g.max_blocks : 1;
+    return g;
+  }
+
+  // The engine inputs of some rows of a batch, in row order: the prompts, each starting 16-byte aligned (the fast hash path),
+  // with 64 bytes of tail; model seeds; adapter ids in the snapshot's dictionary.  With a latency scorer also the latency
+  // fold-in's inputs (predictedlatency/plugin.go:276-290, :315-343), which every profile of a call shares.
+  struct PackedRequests {
+    std::vector<uint8_t> bytes;
+    std::vector<int64_t> off;
+    std::vector<int32_t> len, adapter, in_tokens;
+    std::vector<uint64_t> seed;
+    std::vector<double> ttft_slo, tpot_slo;
+  };
+  PackedRequests Pack(const std::vector<InferenceRequest>& requests, const std::vector<int>& rows) const {
+    const size_t n = rows.size();
+    PackedRequests p;
+    p.off.assign(n + 1, 0);
+    p.len.resize(n);
+    p.adapter.resize(n);
+    p.seed.resize(n);
+    if (latency_scorer_) {
+      p.in_tokens.resize(n);
+      p.ttft_slo.resize(n);
+      p.tpot_slo.resize(n);
+    }
+    size_t total = 64;
+    for (int r : rows) total += (requests[(size_t)r].Prompt.size() + 15) / 16 * 16;
+    p.bytes.reserve(total);
+    for (size_t i = 0; i < n; i++) {
+      const InferenceRequest& q = requests[(size_t)rows[i]];
+      if (latency_scorer_) {
+        p.in_tokens[i] = CountFields(q.Prompt);
+        p.ttft_slo[i] = SloHeader(q, "x-slo-ttft-ms");
+        p.tpot_slo[i] = SloHeader(q, "x-slo-tpot-ms");
+      }
+      while (p.bytes.size() % 16) p.bytes.push_back(0);
+      p.off[i] = (int64_t)p.bytes.size();
+      p.len[i] = (int32_t)q.Prompt.size();
+      p.bytes.insert(p.bytes.end(), q.Prompt.begin(), q.Prompt.end());
+      p.seed[i] = eppscore_model_seed(q.TargetModel.data(), q.TargetModel.size(), q.CacheSalt.data(), q.CacheSalt.size());
+      auto it = adapter_ids_.find(q.TargetModel);
+      p.adapter[i] = it == adapter_ids_.end() ? -1 : it->second;
+    }
+    p.off[n] = (int64_t)p.bytes.size();
+    p.bytes.resize(p.bytes.size() + 64, 0);
+    return p;
+  }
+  // An engine batch over a packing: its request fields, and where the engine writes totalBlocks and (when it hashes) the block
+  // hashes.  The route sets request_base, cand_mask and the pick outputs.
+  static eppscore_batch BatchOf(const PackedRequests& p, const PrefixGeometry& g, uint16_t* total_blocks, uint64_t* hashes_out) {
+    eppscore_batch b{};
+    b.struct_size = sizeof(b);
+    b.R = (int32_t)p.len.size();
+    b.prompt_bytes = g.want_prefix ? p.bytes.data() : nullptr;
+    b.prompt_off = p.off.data();
+    b.prompt_len = p.len.data();
+    b.model_seed = p.seed.data();
+    b.block_chars = g.block_tokens * 4;
+    b.max_blocks = g.max_blocks;
+    b.adapter_id = p.adapter.data();
+    if (!p.in_tokens.empty()) {
+      b.input_tokens = p.in_tokens.data();
+      b.ttft_slo = p.ttft_slo.data();
+      b.tpot_slo = p.tpot_slo.data();
+    }
+    b.total_blocks = total_blocks;
+    b.hashes_out = g.want_prefix ? hashes_out : nullptr;
+    return b;
+  }
+
+  // The host filter chain (scheduler_profile.go:130-149) for one request: the positions of `endpoints` it keeps.
+  static std::vector<int> Candidates(const std::vector<std::shared_ptr<Filter>>& filters, const InferenceRequest& q,
+                                     const std::vector<Endpoint>& endpoints) {
+    std::vector<int> cand(endpoints.size());
+    std::iota(cand.begin(), cand.end(), 0);
+    for (auto& f : filters) {
+      cand = f->Filter_(q, endpoints, cand);
+      if (cand.empty()) break;
+    }
+    return cand;
+  }
+  // The candidate mask of `rows` of `requests` under a profile's host filters, mw words per row.  Its bits are endpoint ids, so
+  // an id without an endpoint in this list is never a candidate.
+  static std::vector<uint32_t> CandidateMask(const std::vector<std::shared_ptr<Filter>>& filters, const std::vector<InferenceRequest>& requests,
+                                             const std::vector<int>& rows, const std::vector<Endpoint>& endpoints, const std::vector<int>& ids,
+                                             int mw) {
+    std::vector<uint32_t> mask(rows.size() * (size_t)mw, 0u);
+    for (size_t i = 0; i < rows.size(); i++)
+      for (int m : Candidates(filters, requests[(size_t)rows[i]], endpoints)) mask[i * (size_t)mw + (ids[m] >> 5)] |= 1u << (ids[m] & 31);
+    return mask;
+  }
+
+  // The endpoint the engine returned as id (pos_of_id: id -> position in the list, -1 for none) as a ScoredEndpoint; `what`
+  // ("picked" or "listed") names the engine's error when the id has no endpoint in the list.
+  static ScoredEndpoint Scored(int32_t id, double score, const std::vector<Endpoint>& endpoints, const std::vector<int>& pos_of_id,
+                               const char* what) {
+    if (id >= (int32_t)pos_of_id.size() || pos_of_id[(size_t)id] < 0)
+      throw SchedulingError(std::string("engine ") + what + " an endpoint that is not in the candidate list");
+    ScoredEndpoint se;
+    se.Index = pos_of_id[(size_t)id];
+    se.Endpoint_ = &endpoints[(size_t)se.Index];
+    se.Score = score;
+    return se;
+  }
+  // Entries 1..k-1 of a request's list from the engine (entry 0 is the pick), onto its TargetEndpoints; -1 past the last candidate.
+  static void AppendList(std::vector<ScoredEndpoint>& te, const int32_t* list_ids, const double* list_scores, int k,
+                         const std::vector<Endpoint>& endpoints, const std::vector<int>& pos_of_id) {
+    for (int i = 1; i < k; i++) {
+      if (list_ids[i] < 0) break;
+      te.push_back(Scored(list_ids[i], list_scores[i], endpoints, pos_of_id, "listed"));
+    }
+  }
+
   std::vector<BatchItem> ScheduleBatchSingle(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints,
                                              int64_t request_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size();
     std::vector<BatchItem> out((size_t)R);
-    lat_ctx_.assign(cfg_.LatencyPredictionInfo ? (size_t)R : 0, LatencyCtx{});
-    last_hashes_.clear();
-    last_nh_.clear();
+    last_.Clear(cfg_.LatencyPredictionInfo ? (size_t)R : 0);
     if (R == 0) return out;
     if (M == 0) {  // scheduler_profile.go:119-121 → single_profile_handler.go:89-91
       for (auto& o : out) o.error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
@@ -679,98 +771,22 @@ class Scheduler {
     std::vector<int> pos_of_id((size_t)Mx, -1);
     for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
     PackSnapshot(endpoints, ids, Mx, requests);
-    // --- filters → candidate mask (rows are ids; ids without an endpoint in this list are never candidates) ---
-    const int mw = (Mx + 31) / 32;
+    std::vector<int> rows((size_t)R);
+    std::iota(rows.begin(), rows.end(), 0);
     std::vector<uint32_t> mask;
-    const bool have_filters = !cfg_.Profile.filters().empty();
-    const bool need_mask = have_filters || Mx != M;  // a pure permutation of the rows has no holes: no mask, the fast path stays
-    if (need_mask) {
-      mask.assign((size_t)R * mw, 0u);
-      std::vector<int> all((size_t)M);
-      for (int m = 0; m < M; m++) all[m] = m;
-      for (int r = 0; r < R; r++) {
-        std::vector<int> cand = all;
-        for (auto& f : cfg_.Profile.filters()) {
-          cand = f->Filter_(requests[r], endpoints, cand);
-          if (cand.empty()) break;
-        }
-        for (int m : cand) mask[(size_t)r * mw + (ids[m] >> 5)] |= 1u << (ids[m] & 31);
-      }
-    }
-    // --- PrepareRequestData inputs (approximateprefix/plugin.go:140-165) ---
-    int block_tokens = cfg_.Prefix.BlockSizeTokens;                        // GetBlockSize: endpoints[0] when autotuning
-    if (cfg_.Prefix.AutoTune && endpoints[0].GetMetrics()->CacheBlockSize > 0) block_tokens = endpoints[0].GetMetrics()->CacheBlockSize;
-    int max_blocks = cfg_.Prefix.MaxPrefixBlocksToMatch;
-    if (cfg_.Prefix.MaxPrefixTokensToMatch > 0 && block_tokens > 0) max_blocks = cfg_.Prefix.MaxPrefixTokensToMatch / block_tokens;
-    std::vector<uint8_t> bytes;
-    std::vector<int64_t> off((size_t)R + 1, 0);
-    std::vector<int32_t> len((size_t)R), adapter((size_t)R), in_tokens;
-    std::vector<double> ttft_slo, tpot_slo;
-    if (latency_scorer_) {  // predictedlatency/plugin.go:276-290, :315-343
-      in_tokens.resize((size_t)R);
-      ttft_slo.assign((size_t)R, 0.0);
-      tpot_slo.assign((size_t)R, 0.0);
-      for (int r = 0; r < R; r++) {
-        in_tokens[r] = CountFields(requests[r].Prompt);
-        ttft_slo[r] = SloHeader(requests[r], "x-slo-ttft-ms");
-        tpot_slo[r] = SloHeader(requests[r], "x-slo-tpot-ms");
-      }
-    }
-    if (running_) {  // PreRequest's inputs: the request id and avgTPOTSLO, the same header rule
-      last_rid_.resize((size_t)R);
-      last_tpot_.resize((size_t)R);
-      for (int r = 0; r < R; r++) {
-        last_rid_[r] = requests[r].RequestId;
-        last_tpot_[r] = SloHeader(requests[r], "x-slo-tpot-ms");
-      }
-    }
-    std::vector<uint64_t> seed((size_t)R);
-    for (int r = 0; r < R; r++) {
-      while (bytes.size() % 16) bytes.push_back(0);  // 16-byte aligned starts: the fast hash path
-      off[r] = (int64_t)bytes.size();
-      len[r] = (int32_t)requests[r].Prompt.size();
-      bytes.insert(bytes.end(), requests[r].Prompt.begin(), requests[r].Prompt.end());
-      seed[r] = eppscore_model_seed(requests[r].TargetModel.data(), requests[r].TargetModel.size(),
-                                    requests[r].CacheSalt.data(), requests[r].CacheSalt.size());
-      auto it = adapter_ids_.find(requests[r].TargetModel);
-      adapter[r] = it == adapter_ids_.end() ? -1 : it->second;
-    }
-    off[R] = (int64_t)bytes.size();
-    bytes.resize(bytes.size() + 64, 0);
-    if (inflight_) {  // the estimator's inputs, for PreRequest
-      last_size_.resize((size_t)R);
-      last_hint_.resize((size_t)R);
-      last_chars_.resize((size_t)R);
-      for (int r = 0; r < R; r++) EstimateInputs(requests[r], &last_size_[r], &last_hint_[r], &last_chars_[r]);
-    }
-    const bool want_prefix = max_blocks > 0 && block_tokens > 0;
+    const bool need_mask = !cfg_.Profile.filters().empty() || Mx != M;  // a pure permutation of the rows has no holes: no mask, the fast path stays
+    if (need_mask) mask = CandidateMask(cfg_.Profile.filters(), requests, rows, endpoints, ids, (Mx + 31) / 32);
+    const PrefixGeometry g = Geometry(endpoints);
+    const PackedRequests p = Pack(requests, rows);
+    last_.Fill(requests, g.stride, inflight_, running_);
     std::vector<int32_t> pick((size_t)R), ties((size_t)R);
     std::vector<double> score((size_t)R);
-    last_nh_.assign((size_t)R, 0);
-    last_stride_ = want_prefix ? max_blocks : 1;
-    last_hashes_.assign((size_t)R * last_stride_, 0);
-    eppscore_batch b{};
-    b.struct_size = sizeof(b);
-    b.R = R;
+    eppscore_batch b = BatchOf(p, g, last_.nh.data(), last_.hashes.data());
     b.request_base = request_base;
-    b.prompt_bytes = want_prefix ? bytes.data() : nullptr;
-    b.prompt_off = off.data();
-    b.prompt_len = len.data();
-    b.model_seed = seed.data();
-    b.block_chars = block_tokens * 4;
-    b.max_blocks = max_blocks;
-    b.adapter_id = adapter.data();
     b.cand_mask = need_mask ? mask.data() : nullptr;
-    if (latency_scorer_) {
-      b.input_tokens = in_tokens.data();
-      b.ttft_slo = ttft_slo.data();
-      b.tpot_slo = tpot_slo.data();
-    }
     b.pick = pick.data();
     b.pick_score = score.data();
     b.tie_count = ties.data();
-    b.total_blocks = last_nh_.data();
-    b.hashes_out = want_prefix ? last_hashes_.data() : nullptr;
     const int topk = cfg_.Profile.picker().MaxNumOfEndpoints;
     // k > 8: the wide lists, except max-score with seeded-random ties, whose device order puts positions >= 1 of a tie class
     // in priority order where the score map's route has ascending index
@@ -789,22 +805,18 @@ class Scheduler {
       t.k = klist;
       t.endpoints = topk_ids.data();
       t.scores = topk_scores.data();
-      const char* what = engine_wide ? "eppscore_schedule_batch_topk_wide: " : "eppscore_schedule_batch_topk: ";
-      if ((engine_wide ? eppscore_schedule_batch_topk_wide(eng_, &b, &t) : eppscore_schedule_batch_topk(eng_, &b, &t)) != EPPSCORE_OK)
-        throw SchedulingError(std::string(what) + eppscore_last_error(eng_));
+      Check(engine_wide ? eppscore_schedule_batch_topk_wide(eng_, &b, &t) : eppscore_schedule_batch_topk(eng_, &b, &t),
+            engine_wide ? "eppscore_schedule_batch_topk_wide" : "eppscore_schedule_batch_topk");
     } else {
       if (topk > 1) {  // k > 8, max-score (seeded-random ties or no wide call): the whole weightedScorePerEndpoint map, NaN for non-candidates (scheduler_profile.go:155-174)
         all_scores.resize((size_t)R * Mx);
         b.scores_out = all_scores.data();
       }
       if (inorder_) {  // the estimates go in with the batch: the call adds each pick's load in request order
-        std::vector<int64_t> est((size_t)R);
-        if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
-          throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
-        if (eppscore_schedule_batch_inorder(eng_, &b, est.data()) != EPPSCORE_OK)
-          throw SchedulingError(std::string("eppscore_schedule_batch_inorder: ") + eppscore_last_error(eng_));
-      } else if (eppscore_schedule_batch(eng_, &b) != EPPSCORE_OK) {
-        throw SchedulingError(std::string("eppscore_schedule_batch: ") + eppscore_last_error(eng_));
+        const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
+        Check(eppscore_schedule_batch_inorder(eng_, &b, est.data()), "eppscore_schedule_batch_inorder");
+      } else {
+        Check(eppscore_schedule_batch(eng_, &b), "eppscore_schedule_batch");
       }
     }
     last_endpoints_ = &endpoints;
@@ -815,28 +827,14 @@ class Scheduler {
         out[r].error = "failed to run scheduler profile '" + cfg_.ProfileName + "'";
         continue;
       }
-      if (pick[r] >= Mx || pos_of_id[(size_t)pick[r]] < 0) throw SchedulingError("engine picked an endpoint that is not in the candidate list");
-      ScoredEndpoint se;
-      se.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)pick[r]]];
-      se.Index = pos_of_id[(size_t)pick[r]];
-      se.Score = score[r];
+      ScoredEndpoint se = Scored(pick[r], score[r], endpoints, pos_of_id, "picked");
       se.TieCount = ties[r];
-      out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints.push_back(se);
+      auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
+      te.push_back(se);
       out[r].result.PrimaryProfileName = cfg_.ProfileName;
-      if (engine_topk) {  // entries 1..k-1 of the picker's order (entry 0 is the pick); -1 past the last candidate
-        auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
-        for (int i = 1; i < klist; i++) {
-          const int32_t id = topk_ids[(size_t)r * klist + i];
-          if (id < 0) break;
-          if (id >= Mx || pos_of_id[(size_t)id] < 0) throw SchedulingError("engine listed an endpoint that is not in the candidate list");
-          ScoredEndpoint o2;
-          o2.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)id]];
-          o2.Index = pos_of_id[(size_t)id];
-          o2.Score = topk_scores[(size_t)r * klist + i];
-          te.push_back(o2);
-        }
+      if (engine_topk) {
+        AppendList(te, topk_ids.data() + (size_t)r * klist, topk_scores.data() + (size_t)r * klist, klist, endpoints, pos_of_id);
       } else if (topk > 1) {  // picker/maxscore/picker.go:104-106: the next best candidates, descending score
-        auto& te = out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints;
         for (const auto& pr : TopK(all_scores.data() + (size_t)r * Mx, Mx, topk)) {  // (id, score), NaN rows skipped
           const int pos = pos_of_id[(size_t)pr.first];
           if (pos < 0 || pos == se.Index) continue;
@@ -849,23 +847,14 @@ class Scheduler {
         }
       }
     }
-    if (cfg_.LatencyPredictionInfo) {
-      std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>> runs((size_t)R);
-      std::vector<int> rows((size_t)R);
-      for (int r = 0; r < R; r++) {
-        rows[(size_t)r] = r;
-        if (out[r].error.empty()) runs[(size_t)r].emplace_back(cfg_.ProfileName, &out[r].result.ProfileResults[cfg_.ProfileName]);
-      }
-      FillLatency(runs, rows, requests, endpoints, ids, last_hashes_.data(), last_nh_.data(), last_stride_, in_tokens.data(),
-                  ttft_slo.data(), tpot_slo.data(), cfg_.PrefixMatchInfo && want_prefix, block_tokens);
-      for (int r = 0; r < R; r++) AttachLatency(out[r], lat_ctx_[(size_t)r], endpoints, ids);
-    } else if (cfg_.PrefixMatchInfo && want_prefix) {
-      std::vector<std::vector<ScoredEndpoint*>> targets((size_t)R);
+    if (cfg_.LatencyPredictionInfo || cfg_.PrefixMatchInfo) {
+      TargetRuns runs((size_t)R);
       for (int r = 0; r < R; r++)
-        if (out[r].error.empty())
-          for (ScoredEndpoint& t : out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints) targets[(size_t)r].push_back(&t);
-      FillPrefixMatch(targets, last_hashes_.data(), last_nh_.data(), last_stride_, ids, block_tokens);
+        if (out[r].error.empty()) runs[(size_t)r].emplace_back(cfg_.ProfileName, &out[r].result.ProfileResults[cfg_.ProfileName]);
+      FillTargetInfo(runs, rows, requests, endpoints, ids, last_.hashes.data(), last_.nh.data(), p, g);
     }
+    if (cfg_.LatencyPredictionInfo)
+      for (int r = 0; r < R; r++) AttachLatency(out[r], last_.lat[(size_t)r], endpoints, ids);
     return out;
   }
 
@@ -876,25 +865,18 @@ class Scheduler {
   void PreRequest(const std::vector<BatchItem>& results) {
     RecordPrefixCacheMatch(results);
     RecordDispatch(results);
-    if (!last_endpoints_ || (last_hashes_.empty() && !inflight_ && !running_)) return;
+    if (!last_endpoints_ || (last_.hashes.empty() && !inflight_ && !running_)) return;
     if (!cfg_.Profiles.empty()) return PreRequestProfiles(results);
     const int R = (int)results.size();
     std::vector<int32_t> pick((size_t)R, -1);
     for (int r = 0; r < R; r++)
       if (results[r].error.empty()) pick[r] = last_ids_[(size_t)results[r].result.ProfileResults.at(cfg_.ProfileName).TargetEndpoints[0].Index];
-    if (!last_hashes_.empty()) {
-      std::vector<int32_t> cap((size_t)last_rows_, 0);
-      for (size_t m = 0; m < last_endpoints_->size(); m++)  // makeserver, plugin.go:207-216
-        cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks > 0) ? (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks : 0;
-      if (eppscore_commit_picks(eng_, R, pick.data(), last_hashes_.data(), last_nh_.data(), last_stride_, cap.data()) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_commit_picks: ") + eppscore_last_error(eng_));
-    }
-    if (inflight_ && !inorder_ && (int)last_size_.size() == R) {  // (in order: ScheduleBatch added the load already)
-      std::vector<int64_t> est((size_t)R);
-      if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
-      if (eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
+    if (!last_.hashes.empty())
+      Check(eppscore_commit_picks(eng_, R, pick.data(), last_.hashes.data(), last_.nh.data(), last_.stride, LruCapacities().data()),
+            "eppscore_commit_picks");
+    if (inflight_ && !inorder_ && (int)last_.size.size() == R) {  // (in order: ScheduleBatch added the load already)
+      const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
+      Check(eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr), "eppscore_inflight_add");
     }
     RunningAdd(pick);
   }
@@ -902,21 +884,20 @@ class Scheduler {
   // requestcontrol_hooks.go:73-86: (pick[r], request id, tpot) into the running-request queues, for PreRequest
   void RunningAdd(const std::vector<int32_t>& pick) {
     const int R = (int)pick.size();
-    if (running_ && (int)last_rid_.size() == R) {
+    if (running_ && (int)last_.rid.size() == R) {
       std::vector<int32_t> ep((size_t)R, -1);
       std::vector<uint64_t> key((size_t)R, 0);
       for (int r = 0; r < R; r++) {
-        if (pick[r] < 0 || last_rid_[r].empty()) continue;  // no target / missing x-request-id: not tracked
+        if (pick[r] < 0 || last_.rid[r].empty()) continue;  // no target / missing x-request-id: not tracked
         ep[r] = pick[r];
-        key[r] = KeyFor(last_rid_[r]);
+        key[r] = KeyFor(last_.rid[r]);
       }
       std::vector<uint8_t> added((size_t)R, 0);
-      if (eppscore_running_add(eng_, R, 0, ep.data(), key.data(), last_tpot_.data(), added.data(), nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_running_add: ") + eppscore_last_error(eng_));
+      Check(eppscore_running_add(eng_, R, 0, ep.data(), key.data(), last_.tpot.data(), added.data(), nullptr), "eppscore_running_add");
       for (int r = 0; r < R; r++)
         if (ep[r] >= 0) {
-          if (added[r]) running_keys_[last_rid_[r]].endpoints.push_back(ep[r]);
-          else ReleaseKeyIfUnused(last_rid_[r]);  // refused (already live there, or a negative tpot)
+          if (added[r]) running_keys_[last_.rid[r]].endpoints.push_back(ep[r]);
+          else ReleaseKeyIfUnused(last_.rid[r]);  // refused (already live there, or a negative tpot)
         }
     }
   }
@@ -941,13 +922,11 @@ class Scheduler {
     if (pr == result.ProfileResults.end() || pr->second.TargetEndpoints.empty() || !pr->second.TargetEndpoints[0].Endpoint_) return;
     const int32_t id = ServerId(pr->second.TargetEndpoints[0].Endpoint_->GetMetadata()->NamespacedName_.String());
     if (id < 0) return;
-    int64_t size = 0, est = 0;
+    int64_t size = 0;
     int32_t hint = -1, chars = 0;
     EstimateInputs(request, &size, &hint, &chars);
-    if (eppscore_estimate_tokens(eng_, 1, 0, &size, &hint, &chars, &est, nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
-    if (eppscore_inflight_release(eng_, 1, 0, &id, &est, nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_inflight_release: ") + eppscore_last_error(eng_));
+    const std::vector<int64_t> est = EstimateTokens(1, &size, &hint, &chars);
+    Check(eppscore_inflight_release(eng_, 1, 0, &id, est.data(), nullptr), "eppscore_inflight_release");
   }
 
   // ResponseBody at start of stream (inflightload/producer.go:137-160): with several profiles, the "prefill" profile's target
@@ -962,13 +941,10 @@ class Scheduler {
   void RemovePod(const std::string& namespaced_name) {
     auto it = server_ids_.find(namespaced_name);
     if (it == server_ids_.end()) return;
-    if (eppscore_prefix_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_prefix_remove_endpoint: ") + eppscore_last_error(eng_));
-    if (inflight_ && eppscore_inflight_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_inflight_remove_endpoint: ") + eppscore_last_error(eng_));
+    Check(eppscore_prefix_remove_endpoint(eng_, it->second), "eppscore_prefix_remove_endpoint");
+    if (inflight_) Check(eppscore_inflight_remove_endpoint(eng_, it->second), "eppscore_inflight_remove_endpoint");
     if (running_) {  // the engine's one divergence: the recycled id's queue starts empty (include/eppscore.h)
-      if (eppscore_running_remove_endpoint(eng_, it->second) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_running_remove_endpoint: ") + eppscore_last_error(eng_));
+      Check(eppscore_running_remove_endpoint(eng_, it->second), "eppscore_running_remove_endpoint");
       for (auto k = running_keys_.begin(); k != running_keys_.end();) {
         auto& v = k->second.endpoints;
         v.erase(std::remove(v.begin(), v.end(), it->second), v.end());
@@ -985,8 +961,7 @@ class Scheduler {
     const int id = ServerId(namespaced_name);
     if (!inflight_ || id < 0) return {0, 0};
     std::vector<int64_t> req((size_t)id + 1), tok((size_t)id + 1);
-    if (eppscore_inflight_get(eng_, req.data(), tok.data(), id + 1) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_inflight_get: ") + eppscore_last_error(eng_));
+    Check(eppscore_inflight_get(eng_, req.data(), tok.data(), id + 1), "eppscore_inflight_get");
     return {req[(size_t)id], tok[(size_t)id]};
   }
   // getEndpointMinTPOTSLO / getEndpointRunningRequestCount (plugin.go:347-363) of one server from the engine's queues:
@@ -996,8 +971,7 @@ class Scheduler {
     if (!running_ || id < 0) return {0.0, 0};
     std::vector<double> mn((size_t)id + 1);
     std::vector<int32_t> cnt((size_t)id + 1);
-    if (eppscore_running_get(eng_, mn.data(), cnt.data(), id + 1) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_running_get: ") + eppscore_last_error(eng_));
+    Check(eppscore_running_get(eng_, mn.data(), cnt.data(), id + 1), "eppscore_running_get");
     return {mn[(size_t)id], cnt[(size_t)id]};
   }
   size_t TrackedRequestIds() const { return running_keys_.size(); }  // ids with a live queue entry (their keys are kept)
@@ -1007,7 +981,7 @@ class Scheduler {
   }
   uint64_t RemappedBatches() const { return remapped_batches_; }  // batches whose list was not ids 0..M-1 in order
 
-  const std::vector<uint16_t>& LastTotalBlocks() const { return last_nh_; }
+  const std::vector<uint16_t>& LastTotalBlocks() const { return last_.nh; }
   // The prefix-indexer histograms PreRequest records with SchedulerConfig::PrefixMatchInfo (empty without it).
   const PrefixIndexerHistograms& PrefixIndexerMetrics() const { return prefix_metrics_; }
   // The dispatch record PreRequest kept for a request id with SchedulerConfig::LatencyPredictionInfo, or nullptr (none kept, or
@@ -1021,35 +995,51 @@ class Scheduler {
   eppscore_engine* engine() { return eng_; }
 
  private:
-  // One eppscore_prefix_match call for an engine batch that hashed its prompts: targets[i] are request i's TargetEndpoints
-  // entries (every profile's), hashes / nh / stride the batch's hashes_out, ids the list position -> endpoint id map.  Each
-  // entry gets {matchBlocks at its endpoint, totalBlocks, the batch's block size} (plugin.go:140-153).  A request's endpoints
-  // are listed once each, so k never passes the number of endpoint rows.
-  void FillPrefixMatch(const std::vector<std::vector<ScoredEndpoint*>>& targets, const uint64_t* hashes, const uint16_t* nh,
-                       int32_t stride, const std::vector<int>& ids, int block_tokens) {
-    const int n = (int)targets.size();
+  // Per row of an engine call, the (profile name, result) pairs of every profile that ran for the row's request.
+  using TargetRuns = std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>>;
+
+  // After an engine call: every TargetEndpoints entry of `runs` (row i is requests[rows[i]], packed as p) gets its
+  // LatencyPredictionInfo with SchedulerConfig::LatencyPredictionInfo, and its PrefixCacheMatchInfo with
+  // SchedulerConfig::PrefixMatchInfo when the call hashed the prompts into hashes / nh.
+  void FillTargetInfo(const TargetRuns& runs, const std::vector<int>& rows, const std::vector<InferenceRequest>& requests,
+                      const std::vector<Endpoint>& endpoints, const std::vector<int>& ids, const uint64_t* hashes, const uint16_t* nh,
+                      const PackedRequests& p, const PrefixGeometry& g) {
+    if (cfg_.LatencyPredictionInfo)
+      FillLatency(runs, rows, requests, endpoints, ids, hashes, nh, p, g, cfg_.PrefixMatchInfo && g.want_prefix);
+    else if (cfg_.PrefixMatchInfo && g.want_prefix)
+      FillPrefixMatch(runs, hashes, nh, ids, g);
+  }
+
+  // One eppscore_prefix_match call for an engine call that hashed its prompts: hashes / nh its hashes_out and total_blocks, ids
+  // the list position -> endpoint id map.  Each TargetEndpoints entry of `runs` gets {matchBlocks at its endpoint, totalBlocks,
+  // the batch's block size} (plugin.go:140-153).  A request's endpoints are listed once each, so k never passes the number of
+  // endpoint rows.
+  void FillPrefixMatch(const TargetRuns& runs, const uint64_t* hashes, const uint16_t* nh, const std::vector<int>& ids,
+                       const PrefixGeometry& g) {
+    const int n = (int)runs.size();
     std::vector<std::vector<int32_t>> cols((size_t)n);
     size_t k = 0;
     for (int i = 0; i < n; i++) {
-      for (const ScoredEndpoint* t : targets[(size_t)i]) {
-        const int32_t id = ids[(size_t)t->Index];
-        if (std::find(cols[(size_t)i].begin(), cols[(size_t)i].end(), id) == cols[(size_t)i].end()) cols[(size_t)i].push_back(id);
-      }
+      for (const auto& run : runs[(size_t)i])
+        for (const ScoredEndpoint& t : run.second->TargetEndpoints) {
+          const int32_t id = ids[(size_t)t.Index];
+          if (std::find(cols[(size_t)i].begin(), cols[(size_t)i].end(), id) == cols[(size_t)i].end()) cols[(size_t)i].push_back(id);
+        }
       k = std::max(k, cols[(size_t)i].size());
     }
     if (n == 0 || k == 0) return;
-    if (block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+    if (g.block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
     std::vector<int32_t> eps((size_t)n * k, -1);
     for (int i = 0; i < n; i++) std::copy(cols[(size_t)i].begin(), cols[(size_t)i].end(), eps.begin() + (ptrdiff_t)((size_t)i * k));
     std::vector<uint16_t> match((size_t)n * k, 0);
-    if (eppscore_prefix_match(eng_, n, (int32_t)k, 0, hashes, nh, stride, eps.data(), match.data(), nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_prefix_match: ") + eppscore_last_error(eng_));
+    Check(eppscore_prefix_match(eng_, n, (int32_t)k, 0, hashes, nh, g.stride, eps.data(), match.data(), nullptr), "eppscore_prefix_match");
     for (int i = 0; i < n; i++)
-      for (ScoredEndpoint* t : targets[(size_t)i]) {
-        const auto& c = cols[(size_t)i];
-        const size_t j = (size_t)(std::find(c.begin(), c.end(), ids[(size_t)t->Index]) - c.begin());
-        t->PrefixMatch = PrefixCacheMatchInfo{match[(size_t)i * k + j], nh[i], (uint16_t)block_tokens};
-      }
+      for (const auto& run : runs[(size_t)i])
+        for (ScoredEndpoint& t : run.second->TargetEndpoints) {
+          const auto& c = cols[(size_t)i];
+          const size_t j = (size_t)(std::find(c.begin(), c.end(), ids[(size_t)t.Index]) - c.begin());
+          t.PrefixMatch = PrefixCacheMatchInfo{match[(size_t)i * k + j], nh[i], (uint16_t)g.block_tokens};
+        }
   }
 
   // A batch row's share of the predicted-latency producer's request context: the request id and SLOs, the info of every endpoint
@@ -1063,6 +1053,60 @@ class Scheduler {
     double ttft_slo = 0.0, tpot_slo = 0.0;
     std::map<int32_t, std::optional<LatencyPredictionInfo>> by_id;  // endpoint id -> its info
     std::map<std::string, std::pair<std::optional<LatencyPredictionInfo>, double>> by_name;  // Name -> (info, prefix score)
+  };
+
+  // What the last engine batch leaves for PreRequest, per request in batch order.  PreRequest checks the sizes: the estimator
+  // inputs are filled only with the inflight-load producer, the request ids and TPOT SLOs only with TrackRunningRequests, and a
+  // batch that returns before Fill (no requests, no endpoints on the single route, the small-batch host route) leaves them as
+  // they were.
+  struct BatchRecord {
+    std::vector<uint64_t> hashes;  // the engine's hashes_out, stride per request
+    std::vector<uint16_t> nh;      // its total_blocks
+    int32_t stride = 1;
+    std::vector<int64_t> size;     // SimpleTokenEstimator's inputs (EstimateInputs)
+    std::vector<int32_t> hint, chars;
+    std::vector<std::string> rid;  // the request id and avgTPOTSLO (x-slo-tpot-ms)
+    std::vector<double> tpot;
+    std::vector<LatencyCtx> lat;   // SchedulerConfig::LatencyPredictionInfo
+
+    void Clear(size_t lat_rows) {
+      hashes.clear();
+      nh.clear();
+      lat.assign(lat_rows, LatencyCtx{});
+    }
+    void Fill(const std::vector<InferenceRequest>& requests, int32_t hash_stride, bool inflight, bool running) {
+      const size_t R = requests.size();
+      stride = hash_stride;
+      nh.assign(R, 0);
+      hashes.assign(R * (size_t)stride, 0);
+      if (inflight) {
+        size.resize(R);
+        hint.resize(R);
+        chars.resize(R);
+        for (size_t r = 0; r < R; r++) EstimateInputs(requests[r], &size[r], &hint[r], &chars[r]);
+      }
+      if (running) {
+        rid.resize(R);
+        tpot.resize(R);
+        for (size_t r = 0; r < R; r++) {
+          rid[r] = requests[r].RequestId;
+          tpot[r] = SloHeader(requests[r], "x-slo-tpot-ms");
+        }
+      }
+    }
+    // A later piece of the same batch.
+    void Append(BatchRecord& piece) {
+      auto append = [](auto& to, auto& from) { to.insert(to.end(), std::make_move_iterator(from.begin()), std::make_move_iterator(from.end())); };
+      append(hashes, piece.hashes);
+      append(nh, piece.nh);
+      stride = piece.stride;
+      append(size, piece.size);
+      append(hint, piece.hint);
+      append(chars, piece.chars);
+      append(rid, piece.rid);
+      append(tpot, piece.tpot);
+      append(lat, piece.lat);
+    }
   };
 
   // The final result's SchedulingResult::TargetLatency from the row's LatencyCtx: every profile's TargetEndpoints, in the order
@@ -1080,15 +1124,14 @@ class Scheduler {
     }
   }
 
-  // One eppscore_predict_latency call for an engine batch piece: runs[i] are piece row i's (profile name, result) pairs (rows[i]
-  // its index in `requests`), hashes / nh / stride the piece's hashes_out (all zero when the engine did not hash), ids the list
-  // position -> endpoint id map.  Every TargetEndpoints entry's LatencyPredictionInfo goes into the row's LatencyCtx (AttachLatency
+  // One eppscore_predict_latency call for an engine call: runs[i] are row i's (profile name, result) pairs (rows[i] its index in
+  // `requests`, p its packing), hashes / nh the call's hashes_out and total_blocks (all zero when the engine did not hash), ids
+  // the list position -> endpoint id map.  Every TargetEndpoints entry's LatencyPredictionInfo goes into the row's LatencyCtx (AttachLatency
   // puts it on the final result); with fill_match the entry also gets its PrefixMatch (as FillPrefixMatch gives it).  The row's
   // LatencyCtx also gets each target name's values at the last candidate of that name.
-  void FillLatency(const std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>>& runs, const std::vector<int>& rows,
-                   const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints, const std::vector<int>& ids,
-                   const uint64_t* hashes, const uint16_t* nh, int32_t stride, const int32_t* in_tokens, const double* ttft_slo,
-                   const double* tpot_slo, bool fill_match, int block_tokens) {
+  void FillLatency(const TargetRuns& runs, const std::vector<int>& rows, const std::vector<InferenceRequest>& requests,
+                   const std::vector<Endpoint>& endpoints, const std::vector<int>& ids, const uint64_t* hashes, const uint16_t* nh,
+                   const PackedRequests& p, const PrefixGeometry& g, bool fill_match) {
     const int n = (int)runs.size();
     std::map<std::string, int> last_of_name;  // Name -> the last candidate position with it
     for (size_t m = 0; m < endpoints.size(); m++) last_of_name[endpoints[m].GetMetadata()->NamespacedName_.Name] = (int)m;
@@ -1110,20 +1153,14 @@ class Scheduler {
       k = std::max(k, cols[(size_t)i].size());
     }
     if (n == 0 || k == 0) return;
-    if (fill_match && block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
-    std::vector<int32_t> eps((size_t)n * k, -1), tok((size_t)n);
-    std::vector<double> tslo((size_t)n), pslo((size_t)n);
-    for (int i = 0; i < n; i++) {
-      std::copy(cols[(size_t)i].begin(), cols[(size_t)i].end(), eps.begin() + (ptrdiff_t)((size_t)i * k));
-      tok[(size_t)i] = in_tokens[i];
-      tslo[(size_t)i] = ttft_slo[i];
-      pslo[(size_t)i] = tpot_slo[i];
-    }
+    if (fill_match && g.block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+    std::vector<int32_t> eps((size_t)n * k, -1);
+    for (int i = 0; i < n; i++) std::copy(cols[(size_t)i].begin(), cols[(size_t)i].end(), eps.begin() + (ptrdiff_t)((size_t)i * k));
     std::vector<eppscore_latency_info> info((size_t)n * k);
     std::vector<uint16_t> match((size_t)n * k);  // (also the prefix cache score when no prediction was stored)
-    if (eppscore_predict_latency(eng_, n, (int32_t)k, 0, hashes, nh, stride, tok.data(), tslo.data(), pslo.data(), eps.data(), info.data(),
-                                 match.data(), nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_predict_latency: ") + eppscore_last_error(eng_));
+    Check(eppscore_predict_latency(eng_, n, (int32_t)k, 0, hashes, nh, g.stride, p.in_tokens.data(), p.ttft_slo.data(), p.tpot_slo.data(),
+                                   eps.data(), info.data(), match.data(), nullptr),
+          "eppscore_predict_latency");
     auto as_info = [](const eppscore_latency_info& x) -> std::optional<LatencyPredictionInfo> {
       if (!x.present) return std::nullopt;
       LatencyPredictionInfo v;
@@ -1138,17 +1175,17 @@ class Scheduler {
     };
     for (int i = 0; i < n; i++) {
       const InferenceRequest& q = requests[(size_t)rows[(size_t)i]];
-      LatencyCtx& ctx = lat_ctx_[(size_t)rows[(size_t)i]];
+      LatencyCtx& ctx = last_.lat[(size_t)rows[(size_t)i]];
       ctx.set = true;
       ctx.rid = q.RequestId;
-      ctx.ttft_slo = ttft_slo[i];
-      ctx.tpot_slo = tpot_slo[i];
+      ctx.ttft_slo = p.ttft_slo[(size_t)i];
+      ctx.tpot_slo = p.tpot_slo[(size_t)i];
       for (const auto& run : runs[(size_t)i]) {
         for (ScoredEndpoint& t : run.second->TargetEndpoints) {
           const int32_t id = ids[(size_t)t.Index];
           const size_t j = (size_t)i * k + col_of(i, id);
           ctx.by_id[id] = as_info(info[j]);
-          if (fill_match) t.PrefixMatch = PrefixCacheMatchInfo{match[j], nh[i], (uint16_t)block_tokens};
+          if (fill_match) t.PrefixMatch = PrefixCacheMatchInfo{match[j], nh[i], (uint16_t)g.block_tokens};
           const std::string& name = endpoints[(size_t)t.Index].GetMetadata()->NamespacedName_.Name;
           const size_t a = (size_t)i * k + col_of(i, ids[(size_t)last_of_name[name]]);
           const double score = nh[i] ? (double)match[a] / (double)nh[i] : 0.0;  // match/total, NaN (0/0) => 0
@@ -1162,8 +1199,8 @@ class Scheduler {
   // TTFT and prefix score at the "prefill" profile's target when it has one, else at the primary target; TPOT at the primary.
   void RecordDispatch(const std::vector<BatchItem>& results) {
     if (!cfg_.LatencyPredictionInfo) return;
-    for (size_t r = 0; r < results.size() && r < lat_ctx_.size(); r++) {
-      const LatencyCtx& ctx = lat_ctx_[r];
+    for (size_t r = 0; r < results.size() && r < last_.lat.size(); r++) {
+      const LatencyCtx& ctx = last_.lat[r];
       const BatchItem& it = results[r];
       if (!ctx.set || ctx.rid.empty() || !it.error.empty()) continue;
       auto target = [&](const std::string& profile) -> const Endpoint* {
@@ -1248,8 +1285,7 @@ class Scheduler {
     if (id < 0 || std::find(v.begin(), v.end(), id) == v.end()) return;
     const uint64_t key = k->second.key;
     uint8_t removed = 0;
-    if (eppscore_running_remove(eng_, 1, 0, &id, &key, &removed, nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_running_remove: ") + eppscore_last_error(eng_));
+    Check(eppscore_running_remove(eng_, 1, 0, &id, &key, &removed, nullptr), "eppscore_running_remove");
     v.erase(std::find(v.begin(), v.end(), id));
     if (v.empty()) running_keys_.erase(k);
   }
@@ -1262,9 +1298,7 @@ class Scheduler {
                                                std::map<unsigned, int64_t>& set_base) {
     const int R = (int)requests.size(), M = (int)endpoints.size(), P = (int)cfg_.Profiles.size();
     std::vector<BatchItem> out((size_t)R);
-    lat_ctx_.assign(cfg_.LatencyPredictionInfo ? (size_t)R : 0, LatencyCtx{});
-    last_hashes_.clear();
-    last_nh_.clear();
+    last_.Clear(cfg_.LatencyPredictionInfo ? (size_t)R : 0);
     if (R == 0) return out;
     std::vector<std::string> names;
     for (const auto& np : cfg_.Profiles) names.push_back(np.first);
@@ -1289,35 +1323,14 @@ class Scheduler {
         if (keep)
           for (int m = 0; m < M; m++)
             if (keep(endpoints[(size_t)m])) row[(size_t)ids[m] >> 5] |= 1u << (ids[m] & 31);
-        if (eppscore_set_profile_endpoints(eng_, p, keep ? row.data() : nullptr, mw) != EPPSCORE_OK)
-          throw SchedulingError(std::string("eppscore_set_profile_endpoints: ") + eppscore_last_error(eng_));
+        Check(eppscore_set_profile_endpoints(eng_, p, keep ? row.data() : nullptr, mw), "eppscore_set_profile_endpoints");
       }
       PackSnapshot(endpoints, ids, Mx, requests);
     }
     std::vector<int> pos_of_id((size_t)Mx, -1);
     for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
-    int block_tokens = cfg_.Prefix.BlockSizeTokens;
-    if (M > 0 && cfg_.Prefix.AutoTune && endpoints[0].GetMetrics()->CacheBlockSize > 0) block_tokens = endpoints[0].GetMetrics()->CacheBlockSize;
-    int max_blocks = cfg_.Prefix.MaxPrefixBlocksToMatch;
-    if (cfg_.Prefix.MaxPrefixTokensToMatch > 0 && block_tokens > 0) max_blocks = cfg_.Prefix.MaxPrefixTokensToMatch / block_tokens;
-    const bool want_prefix = max_blocks > 0 && block_tokens > 0;
-    last_stride_ = want_prefix ? max_blocks : 1;
-    last_nh_.assign((size_t)R, 0);
-    last_hashes_.assign((size_t)R * last_stride_, 0);
-    if (inflight_) {
-      last_size_.resize((size_t)R);
-      last_hint_.resize((size_t)R);
-      last_chars_.resize((size_t)R);
-      for (int r = 0; r < R; r++) EstimateInputs(requests[r], &last_size_[r], &last_hint_[r], &last_chars_[r]);
-    }
-    if (running_) {  // PreRequest's inputs: the request id and avgTPOTSLO
-      last_rid_.resize((size_t)R);
-      last_tpot_.resize((size_t)R);
-      for (int r = 0; r < R; r++) {
-        last_rid_[r] = requests[r].RequestId;
-        last_tpot_[r] = SloHeader(requests[r], "x-slo-tpot-ms");
-      }
-    }
+    const PrefixGeometry g = Geometry(endpoints);
+    last_.Fill(requests, g.stride, inflight_, running_);
     // every profile's result per request (empty TargetEndpoints: the profile ran and found no endpoint)
     std::vector<std::map<std::string, ProfileRunResult>> got((size_t)R);
     std::vector<unsigned> distinct;
@@ -1329,34 +1342,9 @@ class Scheduler {
       for (int r = 0; r < R; r++)
         if (out[r].error.empty() && sets[r] == S) rows.push_back(r);
       const int n = (int)rows.size();
-      std::vector<uint8_t> bytes;
-      std::vector<int64_t> off((size_t)n + 1, 0);
-      std::vector<int32_t> len((size_t)n), adapter((size_t)n), in_tokens;
-      std::vector<uint64_t> seed((size_t)n), hashes((size_t)n * last_stride_, 0);
+      const PackedRequests packed = Pack(requests, rows);
+      std::vector<uint64_t> hashes((size_t)n * g.stride, 0);
       std::vector<uint16_t> nh((size_t)n, 0);
-      std::vector<double> ttft_slo, tpot_slo;
-      if (latency_scorer_) {  // the latency fold-in's per-request inputs, once for every profile (predictedlatency/plugin.go:276-290)
-        in_tokens.resize((size_t)n);
-        ttft_slo.resize((size_t)n);
-        tpot_slo.resize((size_t)n);
-      }
-      for (int i = 0; i < n; i++) {
-        const InferenceRequest& q = requests[(size_t)rows[i]];
-        if (latency_scorer_) {
-          in_tokens[i] = CountFields(q.Prompt);
-          ttft_slo[i] = SloHeader(q, "x-slo-ttft-ms");
-          tpot_slo[i] = SloHeader(q, "x-slo-tpot-ms");
-        }
-        while (bytes.size() % 16) bytes.push_back(0);  // 16-byte aligned starts: the fast hash path
-        off[i] = (int64_t)bytes.size();
-        len[i] = (int32_t)q.Prompt.size();
-        bytes.insert(bytes.end(), q.Prompt.begin(), q.Prompt.end());
-        seed[i] = eppscore_model_seed(q.TargetModel.data(), q.TargetModel.size(), q.CacheSalt.data(), q.CacheSalt.size());
-        auto it = adapter_ids_.find(q.TargetModel);
-        adapter[i] = it == adapter_ids_.end() ? -1 : it->second;
-      }
-      off[n] = (int64_t)bytes.size();
-      bytes.resize(bytes.size() + 64, 0);
       std::vector<int> prof;
       for (int p = 0; p < P; p++)
         if (S & (1u << p)) prof.push_back(p);
@@ -1390,95 +1378,43 @@ class Scheduler {
         x.struct_size = sizeof(x);
         x.profile = prof[k];
         if (!filters.empty() || Mx != M) {  // host filters and rows without an endpoint in this list
-          masks[k].assign((size_t)n * mw, 0u);
-          std::vector<int> all((size_t)M);
-          for (int m = 0; m < M; m++) all[m] = m;
-          for (int i = 0; i < n; i++) {
-            std::vector<int> cand = all;
-            for (auto& f : filters) {
-              cand = f->Filter_(requests[(size_t)rows[i]], endpoints, cand);
-              if (cand.empty()) break;
-            }
-            for (int m : cand) masks[k][(size_t)i * mw + (ids[m] >> 5)] |= 1u << (ids[m] & 31);
-          }
+          masks[k] = CandidateMask(filters, requests, rows, endpoints, ids, mw);
           x.cand_mask = masks[k].data();
         }
         x.pick = pick[k].data();
         x.pick_score = score[k].data();
         x.tie_count = ties[k].data();
       }
-      eppscore_batch b{};
-      b.struct_size = sizeof(b);
-      b.R = n;
+      eppscore_batch b = BatchOf(packed, g, nh.data(), hashes.data());
       b.request_base = set_base[S];
       set_base[S] += n;
-      b.prompt_bytes = want_prefix ? bytes.data() : nullptr;
-      b.prompt_off = off.data();
-      b.prompt_len = len.data();
-      b.model_seed = seed.data();
-      b.block_chars = block_tokens * 4;
-      b.max_blocks = max_blocks;
-      b.adapter_id = adapter.data();
-      b.total_blocks = nh.data();
-      b.hashes_out = want_prefix ? hashes.data() : nullptr;
-      if (latency_scorer_) {
-        b.input_tokens = in_tokens.data();
-        b.ttft_slo = ttft_slo.data();
-        b.tpot_slo = tpot_slo.data();
-      }
-      if (lists) {
-        if (eppscore_schedule_batch_profiles_topk(eng_, &b, nr, runs.data(), topk.data()) != EPPSCORE_OK)
-          throw SchedulingError(std::string("eppscore_schedule_batch_profiles_topk: ") + eppscore_last_error(eng_));
-      } else if (eppscore_schedule_batch_profiles(eng_, &b, nr, runs.data()) != EPPSCORE_OK) {
-        throw SchedulingError(std::string("eppscore_schedule_batch_profiles: ") + eppscore_last_error(eng_));
-      }
+      if (lists)
+        Check(eppscore_schedule_batch_profiles_topk(eng_, &b, nr, runs.data(), topk.data()), "eppscore_schedule_batch_profiles_topk");
+      else
+        Check(eppscore_schedule_batch_profiles(eng_, &b, nr, runs.data()), "eppscore_schedule_batch_profiles");
       for (int i = 0; i < n; i++) {
         const int r = rows[i];
-        last_nh_[(size_t)r] = nh[i];
-        std::copy(hashes.begin() + (size_t)i * last_stride_, hashes.begin() + (size_t)(i + 1) * last_stride_,
-                  last_hashes_.begin() + (size_t)r * last_stride_);
+        last_.nh[(size_t)r] = nh[i];
+        std::copy(hashes.begin() + (size_t)i * g.stride, hashes.begin() + (size_t)(i + 1) * g.stride, last_.hashes.begin() + (size_t)r * g.stride);
         for (int k = 0; k < nr; k++) {
           ProfileRunResult& pr = got[(size_t)r][names[(size_t)prof[k]]];
           const int32_t id = pick[k][i];
           if (id < 0) continue;
-          if (id >= Mx || pos_of_id[(size_t)id] < 0) throw SchedulingError("engine picked an endpoint that is not in the candidate list");
-          ScoredEndpoint se;
-          se.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)id]];
-          se.Index = pos_of_id[(size_t)id];
-          se.Score = score[k][i];
+          ScoredEndpoint se = Scored(id, score[k][i], endpoints, pos_of_id, "picked");
           se.TieCount = ties[k][i];
           pr.TargetEndpoints.push_back(se);
           const int kl = topk[(size_t)k].k;
-          for (int j = 1; j < kl; j++) {  // entries 1..k-1 of the picker's order (entry 0 is the pick); -1 past the last candidate
-            const int32_t lid = list_ids[k][(size_t)i * kl + j];
-            if (lid < 0) break;
-            if (lid >= Mx || pos_of_id[(size_t)lid] < 0) throw SchedulingError("engine listed an endpoint that is not in the candidate list");
-            ScoredEndpoint o2;
-            o2.Endpoint_ = &endpoints[(size_t)pos_of_id[(size_t)lid]];
-            o2.Index = pos_of_id[(size_t)lid];
-            o2.Score = list_scores[k][(size_t)i * kl + j];
-            pr.TargetEndpoints.push_back(o2);
-          }
+          AppendList(pr.TargetEndpoints, list_ids[k].data() + (size_t)i * kl, list_scores[k].data() + (size_t)i * kl, kl, endpoints, pos_of_id);
         }
       }
-      if (cfg_.LatencyPredictionInfo) {  // every run's entries of this call's requests, before the next piece's snapshot
-        std::vector<std::vector<std::pair<std::string, ProfileRunResult*>>> lruns((size_t)n);
+      if (cfg_.LatencyPredictionInfo || cfg_.PrefixMatchInfo) {  // every run's entries of this call's requests, before the next piece's snapshot
+        TargetRuns truns((size_t)n);
         for (int i = 0; i < n; i++)
           for (int k = 0; k < nr; k++) {
             auto it = got[(size_t)rows[i]].find(names[(size_t)prof[k]]);
-            if (it != got[(size_t)rows[i]].end()) lruns[(size_t)i].emplace_back(it->first, &it->second);
+            if (it != got[(size_t)rows[i]].end()) truns[(size_t)i].emplace_back(it->first, &it->second);
           }
-        FillLatency(lruns, rows, requests, endpoints, ids, hashes.data(), nh.data(), last_stride_, in_tokens.data(), ttft_slo.data(),
-                    tpot_slo.data(), cfg_.PrefixMatchInfo && want_prefix, block_tokens);
-      } else if (cfg_.PrefixMatchInfo && want_prefix) {  // every run's entries of this call's requests, against the call's hashes
-        std::vector<std::vector<ScoredEndpoint*>> targets((size_t)n);
-        for (int i = 0; i < n; i++)
-          for (int k = 0; k < nr; k++) {
-            auto it = got[(size_t)rows[i]].find(names[(size_t)prof[k]]);
-            if (it != got[(size_t)rows[i]].end())
-              for (ScoredEndpoint& t : it->second.TargetEndpoints) targets[(size_t)i].push_back(&t);
-          }
-        FillPrefixMatch(targets, hashes.data(), nh.data(), last_stride_, ids, block_tokens);
+        FillTargetInfo(truns, rows, requests, endpoints, ids, hashes.data(), nh.data(), packed, g);
       }
     }
     for (int r = 0; r < R; r++) {
@@ -1498,7 +1434,7 @@ class Scheduler {
       } catch (const SchedulingError& ex) {
         out[r].error = ex.what();
       }
-      if (cfg_.LatencyPredictionInfo) AttachLatency(out[r], lat_ctx_[(size_t)r], endpoints, ids);
+      if (cfg_.LatencyPredictionInfo) AttachLatency(out[r], last_.lat[(size_t)r], endpoints, ids);
     }
     last_endpoints_ = &endpoints;
     last_ids_ = ids;
@@ -1530,22 +1466,17 @@ class Scheduler {
         load_req.push_back(r);
       }
     }
-    if (!last_hashes_.empty()) {
-      std::vector<int32_t> cap((size_t)last_rows_, 0);
-      for (size_t m = 0; m < last_endpoints_->size(); m++)  // makeserver, plugin.go:207-216
-        cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks > 0) ? (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks : 0;
+    if (!last_.hashes.empty()) {
       const int32_t* picks[2] = {primary.data(), prefill.data()};
-      if (eppscore_commit_picks_profiles(eng_, R, has_prefill ? 2 : 1, picks, last_hashes_.data(), last_nh_.data(), last_stride_, cap.data(),
-                                         0, 0, nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_commit_picks_profiles: ") + eppscore_last_error(eng_));
+      Check(eppscore_commit_picks_profiles(eng_, R, has_prefill ? 2 : 1, picks, last_.hashes.data(), last_.nh.data(), last_.stride,
+                                           LruCapacities().data(), 0, 0, nullptr),
+            "eppscore_commit_picks_profiles");
     }
-    if (inflight_ && (int)last_size_.size() == R && !load_ep.empty()) {
-      std::vector<int64_t> est((size_t)R), tok(load_ep.size());
-      if (eppscore_estimate_tokens(eng_, R, 0, last_size_.data(), last_hint_.data(), last_chars_.data(), est.data(), nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
+    if (inflight_ && (int)last_.size.size() == R && !load_ep.empty()) {
+      const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
+      std::vector<int64_t> tok(load_ep.size());
       for (size_t i = 0; i < load_ep.size(); i++) tok[i] = est[(size_t)load_req[i]];
-      if (eppscore_inflight_add(eng_, (int32_t)load_ep.size(), 0, load_ep.data(), tok.data(), nullptr) != EPPSCORE_OK)
-        throw SchedulingError(std::string("eppscore_inflight_add: ") + eppscore_last_error(eng_));
+      Check(eppscore_inflight_add(eng_, (int32_t)load_ep.size(), 0, load_ep.data(), tok.data(), nullptr), "eppscore_inflight_add");
     }
     RunningAdd(primary);  // the primary target only; the prefill target is not queued (requestcontrol_hooks.go:55-95)
   }
@@ -1561,14 +1492,28 @@ class Scheduler {
       if (id >= 0) eps.push_back(id);
     }
     if (eps.empty()) return;
-    int64_t size = 0, est = 0;
+    int64_t size = 0;
     int32_t hint = -1, chars = 0;
     EstimateInputs(request, &size, &hint, &chars);
-    if (eppscore_estimate_tokens(eng_, 1, 0, &size, &hint, &chars, &est, nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_estimate_tokens: ") + eppscore_last_error(eng_));
-    std::vector<int64_t> tok(eps.size(), est);
-    if (eppscore_inflight_release(eng_, (int32_t)eps.size(), 0, eps.data(), tok.data(), nullptr) != EPPSCORE_OK)
-      throw SchedulingError(std::string("eppscore_inflight_release: ") + eppscore_last_error(eng_));
+    std::vector<int64_t> tok(eps.size(), EstimateTokens(1, &size, &hint, &chars)[0]);
+    Check(eppscore_inflight_release(eng_, (int32_t)eps.size(), 0, eps.data(), tok.data(), nullptr), "eppscore_inflight_release");
+  }
+
+  // SimpleTokenEstimator (eppscore_estimate_tokens) over n requests' EstimateInputs.
+  std::vector<int64_t> EstimateTokens(int32_t n, const int64_t* size, const int32_t* hint, const int32_t* chars) const {
+    std::vector<int64_t> est((size_t)n);
+    Check(eppscore_estimate_tokens(eng_, n, 0, size, hint, chars, est.data(), nullptr), "eppscore_estimate_tokens");
+    return est;
+  }
+
+  // makeserver (plugin.go:207-216): the LRU capacity of each endpoint row of the last engine batch, for its commit.
+  std::vector<int32_t> LruCapacities() const {
+    std::vector<int32_t> cap((size_t)last_rows_, 0);
+    for (size_t m = 0; m < last_endpoints_->size(); m++) {
+      const int blocks = (*last_endpoints_)[m].GetMetrics()->CacheNumBlocks;
+      cap[(size_t)last_ids_[m]] = (cfg_.Prefix.AutoTune && blocks > 0) ? blocks : 0;
+    }
+    return cap;
   }
 
   // Stable endpoint ids of a candidate list (see ScheduleBatch): ids[i] is endpoint i's row, *rows the number of rows; true when
@@ -1695,7 +1640,7 @@ class Scheduler {
       lp.composite_kv = latency_scorer_->CompositeKVWeight;
       lp.composite_queue = latency_scorer_->CompositeQueueWeight;
       lp.composite_prefix = latency_scorer_->CompositePrefixWeight;
-      if (eppscore_set_latency_params(eng_, &lp) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_set_latency_params: ") + eppscore_last_error(eng_));
+      Check(eppscore_set_latency_params(eng_, &lp), "eppscore_set_latency_params");
     }
     for (int i = 0; i < N; i++) {
       const int m = ids[(size_t)i];
@@ -1734,7 +1679,7 @@ class Scheduler {
       s.prefill_role = prefill.data();
     }
     s.epoch = ++epoch_;
-    if (eppscore_set_snapshot(eng_, &s) != EPPSCORE_OK) throw SchedulingError(std::string("eppscore_set_snapshot: ") + eppscore_last_error(eng_));
+    Check(eppscore_set_snapshot(eng_, &s), "eppscore_set_snapshot");
   }
 
   SchedulerConfig cfg_;
@@ -1745,9 +1690,7 @@ class Scheduler {
   const LatencyScorer* latency_scorer_ = nullptr;
   std::unordered_map<std::string, int> adapter_ids_;
   uint64_t epoch_ = 0;
-  std::vector<uint64_t> last_hashes_;
-  std::vector<uint16_t> last_nh_;
-  int32_t last_stride_ = 1;
+  BatchRecord last_;  // the last engine batch's per-request record, for PreRequest
   const std::vector<Endpoint>* last_endpoints_ = nullptr;
   std::vector<int> last_ids_;                       // list position -> endpoint id of the last engine batch
   int last_rows_ = 0;
@@ -1757,15 +1700,10 @@ class Scheduler {
   bool inflight_ = false;    // SchedulerConfig::InFlightLoad
   bool token_load_ = false;  // the profile has a token-load scorer
   bool inorder_ = false;     // SchedulerConfig::InOrderInFlightLoad
-  std::vector<int64_t> last_size_;  // estimator inputs of the last engine batch, per request
-  std::vector<int32_t> last_hint_, last_chars_;
   bool running_ = false;  // PredictedLatencyProducer::TrackRunningRequests
-  std::vector<std::string> last_rid_;  // PreRequest's inputs of the last engine batch, per request
-  std::vector<double> last_tpot_;
   std::unordered_map<std::string, KeyUse> running_keys_;
   uint64_t next_key_ = 1;
   PrefixIndexerHistograms prefix_metrics_;
-  std::vector<LatencyCtx> lat_ctx_;  // the last batch's rows (SchedulerConfig::LatencyPredictionInfo)
   std::unordered_map<std::string, epp::PredictedLatencyAtDispatch> dispatch_;
 };
 
