@@ -142,7 +142,8 @@ struct eppscore_engine {
         s_subset,  // candidate rows subset ∧ cand_mask of a run on a profile with an endpoint subset
         // an in-order batch's slice (schedule_inorder): match rows, totals and candidate min / max.  Allocated by the first call
         // outside a capture for a fixed number of rows and never reallocated, like `wide`.
-        s_io_match, s_io_total, s_io_minmax;
+        s_io_match, s_io_total, s_io_minmax,
+        s_pmatch;  // pick_match of an in-order batch that commits as it schedules
     int32_t io_rows = 0;
     // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide).  Allocated by the first call that
     // needs them and never reallocated, so a graph captured after that call keeps pointing at live memory.
@@ -165,6 +166,7 @@ struct eppscore_engine {
   PinnedBuf h_res;
   int32_t wide_rows = 0;
   int32_t io_cluster = 0;          // CTAs per cluster of inorder_pick_kernel (0: not decided yet)
+  int32_t io_index_cluster = 0;    // CTAs per cluster of inorder_index_kernel (0: not decided yet)
   int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
@@ -457,6 +459,7 @@ struct DevBatch {  // all device pointers
   uint16_t* match_blocks;   // profile-independent outputs, written by the kernels of run 0
   uint16_t* total_blocks;
   uint64_t* hashes_out;
+  uint16_t* pick_match;     // [R] an in-order batch's matchBlocks at each pick (schedule_inorder_index)
   int32_t n_runs;
   DevRun run[EPPSCORE_MAX_PROFILES];
 };
@@ -503,6 +506,7 @@ void for_each_row_array(DevBatch& d, size_t M, F&& f) {
   f(d.match_blocks, M, Rows::out, &Scratch::s_match);
   f(d.total_blocks, 1, Rows::small, &Scratch::s_total);
   f(d.hashes_out, (size_t)d.max_blocks, Rows::out, &Scratch::s_hashes);  // (a host batch never has hashes_in with it)
+  f(d.pick_match, 1, Rows::small, &Scratch::s_pmatch);
 }
 
 // Rows [base, base + n) of a batch.
@@ -1526,21 +1530,36 @@ constexpr size_t kInOrderSliceBytes = 32ull << 20;
 // picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
 // inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
 // so the next slice continues from them.
-int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
+// lru_capacity (host, [M] or NULL) -> a padded host vector the index can copy; validates the values
+int32_t pad_caps(eppscore_engine* e, const int32_t* lru_capacity, std::vector<int32_t>* out) {
+  out->clear();
+  if (!lru_capacity) return EPPSCORE_OK;
+  out->assign((size_t)e->geo.Mpad, 0);
+  const int32_t n = e->M > 0 ? e->M : e->geo.Mpad;
+  for (int32_t i = 0; i < n; i++) (*out)[i] = lru_capacity[i] > 0 ? lru_capacity[i] : 0;
+  return EPPSCORE_OK;
+}
+// A reserved index reports a mutation it skipped for lack of room to the next index call outside a capture, which is refused.
+int32_t index_skips(eppscore_engine* e, bool exact, const char* what) {
+  if (!e->index->reserved()) return EPPSCORE_OK;
+  bool skipped = false;
+  CK(e, e->index->new_skips(exact, e->stream, &skipped));
+  if (!skipped) return EPPSCORE_OK;
+  return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + ": an earlier index mutation found no room within eppscore_prefix_reserve's "
+                                        "sizes and was skipped whole (stats.index_error bit 4); this call was not run");
+}
+int32_t index_status(eppscore_engine* e, cudaError_t c, const char* what) {
+  if (c == cudaSuccess) return EPPSCORE_OK;
+  if (c == cudaErrorInvalidValue)
+    return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + ": an LRU capacity above the engine's lru_capacity_max (the per-endpoint regions were sized at the first Add)");
+  return cuda_fail(e, c, what);
+}
+
+// The slice-independent arguments of the in-order walk for profile 0 of the current snapshot; *minmax: whether the profile has
+// a queue or running scorer (the walk then reads the candidates' min / max).
+InOrderArgs inorder_args(eppscore_engine* e, bool* minmax) {
   const Profile& P = e->prof[0];
   const eppscore_config& c = P.cfg;
-  if (!sc.s_io_match.p) {
-    if (is_capturing(s))
-      return fail(e, EPPSCORE_ERR_CAPACITY,
-                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
-                  "CUDA-graph capture first");
-    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
-    if (sc.rows > 0) rows = std::min(rows, sc.rows);
-    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
-    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
-    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
-    sc.io_rows = rows;
-  }
   InOrderArgs a{};
   a.M = e->M;
   a.Mpad = e->geo.Mpad;
@@ -1549,7 +1568,7 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
   a.A = e->A;
   a.mask_words = (e->M + 31) / 32;
   a.n_scorers = c.n_scorers;
-  bool minmax = false;
+  *minmax = false;
   static const double cls_score[4] = {0.0, 0.6, 0.8, 1.0};  // lora_affinity.go:84-99
   for (int i = 0; i < c.n_scorers; i++) {
     const int k = c.scorer_kind[i];
@@ -1558,7 +1577,7 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
     const bool static_term = k == EPPSCORE_SCORER_KV_CACHE || (k >= EPPSCORE_SCORER_ENDPOINT_COL0 && k < EPPSCORE_SCORER_ENDPOINT_COL0 + 4);
     a.term[i] = static_term ? P.term[i].as<double>() : nullptr;
     for (int q = 0; q < 4; q++) a.lora_term[i][q] = clamp01_host(cls_score[q]) * c.scorer_weight[i];
-    minmax = minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
+    *minmax = *minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
   }
   a.pick_mode = c.pick_mode;
   a.tie_mode = c.tie_mode;
@@ -1572,22 +1591,49 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
   a.cls_hi = e->cls_hi.as<uint32_t>();
   a.inflight_req = e->inflight_req.as<int64_t>();
   a.inflight_tok = e->inflight_tok.as<int64_t>();
+  return a;
+}
+// A slice's per-request arguments of the walk.
+void inorder_slice(InOrderArgs& a, const DevBatch& q) {
+  a.R = q.R;
+  a.request_base = q.request_base;
+  a.adapter_id = q.adapter_id;
+  a.cand_mask = q.run[0].cand_mask;
+  a.tokens = q.tokens;
+  a.pick = q.run[0].pick;
+  a.pick_score = q.run[0].pick_score;
+  a.tie_count = q.run[0].tie_count;
+}
+
+// eppscore_schedule_batch_inorder on device buffers, asynchronous on `s`.  Per slice of rows: the batch kernels of
+// schedule_device with their match_out route (the prefix match counts and totals, which depend on no load; their provisional
+// picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
+// inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
+// so the next slice continues from them.
+int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
+  if (!sc.s_io_match.p) {
+    if (is_capturing(s))
+      return fail(e, EPPSCORE_ERR_CAPACITY,
+                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
+                  "CUDA-graph capture first");
+    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
+    if (sc.rows > 0) rows = std::min(rows, sc.rows);
+    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
+    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
+    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
+    sc.io_rows = rows;
+  }
+  bool minmax = false;
+  InOrderArgs a = inorder_args(e, &minmax);
   for (int32_t base = 0; base < d.R; base += sc.io_rows) {
     DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
     q.match_blocks = sc.s_io_match.as<uint16_t>();
     if (!q.total_blocks) q.total_blocks = sc.s_io_total.as<uint16_t>();
     int32_t rc = schedule_device(e, q, s, sc);
     if (rc != EPPSCORE_OK) return rc;
-    a.R = q.R;
-    a.request_base = q.request_base;
+    inorder_slice(a, q);
     a.match = q.match_blocks;
     a.total = q.total_blocks;
-    a.adapter_id = q.adapter_id;
-    a.cand_mask = q.run[0].cand_mask;
-    a.tokens = q.tokens;
-    a.pick = q.run[0].pick;
-    a.pick_score = q.run[0].pick_score;
-    a.tie_count = q.run[0].tie_count;
     a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
     if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
     const int launched = launch_inorder_pick(a, e->io_cluster, s);
@@ -1601,17 +1647,107 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
   return EPPSCORE_OK;
 }
 
-// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk, _inorder): the runs (profile + per-profile filter
-// result and outputs) of one batch, as make_batch takes them.  `inorder`: the batch's single run is scheduled in arrival order
-// against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates.
+// eppscore_schedule_batch_inorder_index on device buffers, asynchronous on `s`, as an index mutation the caller has ordered
+// (schedule_batch_inorder_index).  The slices are those of schedule_inorder (its scratch and row count, plus a hash scratch of
+// the same rows).  Per slice: the hash stage in its plain form (hashes and totals into the scratch, or the caller's hashes_out
+// / total_blocks; supplied hashes are read where they are), the candidates' min / max, the room for the slice's Σ n_hashes
+// (DeviceIndex::ordered_room), then inorder_index_kernel, which reads each request's match counts from the index as it stands
+// and commits the request's blocks at its pick before the next request probes.
+int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, const DeviceIndex::OrderedRefs& refs,
+                               bool capturing) {
+  const int32_t mb = d.max_blocks;
+  const bool hashing = !d.hashes_in && d.prompt_bytes;
+  if (hashing && mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
+  if (d.hashes_in && (!d.n_hashes_in || d.hash_stride <= 0)) return fail(e, EPPSCORE_ERR_INVALID, "hashes_in needs n_hashes_in and hash_stride");
+  if (!sc.s_io_match.p) {
+    if (capturing)
+      return fail(e, EPPSCORE_ERR_CAPACITY,
+                  "the first in-order call on a stream allocates its slice scratch: make one call outside the CUDA-graph capture "
+                  "first");
+    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
+    if (sc.rows > 0) rows = std::min(rows, sc.rows);
+    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
+    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
+    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
+    sc.io_rows = rows;
+  }
+  const size_t hash_bytes = hashing && !d.hashes_out ? (size_t)std::min(sc.io_rows, d.R) * mb * 8 : 0;
+  if (hash_bytes > sc.s_hashes.bytes) {
+    if (capturing) return fail(e, EPPSCORE_ERR_CAPACITY, "schedule_batch_inorder_index under CUDA-graph capture: the hash scratch "
+                                                         "is smaller than this batch needs (make the same call outside the capture first)");
+    CK(e, sc.s_hashes.reserve(hash_bytes));
+  }
+  bool wait_snapshot = false;
+  if (int32_t rc = reader_begin(e, s, nullptr, &wait_snapshot); rc != EPPSCORE_OK) return rc;
+  bool minmax = false;
+  InOrderArgs a = inorder_args(e, &minmax);
+  InOrderIndexArgs ix{};
+  ix.tv = refs.tv;
+  ix.lv = refs.lv;
+  ix.cap_req = refs.cap_req;
+  for (int32_t base = 0; base < d.R; base += sc.io_rows) {
+    const DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
+    uint16_t* total = q.total_blocks ? q.total_blocks : sc.s_io_total.as<uint16_t>();
+    if (hashing) {
+      HashArgs h{};
+      h.R = q.R;
+      h.bytes = q.prompt_bytes;
+      h.off = q.prompt_off;
+      h.len = q.prompt_len;
+      h.seed = q.model_seed;
+      h.block_chars = q.block_chars;
+      h.max_blocks = mb;
+      h.hashes = q.hashes_out ? q.hashes_out : sc.s_hashes.as<uint64_t>();
+      h.stride = mb;
+      h.n_hashes = total;
+      h.stage_mask = e->hash_stage_mask;
+      e->launches += launch_hash_prompts(h, s, e->sm_count);
+      ix.hashes = h.hashes;
+      ix.stride = mb;
+    } else if (q.hashes_in) {
+      CK(e, cudaMemcpyAsync(total, q.n_hashes_in, (size_t)q.R * 2, cudaMemcpyDeviceToDevice, s));
+      ix.hashes = q.hashes_in;
+      ix.stride = q.hash_stride;
+    } else {  // no prompts: every request has 0 blocks
+      CK(e, cudaMemsetAsync(total, 0, (size_t)q.R * 2, s));
+      ix.hashes = nullptr;
+      ix.stride = 1;
+    }
+    CK(e, cudaGetLastError());
+    inorder_slice(a, q);
+    a.match = nullptr;
+    a.total = total;
+    a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
+    ix.pick_match = q.pick_match;
+    if (wait_snapshot && base == 0) CK(e, cudaStreamWaitEvent(s, e->ev_snapshot, 0));
+    if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
+    if (int32_t rc = index_status(e, e->index->ordered_room(q.R, total, s), "schedule_batch_inorder_index"); rc != EPPSCORE_OK) return rc;
+    const int launched = launch_inorder_index(a, ix, e->io_index_cluster, s);
+    if (launched < 0) {
+      cudaGetLastError();
+      return cuda_fail(e, (cudaError_t)-launched, "inorder_index_kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
+    CK(e, e->index->ordered_end(s, capturing));
+  }
+  return EPPSCORE_OK;
+}
+
+// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk, _inorder, _inorder_index): the runs (profile + per-profile
+// filter result and outputs) of one batch, as make_batch takes them.  `inorder`: the batch's single run is scheduled in arrival
+// order against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates; with `ordered` also against
+// the prefix index, committing as it goes (schedule_inorder_index), with pick_match [R] (optional) its output.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
-                       const eppscore_topk* topk, bool wide = false, bool inorder = false, const int64_t* tokens = nullptr) {
+                       const eppscore_topk* topk, bool wide = false, bool inorder = false, const int64_t* tokens = nullptr,
+                       const DeviceIndex::OrderedRefs* ordered = nullptr, uint16_t* pick_match = nullptr) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
   int32_t rc = EPPSCORE_OK;
   DevBatch d = make_batch(e, *b, n_runs, runs, topk, wide);
   d.tokens = tokens;
+  d.pick_match = pick_match;
   const size_t M = (size_t)e->M;
   bool any_wide = false;
   for (int i = 0; i < n_runs; i++) any_wide = any_wide || d.run[i].wide;
@@ -1621,7 +1757,7 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     if (!inorder) return any_wide ? schedule_wide(e, x, st, sc) : schedule_device(e, x, st, sc);
     bool capturing = false;
     int32_t rc = producer_begin(e, st, &capturing);
-    if (rc == EPPSCORE_OK) rc = schedule_inorder(e, x, st, sc);
+    if (rc == EPPSCORE_OK) rc = ordered ? schedule_inorder_index(e, x, st, sc, *ordered, capturing) : schedule_inorder(e, x, st, sc);
     if (rc == EPPSCORE_OK) rc = producer_end(e, st, capturing, counters_feed_scorer(e));
     return rc;
   };
@@ -1792,6 +1928,40 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   return schedule_batch(e, b, 1, nullptr, t, wide);
 }
 
+// What both in-order calls refuse, and the cluster shape of their walk (decided once per engine, before the first call launches
+// anything).  *done: nothing to run (R == 0).
+int32_t inorder_prologue(eppscore_engine* e, const eppscore_batch* b, const char* what, bool index, bool* done) {
+  *done = false;
+  const std::string w(what);
+  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
+  if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
+  if (cfg_has(e->prof[0].cfg, EPPSCORE_SCORER_LATENCY))
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": the latency scorer's inputs are PreRequest state the call does not order");
+  if (e->have_snapshot && e->snapshot_has_tokens)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": the snapshot supplies inflight_tokens; the in-order view needs the engine's counters");
+  if (b->dense_feat || b->scores_out || b->match_blocks || b->pred_out || b->filter_mask_out)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": dense_feat, scores_out, match_blocks, pred_out and filter_mask_out are not available");
+  if (!b->pick || !b->pick_score || !b->tie_count) return fail(e, EPPSCORE_ERR_INVALID, "pick/pick_score/tie_count required");
+  if (b->location != 0 && b->location != 1) return fail(e, EPPSCORE_ERR_INVALID, "location must be 0 or 1");
+  if (b->R == 0) {
+    *done = true;
+    return EPPSCORE_OK;
+  }
+  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, w + " before set_snapshot");
+  if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
+  CK(e, cudaSetDevice(e->device));
+  int32_t& shape = index ? e->io_index_cluster : e->io_cluster;
+  if (shape == 0) {
+    const int C = index ? inorder_index_cluster_size(e->geo.Mpad) : inorder_cluster_size(e->geo.Mpad);
+    if (C < 0) return cuda_fail(e, (cudaError_t)-C, index ? "inorder_index_kernel cluster attributes" : "inorder_pick_kernel cluster attributes");
+    if (C == 0)
+      return fail(e, EPPSCORE_ERR_CAPACITY, w + ": no thread-block cluster of this device holds max_endpoints "
+                                                "endpoints (8192 needs the non-portable cluster size 16)");
+    shape = C;
+  }
+  return EPPSCORE_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1812,29 +1982,43 @@ int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_bat
 
 int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens) {
   if (!e) return EPPSCORE_ERR_INVALID;
-  if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
-  if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
-  if (cfg_has(e->prof[0].cfg, EPPSCORE_SCORER_LATENCY))
-    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: the latency scorer's inputs are PreRequest state the call does not order");
-  if (e->have_snapshot && e->snapshot_has_tokens)
-    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: the snapshot supplies inflight_tokens; the in-order view needs the engine's counters");
-  if (b->dense_feat || b->scores_out || b->match_blocks || b->pred_out || b->filter_mask_out)
-    return fail(e, EPPSCORE_ERR_INVALID, "schedule_batch_inorder: dense_feat, scores_out, match_blocks, pred_out and filter_mask_out are not available");
-  if (!b->pick || !b->pick_score || !b->tie_count) return fail(e, EPPSCORE_ERR_INVALID, "pick/pick_score/tie_count required");
-  if (b->location != 0 && b->location != 1) return fail(e, EPPSCORE_ERR_INVALID, "location must be 0 or 1");
-  if (b->R == 0) return EPPSCORE_OK;
-  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, "schedule_batch_inorder before set_snapshot");
-  if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
-  CK(e, cudaSetDevice(e->device));
-  if (e->io_cluster == 0) {  // the cluster shape, decided once per engine and before the first call launches anything
-    const int C = inorder_cluster_size(e->geo.Mpad);
-    if (C < 0) return cuda_fail(e, (cudaError_t)-C, "inorder_pick_kernel cluster attributes");
-    if (C == 0)
-      return fail(e, EPPSCORE_ERR_CAPACITY, "schedule_batch_inorder: no thread-block cluster of this device holds max_endpoints "
-                                            "endpoints (8192 needs the non-portable cluster size 16)");
-    e->io_cluster = C;
-  }
+  bool done = false;
+  const int32_t rc = inorder_prologue(e, b, "schedule_batch_inorder", false, &done);
+  if (rc != EPPSCORE_OK || done) return rc;
   return schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens);
+}
+
+int32_t eppscore_schedule_batch_inorder_index(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                              const eppscore_inorder_index* x) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  const char* what = "schedule_batch_inorder_index";
+  if (!x || x->struct_size != sizeof(eppscore_inorder_index)) return fail(e, EPPSCORE_ERR_INVALID, "inorder_index NULL or struct_size mismatch");
+  bool done = false;
+  int32_t rc = inorder_prologue(e, b, what, true, &done);
+  if (rc != EPPSCORE_OK || done) return rc;
+  // the call is an index mutation on the stream the batch runs on: ordered like eppscore_commit_picks_device
+  cudaStream_t cs = b->location == 1 && b->stream ? (cudaStream_t)b->stream : e->stream;
+  const bool capturing = is_capturing(cs);
+  if (capturing && !e->index->reserved())
+    return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + " under CUDA-graph capture: reserve the prefix index before capturing "
+                                          "commits (eppscore_prefix_reserve)");
+  if (capturing && x->lru_capacity)
+    return fail(e, EPPSCORE_ERR_INVALID, std::string(what) + " under CUDA-graph capture: lru_capacity must be NULL (create the "
+                                         "endpoints' LRUs outside the capture, e.g. eppscore_prefix_add with n = 0)");
+  if (!capturing && (rc = index_skips(e, false, what)) != EPPSCORE_OK) return rc;
+  std::vector<int32_t> caps;
+  if ((rc = pad_caps(e, x->lru_capacity, &caps)) != EPPSCORE_OK) return rc;
+  if (!capturing) {  // after every earlier batch that reads the index and every earlier mutation (inside a capture: the graph's edges)
+    if ((rc = pending_wait(e, cs)) != EPPSCORE_OK) return rc;
+    if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
+  }
+  DeviceIndex::OrderedRefs refs{};
+  if ((rc = index_status(e, e->index->ordered_begin(caps.empty() ? nullptr : caps.data(), cs, &refs), what)) != EPPSCORE_OK) return rc;
+  rc = schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, &refs, x->pick_match);
+  if (rc != EPPSCORE_OK || capturing) return rc;
+  CK(e, cudaEventRecord(e->ev_table, cs));  // later readers on other streams, and later mutations on the engine stream, follow it
+  if (cs != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_table, 0));
+  return EPPSCORE_OK;
 }
 
 int32_t eppscore_add_profile(eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) {
@@ -2019,31 +2203,6 @@ int32_t eppscore_count_fields(eppscore_engine* e, int32_t R, int32_t location, c
   const int32_t* d_len = st.in(prompt_len, R);
   int32_t* d_out = st.out(out, R);
   return st.finish([&] { return eppscore_count_fields(e, R, 1, d_bytes, d_off, d_len, d_out, e->stream); });
-}
-
-// lru_capacity (host, [M] or NULL) -> a padded host vector the index can copy; validates the values
-static int32_t pad_caps(eppscore_engine* e, const int32_t* lru_capacity, std::vector<int32_t>* out) {
-  out->clear();
-  if (!lru_capacity) return EPPSCORE_OK;
-  out->assign((size_t)e->geo.Mpad, 0);
-  const int32_t n = e->M > 0 ? e->M : e->geo.Mpad;
-  for (int32_t i = 0; i < n; i++) (*out)[i] = lru_capacity[i] > 0 ? lru_capacity[i] : 0;
-  return EPPSCORE_OK;
-}
-// A reserved index reports a mutation it skipped for lack of room to the next index call outside a capture, which is refused.
-static int32_t index_skips(eppscore_engine* e, bool exact, const char* what) {
-  if (!e->index->reserved()) return EPPSCORE_OK;
-  bool skipped = false;
-  CK(e, e->index->new_skips(exact, e->stream, &skipped));
-  if (!skipped) return EPPSCORE_OK;
-  return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + ": an earlier index mutation found no room within eppscore_prefix_reserve's "
-                                        "sizes and was skipped whole (stats.index_error bit 4); this call was not run");
-}
-static int32_t index_status(eppscore_engine* e, cudaError_t c, const char* what) {
-  if (c == cudaSuccess) return EPPSCORE_OK;
-  if (c == cudaErrorInvalidValue)
-    return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + ": an LRU capacity above the engine's lru_capacity_max (the per-endpoint regions were sized at the first Add)");
-  return cuda_fail(e, c, what);
 }
 
 // PreRequest for R requests with n_picks picks each (eppscore_commit_picks[_device|_profiles]): host arrays are staged and the

@@ -10,9 +10,13 @@
 //                          CTA reduces to a winner, the cluster merges the CTA winners through distributed shared memory behind
 //                          barrier.cluster, and the owner of the pick adds the request's tokens.
 // The prefix match counts and totals come from the ordinary batch kernels (their match_out route), which depend on no load.
+//   inorder_index_kernel   the same walk ordered against the prefix index too (eppscore_schedule_batch_inorder_index): each
+//                          request's match counts are probed from the index as the earlier requests' Adds left it, and the CTA
+//                          that owns the pick runs the index's commit program (IndexProgram::commit) for the request's Add.
 #include <cooperative_groups.h>
 
 #include "device_common.cuh"
+#include "index_device.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -90,8 +94,17 @@ struct InOrderReq {
   long long tokens;
 };
 
-template <bool RND>
-__global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(const __grid_constant__ InOrderArgs a) {
+// The hit slots of one round of a request's probes, staged in shared memory (IDX): the cnt word and ep[0..10) of each.
+struct InOrderHits {
+  uint32_t raw[kCommitThreads];
+  uint32_t ep[kCommitThreads][kInlineEps / 2];  // ep pairs as the slot holds them; in row mode ep[0] is the row id
+  uint32_t first[2];                            // first miss of the current round (double-buffered, reset one round ahead)
+};
+
+// The walk, in the in-flight form (IDX false: inorder_pick_kernel) or the index form (IDX true: inorder_index_kernel, CTAs of
+// kCommitThreads threads; dynamic shared memory = the terms, then the CommitSmem of IndexProgram).
+template <bool RND, bool IDX>
+__device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrderIndexArgs& ix) {
   extern __shared__ __align__(16) double s_term[];  // [n_scorers][blockDim.x]: the request-independent terms of each thread's endpoint
   __shared__ InOrderBest s_warp[kInOrderWarps];
   __shared__ InOrderBest s_cta[2];  // the CTA's winner of the last two requests (read by the other CTAs of the cluster)
@@ -136,10 +149,54 @@ __global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(con
     return x;
   };
 
+  // IDX: the index as the walk mutates it.  Every read goes through DevX's relaxed GPU-scope loads (never the read-only path:
+  // the table changes under this kernel); barrier.cluster orders a commit before the next request's probes.
+  DevX dx;
+  InOrderHits* hits = nullptr;
+  uint32_t parity = 0;
+  if constexpr (IDX) {
+    __shared__ InOrderHits s_hits;
+    hits = &s_hits;
+    if (tid < 2) hits->first[tid] = 0xFFFFFFFFu;
+  }
+
   cluster.sync();  // every CTA of the cluster is running before any reads another's shared memory
   InOrderReq cur = load(0);
   for (int r = 0; r < a.R; r++) {
     const InOrderReq nxt = load(r + 1);
+    if constexpr (IDX) {
+      // ---- matchLongestPrefix (plugin.go:219-235) at this thread's endpoint, against the index after requests 0..r-1's Adds:
+      // T probes per round up to the first global miss, the hit slots staged in shared memory, then every thread counts the
+      // hits whose set holds its endpoint (slot_holds: an inline member or bit m of the row) ----
+      const uint32_t n = (uint32_t)cur.total;
+      const uint64_t* h = ix.hashes + (size_t)r * ix.stride;
+      const TableView* tv = ix.tv;
+      uint32_t c = 0;
+      for (uint32_t base = 0; base < n; base += (uint32_t)T) {
+        const bool in = base + tid < n;
+        uint32_t raw = 0;
+        TSlot* sl = in ? table_find(dx, tv, __ldg(reinterpret_cast<const unsigned long long*>(h) + base + tid), &raw) : nullptr;
+        if (sl) {
+          hits->raw[tid] = raw;
+          const uint32_t* w = reinterpret_cast<const uint32_t*>(sl) + 3;
+#pragma unroll
+          for (int k = 0; k < kInlineEps / 2; k++) hits->ep[tid][k] = dx.ld32(w + k);
+        }
+        const uint32_t miss = __ballot_sync(0xffffffffu, in && !sl);
+        if (lane == 0 && miss) atomicMin(&hits->first[parity], (uint32_t)(warp * 32 + __ffs(miss) - 1));
+        __syncthreads();
+        const uint32_t first = hits->first[parity];
+        if (tid == 0) hits->first[parity ^ 1] = 0xFFFFFFFFu;
+        uint32_t nh = n - base < (uint32_t)T ? n - base : (uint32_t)T;
+        nh = first < nh ? first : nh;
+        if (real)
+          for (uint32_t k = 0; k < nh; k++) c += staged_holds(dx, tv, hits->raw[k], hits->ep[k], (uint32_t)m) ? 1u : 0u;
+        __syncthreads();  // the staged hits are read before the next round overwrites them
+        parity ^= 1;
+        if (first != 0xFFFFFFFFu) break;
+      }
+      cur.c = (int32_t)c;
+    }
     // ---- Score (scheduler_profile.go:151-174): profile order from 0.0, the operations of score_matrix_kernel ----
     double acc = 0.0;
     for (int s = 0; s < a.n_scorers; s++) {
@@ -211,6 +268,27 @@ __global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(con
       a.pick_score[r] = pick >= 0 ? score : 0.0;
       a.tie_count[r] = cnt;
     }
+    if constexpr (IDX) {
+      // PrefixCacheMatchInfo at the target (plugin.go:199-204), before the request's own Add
+      if (ix.pick_match && (pick >= 0 ? pick == m : m == 0)) ix.pick_match[r] = pick >= 0 ? (uint16_t)cur.c : (uint16_t)0;
+      // indexer.Add(hashes[r], pick) (plugin.go:169-197) by the CTA that owns the pick: CTA-uniform, as IndexProgram needs
+      if (pick >= 0 && pick / T == (int)cluster.block_rank()) {
+        __shared__ int32_t s_pick;
+        if (tid == 0) s_pick = pick;  // (read inside the program's first parallel section, behind its barrier)
+        CommitArgs ca{};
+        ca.R = 1;
+        ca.pick = &s_pick;
+        ca.hashes = ix.hashes + (size_t)r * ix.stride;
+        ca.n_hashes = a.total + r;
+        ca.stride = ix.stride;
+        ca.cap_req = ix.cap_req;
+        ca.n_picks = 1;
+        CommitSmem* sm = reinterpret_cast<CommitSmem*>(s_term + (size_t)kMaxSteps * T);
+        IndexProgram<DevX> prog(dx, ix.tv, ix.lv, sm, (uint32_t)pick);
+        prog.commit(ca);
+      }
+      cluster.sync();  // request r's Add is visible to every CTA's probes of request r + 1
+    }
     cur = nxt;
   }
   if (m < a.Mpad) {
@@ -218,6 +296,17 @@ __global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(con
     a.inflight_req[m] = req;
   }
   cluster.sync();  // no CTA leaves while another may still read its winners
+}
+
+template <bool RND>
+__global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(const __grid_constant__ InOrderArgs a) {
+  inorder_walk<RND, false>(a, InOrderIndexArgs{});
+}
+
+template <bool RND>
+__global__ void __launch_bounds__(kCommitThreads, 1) inorder_index_kernel(const __grid_constant__ InOrderArgs a,
+                                                                          const __grid_constant__ InOrderIndexArgs ix) {
+  inorder_walk<RND, true>(a, ix);
 }
 
 int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count) {
@@ -284,6 +373,61 @@ int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s) {
   }
   const cudaLaunchConfig_t cfg = pick_config<false>(a.Mpad, C, s, at);
   return launched_one(cudaLaunchKernelEx(&cfg, inorder_pick_kernel<false>, a));
+}
+
+// The index form: C CTAs of kCommitThreads threads (IndexProgram's CTA), thread t of CTA c owning endpoint c * 512 + t (threads
+// past Mpad idle), so C = Mpad / 512 up to 16 (one CTA below 512 endpoints).  Dynamic shared memory: the terms of 512 threads,
+// then the CommitSmem of the program (136 KiB, plus 13 KiB of static shared memory: one CTA per SM).
+static size_t index_smem() { return (size_t)kMaxSteps * 8 * kCommitThreads + sizeof(CommitSmem); }
+
+static cudaLaunchConfig_t index_config(int C, cudaStream_t s, cudaLaunchAttribute* at) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(C);
+  cfg.blockDim = dim3(kCommitThreads);
+  cfg.dynamicSmemBytes = index_smem();
+  cfg.stream = s;
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = C;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+template <bool RND>
+static int index_cluster_size(int Mpad) {
+  auto kernel = inorder_index_kernel<RND>;
+  cudaError_t c = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)index_smem());
+  if (c != cudaSuccess) return -(int)c;
+  const int C = Mpad <= kCommitThreads ? 1 : (Mpad + kCommitThreads - 1) / kCommitThreads;
+  if (C > 16) return 0;
+  cudaLaunchAttribute at[1];
+  const cudaLaunchConfig_t cfg = index_config(C, nullptr, at);
+  int clusters = 0;
+  c = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
+  if (c == cudaSuccess && clusters >= 1) return C;
+  cudaGetLastError();
+  return 0;
+}
+
+int inorder_index_cluster_size(int Mpad) {
+  const int a = index_cluster_size<false>(Mpad);
+  if (a <= 0) return a;
+  const int b = index_cluster_size<true>(Mpad);
+  return b <= 0 ? b : a;  // (both forms have the same shape)
+}
+
+int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s) {
+  if (a.R <= 0) return 0;
+  cudaLaunchAttribute at[1];
+  if (a.pick_mode != 0) {
+    const cudaLaunchConfig_t cfg = index_config(C, s, at);
+    return launched_one(cudaLaunchKernelEx(&cfg, inorder_index_kernel<true>, a, ix));
+  }
+  const cudaLaunchConfig_t cfg = index_config(C, s, at);
+  return launched_one(cudaLaunchKernelEx(&cfg, inorder_index_kernel<false>, a, ix));
 }
 
 }  // namespace eppscore

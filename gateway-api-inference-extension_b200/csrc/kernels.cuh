@@ -326,6 +326,19 @@ int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count);  
 // cluster shape fits, or -(cudaError_t)
 int inorder_cluster_size(int Mpad);
 int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s);            // one cluster of C CTAs
+// The walk in index order (eppscore_schedule_batch_inorder_index): request r's match counts are read from the index as it
+// stands after requests 0..r-1's commits, and the CTA that owns r's pick commits r's blocks (IndexProgram::commit) before
+// request r + 1 probes.  a.match is unused; a.total holds n_hashes.
+struct InOrderIndexArgs {
+  TableView* tv;
+  LruView* lv;
+  const uint64_t* hashes;   // [R][stride]
+  int32_t stride;
+  const int32_t* cap_req;   // [n_endpoints] CacheNumBlocks or null
+  uint16_t* pick_match;     // [R] the pick's match count as the request was scored, or null
+};
+int inorder_index_cluster_size(int Mpad);  // as inorder_cluster_size, for launch_inorder_index's CTAs of kCommitThreads
+int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s);
 
 // predicted-latency producer's running-request queues (running_kernel.cu).  Table slot: {key, meta}, meta = endpoint + 1
 // (| kRunTomb once removed), {0, 0} empty; tpot[] holds the entry's tpot bits, owner[] / rm[] the (gen << 32 | r) bids of

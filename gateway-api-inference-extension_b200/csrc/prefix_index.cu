@@ -16,96 +16,9 @@
 #include <vector>
 
 #include "../../include/eppscore.h"
+#include "index_device.cuh"
 
 namespace eppscore {
-
-// ---------------------------------------------------------------------------------------------
-// execution policy: CUDA threads of one CTA
-// ---------------------------------------------------------------------------------------------
-struct DevX {
-  template <class F>
-  __device__ __forceinline__ void par(F f) {
-    __syncthreads();  // everything the previous section wrote is visible, every uniform read before this point is done
-    f((int)threadIdx.x);
-    __syncthreads();
-  }
-  // in-place exclusive scan of arr[0..kCommitThreads); returns the total (uniform)
-  __device__ __forceinline__ uint32_t scan(uint32_t* arr, uint32_t* /*unused*/) {
-    __shared__ uint32_t wt[kCommitThreads / 32];
-    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    __syncthreads();
-    const uint32_t v = arr[tid];
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o) inc += t;
-    }
-    if (lane == 31) wt[w] = inc;
-    __syncthreads();
-    uint32_t base = 0, total = 0;
-#pragma unroll
-    for (int i = 0; i < kCommitThreads / 32; i++) {
-      const uint32_t t = wt[i];
-      if (i < w) base += t;
-      total += t;
-    }
-    arr[tid] = base + inc - v;
-    __syncthreads();
-    return total;
-  }
-  // Index structures are read and written at GPU scope (L2), never through a stale L1 line, and every access is a
-  // compiler barrier: the intrinsics (__ldcg) are plain asm statements the compiler may hoist out of a spin loop or CSE
-  // across a lock acquisition — a stale `key` of a slot that another CTA was still creating made a second slot for the
-  // same hash (r2 first GPU run: one member of a 200-endpoint set missing).
-  __device__ __forceinline__ uint32_t ld32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-  }
-  __device__ __forceinline__ uint64_t ld64(const uint64_t* p) {
-    uint64_t v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-  }
-  __device__ __forceinline__ uint32_t ld16(const uint16_t* p) {
-    uint16_t v;
-    asm volatile("ld.relaxed.gpu.global.u16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
-    return v;
-  }
-  __device__ __forceinline__ void st32(uint32_t* p, uint32_t v) { asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-  __device__ __forceinline__ void st64(uint64_t* p, uint64_t v) { asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
-  __device__ __forceinline__ void st16(uint16_t* p, uint16_t v) { asm volatile("st.relaxed.gpu.global.u16 [%0], %1;" ::"l"(p), "h"(v) : "memory"); }
-  __device__ __forceinline__ uint32_t ld_acquire32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-  }
-  __device__ __forceinline__ void st_release32(uint32_t* p, uint32_t v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-  }
-  __device__ __forceinline__ uint32_t cas32(uint32_t* p, uint32_t cmp, uint32_t val) { return atomicCAS(p, cmp, val); }
-  __device__ __forceinline__ uint32_t cas_acquire32(uint32_t* p, uint32_t cmp, uint32_t val) {
-    uint32_t old;
-    asm volatile("atom.acquire.gpu.global.cas.b32 %0, [%1], %2, %3;" : "=r"(old) : "l"(p), "r"(cmp), "r"(val) : "memory");
-    return old;
-  }
-  __device__ __forceinline__ uint64_t cas64(uint64_t* p, uint64_t cmp, uint64_t val) {
-    return atomicCAS(reinterpret_cast<unsigned long long*>(p), (unsigned long long)cmp, (unsigned long long)val);
-  }
-  __device__ __forceinline__ void add64(unsigned long long* p, unsigned long long v) { atomicAdd(p, v); }
-  __device__ __forceinline__ void fence() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-  __device__ __forceinline__ void lock(uint32_t* p) {
-    while (cas_acquire32(p, 0u, 1u) != 0u) {
-    }
-  }
-  __device__ __forceinline__ void unlock(uint32_t* p) { st_release32(p, 0u); }
-  __device__ __forceinline__ uint64_t smem_cas64(uint64_t* p, uint64_t cmp, uint64_t val) {
-    return atomicCAS(reinterpret_cast<unsigned long long*>(p), (unsigned long long)cmp, (unsigned long long)val);
-  }
-  __device__ __forceinline__ void smem_max32(uint32_t* p, uint32_t v) { atomicMax(p, v); }
-  __device__ __forceinline__ void smem_add32(uint32_t* p, uint32_t v) { atomicAdd(p, v); }
-};
 
 // ---------------------------------------------------------------------------------------------
 // kernels
@@ -306,6 +219,26 @@ __global__ void __launch_bounds__(kRoomThreads) index_room_kernel(TableView* tv,
     for (int w = 0; w < kRoomThreads / 32; w++) total += part[w];
     DevX x;
     RoomOps<DevX>::decide(x, tv, total);
+  }
+}
+
+// Σ n_hashes[0..R): the touches a batch that commits as it schedules may make (every request's pick is still unknown).  decide:
+// take the room decision for them (a reserved index), else write the sum to *out.
+__global__ void __launch_bounds__(kRoomThreads) index_room_rows_kernel(TableView* tv, const uint16_t* n_hashes, int32_t R, int decide,
+                                                                       unsigned long long* out) {
+  __shared__ unsigned long long part[kRoomThreads / 32];
+  unsigned long long t = 0;
+  for (int32_t r = threadIdx.x; r < R; r += kRoomThreads) t += n_hashes[r];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned long long total = 0;
+    for (int w = 0; w < kRoomThreads / 32; w++) total += part[w];
+    DevX x;
+    if (decide) RoomOps<DevX>::decide(x, tv, total);
+    else *out = total;
   }
 }
 
@@ -624,6 +557,45 @@ cudaError_t DeviceIndex::commit(int32_t R, int32_t n_picks, const int32_t* const
     IX_CK(snapshot_after(s));
   }
   return cudaSuccess;
+}
+
+cudaError_t DeviceIndex::ordered_begin(const int32_t* cap_req_host, cudaStream_t s, OrderedRefs* out) {
+  uint32_t want = 0;
+  if (cap_req_host)
+    for (int32_t i = 0; i < n_endpoints_; i++) want = std::max(want, (uint32_t)std::max(cap_req_host[i], 0));
+  IX_CK(ensure_lru(want, s));
+  if (want > lv_.max_cap) return cudaErrorInvalidValue;  // the LRU regions were sized for a smaller largest capacity
+  if (cap_req_host) IX_CK(cudaMemcpyAsync(d_capreq_, cap_req_host, (size_t)n_endpoints_ * 4, cudaMemcpyHostToDevice, s));
+  out->tv = d_tv_;
+  out->lv = d_lv_;
+  out->cap_req = cap_req_host ? d_capreq_ : nullptr;
+  return cudaSuccess;
+}
+
+cudaError_t DeviceIndex::ordered_room(int32_t R, const uint16_t* n_hashes, cudaStream_t s) {
+  if (R <= 0) return cudaSuccess;
+  if (reserved_) {  // room decided on the device: nothing here waits on the host
+    index_room_rows_kernel<<<1, kRoomThreads, 0, s>>>(d_tv_, n_hashes, R, 1, nullptr);
+    table_clear_spare_kernel<<<kRebuildCtas, kRebuildThreads, 0, s>>>(d_tv_);
+    table_rebuild_kernel<<<kRebuildCtas, kRebuildThreads, 0, s>>>(d_tv_);
+    launches_ += 3;
+    return cudaGetLastError();
+  }
+  unsigned long long* d_t = reinterpret_cast<unsigned long long*>(d_scratch_);
+  unsigned long long t = 0;
+  index_room_rows_kernel<<<1, kRoomThreads, 0, s>>>(d_tv_, n_hashes, R, 0, d_t);
+  launches_++;
+  IX_CK(cudaMemcpyAsync(&t, d_t, 8, cudaMemcpyDeviceToHost, s));
+  IX_CK(cudaStreamSynchronize(s));
+  return ensure_room(std::max<int64_t>((int64_t)t, 1), s);
+}
+
+cudaError_t DeviceIndex::ordered_end(cudaStream_t s, bool capturing) {
+  if (capturing) {
+    captured_ = true;
+    return cudaSuccess;
+  }
+  return snapshot_after(s);
 }
 
 void DeviceIndex::match(int32_t R, int32_t k, int32_t limit, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,

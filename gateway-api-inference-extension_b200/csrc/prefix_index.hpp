@@ -47,6 +47,22 @@ class DeviceIndex {
   cudaError_t commit(int32_t R, int32_t n_picks, const int32_t* const* picks, const uint64_t* hashes, const uint16_t* n_hashes, int32_t stride,
                      const int32_t* cap_req_host, int32_t single_cap, int32_t ep_first, int32_t n_eps, int64_t max_touches,
                      cudaStream_t s, bool capturing = false);
+  // The index side of a batch that commits as it schedules (eppscore_schedule_batch_inorder_index), all on `s`:
+  //   ordered_begin  before anything is launched: ensures the LRU regions for the largest of cap_req_host (optional
+  //                  [n_endpoints] CacheNumBlocks), stages the capacities and returns what the walk kernel commits through;
+  //   ordered_room   per slice, once its n_hashes are on the device: room for Σ n_hashes[0..R) touches.  A reserved index
+  //                  decides it on the device (RoomOps: proceed, rebuild or skip the slice's commits whole); an unreserved one
+  //                  reads the sum back (synchronous) and grows on the host as a commit does;
+  //   ordered_end    after each slice's walk: the counters' copy-back the next slice's room reads, or (inside a capture) marks
+  //                  the index captured.
+  struct OrderedRefs {
+    TableView* tv;
+    LruView* lv;
+    const int32_t* cap_req;  // device [n_endpoints] or null
+  };
+  cudaError_t ordered_begin(const int32_t* cap_req_host, cudaStream_t s, OrderedRefs* out);
+  cudaError_t ordered_room(int32_t R, const uint16_t* n_hashes, cudaStream_t s);
+  cudaError_t ordered_end(cudaStream_t s, bool capturing);
   // matchLongestPrefix of R requests (device arrays, R >= 1) read at k endpoints each: out[r*k + j] = the hit blocks before
   // request r's first miss whose set holds endpoints[r*k + j]; 0 for entries outside [0, limit).  One launch of a fixed shape,
   // async on `s`; reads the index through its descriptor.

@@ -854,18 +854,31 @@ PT_HD TSlot* table_find(X& x, const TableView* tv, uint64_t h, uint32_t* raw) {
   return hit;
 }
 
-// Whether endpoint p is in the set of a slot table_find returned: a compare against the inline members, or bit p of the row.
-template <class X>
-PT_HD bool slot_holds(X& x, const TableView* tv, TSlot* s, uint32_t raw, uint32_t p) {
+// The membership rule of a set given its cnt word `raw`: a compare against the inline members (member(k) = ep[k]), or bit p of
+// the row (row() = its id).  slot_holds reads them from the slot, staged_holds from a copy of the slot's ep words.
+template <class X, class Row, class Member>
+PT_HD bool set_holds(X& x, const TableView* tv, uint32_t raw, uint32_t p, Row row, Member member) {
   if (raw & kCntRow) {
     if ((p >> 5) >= tv->row_words) return false;
-    const uint32_t r = x.ld32(slot_row_id(s));
+    const uint32_t r = row();
     return (x.ld32(&tv->ovf_rows[(size_t)r * tv->row_words + (p >> 5)]) >> (p & 31)) & 1u;
   }
   const uint32_t c = raw & kCntMask;
   for (uint32_t k = 0; k < c; k++)
-    if (x.ld16(&s->ep[k]) == p) return true;
+    if (member(k) == p) return true;
   return false;
+}
+// Whether endpoint p is in the set of a slot table_find returned.
+template <class X>
+PT_HD bool slot_holds(X& x, const TableView* tv, TSlot* s, uint32_t raw, uint32_t p) {
+  return set_holds(x, tv, raw, p, [&] { return x.ld32(slot_row_id(s)); }, [&](uint32_t k) { return x.ld16(&s->ep[k]); });
+}
+// The same for a slot whose ep[0..kInlineEps) were copied as kInlineEps / 2 words (ep[2i] | ep[2i+1] << 16, as the slot holds
+// them; in row mode word 0 is the row id).
+template <class X>
+PT_HD bool staged_holds(X& x, const TableView* tv, uint32_t raw, const uint32_t* ep_words, uint32_t p) {
+  return set_holds(x, tv, raw, p, [&] { return ep_words[0]; },
+                   [&](uint32_t k) { return (ep_words[k >> 1] >> ((k & 1) * 16)) & 0xFFFFu; });
 }
 
 // indexer.Get (indexer.go:86-102) for one hash, read-only: writes the set as a natural-order bitset, returns its size.

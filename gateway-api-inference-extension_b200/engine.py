@@ -184,7 +184,10 @@ class Engine:
         call, topk = ((self._lib.eppscore_schedule_batch_topk_wide, topk_wide) if topk_wide else
                       (self._lib.eppscore_schedule_batch_topk, topk))
         a = _Args(device)
-        if _inorder is not None:  # schedule_inorder: (tokens,)
+        if _inorder is not None and len(_inorder) > 1:  # schedule_inorder_index: (tokens, InOrderIndex)
+            tok, ix = a.ptr(_inorder[0], np.int64), _inorder[1]
+            call = lambda h, bp: self._lib.eppscore_schedule_batch_inorder_index(h, bp, tok, C.byref(ix))
+        elif _inorder is not None:  # schedule_inorder: (tokens,)
             tok = a.ptr(_inorder[0], np.int64)
             call = lambda h, bp: self._lib.eppscore_schedule_batch_inorder(h, bp, tok)
         else:
@@ -266,6 +269,30 @@ class Engine:
             if kw.get(k):
                 raise ValueError(f"schedule_inorder does not take {k}")
         return self.schedule(R, _inorder=(tokens,), **kw)
+
+    def schedule_inorder_index(self, R, tokens=None, lru_capacity=None, **kw):
+        """eppscore_schedule_batch_inorder_index: `schedule_inorder` with request r also scored against the prefix index as
+        requests 0..r-1's commits left it, and each request's blocks committed at its pick inside the call (do not commit the
+        batch again).  lru_capacity: host int32[M] CacheNumBlocks or None.  Host mode returns the `schedule_inorder` dict plus
+        pick_match uint16[R] (matchBlocks at each pick before its own Add); device mode fills `out` asynchronously on `stream`,
+        pick_match included when `out` has it."""
+        for k in ("want_match", "want_scores", "want_pred", "want_filter_mask", "topk", "topk_wide"):
+            if kw.get(k):
+                raise ValueError(f"schedule_inorder_index does not take {k}")
+        x = capi.InOrderIndex()
+        x.struct_size = C.sizeof(capi.InOrderIndex)
+        caps = None if lru_capacity is None else np.ascontiguousarray(lru_capacity, np.int32)
+        x.lru_capacity = None if caps is None else caps.ctypes.data
+        if kw.get("device"):
+            out = kw.get("out") or {}
+            pm = out.get("pick_match")
+            x.pick_match = None if pm is None else _Args(True).ptr(pm, None)
+            return self.schedule(R, _inorder=(tokens, x), **kw)
+        pick_match = np.zeros(R, np.uint16)
+        x.pick_match = pick_match.ctypes.data
+        res = self.schedule(R, _inorder=(tokens, x), **kw)
+        res["pick_match"] = pick_match
+        return res
 
     # ------------------------------------------------------------------ several scheduler profiles
     def add_profile(self, scorers, pick_mode=0, filters=()) -> int:

@@ -146,6 +146,11 @@ struct PrefixIndexerHistograms {
 extern "C" int32_t eppscore_schedule_batch_inorder(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens)
     __attribute__((weak));
 inline bool EngineHasInOrderLoad() { return &eppscore_schedule_batch_inorder != nullptr; }
+// eppscore_schedule_batch_inorder_index (the same, ordered against the prefix index too) likewise: EngineHasInOrderPrefixIndex()
+// tells.  Without it a config with SchedulerConfig::InOrderPrefixIndex is refused when the Scheduler is built.
+extern "C" int32_t eppscore_schedule_batch_inorder_index(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                                         const eppscore_inorder_index* x) __attribute__((weak));
+inline bool EngineHasInOrderPrefixIndex() { return &eppscore_schedule_batch_inorder_index != nullptr; }
 
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
@@ -362,6 +367,15 @@ struct SchedulerConfig {
   // sequence.  Refused with a latency scorer, with the Profiles list, with MaxNumOfEndpoints > 1, without InFlightLoad and with
   // an engine library without the call.
   bool InOrderInFlightLoad = false;
+  // Opt-in (off by default), with InOrderInFlightLoad and the approximate-prefix producer (prefix hashing on): every engine batch
+  // goes through eppscore_schedule_batch_inorder_index, so request r is also scored against the prefix index as requests
+  // 0..r-1's Adds left it (approximateprefix/plugin.go:169-197 before :219-235), and each request's blocks are added at its
+  // pick inside the call, with LruCapacities().  PreRequest then does not commit that batch again, and with PrefixMatchInfo the
+  // target's PrefixCacheMatchInfo is the pick's match as the request was scored, before its own Add (plugin.go:199-204).  A
+  // batch cut into LoRA pieces runs its pieces in order, each committing before the next is scheduled.  Refused with
+  // LatencyPredictionInfo (eppscore_predict_latency after the batch would read the index the batch left), without
+  // InOrderInFlightLoad or prefix hashing, and with an engine library without the call.
+  bool InOrderPrefixIndex = false;
 };
 
 class Scheduler {
@@ -464,7 +478,7 @@ class Scheduler {
       throw SchedulingError("maxNumOfEndpoints > 1 with a stochastic picker needs an engine library with eppscore_schedule_batch_topk");
     if (cfg.InFlightLoad && !EngineHasInFlightLoad())
       throw SchedulingError("the inflight-load-producer needs an engine library with eppscore_inflight_add");
-    if (cfg.PrefixMatchInfo && !EngineHasPrefixMatch())
+    if (cfg.PrefixMatchInfo && !cfg0.InOrderPrefixIndex && !EngineHasPrefixMatch())  // (in order: the call returns the match)
       throw SchedulingError("SchedulerConfig::PrefixMatchInfo needs an engine library with eppscore_prefix_match");
     if (cfg.LatencyPredictionInfo && !EngineHasPredictLatency())
       throw SchedulingError("SchedulerConfig::LatencyPredictionInfo needs an engine library with eppscore_predict_latency");
@@ -479,6 +493,16 @@ class Scheduler {
       if (!EngineHasInOrderLoad())
         throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs an engine library with eppscore_schedule_batch_inorder");
       inorder_ = true;
+    }
+    if (cfg0.InOrderPrefixIndex) {
+      if (!cfg0.InOrderInFlightLoad) throw SchedulingError("SchedulerConfig::InOrderPrefixIndex needs InOrderInFlightLoad");
+      if (!Geometry({}).want_prefix) throw SchedulingError("SchedulerConfig::InOrderPrefixIndex needs the approximate-prefix producer (prefix hashing)");
+      if (cfg.LatencyPredictionInfo)
+        throw SchedulingError("SchedulerConfig::InOrderPrefixIndex cannot give LatencyPredictionInfo: the prediction would read the "
+                              "prefix index the batch left");
+      if (!EngineHasInOrderPrefixIndex())
+        throw SchedulingError("SchedulerConfig::InOrderPrefixIndex needs an engine library with eppscore_schedule_batch_inorder_index");
+      inorder_index_ = true;
     }
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
@@ -795,6 +819,7 @@ class Scheduler {
     const bool engine_topk = (topk > 1 && topk <= EPPSCORE_MAX_TOPK && EngineHasTopK()) || engine_wide;
     const int klist = engine_wide ? std::min(topk, cfg_.MaxEndpoints) : topk;  // entries past max_endpoints would all be -1
     std::vector<double> all_scores;
+    std::vector<uint16_t> pick_match;  // InOrderPrefixIndex: matchBlocks at each pick before its own Add
     std::vector<int32_t> topk_ids;
     std::vector<double> topk_scores;
     if (engine_topk) {  // the picker's first k endpoints, ordered on the device (eppscore_topk)
@@ -812,7 +837,19 @@ class Scheduler {
         all_scores.resize((size_t)R * Mx);
         b.scores_out = all_scores.data();
       }
-      if (inorder_) {  // the estimates go in with the batch: the call adds each pick's load in request order
+      if (inorder_index_) {  // ... and each pick's blocks, in request order: PreRequest commits nothing more
+        const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
+        last_endpoints_ = &endpoints;  // (LruCapacities reads the batch's list)
+        last_ids_ = ids;
+        last_rows_ = Mx;
+        const std::vector<int32_t> caps = LruCapacities();
+        pick_match.assign((size_t)R, 0);
+        eppscore_inorder_index x{};
+        x.struct_size = sizeof(x);
+        x.lru_capacity = caps.data();
+        x.pick_match = pick_match.data();
+        Check(eppscore_schedule_batch_inorder_index(eng_, &b, est.data(), &x), "eppscore_schedule_batch_inorder_index");
+      } else if (inorder_) {  // the estimates go in with the batch: the call adds each pick's load in request order
         const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
         Check(eppscore_schedule_batch_inorder(eng_, &b, est.data()), "eppscore_schedule_batch_inorder");
       } else {
@@ -847,7 +884,13 @@ class Scheduler {
         }
       }
     }
-    if (cfg_.LatencyPredictionInfo || cfg_.PrefixMatchInfo) {
+    if (inorder_index_ && cfg_.PrefixMatchInfo && g.want_prefix) {  // the target is the only entry (MaxNumOfEndpoints 1)
+      if (g.block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+      for (int r = 0; r < R; r++)
+        if (out[r].error.empty())
+          out[r].result.ProfileResults[cfg_.ProfileName].TargetEndpoints[0].PrefixMatch =
+              PrefixCacheMatchInfo{pick_match[(size_t)r], last_.nh[(size_t)r], (uint16_t)g.block_tokens};
+    } else if (cfg_.LatencyPredictionInfo || cfg_.PrefixMatchInfo) {
       TargetRuns runs((size_t)R);
       for (int r = 0; r < R; r++)
         if (out[r].error.empty()) runs[(size_t)r].emplace_back(cfg_.ProfileName, &out[r].result.ProfileResults[cfg_.ProfileName]);
@@ -859,9 +902,10 @@ class Scheduler {
   }
 
  public:
-  // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index; with the
-  // inflight-load-producer also counts every scheduled request, with its estimated tokens, on its TargetEndpoints[0]
-  // (inflightload/producer.go:101-120), unless InOrderInFlightLoad counted it while scheduling.
+  // PreRequest for the last ScheduleBatch (approximateprefix/plugin.go:169-197): records the picks in the index, unless
+  // InOrderPrefixIndex recorded them while scheduling; with the inflight-load-producer also counts every scheduled request, with
+  // its estimated tokens, on its TargetEndpoints[0] (inflightload/producer.go:101-120), unless InOrderInFlightLoad counted it
+  // while scheduling.
   void PreRequest(const std::vector<BatchItem>& results) {
     RecordPrefixCacheMatch(results);
     RecordDispatch(results);
@@ -871,7 +915,7 @@ class Scheduler {
     std::vector<int32_t> pick((size_t)R, -1);
     for (int r = 0; r < R; r++)
       if (results[r].error.empty()) pick[r] = last_ids_[(size_t)results[r].result.ProfileResults.at(cfg_.ProfileName).TargetEndpoints[0].Index];
-    if (!last_.hashes.empty())
+    if (!last_.hashes.empty() && !inorder_index_)  // (in order against the index: ScheduleBatch committed the batch already)
       Check(eppscore_commit_picks(eng_, R, pick.data(), last_.hashes.data(), last_.nh.data(), last_.stride, LruCapacities().data()),
             "eppscore_commit_picks");
     if (inflight_ && !inorder_ && (int)last_.size.size() == R) {  // (in order: ScheduleBatch added the load already)
@@ -1700,6 +1744,7 @@ class Scheduler {
   bool inflight_ = false;    // SchedulerConfig::InFlightLoad
   bool token_load_ = false;  // the profile has a token-load scorer
   bool inorder_ = false;     // SchedulerConfig::InOrderInFlightLoad
+  bool inorder_index_ = false;  // SchedulerConfig::InOrderPrefixIndex
   bool running_ = false;  // PredictedLatencyProducer::TrackRunningRequests
   std::unordered_map<std::string, KeyUse> running_keys_;
   uint64_t next_key_ = 1;

@@ -366,12 +366,53 @@ int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppsc
  * its provisional picks are overwritten), which a match-only pre-pass could avoid; today the in-order walk dominates.  The
  * cluster shape is decided by the engine's first call, before anything is launched: ERR_CAPACITY when no cluster of the device
  * holds max_endpoints endpoints (8192 needs the non-portable cluster size 16).
- * Not ordered: the prefix index (request r+1 does not see the blocks request r adds; commit after the call), the latency
- * scorer's running queues, top-k lists, several profiles, and requests on other GPU shards (each engine orders its own batch).
+ * Not ordered: the prefix index (request r+1 does not see the blocks request r adds; commit after the call, or use
+ * eppscore_schedule_batch_inorder_index), the latency scorer's running queues, top-k lists, several profiles, and requests on
+ * other GPU shards (each engine orders its own batch).
  * ERR_INVALID before anything is launched: a profile 0 with the latency scorer, a current snapshot that supplies
  * inflight_tokens, dense_feat / scores_out / match_blocks / pred_out / filter_mask_out set, and what eppscore_schedule_batch
  * refuses.  ERR_NO_SNAPSHOT before eppscore_set_snapshot. */
 int32_t eppscore_schedule_batch_inorder(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens);
+
+/* The index side of eppscore_schedule_batch_inorder_index. */
+typedef struct eppscore_inorder_index {
+  int32_t struct_size;          /* sizeof(eppscore_inorder_index) */
+  const int32_t *lru_capacity;  /* HOST [M] CacheNumBlocks per endpoint (autotune), NULL/<=0 = default; NULL under capture */
+  uint16_t *pick_match;         /* optional [R], where b->location says: matchBlocks of pick[r] as request r was scored */
+} eppscore_inorder_index;
+
+/* A batch in arrival order against the in-flight load AND the prefix index: the outputs (pick, pick_score, tie_count,
+ * total_blocks, hashes_out, x->pick_match), the in-flight counters and the whole prefix index afterwards (every LRU's keys oldest
+ * -> newest, every set, len(hashToPods)) equal, bit for bit, what this loop gives:
+ *     for r in 0 .. R-1:
+ *         eppscore_schedule_batch(request r alone, request_base = b->request_base + r, hashes_out)
+ *         pick_match[r] = eppscore_prefix_match(request r's hashes, at pick[r])     (before its own Add)
+ *         eppscore_inflight_add(1, &pick[r], &tokens[r])
+ *         eppscore_commit_picks(1, &pick[r], hashes[r], n_hashes[r], x->lru_capacity)
+ * so request r's prefix scorer sees the blocks requests 0..r-1 were sent with, as R consecutive Schedule + PreRequest calls of
+ * the reference do (approximateprefix/plugin.go:169-204): a window of requests sharing a new prefix follows the first of them.
+ * pick_match is PrefixCacheMatchInfo.matchBlocks at the target as the reference records it; an eppscore_prefix_match after the
+ * call would see the batch's own Adds.  A request with pick -1 adds nothing anywhere.
+ * Scope, validation, the cluster-shape decision and the first-call-outside-capture rule are those of
+ * eppscore_schedule_batch_inorder (the walk runs in CTAs of 512 threads, one endpoint per thread).  The call is also an index
+ * mutation, waited for and ordered like eppscore_commit_picks_device: it reports an earlier skipped mutation (ERR_CAPACITY), it
+ * refuses an unreserved index and a non-NULL lru_capacity under capture, and it ensures the LRU regions before anything is
+ * launched.  Device arrays run on b->stream; later readers and index mutations on other streams are ordered after it.
+ * Room is decided once per slice of rows (the slices of eppscore_schedule_batch_inorder), before that slice's walk, for the
+ * slice's sum of n_hashes.  An unreserved index grows on the host as a commit does (a synchronous read of the sum).  On a reserved
+ * index the decision runs on the device and may rebuild in place; a slice that finds no room is walked WITHOUT commits, all or
+ * nothing as a commit is: its outputs equal eppscore_schedule_batch_inorder's on the frozen index, the index stays
+ * bit-identical, stats.index_error bit 4 and the skip counter are set, and the next index call reports it.
+ * Per slice: the hash stage (no R x M match route), the candidates' min / max, the room, then one thread-block cluster walks the
+ * requests in order: each request's blocks are probed up to the first miss, every endpoint's thread counts the hit blocks whose
+ * set holds it, the request is scored and picked as in eppscore_schedule_batch_inorder, and the CTA that owns the pick runs the
+ * index's commit program for that one Add before the cluster barrier that the next request's probes wait for.
+ * Not covered: several picks per request (the "prefill" profile's Add), several profiles and top-k lists, the latency scorer's
+ * running queues, and replication across GPU shards (each engine commits its own batch inside the call; replaying an
+ * all-gathered commit stream on top would apply its commits twice, so sharding.gather_commit_stream belongs to the
+ * batch-wide path).  ERR_INVALID: x NULL or a wrong struct_size, and what eppscore_schedule_batch_inorder refuses. */
+int32_t eppscore_schedule_batch_inorder_index(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens,
+                                              const eppscore_inorder_index *x);
 
 /* ---- several scheduler profiles (see eppscore_profile) ---- */
 /* Adds a profile; *id_out receives its id (1, 2, ...).  With a snapshot present the profile is prepared for it at once, on the
