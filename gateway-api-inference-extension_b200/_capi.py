@@ -85,6 +85,10 @@ class InOrderIndex(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("lru_capacity", C.c_void_p), ("pick_match", C.c_void_p)]
 
 
+class InOrderRunning(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("request_key", C.c_void_p), ("added_out", C.c_void_p)]
+
+
 class TopK(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("k", C.c_int32), ("endpoints", C.c_void_p), ("scores", C.c_void_p)]
 
@@ -121,6 +125,8 @@ ABI_SYMBOLS = [
     ("eppscore_schedule_batch_topk_wide", C.c_int32, [_P, C.POINTER(Batch), C.POINTER(TopK)]),
     ("eppscore_schedule_batch_inorder", C.c_int32, [_P, C.POINTER(Batch), _P]),
     ("eppscore_schedule_batch_inorder_index", C.c_int32, [_P, C.POINTER(Batch), _P, C.POINTER(InOrderIndex)]),
+    ("eppscore_schedule_batch_inorder_latency", C.c_int32, [_P, C.POINTER(Batch), _P, C.POINTER(InOrderIndex),
+                                                            C.POINTER(InOrderRunning)]),
     ("eppscore_add_profile", C.c_int32, [_P, C.POINTER(Profile), C.POINTER(C.c_int32)]),
     ("eppscore_set_profile_endpoints", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_schedule_batch_profiles", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun)]),

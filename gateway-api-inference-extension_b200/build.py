@@ -20,7 +20,7 @@ PART_SOURCES = [("score_matrix.cu", f"score_matrix_p{k}.o", [f"-DEPP_MATRIX_PART
 # host-only C++ compiled by g++ directly (AVX-512 intrinsics: kept away from nvcc's front end); the ISA flags apply to this
 # file alone and its one entry point is only called after a run-time CPU check (host_path.cu)
 CPP_SOURCES = [("host_hash_simd.cpp", ["-mavx512f", "-mavx512dq"])]
-HEADERS = ["kernels.cuh", "device_common.cuh", "xxh64.cuh", "prefix_index.hpp", "prefix_table.cuh", "index_device.cuh", "cuda_owners.hpp", "lat_pair.cuh",
+HEADERS = ["kernels.cuh", "device_common.cuh", "xxh64.cuh", "prefix_index.hpp", "prefix_table.cuh", "index_device.cuh", "cuda_owners.hpp", "lat_pair.cuh", "running_slot.cuh",
            os.path.join("..", "..", "include", "eppscore.h")]
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -143,7 +143,8 @@ struct eppscore_engine {
         // an in-order batch's slice (schedule_inorder): match rows, totals and candidate min / max.  Allocated by the first call
         // outside a capture for a fixed number of rows and never reallocated, like `wide`.
         s_io_match, s_io_total, s_io_minmax,
-        s_pmatch;  // pick_match of an in-order batch that commits as it schedules
+        s_pmatch,  // pick_match of an in-order batch that commits as it schedules
+        s_rkey, s_added;  // request keys and added_out of an in-order batch that adds to the running-request queues
     int32_t io_rows = 0;
     // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide).  Allocated by the first call that
     // needs them and never reallocated, so a graph captured after that call keeps pointing at live memory.
@@ -167,6 +168,7 @@ struct eppscore_engine {
   int32_t wide_rows = 0;
   int32_t io_cluster = 0;          // CTAs per cluster of inorder_pick_kernel (0: not decided yet)
   int32_t io_index_cluster = 0;    // CTAs per cluster of inorder_index_kernel (0: not decided yet)
+  int32_t io_lat_cluster = 0, io_lat_index_cluster = 0;  // the same for their latency forms (the _lat kernels)
   int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
@@ -460,6 +462,8 @@ struct DevBatch {  // all device pointers
   uint16_t* total_blocks;
   uint64_t* hashes_out;
   uint16_t* pick_match;     // [R] an in-order batch's matchBlocks at each pick (schedule_inorder_index)
+  const uint64_t* request_key;  // [R] an in-order latency batch's running-request keys (eppscore_inorder_running)
+  uint8_t* added_out;       // [R] its added flags
   int32_t n_runs;
   DevRun run[EPPSCORE_MAX_PROFILES];
 };
@@ -507,6 +511,8 @@ void for_each_row_array(DevBatch& d, size_t M, F&& f) {
   f(d.total_blocks, 1, Rows::small, &Scratch::s_total);
   f(d.hashes_out, (size_t)d.max_blocks, Rows::out, &Scratch::s_hashes);  // (a host batch never has hashes_in with it)
   f(d.pick_match, 1, Rows::small, &Scratch::s_pmatch);
+  f(d.request_key, 1, Rows::in, &Scratch::s_rkey);
+  f(d.added_out, 1, Rows::small, &Scratch::s_added);
 }
 
 // Rows [base, base + n) of a batch.
@@ -1578,6 +1584,8 @@ InOrderArgs inorder_args(eppscore_engine* e, bool* minmax) {
     a.term[i] = static_term ? P.term[i].as<double>() : nullptr;
     for (int q = 0; q < 4; q++) a.lora_term[i][q] = clamp01_host(cls_score[q]) * c.scorer_weight[i];
     *minmax = *minmax || k == EPPSCORE_SCORER_QUEUE || k == EPPSCORE_SCORER_RUNNING;
+    // the latency scorer's composite fallback: maxQ over the candidates is the queue maximum (plugin.go:338-344)
+    *minmax = *minmax || (k == EPPSCORE_SCORER_LATENCY && !e->lat_args.has_predictions);
   }
   a.pick_mode = c.pick_mode;
   a.tie_mode = c.tie_mode;
@@ -1593,6 +1601,23 @@ InOrderArgs inorder_args(eppscore_engine* e, bool* minmax) {
   a.inflight_tok = e->inflight_tok.as<int64_t>();
   return a;
 }
+// The latency form's arguments (eppscore_schedule_batch_inorder_latency): the snapshot's fold-in and the running-request queues.
+InOrderLatArgs inorder_lat_args(eppscore_engine* e) {
+  InOrderLatArgs lt{};
+  lt.lat = e->lat_args;
+  lt.run = e->run_desc.as<RunDev>();
+  lt.n_ep = e->cfg.max_endpoints;
+  return lt;
+}
+// A slice's per-request inputs of the latency form; `fields`: its device-counted input tokens when the batch supplies none.
+void inorder_lat_slice(InOrderLatArgs& lt, const DevBatch& q, const int32_t* fields) {
+  lt.lat.input_tokens = q.input_tokens ? q.input_tokens : fields;
+  lt.lat.ttft_slo = q.ttft_slo;
+  lt.lat.tpot_slo = q.tpot_slo;
+  lt.request_key = q.request_key;
+  lt.added_out = q.added_out;
+}
+
 // A slice's per-request arguments of the walk.
 void inorder_slice(InOrderArgs& a, const DevBatch& q) {
   a.R = q.R;
@@ -1609,8 +1634,9 @@ void inorder_slice(InOrderArgs& a, const DevBatch& q) {
 // schedule_device with their match_out route (the prefix match counts and totals, which depend on no load; their provisional
 // picks are overwritten), the candidates' queue / running min / max when the profile has those scorers, then
 // inorder_pick_kernel, which reads the in-flight counters, walks the slice's requests in order and writes the counters back,
-// so the next slice continues from them.
-int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc) {
+// so the next slice continues from them.  lat: the latency form (inorder_pick_lat_kernel), whose input token counts are those
+// schedule_device counted into sc.s_fields when the batch supplies none.
+int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, bool lat) {
   if (!sc.s_io_match.p) {
     if (is_capturing(s))
       return fail(e, EPPSCORE_ERR_CAPACITY,
@@ -1625,6 +1651,7 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
   }
   bool minmax = false;
   InOrderArgs a = inorder_args(e, &minmax);
+  InOrderLatArgs lt = inorder_lat_args(e);
   for (int32_t base = 0; base < d.R; base += sc.io_rows) {
     DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
     q.match_blocks = sc.s_io_match.as<uint16_t>();
@@ -1636,7 +1663,8 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
     a.total = q.total_blocks;
     a.minmax = minmax ? sc.s_io_minmax.as<long long>() : nullptr;
     if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
-    const int launched = launch_inorder_pick(a, e->io_cluster, s);
+    inorder_lat_slice(lt, q, q.prompt_bytes && q.prompt_off ? sc.s_fields.as<int32_t>() : nullptr);
+    const int launched = lat ? launch_inorder_pick(a, e->io_lat_cluster, s, &lt) : launch_inorder_pick(a, e->io_cluster, s);
     if (launched < 0) {
       cudaGetLastError();
       return cuda_fail(e, (cudaError_t)-launched, "inorder_pick_kernel launch");
@@ -1652,9 +1680,10 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
 // the same rows).  Per slice: the hash stage in its plain form (hashes and totals into the scratch, or the caller's hashes_out
 // / total_blocks; supplied hashes are read where they are), the candidates' min / max, the room for the slice's Σ n_hashes
 // (DeviceIndex::ordered_room), then inorder_index_kernel, which reads each request's match counts from the index as it stands
-// and commits the request's blocks at its pick before the next request probes.
+// and commits the request's blocks at its pick before the next request probes.  lat: the latency form (inorder_index_lat_kernel),
+// which counts the input tokens of the prompt bytes itself when the batch supplies none.
 int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, const DeviceIndex::OrderedRefs& refs,
-                               bool capturing) {
+                               bool capturing, bool lat) {
   const int32_t mb = d.max_blocks;
   const bool hashing = !d.hashes_in && d.prompt_bytes;
   if (hashing && mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
@@ -1679,8 +1708,15 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
   }
   bool wait_snapshot = false;
   if (int32_t rc = reader_begin(e, s, nullptr, &wait_snapshot); rc != EPPSCORE_OK) return rc;
+  const bool count = lat && !d.input_tokens && d.prompt_bytes && d.prompt_off;
+  if (count && (size_t)std::min(sc.io_rows, d.R) * 4 > sc.s_fields.bytes) {
+    if (capturing) return fail(e, EPPSCORE_ERR_CAPACITY, "schedule_batch_inorder_latency under CUDA-graph capture: the input-token "
+                                                         "scratch is smaller than this batch needs (make the same call outside the capture first)");
+    CK(e, sc.s_fields.reserve((size_t)std::min(sc.io_rows, d.R) * 4));
+  }
   bool minmax = false;
   InOrderArgs a = inorder_args(e, &minmax);
+  InOrderLatArgs lt = inorder_lat_args(e);
   InOrderIndexArgs ix{};
   ix.tv = refs.tv;
   ix.lv = refs.lv;
@@ -1714,6 +1750,9 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
       ix.stride = 1;
     }
     CK(e, cudaGetLastError());
+    if (count)
+      e->launches += launch_count_fields(q.prompt_bytes, q.prompt_off, q.prompt_len, q.R, sc.s_fields.as<int32_t>(), s, e->sm_count);
+    inorder_lat_slice(lt, q, count ? sc.s_fields.as<int32_t>() : nullptr);
     inorder_slice(a, q);
     a.match = nullptr;
     a.total = total;
@@ -1722,7 +1761,7 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
     if (wait_snapshot && base == 0) CK(e, cudaStreamWaitEvent(s, e->ev_snapshot, 0));
     if (minmax) e->launches += launch_inorder_minmax(a, s, e->sm_count);
     if (int32_t rc = index_status(e, e->index->ordered_room(q.R, total, s), "schedule_batch_inorder_index"); rc != EPPSCORE_OK) return rc;
-    const int launched = launch_inorder_index(a, ix, e->io_index_cluster, s);
+    const int launched = lat ? launch_inorder_index(a, ix, e->io_lat_index_cluster, s, &lt) : launch_inorder_index(a, ix, e->io_index_cluster, s);
     if (launched < 0) {
       cudaGetLastError();
       return cuda_fail(e, (cudaError_t)-launched, "inorder_index_kernel launch");
@@ -1734,13 +1773,19 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
   return EPPSCORE_OK;
 }
 
-// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk, _inorder, _inorder_index): the runs (profile + per-profile
-// filter result and outputs) of one batch, as make_batch takes them.  `inorder`: the batch's single run is scheduled in arrival
-// order against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates; with `ordered` also against
-// the prefix index, committing as it goes (schedule_inorder_index), with pick_match [R] (optional) its output.
+int32_t run_make_room(eppscore_engine* e, cudaStream_t st, int64_t R, bool capturing);
+int32_t run_copy_back(eppscore_engine* e, cudaStream_t st, bool capturing);
+int32_t count_reads_wait(eppscore_engine* e, cudaStream_t st);
+
+// eppscore_schedule_batch(_topk, _topk_wide, _profiles, _profiles_topk, _inorder, _inorder_index, _inorder_latency): the runs
+// (profile + per-profile filter result and outputs) of one batch, as make_batch takes them.  `inorder`: the batch's single run is
+// scheduled in arrival order against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates; with
+// `ordered` also against the prefix index, committing as it goes (schedule_inorder_index), with pick_match [R] (optional) its
+// output; with `running` also with the latency scorer against the running-request queues, adding as it goes when it has keys.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
                        const eppscore_topk* topk, bool wide = false, bool inorder = false, const int64_t* tokens = nullptr,
-                       const DeviceIndex::OrderedRefs* ordered = nullptr, uint16_t* pick_match = nullptr) {
+                       const DeviceIndex::OrderedRefs* ordered = nullptr, uint16_t* pick_match = nullptr,
+                       const eppscore_inorder_running* running = nullptr) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
@@ -1748,17 +1793,32 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   DevBatch d = make_batch(e, *b, n_runs, runs, topk, wide);
   d.tokens = tokens;
   d.pick_match = pick_match;
+  d.request_key = running ? running->request_key : nullptr;
+  d.added_out = running ? running->added_out : nullptr;
   const size_t M = (size_t)e->M;
   bool any_wide = false;
   for (int i = 0; i < n_runs; i++) any_wide = any_wide || d.run[i].wide;
   // What one piece of the batch runs on `st` with scratch set `sc`.  The in-order step reads and writes the in-flight counters,
-  // so it is ordered as a producer mutation.
+  // so it is ordered as a producer mutation; with request keys it also adds to the running-request queues, with the room for
+  // its R adds made once, before the walk (run_make_room and the pre-add compaction of eppscore_running_add), and the view
+  // published behind it.
   auto step = [&](const DevBatch& x, cudaStream_t st, Scratch& sc) -> int32_t {
     if (!inorder) return any_wide ? schedule_wide(e, x, st, sc) : schedule_device(e, x, st, sc);
+    const bool adds = x.request_key != nullptr;
     bool capturing = false;
     int32_t rc = producer_begin(e, st, &capturing);
-    if (rc == EPPSCORE_OK) rc = ordered ? schedule_inorder_index(e, x, st, sc, *ordered, capturing) : schedule_inorder(e, x, st, sc);
-    if (rc == EPPSCORE_OK) rc = producer_end(e, st, capturing, counters_feed_scorer(e));
+    if (rc == EPPSCORE_OK && adds && !capturing) rc = count_reads_wait(e, st);
+    if (rc == EPPSCORE_OK && adds) rc = run_make_room(e, st, x.R, capturing);
+    if (rc != EPPSCORE_OK) return rc;
+    if (adds) e->launches += launch_running_compact(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, x.R, e->sm_count, st);
+    rc = ordered ? schedule_inorder_index(e, x, st, sc, *ordered, capturing, running != nullptr)
+                 : schedule_inorder(e, x, st, sc, running != nullptr);
+    if (rc == EPPSCORE_OK && adds) {
+      e->launches += launch_running_finalize(e->run_desc.as<RunDev>(), e->cfg.max_endpoints, st);
+      e->run_bound_live += x.R;
+      rc = run_copy_back(e, st, capturing);
+    }
+    if (rc == EPPSCORE_OK) rc = producer_end(e, st, capturing, counters_feed_scorer(e) | (adds ? running_feeds_scorer(e) : 0u));
     return rc;
   };
   if (b->location == 1) {
@@ -1833,14 +1893,15 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   // one is aligned, and `results` lists the copies from there to the caller.
   DevBatch pinned = d;
   std::vector<Copy> results, d2h;
-  size_t h_end[9] = {};  // by element size: the end of the 8-byte arrays, then of the 4- and 2-byte ones
+  size_t h_end[9] = {};  // by element size: the end of the 8-byte arrays, then of the 4-, 2- and 1-byte ones
   auto via_pinned = [](auto* p, Rows kind) { return p && (kind == Rows::small || kind == Rows::result); };
   for_each_row_array(pinned, M, [&](auto*& p, size_t per, Rows kind, auto) {
     if (via_pinned(p, kind)) h_end[sizeof *p] += (size_t)b->R * per * sizeof *p;
   });
   h_end[4] += h_end[8];
   h_end[2] += h_end[4];
-  CK(e, e->h_res.reserve(h_end[2]));
+  h_end[1] += h_end[2];
+  CK(e, e->h_res.reserve(h_end[1]));
   for_each_row_array(pinned, M, [&](auto*& p, size_t per, Rows kind, auto) {
     if (!via_pinned(p, kind)) return;
     const size_t bytes = (size_t)b->R * per * sizeof *p;
@@ -1928,15 +1989,21 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, const eppsco
   return schedule_batch(e, b, 1, nullptr, t, wide);
 }
 
-// What both in-order calls refuse, and the cluster shape of their walk (decided once per engine, before the first call launches
-// anything).  *done: nothing to run (R == 0).
-int32_t inorder_prologue(eppscore_engine* e, const eppscore_batch* b, const char* what, bool index, bool* done) {
+// What the in-order calls refuse, and the cluster shape of their walk (decided once per engine and form, before the first call
+// launches anything).  q: the latency form's running-request side (eppscore_schedule_batch_inorder_latency), else nullptr.
+// *done: nothing to run (R == 0).
+int32_t inorder_prologue(eppscore_engine* e, const eppscore_batch* b, const char* what, bool index, const eppscore_inorder_running* q,
+                         bool* done) {
   *done = false;
   const std::string w(what);
   if (!b || b->struct_size != sizeof(eppscore_batch)) return fail(e, EPPSCORE_ERR_INVALID, "batch NULL or struct_size mismatch");
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
-  if (cfg_has(e->prof[0].cfg, EPPSCORE_SCORER_LATENCY))
+  const bool lat = cfg_has(e->prof[0].cfg, EPPSCORE_SCORER_LATENCY);
+  if (lat && !q)
     return fail(e, EPPSCORE_ERR_INVALID, w + ": the latency scorer's inputs are PreRequest state the call does not order");
+  if (q && !lat) return fail(e, EPPSCORE_ERR_INVALID, w + ": profile 0 has no latency scorer");
+  if (q && e->prof[0].cfg.n_filters > 0)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": the device filters (prefix-cache-affinity, slo-headroom-tier) are not ordered");
   if (e->have_snapshot && e->snapshot_has_tokens)
     return fail(e, EPPSCORE_ERR_INVALID, w + ": the snapshot supplies inflight_tokens; the in-order view needs the engine's counters");
   if (b->dense_feat || b->scores_out || b->match_blocks || b->pred_out || b->filter_mask_out)
@@ -1949,10 +2016,20 @@ int32_t inorder_prologue(eppscore_engine* e, const eppscore_batch* b, const char
   }
   if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, w + " before set_snapshot");
   if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
+  if (q) {
+    if (!e->lat_args.enabled)
+      return fail(e, EPPSCORE_ERR_INVALID, w + ": the snapshot was prepared without latency params");
+    if (q->request_key && (e->snapshot_has_min_tpot || e->snapshot_has_dispatched))
+      return fail(e, EPPSCORE_ERR_INVALID, w + ": the snapshot supplies min_tpot_slo or dispatched; the in-order view needs the "
+                                               "engine's running-request queues");
+    if (q->request_key && b->location == 0 && b->tpot_slo)
+      for (int32_t r = 0; r < b->R; r++)
+        if (std::isnan(b->tpot_slo[r])) return fail(e, EPPSCORE_ERR_INVALID, w + ": tpot_slo is NaN");
+  }
   CK(e, cudaSetDevice(e->device));
-  int32_t& shape = index ? e->io_index_cluster : e->io_cluster;
+  int32_t& shape = index ? (q ? e->io_lat_index_cluster : e->io_index_cluster) : (q ? e->io_lat_cluster : e->io_cluster);
   if (shape == 0) {
-    const int C = index ? inorder_index_cluster_size(e->geo.Mpad) : inorder_cluster_size(e->geo.Mpad);
+    const int C = index ? inorder_index_cluster_size(e->geo.Mpad, q != nullptr) : inorder_cluster_size(e->geo.Mpad, q != nullptr);
     if (C < 0) return cuda_fail(e, (cudaError_t)-C, index ? "inorder_index_kernel cluster attributes" : "inorder_pick_kernel cluster attributes");
     if (C == 0)
       return fail(e, EPPSCORE_ERR_CAPACITY, w + ": no thread-block cluster of this device holds max_endpoints "
@@ -1983,18 +2060,21 @@ int32_t eppscore_schedule_batch_topk_wide(eppscore_engine* e, const eppscore_bat
 int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens) {
   if (!e) return EPPSCORE_ERR_INVALID;
   bool done = false;
-  const int32_t rc = inorder_prologue(e, b, "schedule_batch_inorder", false, &done);
+  const int32_t rc = inorder_prologue(e, b, "schedule_batch_inorder", false, nullptr, &done);
   if (rc != EPPSCORE_OK || done) return rc;
   return schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens);
 }
 
-int32_t eppscore_schedule_batch_inorder_index(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
-                                              const eppscore_inorder_index* x) {
-  if (!e) return EPPSCORE_ERR_INVALID;
-  const char* what = "schedule_batch_inorder_index";
+}  // extern "C"
+
+namespace {
+
+// eppscore_schedule_batch_inorder_index, and the index form of eppscore_schedule_batch_inorder_latency (q non-null)
+int32_t inorder_index_call(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens, const eppscore_inorder_index* x,
+                           const eppscore_inorder_running* q, const char* what) {
   if (!x || x->struct_size != sizeof(eppscore_inorder_index)) return fail(e, EPPSCORE_ERR_INVALID, "inorder_index NULL or struct_size mismatch");
   bool done = false;
-  int32_t rc = inorder_prologue(e, b, what, true, &done);
+  int32_t rc = inorder_prologue(e, b, what, true, q, &done);
   if (rc != EPPSCORE_OK || done) return rc;
   // the call is an index mutation on the stream the batch runs on: ordered like eppscore_commit_picks_device
   cudaStream_t cs = b->location == 1 && b->stream ? (cudaStream_t)b->stream : e->stream;
@@ -2014,11 +2094,34 @@ int32_t eppscore_schedule_batch_inorder_index(eppscore_engine* e, const eppscore
   }
   DeviceIndex::OrderedRefs refs{};
   if ((rc = index_status(e, e->index->ordered_begin(caps.empty() ? nullptr : caps.data(), cs, &refs), what)) != EPPSCORE_OK) return rc;
-  rc = schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, &refs, x->pick_match);
+  rc = schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, &refs, x->pick_match, q);
   if (rc != EPPSCORE_OK || capturing) return rc;
   CK(e, cudaEventRecord(e->ev_table, cs));  // later readers on other streams, and later mutations on the engine stream, follow it
   if (cs != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_table, 0));
   return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_schedule_batch_inorder_index(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                              const eppscore_inorder_index* x) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  return inorder_index_call(e, b, tokens, x, nullptr, "schedule_batch_inorder_index");
+}
+
+int32_t eppscore_schedule_batch_inorder_latency(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                                const eppscore_inorder_index* x, const eppscore_inorder_running* q) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  const char* what = "schedule_batch_inorder_latency";
+  if (!q || q->struct_size != sizeof(eppscore_inorder_running))
+    return fail(e, EPPSCORE_ERR_INVALID, "inorder_running NULL or struct_size mismatch");
+  if (x) return inorder_index_call(e, b, tokens, x, q, what);
+  bool done = false;
+  const int32_t rc = inorder_prologue(e, b, what, false, q, &done);
+  if (rc != EPPSCORE_OK || done) return rc;
+  return schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, nullptr, nullptr, q);
 }
 
 int32_t eppscore_add_profile(eppscore_engine* e, const eppscore_profile* p, int32_t* id_out) {

@@ -13,10 +13,16 @@
 //   inorder_index_kernel   the same walk ordered against the prefix index too (eppscore_schedule_batch_inorder_index): each
 //                          request's match counts are probed from the index as the earlier requests' Adds left it, and the CTA
 //                          that owns the pick runs the index's commit program (IndexProgram::commit) for the request's Add.
+//   inorder_pick_lat_kernel, inorder_index_lat_kernel   either walk with the latency scorer ordered against the running-request
+//                          queues (eppscore_schedule_batch_inorder_latency): each thread keeps its endpoint's running count and
+//                          minimum tpot in registers, the cluster reduces request r's tier and headroom ranges (one more
+//                          barrier.cluster), and the owner of the pick adds request r to its queue (requestcontrol_hooks.go:73-86).
 #include <cooperative_groups.h>
 
 #include "device_common.cuh"
 #include "index_device.cuh"
+#include "lat_pair.cuh"
+#include "running_slot.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -94,6 +100,46 @@ struct InOrderReq {
   long long tokens;
 };
 
+// The latency walk's per-request inputs (tile terms of the request, prediction.go:171-185 and :150), loaded one request ahead.
+struct InOrderLatReq {
+  double x, y;     // ttft_input * input_tokens, tpot_input * input_tokens
+  double tslo;     // TTFT SLO
+  double tpot;     // TPOT SLO (avgTPOTSLO): the bound's input and the value the Add queues
+  unsigned long long key;
+};
+
+// One CTA's (or warp's) share of request r's tier selection (plugin.go:177-238): the lowest tier among its candidates and the
+// |headroom| min / max inside it.  The merge keeps the lower tier, or combines the ranges of an equal one: associative and
+// commutative, so any reduction order gives score_matrix_kernel's one-pass result.
+struct LatTier {
+  int rank;
+  double mnT, mxT, mnP, mxP;
+};
+__device__ __forceinline__ LatTier lat_tier_none() {
+  return LatTier{5, 1.7976931348623157e308, -1.7976931348623157e308, 1.7976931348623157e308, -1.7976931348623157e308};
+}
+__device__ __forceinline__ void lat_tier_merge(LatTier& x, const LatTier& o) {
+  const bool better = o.rank < x.rank, same = o.rank == x.rank;
+  x.mnT = (better || (same && o.mnT < x.mnT)) ? o.mnT : x.mnT;
+  x.mxT = (better || (same && o.mxT > x.mxT)) ? o.mxT : x.mxT;
+  x.mnP = (better || (same && o.mnP < x.mnP)) ? o.mnP : x.mnP;
+  x.mxP = (better || (same && o.mxP > x.mxP)) ? o.mxP : x.mxP;
+  x.rank = better ? o.rank : x.rank;
+}
+__device__ __forceinline__ void lat_tier_warp_reduce(LatTier& x) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    LatTier y;
+    y.rank = __shfl_xor_sync(0xffffffffu, x.rank, o);
+    y.mnT = shfl_xor_f64(x.mnT, o);
+    y.mxT = shfl_xor_f64(x.mxT, o);
+    y.mnP = shfl_xor_f64(x.mnP, o);
+    y.mxP = shfl_xor_f64(x.mxP, o);
+    lat_tier_merge(x, y);
+  }
+}
+constexpr int kLatStatic = 6;  // tile slots 0-5: request-independent for the whole walk (kernels.cuh: LatArgs)
+
 // The hit slots of one round of a request's probes, staged in shared memory (IDX): the cnt word and ep[0..10) of each.
 struct InOrderHits {
   uint32_t raw[kCommitThreads];
@@ -102,9 +148,11 @@ struct InOrderHits {
 };
 
 // The walk, in the in-flight form (IDX false: inorder_pick_kernel) or the index form (IDX true: inorder_index_kernel, CTAs of
-// kCommitThreads threads; dynamic shared memory = the terms, then the CommitSmem of IndexProgram).
-template <bool RND, bool IDX>
-__device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrderIndexArgs& ix) {
+// kCommitThreads threads; dynamic shared memory = the terms, then the CommitSmem of IndexProgram).  LAT: with the latency scorer
+// (the _lat kernels): the terms are followed by the kLatStatic static tile slots of each thread's endpoint, before the CommitSmem.
+template <bool RND, bool IDX, bool LAT>
+__device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrderIndexArgs& ix, const InOrderLatArgs& lt) {
+  constexpr int kTermSlots = kMaxSteps + (LAT ? kLatStatic : 0);
   extern __shared__ __align__(16) double s_term[];  // [n_scorers][blockDim.x]: the request-independent terms of each thread's endpoint
   __shared__ InOrderBest s_warp[kInOrderWarps];
   __shared__ InOrderBest s_cta[2];  // the CTA's winner of the last two requests (read by the other CTAs of the cluster)
@@ -149,6 +197,48 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
     return x;
   };
 
+  // LAT: this thread's endpoint in the latency fold-in.  The static tile slots go to shared memory; lim (slot 6) and the idle
+  // bit (slot 7 bit 0) come from the tiles, or with request keys from this endpoint's running count, minimum tpot (bits) and
+  // count at the minimum, which live in registers and move with its own Adds.
+  double* s_lat = s_term + (size_t)kMaxSteps * T;  // [kLatStatic][T]
+  double lim = 0.0;
+  bool idle = false, neutral = false;
+  int run_cnt = 0, run_mincnt = 0;
+  unsigned long long run_min = kRunMinNone;
+  if constexpr (LAT) {
+    const bool tiled = m < a.Mpad;
+    const double* tp = lt.lat.ep + (size_t)(m >> 5) * 256 + (m & 31);
+#pragma unroll
+    for (int i = 0; i < kLatStatic; i++) s_lat[(size_t)i * T + tid] = tiled ? __ldg(tp + 32 * i) : 0.0;
+    if (tiled) {
+      lim = __ldg(tp + 192);
+      const int fl = __ldg(reinterpret_cast<const int*>(tp + 224));
+      idle = fl & 1;
+      neutral = fl & 2;
+    }
+    if (lt.request_key && m < lt.n_ep) {  // (then the snapshot took both values from the queues, as here; a later slice of the
+                                          // call sees the earlier slices' Adds only here)
+      const RunDev* d = lt.run;
+      run_cnt = d->count[m];
+      run_min = d->min_bits[m];
+      run_mincnt = d->min_cnt[m];
+      lim = lat_lim(run_cnt > 0 ? __longlong_as_double((long long)run_min) : 0.0, lt.lat.buffer);
+      idle = lat_idle(run_cnt);
+    }
+  }
+  auto load_lat = [&](int r) {
+    InOrderLatReq x{};
+    if (r >= a.R) return x;
+    const LatArgs& L = lt.lat;
+    const double in_tok = (double)(L.input_tokens ? __ldg(L.input_tokens + r) : 0);  // len(strings.Fields(prompt))
+    x.x = __dmul_rn(L.ttft_input, in_tok);
+    x.y = __dmul_rn(L.tpot_input, in_tok);
+    x.tslo = L.ttft_slo ? __ldg(L.ttft_slo + r) : 0.0;
+    x.tpot = L.tpot_slo ? __ldg(L.tpot_slo + r) : 0.0;
+    x.key = lt.request_key ? __ldg(reinterpret_cast<const unsigned long long*>(lt.request_key) + r) : 0ull;
+    return x;
+  };
+
   // IDX: the index as the walk mutates it.  Every read goes through DevX's relaxed GPU-scope loads (never the read-only path:
   // the table changes under this kernel); barrier.cluster orders a commit before the next request's probes.
   DevX dx;
@@ -162,8 +252,14 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
 
   cluster.sync();  // every CTA of the cluster is running before any reads another's shared memory
   InOrderReq cur = load(0);
+  InOrderLatReq lcur{};  // (loaded one request ahead in the in-flight form; the index form has no registers to spare for that,
+                         // and its probes cover the loads)
+  if constexpr (LAT && !IDX) lcur = load_lat(0);
   for (int r = 0; r < a.R; r++) {
     const InOrderReq nxt = load(r + 1);
+    InOrderLatReq lnxt{};
+    if constexpr (LAT && IDX) lcur = load_lat(r);
+    if constexpr (LAT && !IDX) lnxt = load_lat(r + 1);
     if constexpr (IDX) {
       // ---- matchLongestPrefix (plugin.go:219-235) at this thread's endpoint, against the index after requests 0..r-1's Adds:
       // T probes per round up to the first global miss, the hit slots staged in shared memory, then every thread counts the
@@ -197,6 +293,56 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
       }
       cur.c = (int32_t)c;
     }
+    // ---- The latency scorer (scorer/latency/plugin.go:144-360) at this thread's endpoint: w, the scoreBucket weight ----
+    long long lat_w = 0;
+    if constexpr (LAT) {
+      const LatArgs& L = lt.lat;
+      const double pt = __dmul_rn(L.has_predictions ? L.ttft_prefix : L.wpref,
+                                  cur.total ? __ddiv_rn((double)cur.c, (double)cur.total) : 0.0);  // preparedata_hooks.go:44-58
+      if (L.has_predictions) {
+        const LatPair lp = lat_pair_slots(s_lat[tid], s_lat[(size_t)T + tid], s_lat[(size_t)2 * T + tid], s_lat[(size_t)3 * T + tid],
+                                          s_lat[(size_t)4 * T + tid], s_lat[(size_t)5 * T + tid], lim,
+                                          (idle ? 1 : 0) | (neutral ? 2 : 0), L.tpot_generated, pt, lcur.x, lcur.y, lcur.tslo,
+                                          __dmul_rn(lcur.tpot, L.buffer));
+        const double aT = fabs(lp.hT), aP = fabs(lp.hP);
+        // the lowest tier over the candidates and the |headroom| ranges inside it: warp, CTA, then cluster (barrier.cluster)
+        __shared__ LatTier s_wtier[kInOrderWarps];
+        __shared__ LatTier s_ctier[2];
+        LatTier t = cur.cand ? LatTier{lp.rank, aT, aT, aP, aP} : lat_tier_none();
+        lat_tier_warp_reduce(t);
+        if (lane == 0) s_wtier[warp] = t;
+        __syncthreads();
+        if (warp == 0) {
+          t = lane < nwarps ? s_wtier[lane] : lat_tier_none();
+          lat_tier_warp_reduce(t);
+          if (lane == 0) s_ctier[r & 1] = t;
+        }
+        cluster.sync();
+        t = lane < C ? *cluster.map_shared_rank(&s_ctier[r & 1], lane) : lat_tier_none();
+        lat_tier_warp_reduce(t);
+        // scoreBucket (plugin.go:262-318) with exact divisions, as the oracle
+        const double rgT = __dsub_rn(t.mxT, t.mnT), rgP = __dsub_rn(t.mxP, t.mnP);
+        const bool tok = rgT > 1e-9, pok = rgP > 1e-9;  // plugin.go:41
+        double alpha = L.alpha, beta = L.beta;
+        if (!tok && pok) {                               // plugin.go:275-279
+          alpha = 0.0;
+          beta = 1.0;
+        } else if (!pok && tok) {
+          alpha = 1.0;
+          beta = 0.0;
+        }
+        const bool most = L.strategy_most && t.rank == 0;
+        const double eT = tok ? __ddiv_rn(__dsub_rn(aT, t.mnT), rgT) : 0.5, eP = pok ? __ddiv_rn(__dsub_rn(aP, t.mnP), rgP) : 0.5;
+        const double ec = __dadd_rn(__dmul_rn(alpha, eT), __dmul_rn(beta, eP));
+        lat_w = lp.rank == t.rank ? __double2ll_rz(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1 : 0;
+      } else {
+        // compositeScores (plugin.go:338-360): maxQ over the candidates from 0, the candidates' queue maximum
+        const long long maxq = cur.mx0 > 0 ? cur.mx0 : 0;
+        const long long q = __double_as_longlong(s_lat[(size_t)T + tid]);  // raw WaitingQueueSize
+        const double rel = maxq > 0 ? __ddiv_rn(__ll2double_rn(maxq - q), __ll2double_rn(maxq)) : 1.0;
+        lat_w = __double2ll_rz(round(__dmul_rn(100.0, __dadd_rn(__dadd_rn(s_lat[tid], __dmul_rn(L.wq, rel)), pt))));
+      }
+    }
     // ---- Score (scheduler_profile.go:151-174): profile order from 0.0, the operations of score_matrix_kernel ----
     double acc = 0.0;
     for (int s = 0; s < a.n_scorers; s++) {
@@ -214,6 +360,8 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
         term = prefix_term_direct(cur.c, cur.total, w);                                // prefix/plugin.go:108-110
       } else if (kind == 3) {
         term = a.lora_term[s][cur.cls];
+      } else if (LAT && kind == 5) {
+        term = __dmul_rn(clamp01(__ddiv_rn(__ll2double_rn(lat_w), 100.0)), w);       // float64(w)/100, plugin.go:301-306
       } else if (kind >= 16) {
         term = __dmul_rn(0.0, w);                                                      // pair columns absent
       } else {
@@ -268,6 +416,41 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
       a.pick_score[r] = pick >= 0 ? score : 0.0;
       a.tie_count[r] = cnt;
     }
+    if constexpr (LAT) {
+      // ---- PreRequest: the request joins its target's running-request queue (requestcontrol_hooks.go:73-86), refused for an
+      // empty key, a negative tpot or a pair already live (running_request_tpot_slo_queue.go:127-132) ----
+      uint8_t added = 0;
+      if (pick == m && lcur.key != 0ull) {
+        const RunDev* d = lt.run;
+        const double tp = lcur.tpot;
+        if (tp != tp) {
+          atomicOr(&d->ctr->err, kRunErrInvalid);  // (host arrays are validated before the launch)
+        } else if (!(tp < 0.0)) {
+          const RunDev dv = *d;
+          bool created = false;
+          const long long h = run_find_or_create(dv, lcur.key, m, &created);
+          if (h < 0) atomicOr(&d->ctr->err, kRunErrCapacity);
+          if (created) {
+            const unsigned long long v = tp == 0.0 ? 0ull : (unsigned long long)__double_as_longlong(tp);  // -0.0 as +0.0
+            dv.tpot[h] = v;
+            dv.owner[h] = ((unsigned long long)d->ctr->gen << 32) | (unsigned)r;  // older than any later call's bid: its add is refused
+            atomicAdd(&d->ctr->live, 1ull);
+            run_cnt += 1;
+            if (v < run_min) {
+              run_min = v;
+              run_mincnt = 1;
+            } else if (v == run_min) {
+              run_mincnt += 1;
+            }
+            lim = lat_lim(__longlong_as_double((long long)run_min), lt.lat.buffer);
+            idle = lat_idle(run_cnt);
+            added = 1;
+          }
+        }
+      }
+      if (lt.added_out && (pick >= 0 ? pick == m : m == 0)) lt.added_out[r] = added;
+      lcur = lnxt;
+    }
     if constexpr (IDX) {
       // PrefixCacheMatchInfo at the target (plugin.go:199-204), before the request's own Add
       if (ix.pick_match && (pick >= 0 ? pick == m : m == 0)) ix.pick_match[r] = pick >= 0 ? (uint16_t)cur.c : (uint16_t)0;
@@ -283,7 +466,7 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
         ca.stride = ix.stride;
         ca.cap_req = ix.cap_req;
         ca.n_picks = 1;
-        CommitSmem* sm = reinterpret_cast<CommitSmem*>(s_term + (size_t)kMaxSteps * T);
+        CommitSmem* sm = reinterpret_cast<CommitSmem*>(s_term + (size_t)kTermSlots * T);
         IndexProgram<DevX> prog(dx, ix.tv, ix.lv, sm, (uint32_t)pick);
         prog.commit(ca);
       }
@@ -295,18 +478,39 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
     a.inflight_tok[m] = tok;
     a.inflight_req[m] = req;
   }
+  if constexpr (LAT) {
+    if (lt.request_key && m < lt.n_ep) {  // (running_finalize_kernel publishes the view and advances the generation)
+      const RunDev* d = lt.run;
+      d->count[m] = run_cnt;
+      d->min_bits[m] = run_min;
+      d->min_cnt[m] = run_mincnt;
+    }
+  }
   cluster.sync();  // no CTA leaves while another may still read its winners
 }
 
 template <bool RND>
 __global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_kernel(const __grid_constant__ InOrderArgs a) {
-  inorder_walk<RND, false>(a, InOrderIndexArgs{});
+  inorder_walk<RND, false, false>(a, InOrderIndexArgs{}, InOrderLatArgs{});
 }
 
 template <bool RND>
 __global__ void __launch_bounds__(kCommitThreads, 1) inorder_index_kernel(const __grid_constant__ InOrderArgs a,
                                                                           const __grid_constant__ InOrderIndexArgs ix) {
-  inorder_walk<RND, true>(a, ix);
+  inorder_walk<RND, true, false>(a, ix, InOrderLatArgs{});
+}
+
+template <bool RND>
+__global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_pick_lat_kernel(const __grid_constant__ InOrderArgs a,
+                                                                                 const __grid_constant__ InOrderLatArgs lt) {
+  inorder_walk<RND, false, true>(a, InOrderIndexArgs{}, lt);
+}
+
+template <bool RND>
+__global__ void __launch_bounds__(kCommitThreads, 1) inorder_index_lat_kernel(const __grid_constant__ InOrderArgs a,
+                                                                              const __grid_constant__ InOrderIndexArgs ix,
+                                                                              const __grid_constant__ InOrderLatArgs lt) {
+  inorder_walk<RND, true, true>(a, ix, lt);
 }
 
 int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count) {
@@ -320,13 +524,13 @@ int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count) {
 // The cluster: C CTAs of T = Mpad / C threads, one endpoint per thread.  Up to 16 CTAs when the device grants the non-portable
 // size, else 8 (then max_endpoints 8192 does not fit); fewer at small Mpad, so that a CTA keeps at least 256 endpoints (each
 // CTA is one more arrival at every barrier).  The dynamic shared memory (8 bytes per scorer per thread, at most 32 KiB) needs no
-// opt-in.
+// opt-in; the latency form's (8 more bytes per static tile slot, at most 56 KiB) is opted in by cluster_size.
 template <bool RND>
-static cudaLaunchConfig_t pick_config(int Mpad, int C, cudaStream_t s, cudaLaunchAttribute* at) {
+static cudaLaunchConfig_t pick_config(int Mpad, int C, cudaStream_t s, cudaLaunchAttribute* at, bool lat = false) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(C);
   cfg.blockDim = dim3(Mpad / C);
-  cfg.dynamicSmemBytes = (size_t)kMaxSteps * 8 * (Mpad / C);
+  cfg.dynamicSmemBytes = (size_t)(kMaxSteps + (lat ? kLatStatic : 0)) * 8 * (Mpad / C);
   cfg.stream = s;
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = C;
@@ -337,10 +541,12 @@ static cudaLaunchConfig_t pick_config(int Mpad, int C, cudaStream_t s, cudaLaunc
   return cfg;
 }
 
-template <bool RND>
+template <bool RND, bool LAT>
 static int cluster_size(int Mpad) {
-  auto kernel = inorder_pick_kernel<RND>;
+  auto kernel = LAT ? (const void*)inorder_pick_lat_kernel<RND> : (const void*)inorder_pick_kernel<RND>;
   cudaError_t c = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  if (c == cudaSuccess && LAT)
+    c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (kMaxSteps + kLatStatic) * 8 * kInOrderMaxThreads);
   if (c != cudaSuccess) return -(int)c;
   for (int cmax = 16; cmax >= 8; cmax /= 2) {
     int C = Mpad / 256;
@@ -348,7 +554,7 @@ static int cluster_size(int Mpad) {
     if (C > cmax) C = cmax;
     if (Mpad / C > kInOrderMaxThreads) continue;
     cudaLaunchAttribute at[1];
-    const cudaLaunchConfig_t cfg = pick_config<RND>(Mpad, C, nullptr, at);
+    const cudaLaunchConfig_t cfg = pick_config<RND>(Mpad, C, nullptr, at, LAT);
     int clusters = 0;
     c = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
     if (c == cudaSuccess && clusters >= 1) return C;
@@ -357,16 +563,21 @@ static int cluster_size(int Mpad) {
   return 0;
 }
 
-int inorder_cluster_size(int Mpad) {
-  const int a = cluster_size<false>(Mpad);
+int inorder_cluster_size(int Mpad, bool lat) {
+  const int a = lat ? cluster_size<false, true>(Mpad) : cluster_size<false, false>(Mpad);
   if (a <= 0) return a;
-  const int b = cluster_size<true>(Mpad);
+  const int b = lat ? cluster_size<true, true>(Mpad) : cluster_size<true, false>(Mpad);
   return b <= 0 ? b : (a < b ? a : b);
 }
 
-int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s) {
+int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s, const InOrderLatArgs* lt) {
   if (a.R <= 0) return 0;
   cudaLaunchAttribute at[1];
+  if (lt) {
+    const cudaLaunchConfig_t cfg = pick_config<true>(a.Mpad, C, s, at, true);
+    return launched_one(a.pick_mode != 0 ? cudaLaunchKernelEx(&cfg, inorder_pick_lat_kernel<true>, a, *lt)
+                                         : cudaLaunchKernelEx(&cfg, inorder_pick_lat_kernel<false>, a, *lt));
+  }
   if (a.pick_mode != 0) {
     const cudaLaunchConfig_t cfg = pick_config<true>(a.Mpad, C, s, at);
     return launched_one(cudaLaunchKernelEx(&cfg, inorder_pick_kernel<true>, a));
@@ -377,14 +588,15 @@ int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s) {
 
 // The index form: C CTAs of kCommitThreads threads (IndexProgram's CTA), thread t of CTA c owning endpoint c * 512 + t (threads
 // past Mpad idle), so C = Mpad / 512 up to 16 (one CTA below 512 endpoints).  Dynamic shared memory: the terms of 512 threads,
-// then the CommitSmem of the program (136 KiB, plus 13 KiB of static shared memory: one CTA per SM).
-static size_t index_smem() { return (size_t)kMaxSteps * 8 * kCommitThreads + sizeof(CommitSmem); }
+// then the CommitSmem of the program (136 KiB, plus 13 KiB of static shared memory: one CTA per SM).  The latency form puts the
+// static tile slots (24 KiB) between the two.
+static size_t index_smem(bool lat) { return (size_t)(kMaxSteps + (lat ? kLatStatic : 0)) * 8 * kCommitThreads + sizeof(CommitSmem); }
 
-static cudaLaunchConfig_t index_config(int C, cudaStream_t s, cudaLaunchAttribute* at) {
+static cudaLaunchConfig_t index_config(int C, cudaStream_t s, cudaLaunchAttribute* at, bool lat = false) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(C);
   cfg.blockDim = dim3(kCommitThreads);
-  cfg.dynamicSmemBytes = index_smem();
+  cfg.dynamicSmemBytes = index_smem(lat);
   cfg.stream = s;
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = C;
@@ -395,16 +607,16 @@ static cudaLaunchConfig_t index_config(int C, cudaStream_t s, cudaLaunchAttribut
   return cfg;
 }
 
-template <bool RND>
+template <bool RND, bool LAT>
 static int index_cluster_size(int Mpad) {
-  auto kernel = inorder_index_kernel<RND>;
+  auto kernel = LAT ? (const void*)inorder_index_lat_kernel<RND> : (const void*)inorder_index_kernel<RND>;
   cudaError_t c = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)index_smem());
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)index_smem(LAT));
   if (c != cudaSuccess) return -(int)c;
   const int C = Mpad <= kCommitThreads ? 1 : (Mpad + kCommitThreads - 1) / kCommitThreads;
   if (C > 16) return 0;
   cudaLaunchAttribute at[1];
-  const cudaLaunchConfig_t cfg = index_config(C, nullptr, at);
+  const cudaLaunchConfig_t cfg = index_config(C, nullptr, at, LAT);
   int clusters = 0;
   c = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
   if (c == cudaSuccess && clusters >= 1) return C;
@@ -412,16 +624,21 @@ static int index_cluster_size(int Mpad) {
   return 0;
 }
 
-int inorder_index_cluster_size(int Mpad) {
-  const int a = index_cluster_size<false>(Mpad);
+int inorder_index_cluster_size(int Mpad, bool lat) {
+  const int a = lat ? index_cluster_size<false, true>(Mpad) : index_cluster_size<false, false>(Mpad);
   if (a <= 0) return a;
-  const int b = index_cluster_size<true>(Mpad);
+  const int b = lat ? index_cluster_size<true, true>(Mpad) : index_cluster_size<true, false>(Mpad);
   return b <= 0 ? b : a;  // (both forms have the same shape)
 }
 
-int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s) {
+int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s, const InOrderLatArgs* lt) {
   if (a.R <= 0) return 0;
   cudaLaunchAttribute at[1];
+  if (lt) {
+    const cudaLaunchConfig_t cfg = index_config(C, s, at, true);
+    return launched_one(a.pick_mode != 0 ? cudaLaunchKernelEx(&cfg, inorder_index_lat_kernel<true>, a, ix, *lt)
+                                         : cudaLaunchKernelEx(&cfg, inorder_index_lat_kernel<false>, a, ix, *lt));
+  }
   if (a.pick_mode != 0) {
     const cudaLaunchConfig_t cfg = index_config(C, s, at);
     return launched_one(cudaLaunchKernelEx(&cfg, inorder_index_kernel<true>, a, ix));

@@ -295,7 +295,7 @@ int launch_estimate_tokens(const int64_t* size, const int32_t* hint, const int32
 struct InOrderArgs {
   int32_t M, Mpad, log_epl, RW, A, mask_words;
   int32_t n_scorers;
-  int32_t kind[kMaxSteps];             // eppscore_scorer_kind (no latency scorer)
+  int32_t kind[kMaxSteps];             // eppscore_scorer_kind (the latency scorer only in the walk's latency form)
   double weight[kMaxSteps];
   double lora_term[kMaxSteps][4];      // per LoRA scorer: clamp({0,0.6,0.8,1.0})*w, as Plan::lora_term
   const double* term[kMaxSteps];       // the prepared [Mpad] terms of the kv-cache and endpoint-column scorers, else null
@@ -306,7 +306,8 @@ struct InOrderArgs {
   int32_t R;
   const uint16_t* match;               // [R][M] match counts (the batch kernels' match_out) or null
   const uint16_t* total;               // [R] or null
-  long long* minmax;                   // [R][4]: queue min, max, running min, max over the candidates (or null: no such scorer)
+  long long* minmax;                   // [R][4]: queue min, max, running min, max over the candidates (or null: no such scorer
+                                       // and no latency scorer without predictions)
   const int32_t* adapter_id;           // [R] or null
   const uint32_t* cand_mask;           // [R][mask_words] natural order or null
   const uint32_t* member;              // [Mpad/32] natural-order bits of profile 0's endpoint subset, or null
@@ -322,10 +323,21 @@ struct InOrderArgs {
   int32_t* tie_count;
 };
 int launch_inorder_minmax(const InOrderArgs& a, cudaStream_t s, int sm_count);  // fills a.minmax
-// CTAs per cluster of inorder_pick_kernel at this Mpad on the current device (sets the kernels' cluster attribute): > 0, 0 when no
-// cluster shape fits, or -(cudaError_t)
-int inorder_cluster_size(int Mpad);
-int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s);            // one cluster of C CTAs
+struct RunDev;
+// The latency scorer in the walk (eppscore_schedule_batch_inorder_latency): the snapshot's fold-in (its tiles and scalars, the
+// slice's input_tokens / ttft_slo / tpot_slo) and the running-request queues, which the owner of each pick adds request r to.
+struct InOrderLatArgs {
+  LatArgs lat;
+  RunDev* run;                    // the device descriptor of the queues (kernels.cuh: RunDev)
+  const uint64_t* request_key;    // [R] or null: the queues are read (from the tiles), never changed
+  uint8_t* added_out;             // [R] or null
+  int32_t n_ep;                   // max_endpoints: the length of the queues' per-endpoint arrays
+};
+// CTAs per cluster of inorder_pick_kernel (lat: inorder_pick_lat_kernel) at this Mpad on the current device (sets the kernels'
+// cluster attribute): > 0, 0 when no cluster shape fits, or -(cudaError_t)
+int inorder_cluster_size(int Mpad, bool lat = false);
+// one cluster of C CTAs; lt non-null: the latency form (inorder_pick_lat_kernel)
+int launch_inorder_pick(const InOrderArgs& a, int C, cudaStream_t s, const InOrderLatArgs* lt = nullptr);
 // The walk in index order (eppscore_schedule_batch_inorder_index): request r's match counts are read from the index as it
 // stands after requests 0..r-1's commits, and the CTA that owns r's pick commits r's blocks (IndexProgram::commit) before
 // request r + 1 probes.  a.match is unused; a.total holds n_hashes.
@@ -337,8 +349,8 @@ struct InOrderIndexArgs {
   const int32_t* cap_req;   // [n_endpoints] CacheNumBlocks or null
   uint16_t* pick_match;     // [R] the pick's match count as the request was scored, or null
 };
-int inorder_index_cluster_size(int Mpad);  // as inorder_cluster_size, for launch_inorder_index's CTAs of kCommitThreads
-int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s);
+int inorder_index_cluster_size(int Mpad, bool lat = false);  // as inorder_cluster_size, for launch_inorder_index's CTAs of kCommitThreads
+int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s, const InOrderLatArgs* lt = nullptr);
 
 // predicted-latency producer's running-request queues (running_kernel.cu).  Table slot: {key, meta}, meta = endpoint + 1
 // (| kRunTomb once removed), {0, 0} empty; tpot[] holds the entry's tpot bits, owner[] / rm[] the (gen << 32 | r) bids of
@@ -377,6 +389,10 @@ cudaError_t init_running_kernels();
 // out: optional [R] added / removed flags.
 int launch_running_update(RunDev* dp, unsigned long long cap, int op, const int32_t* endpoint, const uint64_t* key,
                           const double* tpot, int R, int n_ep, uint8_t* out, int sm_count, cudaStream_t s);
+// The pre-add compaction alone (the first three launches of an add), and the end of every call (the view and the generation):
+// for a caller that adds through its own kernel (the in-order walk's Add at each pick).
+int launch_running_compact(RunDev* dp, unsigned long long cap, int R, int sm_count, cudaStream_t s);
+int launch_running_finalize(RunDev* dp, int n_ep, cudaStream_t s);
 int launch_running_drop_endpoint(RunDev* dp, unsigned long long cap, int m, int n_ep, int sm_count, cudaStream_t s);
 int launch_running_rebuild(const RunDev& src, const RunDev& dst, int sm_count, cudaStream_t s);
 

@@ -6,6 +6,7 @@
 //       (lora_affinity.go:84-99 precedence) and — for the sparse fast path — the arg-max summary of the
 //       zero-prefix-match score map G[a][m] (max, arg, count, tie mask).
 #include "device_common.cuh"
+#include "lat_pair.cuh"
 
 namespace eppscore {
 
@@ -138,8 +139,8 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const __grid_co
         tile[3 * 32] = __dadd_rn(a.lat_coef[4], __dmul_rn(a.lat_coef[5], kv));
         tile[4 * 32] = __dmul_rn(a.lat_coef[6], wt);
         tile[5 * 32] = __dmul_rn(a.lat_coef[7], rn);
-        tile[6 * 32] = pod_min > 0.0 ? __dmul_rn(pod_min, a.lat_buffer) : __longlong_as_double(0x7ff0000000000000LL);
-        const bool idle = !(m < M && a.dispatched) || a.dispatched[m] == 0;
+        tile[6 * 32] = lat_lim(pod_min, a.lat_buffer);
+        const bool idle = lat_idle((m < M && a.dispatched) ? a.dispatched[m] : 0);
         const bool neutral = !a.lat_streaming || (m < M && a.prefill && a.prefill[m]);
         tile[7 * 32] = __longlong_as_double((long long)((idle ? 1 : 0) | (neutral ? 2 : 0)));
       } else {

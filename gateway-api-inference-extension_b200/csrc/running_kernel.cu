@@ -13,24 +13,17 @@
 // The apply kernels have the structure of inflight_update_kernel: lanes of a warp that name the same endpoint are combined
 // (__match_any_sync), each group updates a per-CTA shared-memory histogram once, and each CTA issues one global atomic per
 // endpoint it saw, so 64K entries on one endpoint do not serialise on one address.
-#include "kernels.cuh"
+#include "running_slot.cuh"
 
 namespace eppscore {
 
 constexpr int kRunThreads = 512;
 constexpr int kRunPerCta = 4096;  // entries per CTA of the apply kernels: the histogram is zeroed and flushed once per 4096
 
-__device__ __forceinline__ unsigned long long run_hash(unsigned long long key, int m) {
-  unsigned long long x = key ^ ((unsigned long long)(m + 1) * 0x9E3779B97F4A7C15ull);  // splitmix64 finaliser
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-
 __device__ __forceinline__ bool run_live(unsigned long long meta) { return meta != 0ull && !(meta & kRunTomb); }
 
-// claim: one thread per entry.  add (op 0): validates the entry, finds or creates the (endpoint, key) slot — creation is one
-// 16-byte CAS of an empty slot, so two entries of the call with the same pair meet in one slot — and bids (gen << 32 | r) for
+// claim: one thread per entry.  add (op 0): validates the entry, finds or creates the (endpoint, key) slot (run_find_or_create:
+// two entries of the call with the same pair meet in one slot) and bids (gen << 32 | r) for
 // it with atomicMin.  A slot that existed before the call holds an older generation and always wins: the add is refused.
 // remove (op 1): finds the live slot and bids the same way; the lowest r removes it.  slot_of[r] = slot, or -1.
 __global__ void running_claim_kernel(const RunDev* __restrict__ dp, int op, const int32_t* __restrict__ endpoint,
@@ -50,25 +43,29 @@ __global__ void running_claim_kernel(const RunDev* __restrict__ dp, int op, cons
   }
   const unsigned long long k = key[r];
   if (k == 0ull || t < 0.0) return;  // empty x-request-id, negative tpot: refused (running_request_tpot_slo_queue.go:127-132)
-  const unsigned long long want_meta = (unsigned long long)(m + 1);
   const unsigned long long bid = ((unsigned long long)d.ctr->gen << 32) | (unsigned)r;
+  if (op == 0) {
+    bool created;
+    const long long h = run_find_or_create(d, k, m, &created);
+    if (h < 0) {
+      atomicOr(&d.ctr->err, kRunErrCapacity);
+      return;
+    }
+    atomicMin(&d.owner[h], bid);
+    slot_of[r] = (int32_t)h;
+    return;
+  }
+  const unsigned long long want_meta = (unsigned long long)(m + 1);
   unsigned long long h = run_hash(k, m) & d.mask;
   for (unsigned long long i = 0; i <= d.mask; i++, h = (h + 1) & d.mask) {
-    RunSlot cur;
-    if (op == 0) {
-      cur = atomicCAS(&d.slot[h], RunSlot{0ull, 0ull}, RunSlot{k, want_meta});
-      if (cur.key == 0ull && cur.meta == 0ull) cur = RunSlot{k, want_meta};  // created it
-    } else {
-      cur = d.slot[h];  // nothing creates or tombstones slots during a remove's claim
-    }
-    if (cur.key == 0ull && cur.meta == 0ull) return;  // remove: an empty slot ends the chain, the pair is not live
+    const RunSlot cur = d.slot[h];  // nothing creates or tombstones slots during a remove's claim
+    if (cur.key == 0ull && cur.meta == 0ull) return;  // an empty slot ends the chain: the pair is not live
     if (cur.key == k && cur.meta == want_meta) {
-      atomicMin(op == 0 ? &d.owner[h] : &d.rm[h], bid);
+      atomicMin(&d.rm[h], bid);
       slot_of[r] = (int32_t)h;
       return;
     }
   }
-  if (op == 0) atomicOr(&d.ctr->err, kRunErrCapacity);  // no empty slot left: only a graph replayed past its reserve
 }
 
 // apply: the winners of the claim.  add: store tpot, count += n, min = min(min, tpot); an endpoint whose minimum went down
@@ -335,6 +332,19 @@ static int run_grid(unsigned long long cap, int max_ctas) {  // grid-stride pass
   return want < (unsigned long long)max_ctas ? (int)want : max_ctas;
 }
 
+int launch_running_compact(RunDev* dp, unsigned long long cap, int R, int sm_count, cudaStream_t s) {
+  const int g = run_grid(cap, sm_count * 4);
+  running_compact_clear_kernel<<<g, 256, 0, s>>>(dp, R);
+  running_compact_move_kernel<<<g, 256, 0, s>>>(dp, R);
+  running_compact_swap_kernel<<<1, 1, 0, s>>>(dp, R);
+  return 3;
+}
+
+int launch_running_finalize(RunDev* dp, int n_ep, cudaStream_t s) {
+  running_finalize_kernel<<<(n_ep + 255) / 256, 256, 0, s>>>(dp, n_ep);
+  return 1;
+}
+
 // The table passes are grid-stride loops over the descriptor's capacity, so a captured graph stays valid after the table
 // grows: its grid was sized for the capacity at capture time, and its kernels read the table through `dp`.
 int launch_running_update(RunDev* dp, unsigned long long cap, int op, const int32_t* endpoint, const uint64_t* key,
@@ -344,12 +354,7 @@ int launch_running_update(RunDev* dp, unsigned long long cap, int op, const int3
   const int grid = (R + kRunPerCta - 1) / kRunPerCta;
   const int g = run_grid(cap, sm_count * 4);
   if (R > 0) {
-    if (op == 0) {
-      running_compact_clear_kernel<<<g, 256, 0, s>>>(dp, R);
-      running_compact_move_kernel<<<g, 256, 0, s>>>(dp, R);
-      running_compact_swap_kernel<<<1, 1, 0, s>>>(dp, R);
-      n += 3;
-    }
+    if (op == 0) n += launch_running_compact(dp, cap, R, sm_count, s);
     running_claim_kernel<<<(R + 255) / 256, 256, 0, s>>>(dp, op, endpoint, key, tpot, R, n_ep);
     running_apply_kernel<<<grid, kRunThreads, smem, s>>>(dp, op, endpoint, tpot, R, n_ep, out);
     n += 2;
@@ -363,15 +368,13 @@ int launch_running_update(RunDev* dp, unsigned long long cap, int op, const int3
     running_recompute_kernel<<<g, 256, 0, s>>>(dp, 1);
     n += 2;
   }
-  running_finalize_kernel<<<(n_ep + 255) / 256, 256, 0, s>>>(dp, n_ep);
-  return n + 1;
+  return n + launch_running_finalize(dp, n_ep, s);
 }
 
 int launch_running_drop_endpoint(RunDev* dp, unsigned long long cap, int m, int n_ep, int sm_count, cudaStream_t s) {
   const int g = run_grid(cap, sm_count * 4);
   running_drop_endpoint_kernel<<<g, 256, 0, s>>>(dp, m);
-  running_finalize_kernel<<<(n_ep + 255) / 256, 256, 0, s>>>(dp, n_ep);
-  return 2;
+  return 1 + launch_running_finalize(dp, n_ep, s);
 }
 
 int launch_running_rebuild(const RunDev& src, const RunDev& dst, int sm_count, cudaStream_t s) {

@@ -184,7 +184,12 @@ class Engine:
         call, topk = ((self._lib.eppscore_schedule_batch_topk_wide, topk_wide) if topk_wide else
                       (self._lib.eppscore_schedule_batch_topk, topk))
         a = _Args(device)
-        if _inorder is not None and len(_inorder) > 1:  # schedule_inorder_index: (tokens, InOrderIndex)
+        if _inorder is not None and len(_inorder) > 2:  # schedule_inorder_latency: (tokens, InOrderIndex | None, InOrderRunning)
+            tok, ix, q = a.ptr(_inorder[0], np.int64), _inorder[1], _inorder[2]
+            q.request_key = a.ptr(_inorder[3], np.uint64)
+            call = lambda h, bp: self._lib.eppscore_schedule_batch_inorder_latency(h, bp, tok, None if ix is None else C.byref(ix),
+                                                                                   C.byref(q))
+        elif _inorder is not None and len(_inorder) > 1:  # schedule_inorder_index: (tokens, InOrderIndex)
             tok, ix = a.ptr(_inorder[0], np.int64), _inorder[1]
             call = lambda h, bp: self._lib.eppscore_schedule_batch_inorder_index(h, bp, tok, C.byref(ix))
         elif _inorder is not None:  # schedule_inorder: (tokens,)
@@ -292,6 +297,43 @@ class Engine:
         x.pick_match = pick_match.ctypes.data
         res = self.schedule(R, _inorder=(tokens, x), **kw)
         res["pick_match"] = pick_match
+        return res
+
+    def schedule_inorder_latency(self, R, tokens=None, request_key=None, index=False, lru_capacity=None, **kw):
+        """eppscore_schedule_batch_inorder_latency: `schedule_inorder` (index=True: `schedule_inorder_index`) for a profile 0 with
+        the latency scorer, request r's latency scorer seeing the running-request queues after requests 0..r-1 were added to
+        them: each request joins its pick's queue inside the call with key request_key[r] (uint64[R]; None: the queues are read,
+        never changed) and tpot tpot_slo[r].  Host mode returns the `schedule_inorder(_index)` dict plus added bool[R]; device
+        mode fills `out` asynchronously on `stream`, with added_out (uint8[R]) and pick_match when `out` has them."""
+        for k in ("want_match", "want_scores", "want_pred", "want_filter_mask", "topk", "topk_wide"):
+            if kw.get(k):
+                raise ValueError(f"schedule_inorder_latency does not take {k}")
+        x = None
+        if index:
+            x = capi.InOrderIndex()
+            x.struct_size = C.sizeof(capi.InOrderIndex)
+            caps = None if lru_capacity is None else np.ascontiguousarray(lru_capacity, np.int32)
+            x.lru_capacity = None if caps is None else caps.ctypes.data
+        q = capi.InOrderRunning()
+        q.struct_size = C.sizeof(capi.InOrderRunning)
+        if kw.get("device"):
+            out = kw.get("out") or {}
+            dev = _Args(True)
+            if x is not None:
+                pm = out.get("pick_match")
+                x.pick_match = None if pm is None else dev.ptr(pm, None)
+            ad = out.get("added_out")
+            q.added_out = None if ad is None else dev.ptr(ad, None)
+            return self.schedule(R, _inorder=(tokens, x, q, request_key), **kw)
+        added = np.zeros(max(R, 1), np.uint8)
+        q.added_out = added.ctypes.data
+        pick_match = np.zeros(max(R, 1), np.uint16)
+        if x is not None:
+            x.pick_match = pick_match.ctypes.data
+        res = self.schedule(R, _inorder=(tokens, x, q, request_key), **kw)
+        res["added"] = added[:R].astype(bool)
+        if x is not None:
+            res["pick_match"] = pick_match[:R]
         return res
 
     # ------------------------------------------------------------------ several scheduler profiles

@@ -151,6 +151,12 @@ inline bool EngineHasInOrderLoad() { return &eppscore_schedule_batch_inorder != 
 extern "C" int32_t eppscore_schedule_batch_inorder_index(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
                                                          const eppscore_inorder_index* x) __attribute__((weak));
 inline bool EngineHasInOrderPrefixIndex() { return &eppscore_schedule_batch_inorder_index != nullptr; }
+// eppscore_schedule_batch_inorder_latency (either in-order call with the latency scorer ordered against the running-request
+// queues) likewise: EngineHasInOrderLatency() tells.  Without it a config with SchedulerConfig::InOrderRunningRequests is refused.
+extern "C" int32_t eppscore_schedule_batch_inorder_latency(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                                           const eppscore_inorder_index* x, const eppscore_inorder_running* q)
+    __attribute__((weak));
+inline bool EngineHasInOrderLatency() { return &eppscore_schedule_batch_inorder_latency != nullptr; }
 
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
@@ -376,6 +382,17 @@ struct SchedulerConfig {
   // LatencyPredictionInfo (eppscore_predict_latency after the batch would read the index the batch left), without
   // InOrderInFlightLoad or prefix hashing, and with an engine library without the call.
   bool InOrderPrefixIndex = false;
+  // Opt-in (off by default), with InOrderInFlightLoad and a profile with a latency scorer: every engine batch goes through
+  // eppscore_schedule_batch_inorder_latency (its index form with InOrderPrefixIndex), so request r's latency scorer sees the
+  // running-request queues after requests 0..r-1 joined them, as the reference's per-request Schedule + PreRequest sequence
+  // does (requestcontrol_hooks.go:73-86 before scorer/latency/plugin.go:189-202 and prediction.go:149-161).  With
+  // TrackRunningRequests each request is added to its TargetEndpoints[0]'s queue inside the call, under its x-request-id, so
+  // PreRequest does not add it again; ResponseComplete, RequestExpired and RemovePod remove it as before.  Without
+  // TrackRunningRequests the queues are read, never changed.  A batch cut into LoRA pieces runs its pieces in order.  Refused
+  // without InOrderInFlightLoad, with LatencyPredictionInfo (eppscore_predict_latency after the batch would read the queues the
+  // batch left), with device filters, with the Profiles list, with MaxNumOfEndpoints > 1 and with an engine library without
+  // the call.
+  bool InOrderRunningRequests = false;
 };
 
 class Scheduler {
@@ -487,9 +504,10 @@ class Scheduler {
       if (!inflight_) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs the inflight-load-producer (InFlightLoad)");
       if (!cfg0.Profiles.empty()) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad serves the single-profile config, not the Profiles list");
       if (cfg.Profile.picker().MaxNumOfEndpoints > 1) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs maxNumOfEndpoints == 1");
-      for (const auto& w : sc)
-        if (dynamic_cast<const LatencyScorer*>(w.Scorer_.get()))
-          throw SchedulingError("SchedulerConfig::InOrderInFlightLoad cannot order the latency scorer's inputs");
+      if (!cfg0.InOrderRunningRequests)
+        for (const auto& w : sc)
+          if (dynamic_cast<const LatencyScorer*>(w.Scorer_.get()))
+            throw SchedulingError("SchedulerConfig::InOrderInFlightLoad cannot order the latency scorer's inputs");
       if (!EngineHasInOrderLoad())
         throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs an engine library with eppscore_schedule_batch_inorder");
       inorder_ = true;
@@ -500,9 +518,25 @@ class Scheduler {
       if (cfg.LatencyPredictionInfo)
         throw SchedulingError("SchedulerConfig::InOrderPrefixIndex cannot give LatencyPredictionInfo: the prediction would read the "
                               "prefix index the batch left");
-      if (!EngineHasInOrderPrefixIndex())
+      if (!(cfg0.InOrderRunningRequests ? EngineHasInOrderLatency() : EngineHasInOrderPrefixIndex()))  // (the route's one call)
         throw SchedulingError("SchedulerConfig::InOrderPrefixIndex needs an engine library with eppscore_schedule_batch_inorder_index");
       inorder_index_ = true;
+    }
+    if (cfg0.InOrderRunningRequests) {
+      if (!cfg0.InOrderInFlightLoad) throw SchedulingError("SchedulerConfig::InOrderRunningRequests needs InOrderInFlightLoad");
+      if (!cfg0.Profiles.empty()) throw SchedulingError("SchedulerConfig::InOrderRunningRequests serves the single-profile config, not the Profiles list");
+      if (cfg.Profile.picker().MaxNumOfEndpoints > 1) throw SchedulingError("SchedulerConfig::InOrderRunningRequests needs maxNumOfEndpoints == 1");
+      bool lat = false;
+      for (const auto& w : sc) lat = lat || dynamic_cast<const LatencyScorer*>(w.Scorer_.get()) != nullptr;
+      if (!lat) throw SchedulingError("SchedulerConfig::InOrderRunningRequests needs a profile with a latency-scorer");
+      if (!cfg.Profile.device_filters().empty())
+        throw SchedulingError("SchedulerConfig::InOrderRunningRequests does not order the device filters");
+      if (cfg.LatencyPredictionInfo)
+        throw SchedulingError("SchedulerConfig::InOrderRunningRequests cannot give LatencyPredictionInfo: the prediction would read "
+                              "the running-request queues the batch left");
+      if (!EngineHasInOrderLatency())
+        throw SchedulingError("SchedulerConfig::InOrderRunningRequests needs an engine library with eppscore_schedule_batch_inorder_latency");
+      inorder_latency_ = true;
     }
     running_ = cfg.Profile.producer() && cfg.Profile.producer()->TrackRunningRequests;
     if (running_ && !EngineHasRunningQueues())
@@ -837,7 +871,40 @@ class Scheduler {
         all_scores.resize((size_t)R * Mx);
         b.scores_out = all_scores.data();
       }
-      if (inorder_index_) {  // ... and each pick's blocks, in request order: PreRequest commits nothing more
+      if (inorder_latency_) {  // ... and each request joins its pick's running-request queue: PreRequest adds nothing more
+        const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
+        std::vector<int32_t> caps;
+        eppscore_inorder_index x{};
+        if (inorder_index_) {
+          last_endpoints_ = &endpoints;  // (LruCapacities reads the batch's list)
+          last_ids_ = ids;
+          last_rows_ = Mx;
+          caps = LruCapacities();
+          pick_match.assign((size_t)R, 0);
+          x.struct_size = sizeof(x);
+          x.lru_capacity = caps.data();
+          x.pick_match = pick_match.data();
+        }
+        std::vector<uint64_t> key;
+        std::vector<uint8_t> added((size_t)R, 0);
+        if (running_) {  // the batch's x-request-ids (KeyFor); no id: key 0, not tracked
+          key.assign((size_t)R, 0);
+          for (int r = 0; r < R; r++)
+            if (!requests[r].RequestId.empty()) key[(size_t)r] = KeyFor(requests[r].RequestId);
+        }
+        eppscore_inorder_running q{};
+        q.struct_size = sizeof(q);
+        q.request_key = running_ ? key.data() : nullptr;
+        q.added_out = added.data();
+        Check(eppscore_schedule_batch_inorder_latency(eng_, &b, est.data(), inorder_index_ ? &x : nullptr, &q),
+              "eppscore_schedule_batch_inorder_latency");
+        if (running_)
+          for (int r = 0; r < R; r++) {
+            if (key[(size_t)r] == 0) continue;
+            if (added[(size_t)r]) running_keys_[requests[r].RequestId].endpoints.push_back(pick[r]);
+            else ReleaseKeyIfUnused(requests[r].RequestId);  // refused (already live there, a negative tpot, or no pick)
+          }
+      } else if (inorder_index_) {  // ... and each pick's blocks, in request order: PreRequest commits nothing more
         const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
         last_endpoints_ = &endpoints;  // (LruCapacities reads the batch's list)
         last_ids_ = ids;
@@ -922,7 +989,7 @@ class Scheduler {
       const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
       Check(eppscore_inflight_add(eng_, R, 0, pick.data(), est.data(), nullptr), "eppscore_inflight_add");
     }
-    RunningAdd(pick);
+    if (!inorder_latency_) RunningAdd(pick);  // (in order with the running queues: ScheduleBatch added them already)
   }
 
   // requestcontrol_hooks.go:73-86: (pick[r], request id, tpot) into the running-request queues, for PreRequest
@@ -1745,6 +1812,7 @@ class Scheduler {
   bool token_load_ = false;  // the profile has a token-load scorer
   bool inorder_ = false;     // SchedulerConfig::InOrderInFlightLoad
   bool inorder_index_ = false;  // SchedulerConfig::InOrderPrefixIndex
+  bool inorder_latency_ = false;  // SchedulerConfig::InOrderRunningRequests
   bool running_ = false;  // PredictedLatencyProducer::TrackRunningRequests
   std::unordered_map<std::string, KeyUse> running_keys_;
   uint64_t next_key_ = 1;

@@ -367,8 +367,8 @@ int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppsc
  * cluster shape is decided by the engine's first call, before anything is launched: ERR_CAPACITY when no cluster of the device
  * holds max_endpoints endpoints (8192 needs the non-portable cluster size 16).
  * Not ordered: the prefix index (request r+1 does not see the blocks request r adds; commit after the call, or use
- * eppscore_schedule_batch_inorder_index), the latency scorer's running queues, top-k lists, several profiles, and requests on
- * other GPU shards (each engine orders its own batch).
+ * eppscore_schedule_batch_inorder_index), the latency scorer's running queues (use eppscore_schedule_batch_inorder_latency),
+ * top-k lists, several profiles, and requests on other GPU shards (each engine orders its own batch).
  * ERR_INVALID before anything is launched: a profile 0 with the latency scorer, a current snapshot that supplies
  * inflight_tokens, dense_feat / scores_out / match_blocks / pred_out / filter_mask_out set, and what eppscore_schedule_batch
  * refuses.  ERR_NO_SNAPSHOT before eppscore_set_snapshot. */
@@ -408,11 +408,48 @@ typedef struct eppscore_inorder_index {
  * set holds it, the request is scored and picked as in eppscore_schedule_batch_inorder, and the CTA that owns the pick runs the
  * index's commit program for that one Add before the cluster barrier that the next request's probes wait for.
  * Not covered: several picks per request (the "prefill" profile's Add), several profiles and top-k lists, the latency scorer's
- * running queues, and replication across GPU shards (each engine commits its own batch inside the call; replaying an
+ * running queues (eppscore_schedule_batch_inorder_latency with x), and replication across GPU shards (each engine commits its own batch inside the call; replaying an
  * all-gathered commit stream on top would apply its commits twice, so sharding.gather_commit_stream belongs to the
  * batch-wide path).  ERR_INVALID: x NULL or a wrong struct_size, and what eppscore_schedule_batch_inorder refuses. */
 int32_t eppscore_schedule_batch_inorder_index(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens,
                                               const eppscore_inorder_index *x);
+
+/* The running-request side of eppscore_schedule_batch_inorder_latency. */
+typedef struct eppscore_inorder_running {
+  int32_t struct_size;          /* sizeof(eppscore_inorder_running) */
+  const uint64_t *request_key;  /* [R] where b->location says; NULL: the queues are read, never changed */
+  uint8_t *added_out;           /* optional [R]: 1 where request r was added to pick[r]'s queue */
+} eppscore_inorder_running;
+
+/* A batch in arrival order with profile 0's latency scorer ordered too: request r's latency scorer sees the running-request
+ * queues after requests 0..r-1 were added to them, and each request is added to its pick's queue inside the call.  The outputs
+ * (pick, pick_score, tie_count, total_blocks, hashes_out, q->added_out, and x->pick_match in the index form), the in-flight
+ * counters, the running-request view (eppscore_running_get) and, in the index form, the whole prefix index afterwards equal,
+ * bit for bit, what this loop gives:
+ *     for r in 0 .. R-1:
+ *         eppscore_schedule_batch(request r alone, request_base = b->request_base + r)
+ *         [x: pick_match[r] = eppscore_prefix_match(request r's hashes, at pick[r])]
+ *         added_out[r] = eppscore_running_add(1, &pick[r], &request_key[r], &b->tpot_slo[r])
+ *         eppscore_inflight_add(1, &pick[r], &tokens[r])
+ *         [x: eppscore_commit_picks(1, &pick[r], hashes[r], n_hashes[r], x->lru_capacity)]
+ * PreRequest adds the request to its target's queue (predictedlatency/requestcontrol_hooks.go:73-86) and the next Schedule reads
+ * the queue's count (the idle preference, scorer/latency/plugin.go:189-202) and minimum TPOT SLO (the TPOT bound,
+ * prediction.go:149-161): a batch-wide call gives every request of the batch the same view, so in an overloaded fleet every
+ * request picks the same idle endpoint, and a tight TPOT SLO does not tighten its target for the requests after it.
+ * Each request reads b->tpot_slo (the value queued), b->ttft_slo and b->input_tokens (counted from the prompt bytes when absent).
+ * An add is refused (added_out[r] = 0) as eppscore_running_add refuses it: no pick, key 0, tpot < 0, or an (endpoint, key) pair
+ * already live, before the call or from an earlier request of the batch.  x NULL: the in-flight form
+ * (eppscore_schedule_batch_inorder's walk); x set: the index form (eppscore_schedule_batch_inorder_index's walk, with its index
+ * ordering, room and capture rules).  The call is a running-queue mutation too, ordered like eppscore_running_add: room for R adds
+ * is made once per call before the walk (under CUDA-graph capture it needs eppscore_running_reserve, and in the index form
+ * eppscore_prefix_reserve), and the snapshot terms are prepared again behind it.  Per request the walk reduces the lowest tier
+ * and its headroom ranges across the cluster (with predictions, one more cluster barrier than the walk without it); each thread
+ * keeps its endpoint's running count and minimum in registers, and the owner of the pick runs the Add.
+ * ERR_INVALID before anything is launched: q NULL or a wrong struct_size, a profile 0 without the latency scorer or with device
+ * filters, request_key set while the current snapshot supplies min_tpot_slo or dispatched, a NaN tpot_slo in host arrays with
+ * request_key set, a snapshot prepared without latency params, and what the call's form refuses apart from the latency scorer. */
+int32_t eppscore_schedule_batch_inorder_latency(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens,
+                                                const eppscore_inorder_index *x, const eppscore_inorder_running *q);
 
 /* ---- several scheduler profiles (see eppscore_profile) ---- */
 /* Adds a profile; *id_out receives its id (1, 2, ...).  With a snapshot present the profile is prepared for it at once, on the
