@@ -469,7 +469,7 @@ __global__ void __launch_bounds__(kFusedWarps * 32, 5) hash_fused_kernel(HashArg
 // reads it).  The index is not snapshot data, so this kernel still runs concurrently with a snapshot preparation.
 // ---------------------------------------------------------------------------------------------
 constexpr int kWarpTileWarps = 8;
-constexpr int kProbeU = 4;     // PROBE: hashes probed per lane at a time (independent loads in flight)
+constexpr int kProbeU = 4;     // PROBE: hashes probed per lane at a time (both halves of each slot in flight: 128 registers)
 
 template <int BC, bool PROBE>
 __global__ void __launch_bounds__(kWarpTileWarps * 32, 2) hash_warp_kernel(HashArgs a) {
@@ -553,39 +553,40 @@ __global__ void __launch_bounds__(kWarpTileWarps * 32, 2) hash_warp_kernel(HashA
       // ---- PROBE: indexer.Get on the lane's own row, kProbeU blocks at a time, up to the first miss ----
       if (PROBE) {
         for (int i0 = 0; __any_sync(0xffffffffu, p_open && i0 < nb); i0 += kProbeU) {
-          uint64_t h[kProbeU], idx[kProbeU];
-          uint4 lo[kProbeU];
-          bool act[kProbeU], hit[kProbeU];
-#pragma unroll
-          for (int u = 0; u < kProbeU; u++) {
-            act[u] = p_open && i0 + u < nb;
-            h[u] = act[u] ? tile[lane][i0 + u] : 0ULL;
-            idx[u] = h[u] & slot_mask;
-          }
+          // the round's loads first: both 16-byte halves of each home slot (one 32-byte sector), so that the walk below does
+          // not wait on a dependent load per hit for the members 2..9; hashes and home indices are read back from the tile
+          uint4 lo[kProbeU], hi[kProbeU];
 #pragma unroll
           for (int u = 0; u < kProbeU; u++) {
             lo[u] = make_uint4(0u, 0u, kCntFree, 0u);
-            if (act[u]) lo[u] = ldg16(&slots[idx[u]]);
+            hi[u] = make_uint4(0u, 0u, 0u, 0u);
+            if (p_open && i0 + u < nb) {
+              const uint4* sp = reinterpret_cast<const uint4*>(&slots[tile[lane][i0 + u] & slot_mask]);
+              lo[u] = ldg16(sp);
+              hi[u] = ldg16(sp + 1);
+            }
           }
 #pragma unroll
-          for (int u = 0; u < kProbeU; u++) hit[u] = act[u] && table_find(slots, slot_mask, h[u], idx[u], lo[u]);
-#pragma unroll
           for (int u = 0; u < kProbeU; u++) {
-            if (!act[u] || !p_open) continue;
-            if (!hit[u]) {
+            if (!p_open || i0 + u >= nb) continue;
+            const uint64_t h = tile[lane][i0 + u], home = h & slot_mask;
+            uint64_t idx = home;
+            if (!table_find(slots, slot_mask, h, idx, lo[u])) {
               p_open = false;                                   // the first miss ends the matched prefix
               continue;
             }
-            // members 2..9 (the slot's second half, same 32-byte sector as the first), loaded as pick_sparse_kernel loads them
-            uint4 hi = make_uint4(0u, 0u, 0u, 0u);
-            if (!(lo[u].z & kCntRow) && (lo[u].z & kCntMask) > 2u) hi = ldg16(reinterpret_cast<const uint4*>(&slots[idx[u]]) + 1);
+            // members 2..9 (the slot's second half) count only for inline sets of more than two, as pick_sparse_kernel reads
+            // them; a key found past its home slot (a probe chain) has its second half loaded here
+            uint4 h2 = make_uint4(0u, 0u, 0u, 0u);
+            if (!(lo[u].z & kCntRow) && (lo[u].z & kCntMask) > 2u)
+              h2 = idx == home ? hi[u] : ldg16(reinterpret_cast<const uint4*>(&slots[idx]) + 1);
             if (c0 + i0 + u == 0) {
               ref_raw = lo[u].z;                                // the first hit: the reference set
               ref_w = lo[u].w;
-              ref_hi = hi;
+              ref_hi = h2;
               p_n = 1;
               if (ref_raw & kCntRow) p_ok = p_open = false;     // a bitset row: pick_sparse's exception table
-            } else if (lo[u].z != ref_raw || !same_inline_set(ref_w, ref_hi, lo[u].w, hi)) {
+            } else if (lo[u].z != ref_raw || !same_inline_set(ref_w, ref_hi, lo[u].w, h2)) {
               p_ok = p_open = false;                            // a different set: pick_sparse's exception table
             } else {
               p_n++;
