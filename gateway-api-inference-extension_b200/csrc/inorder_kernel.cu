@@ -308,7 +308,7 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
         // the lowest tier over the candidates and the |headroom| ranges inside it: warp, CTA, then cluster (barrier.cluster)
         __shared__ LatTier s_wtier[kInOrderWarps];
         __shared__ LatTier s_ctier[2];
-        LatTier t = cur.cand ? LatTier{lp.rank, aT, aT, aP, aP} : lat_tier_none();
+        LatTier t = cur.cand ? LatTier{lp.rank, lat_min_in(aT), aT, lat_min_in(aP), aP} : lat_tier_none();
         lat_tier_warp_reduce(t);
         if (lane == 0) s_wtier[warp] = t;
         __syncthreads();
@@ -334,7 +334,7 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
         const bool most = L.strategy_most && t.rank == 0;
         const double eT = tok ? __ddiv_rn(__dsub_rn(aT, t.mnT), rgT) : 0.5, eP = pok ? __ddiv_rn(__dsub_rn(aP, t.mnP), rgP) : 0.5;
         const double ec = __dadd_rn(__dmul_rn(alpha, eT), __dmul_rn(beta, eP));
-        lat_w = lp.rank == t.rank ? __double2ll_rz(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1 : 0;
+        lat_w = lp.rank == t.rank ? go_int(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1 : 0;
       } else {
         // compositeScores (plugin.go:338-360): maxQ over the candidates from 0, the candidates' queue maximum
         const long long maxq = cur.mx0 > 0 ? cur.mx0 : 0;

@@ -50,6 +50,15 @@ __device__ __forceinline__ double lat_lim(double pod_min, double buffer) {
 }
 __device__ __forceinline__ bool lat_idle(int dispatched) { return dispatched == 0; }
 
+// An endpoint's |headroom| as it enters its tier's minimum: scoreBucket (plugin.go:262-318) starts the minimum at
+// math.MaxFloat64 and lowers it with h < min, so an infinite headroom (an infinite SLO) leaves it at MaxFloat64, not +Inf.
+__device__ __forceinline__ double lat_min_in(double h) { return h < 1.7976931348623157e308 ? h : 1.7976931348623157e308; }
+
+// Go's int(x) on amd64 (CVTTSD2SQ) for scoreBucket's weight: truncation toward zero, and NaN as math.MinInt64, which the score
+// range then clamps to 0.  The weight is NaN for an infinite headroom in a tier whose range is infinite ((+Inf - MaxFloat64) /
+// +Inf), so NaN is mapped here explicitly rather than left to __double2ll_rz.
+__device__ __forceinline__ long long go_int(double x) { return x == x ? __double2ll_rz(x) : (long long)0x8000000000000000ULL; }
+
 // The inputs of latency_info_kernel beyond the match lookup's (DeviceIndex::latency_info): the engine's prepared snapshot
 // (LatArgs' tiles and scalars) and the running-request view, plus the requests' own inputs and the output records.
 struct LatInfoArgs {

@@ -465,9 +465,10 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
             const int rk = cand ? lp.rank : 5;
             const double aT = fabs(lp.hT), aP = fabs(lp.hP);
             const bool better = rk < rank_l, same = rk == rank_l;
-            mnT = (better || (same && aT < mnT)) ? aT : mnT;
+            const double iT = lat_min_in(aT), iP = lat_min_in(aP);
+            mnT = (better || (same && iT < mnT)) ? iT : mnT;
             mxT = (better || (same && aT > mxT)) ? aT : mxT;
-            mnP = (better || (same && aP < mnP)) ? aP : mnP;
+            mnP = (better || (same && iP < mnP)) ? iP : mnP;
             mxP = (better || (same && aP > mxP)) ? aP : mxP;
             rank_l = better ? rk : rank_l;
           }
@@ -614,12 +615,12 @@ __global__ void __launch_bounds__(kMatrixWarps * 32, TOPK ? 1 : 0) score_matrix_
               const double v = most ? __dmul_rn(comb, 100.0) : __dmul_rn(__dsub_rn(1.0, comb), 100.0);
               const int vn = __double2int_rn(v);
               const bool in_tier = lp.rank == l_sel;
-              w = in_tier ? __double2ll_rz(v) + 1 : 0;                         // float64(int(x) + minWeight + 1); 0 outside the tier
+              w = in_tier ? go_int(v) + 1 : 0;                                 // float64(int(x) + minWeight + 1); 0 outside the tier
               const bool redo = in_tier && (!l_fast || fabs(__dsub_rn(v, (double)vn)) < 1e-9);
               if (__any_sync(0xffffffffu, redo)) {                             // warp-uniform: scoreBucket, plugin.go:281-306, exactly
                 const double eT = l_tok ? __ddiv_rn(dT, l_rgT) : 0.5, eP = l_pok ? __ddiv_rn(dP, l_rgP) : 0.5;
                 const double ec = __dadd_rn(__dmul_rn(l_alpha, eT), __dmul_rn(l_beta, eP));
-                const long long we = __double2ll_rz(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1;
+                const long long we = go_int(most ? __dmul_rn(ec, 100.0) : __dmul_rn(__dsub_rn(1.0, ec), 100.0)) + 1;
                 w = redo ? we : w;
               }
             } else {                                                           // compositeScores, plugin.go:346-360
