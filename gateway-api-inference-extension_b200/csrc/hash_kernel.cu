@@ -467,14 +467,22 @@ __global__ void __launch_bounds__(kFusedWarps * 32, 5) hash_fused_kernel(HashArg
 // new hashes while the tile holds them, exactly as pick_sparse_kernel would, and a request whose matched blocks all carry its
 // first hit's inline set is RESOLVED: its ProbeRec holds the count and the set, and its row of hashes is not written (nothing
 // reads it).  The index is not snapshot data, so this kernel still runs concurrently with a snapshot preparation.
+// With PROBE, A, B and PROBE run per chunk of kProbeChunk blocks of every request, and A skips the requests whose walk ended
+// at a miss while still resolvable: nothing reads their hashes past that miss, so their bytes are never loaded.  Every other
+// request (one that meets a set change or a bitset row, a trailing partial block, the generic path) streams its whole row.
 // ---------------------------------------------------------------------------------------------
 constexpr int kWarpTileWarps = 8;
 constexpr int kProbeU = 4;     // PROBE: hashes probed per lane at a time (both halves of each slot in flight: 128 registers)
+constexpr int kProbeChunk = 4; // PROBE: blocks per request streamed, chained and probed before the next chunk
 
 template <int BC, bool PROBE>
 __global__ void __launch_bounds__(kWarpTileWarps * 32, 2) hash_warp_kernel(HashArgs a) {
+  // phase A's lanes: K blocks of G requests per step, K steps per chunk (the plain form: one request of 32 blocks per step)
+  constexpr int K = PROBE ? kProbeChunk : 32, G = 32 / K;
+  static_assert(K * G == 32 && K % kProbeU == 0, "a chunk is a whole number of probe rounds and divides a warp");
   extern __shared__ __align__(16) unsigned char hw_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int sub = lane / K, kb = lane % K;  // phase A: this lane's request within a step, and its block within the chunk
   uint64_t(*tile)[33] = reinterpret_cast<uint64_t(*)[33]>(hw_smem) + (size_t)warp * 32;
   const int bc = BC ? BC : a.block_chars;
   const int ntiles = (a.R + 31) / 32;
@@ -505,99 +513,108 @@ __global__ void __launch_bounds__(kWarpTileWarps * 32, 2) hash_warp_kernel(HashA
     uint32_t p_n = 0, ref_raw = 0, ref_w = 0;
     uint4 ref_hi = make_uint4(0u, 0u, 0u, 0u);
     for (int c0 = 0; c0 < maxfull; c0 += 32) {
-      const int blk = c0 + lane;
-      // ---- A: body states ----
-      if (BC == 64) {
-        uint4 buf[3][4];  // a ring: request rq digested while rq+1 and rq+2 are in flight (indices compile-time after unrolling)
-        bool on[3];
-        auto fetch = [&](int rq, uint4 (&dst)[4], bool& o) {
-          const int nf = __shfl_sync(0xffffffffu, nf_mine, rq);
-          const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq);
-          o = blk < nf;
-          if (o) {
-            const uint8_t* q = reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * 64;
+      for (int s0 = 0; s0 < 32; s0 += K) {  // chunks of this 32-block window (one in the plain form)
+        const int cb = c0 + s0, blk = cb + kb;
+        // blocks of this lane's request still hashed: a resolved request stops at its first miss (nothing reads its row)
+        const int nf_str = (PROBE && p_ok && !p_open) ? 0 : nf_mine;
+        if (PROBE && !__any_sync(0xffffffffu, cb < nf_str)) break;
+        // ---- A: body states ----
+        if (BC == 64) {
+          uint4 buf[3][4];  // a ring: step st digested while st+1 and st+2 are in flight (indices compile-time after unrolling)
+          bool on[3];
+          auto fetch = [&](int st, uint4 (&dst)[4], bool& o) {
+            const int rq = st * G + sub;
+            const int nf = __shfl_sync(0xffffffffu, nf_str, rq);
+            const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq);
+            o = blk < nf;
+            if (o) {
+              const uint8_t* q = reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * 64;
 #pragma unroll
-            for (int k = 0; k < 4; k++) dst[k] = ldg16(q + 16 * k);
+              for (int k = 0; k < 4; k++) dst[k] = ldg16(q + 16 * k);
+            }
+          };
+          fetch(0, buf[0], on[0]);
+          fetch(1, buf[1], on[1]);
+#pragma unroll (PROBE ? K : 1)  // the probing form: every step unrolled (no spill at 128 registers)
+          for (int st0 = 0; st0 < K; st0 += 3) {
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+              const int st = st0 + j;
+              if (st < K) {
+                const int ns = (j + 2) % 3;
+                on[ns] = false;
+                if (st + 2 < K) fetch(st + 2, buf[ns], on[ns]);
+                if (on[j]) tile[st * G + sub][s0 + kb] = body_state_64(buf[j]);
+              }
+            }
           }
-        };
-        fetch(0, buf[0], on[0]);
-        fetch(1, buf[1], on[1]);
+        } else {
 #pragma unroll 1
-        for (int rq0 = 0; rq0 < 32; rq0 += 3) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) {
-            const int rq = rq0 + j;
-            if (rq < 32) {
-              const int ns = (j + 2) % 3;
-              on[ns] = false;
-              if (rq + 2 < 32) fetch(rq + 2, buf[ns], on[ns]);
-              if (on[j]) tile[rq][lane] = body_state_64(buf[j]);
-            }
+          for (int st = 0; st < K; st++) {
+            const int rq = st * G + sub;
+            const int nf = __shfl_sync(0xffffffffu, nf_str, rq);
+            const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq);
+            if (blk < nf)
+              tile[rq][s0 + kb] = block_body_state<BC>(reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * bc, bc);
           }
         }
-      } else {
-#pragma unroll 1
-        for (int rq = 0; rq < 32; rq++) {
-          const int nf = __shfl_sync(0xffffffffu, nf_mine, rq);
-          const unsigned long long pp = __shfl_sync(0xffffffffu, (unsigned long long)reinterpret_cast<uintptr_t>(d.p), rq);
-          if (blk < nf) tile[rq][lane] = block_body_state<BC>(reinterpret_cast<const uint8_t*>((uintptr_t)pp) + (size_t)blk * bc, bc);
+        __syncwarp();
+        // ---- B: the chain, lane = request ----
+        const int nb = min(K, nf_str - cb);
+        for (int i = 0; i < nb; i++) {
+          prev = xchain_aligned(tile[lane][s0 + i], prev);
+          tile[lane][s0 + i] = prev;
         }
-      }
-      __syncwarp();
-      // ---- B: the chain, lane = request ----
-      const int nb = min(32, nf_mine - c0);
-      for (int i = 0; i < nb; i++) {
-        prev = xchain_aligned(tile[lane][i], prev);
-        tile[lane][i] = prev;
-      }
-      // ---- PROBE: indexer.Get on the lane's own row, kProbeU blocks at a time, up to the first miss ----
-      if (PROBE) {
-        for (int i0 = 0; __any_sync(0xffffffffu, p_open && i0 < nb); i0 += kProbeU) {
-          // the round's loads first: both 16-byte halves of each home slot (one 32-byte sector), so that the walk below does
-          // not wait on a dependent load per hit for the members 2..9; hashes and home indices are read back from the tile
-          uint4 lo[kProbeU], hi[kProbeU];
+        // ---- PROBE: indexer.Get on the lane's own row, kProbeU blocks at a time, up to the first miss ----
+        if (PROBE) {
+          for (int i0 = 0; __any_sync(0xffffffffu, p_open && i0 < nb); i0 += kProbeU) {
+            // the round's loads first: both 16-byte halves of each home slot (one 32-byte sector), so that the walk below does
+            // not wait on a dependent load per hit for the members 2..9; hashes and home indices are read back from the tile
+            uint4 lo[kProbeU], hi[kProbeU];
 #pragma unroll
-          for (int u = 0; u < kProbeU; u++) {
-            lo[u] = make_uint4(0u, 0u, kCntFree, 0u);
-            hi[u] = make_uint4(0u, 0u, 0u, 0u);
-            if (p_open && i0 + u < nb) {
-              const uint4* sp = reinterpret_cast<const uint4*>(&slots[tile[lane][i0 + u] & slot_mask]);
-              lo[u] = ldg16(sp);
-              hi[u] = ldg16(sp + 1);
+            for (int u = 0; u < kProbeU; u++) {
+              lo[u] = make_uint4(0u, 0u, kCntFree, 0u);
+              hi[u] = make_uint4(0u, 0u, 0u, 0u);
+              if (p_open && i0 + u < nb) {
+                const uint4* sp = reinterpret_cast<const uint4*>(&slots[tile[lane][s0 + i0 + u] & slot_mask]);
+                lo[u] = ldg16(sp);
+                hi[u] = ldg16(sp + 1);
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < kProbeU; u++) {
+              if (!p_open || i0 + u >= nb) continue;
+              const uint64_t h = tile[lane][s0 + i0 + u], home = h & slot_mask;
+              uint64_t idx = home;
+              if (!table_find(slots, slot_mask, h, idx, lo[u])) {
+                p_open = false;                                   // the first miss ends the matched prefix
+                continue;
+              }
+              // members 2..9 (the slot's second half) count only for inline sets of more than two, as pick_sparse_kernel reads
+              // them; a key found past its home slot (a probe chain) has its second half loaded here
+              uint4 h2 = make_uint4(0u, 0u, 0u, 0u);
+              if (!(lo[u].z & kCntRow) && (lo[u].z & kCntMask) > 2u)
+                h2 = idx == home ? hi[u] : ldg16(reinterpret_cast<const uint4*>(&slots[idx]) + 1);
+              if (cb + i0 + u == 0) {
+                ref_raw = lo[u].z;                                // the first hit: the reference set
+                ref_w = lo[u].w;
+                ref_hi = h2;
+                p_n = 1;
+                if (ref_raw & kCntRow) p_ok = p_open = false;     // a bitset row: pick_sparse's exception table
+              } else if (lo[u].z != ref_raw || !same_inline_set(ref_w, ref_hi, lo[u].w, h2)) {
+                p_ok = p_open = false;                            // a different set: pick_sparse's exception table
+              } else {
+                p_n++;
+              }
             }
           }
-#pragma unroll
-          for (int u = 0; u < kProbeU; u++) {
-            if (!p_open || i0 + u >= nb) continue;
-            const uint64_t h = tile[lane][i0 + u], home = h & slot_mask;
-            uint64_t idx = home;
-            if (!table_find(slots, slot_mask, h, idx, lo[u])) {
-              p_open = false;                                   // the first miss ends the matched prefix
-              continue;
-            }
-            // members 2..9 (the slot's second half) count only for inline sets of more than two, as pick_sparse_kernel reads
-            // them; a key found past its home slot (a probe chain) has its second half loaded here
-            uint4 h2 = make_uint4(0u, 0u, 0u, 0u);
-            if (!(lo[u].z & kCntRow) && (lo[u].z & kCntMask) > 2u)
-              h2 = idx == home ? hi[u] : ldg16(reinterpret_cast<const uint4*>(&slots[idx]) + 1);
-            if (c0 + i0 + u == 0) {
-              ref_raw = lo[u].z;                                // the first hit: the reference set
-              ref_w = lo[u].w;
-              ref_hi = h2;
-              p_n = 1;
-              if (ref_raw & kCntRow) p_ok = p_open = false;     // a bitset row: pick_sparse's exception table
-            } else if (lo[u].z != ref_raw || !same_inline_set(ref_w, ref_hi, lo[u].w, h2)) {
-              p_ok = p_open = false;                            // a different set: pick_sparse's exception table
-            } else {
-              p_n++;
-            }
-          }
+          if (cb + K >= nf_mine) p_open = false;                  // the whole row matched
         }
-        if (c0 + 32 >= nf_mine) p_open = false;                 // the whole row matched
+        __syncwarp();
       }
       // a resolved row whose walk is over is not written: nothing reads it
       const int nf_out = (PROBE && p_ok && !p_open) ? 0 : nf_mine;
-      __syncwarp();
+      const int blk = c0 + lane;
       // ---- C: hashes out ----
 #pragma unroll 4
       for (int rq = 0; rq < 32; rq++) {
