@@ -89,6 +89,11 @@ class InOrderRunning(C.Structure):
     _fields_ = [("struct_size", C.c_int32), ("request_key", C.c_void_p), ("added_out", C.c_void_p)]
 
 
+class InOrderProfiles(C.Structure):
+    _fields_ = [("struct_size", C.c_int32), ("index", C.c_int32), ("primary_run", C.c_int32), ("prefill_run", C.c_int32),
+                ("run_mask", C.c_void_p), ("lru_capacity", C.c_void_p), ("pick_match", C.c_void_p * MAX_PROFILES)]
+
+
 class TopK(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("k", C.c_int32), ("endpoints", C.c_void_p), ("scores", C.c_void_p)]
 
@@ -130,6 +135,8 @@ ABI_SYMBOLS = [
     ("eppscore_add_profile", C.c_int32, [_P, C.POINTER(Profile), C.POINTER(C.c_int32)]),
     ("eppscore_set_profile_endpoints", C.c_int32, [_P, C.c_int32, _P, C.c_int32]),
     ("eppscore_schedule_batch_profiles", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun)]),
+    ("eppscore_schedule_batch_inorder_profiles", C.c_int32, [_P, C.POINTER(Batch), _P, C.c_int32, C.POINTER(ProfileRun),
+                                                             C.POINTER(InOrderProfiles)]),
     ("eppscore_schedule_batch_profiles_topk", C.c_int32, [_P, C.POINTER(Batch), C.c_int32, C.POINTER(ProfileRun),
                                                           C.POINTER(TopK)]),
     ("eppscore_hash_prompts", C.c_int32, [_P, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),

@@ -144,6 +144,8 @@ struct eppscore_engine {
         // outside a capture for a fixed number of rows and never reallocated, like `wide`.
         s_io_match, s_io_total, s_io_minmax,
         s_pmatch,  // pick_match of an in-order batch that commits as it schedules
+        s_runmask,  // run_mask of an in-order profiles batch
+        s_io_room,  // an in-order profiles slice's totals twice over: the room of its primary and prefill Adds
         s_rkey, s_added;  // request keys and added_out of an in-order batch that adds to the running-request queues
     int32_t io_rows = 0;
     // score rows of a wide top-k batch's slice ([wide_rows][Mpad] float64, schedule_wide).  Allocated by the first call that
@@ -169,6 +171,8 @@ struct eppscore_engine {
   int32_t io_cluster = 0;          // CTAs per cluster of inorder_pick_kernel (0: not decided yet)
   int32_t io_index_cluster = 0;    // CTAs per cluster of inorder_index_kernel (0: not decided yet)
   int32_t io_lat_cluster = 0, io_lat_index_cluster = 0;  // the same for their latency forms (the _lat kernels)
+  int32_t io_prof_cluster[2] = {0, 0};  // the same for the profiles walk, in-flight and index form
+  size_t io_prof_smem[2] = {0, 0};      // the dynamic shared memory the profiles walk may use, per form
   int32_t host_chunk = 8192;       // requests per chunk of a host-location batch (eppscore_set_debug key 3)
   // device-location batches cut into `dev_split` slices over `dev_streams` streams (the caller's + internal ones): the
   // HBM-bound body hashing of slice i+1 runs under the latency-bound chain and probe kernels of slice i
@@ -434,6 +438,7 @@ struct DevRun {
   double* scores_out;
   double* pred_out;
   uint32_t* filter_mask_out;
+  uint16_t* pick_match;  // [R] an in-order profiles batch's matchBlocks at this run's pick (eppscore_inorder_profiles)
   int32_t topk;          // > 0: topk_m / topk_score [R*topk] are written
   int32_t* topk_m;
   double* topk_score;
@@ -464,6 +469,7 @@ struct DevBatch {  // all device pointers
   uint16_t* pick_match;     // [R] an in-order batch's matchBlocks at each pick (schedule_inorder_index)
   const uint64_t* request_key;  // [R] an in-order latency batch's running-request keys (eppscore_inorder_running)
   uint8_t* added_out;       // [R] its added flags
+  const uint8_t* run_mask;  // [R] an in-order profiles batch's runs per request (eppscore_inorder_profiles)
   int32_t n_runs;
   DevRun run[EPPSCORE_MAX_PROFILES];
 };
@@ -506,6 +512,7 @@ void for_each_row_array(DevBatch& d, size_t M, F&& f) {
     f(r.filter_mask_out, mw, Rows::out, &Scratch::s_fmask);
     f(r.topk_m, (size_t)r.topk, Rows::small, &Scratch::s_topk_m);
     f(r.topk_score, (size_t)r.topk, Rows::small, &Scratch::s_topk_s);
+    f(r.pick_match, 1, Rows::small, &Scratch::s_pmatch);
   }
   f(d.match_blocks, M, Rows::out, &Scratch::s_match);
   f(d.total_blocks, 1, Rows::small, &Scratch::s_total);
@@ -513,6 +520,7 @@ void for_each_row_array(DevBatch& d, size_t M, F&& f) {
   f(d.pick_match, 1, Rows::small, &Scratch::s_pmatch);
   f(d.request_key, 1, Rows::in, &Scratch::s_rkey);
   f(d.added_out, 1, Rows::small, &Scratch::s_added);
+  f(d.run_mask, 1, Rows::in, &Scratch::s_runmask);
 }
 
 // Rows [base, base + n) of a batch.
@@ -1561,10 +1569,10 @@ int32_t index_status(eppscore_engine* e, cudaError_t c, const char* what) {
   return cuda_fail(e, c, what);
 }
 
-// The slice-independent arguments of the in-order walk for profile 0 of the current snapshot; *minmax: whether the profile has
-// a queue or running scorer (the walk then reads the candidates' min / max).
-InOrderArgs inorder_args(eppscore_engine* e, bool* minmax) {
-  const Profile& P = e->prof[0];
+// The slice-independent arguments of the in-order walk for profile p (default 0) of the current snapshot; *minmax: whether the
+// profile has a queue or running scorer (the walk then reads the candidates' min / max).
+InOrderArgs inorder_args(eppscore_engine* e, bool* minmax, int p = 0) {
+  const Profile& P = e->prof[p];
   const eppscore_config& c = P.cfg;
   InOrderArgs a{};
   a.M = e->M;
@@ -1618,6 +1626,25 @@ void inorder_lat_slice(InOrderLatArgs& lt, const DevBatch& q, const int32_t* fie
   lt.added_out = q.added_out;
 }
 
+// The slice scratch of the in-order calls on a stream's scratch set: match rows, totals, a candidate min / max per profile run
+// and the profiles walk's room totals, for a fixed number of rows.  Allocated by the first in-order call on the set, which must
+// run outside a CUDA-graph capture, and never reallocated.
+int32_t inorder_scratch(eppscore_engine* e, Scratch& sc, bool capturing) {
+  if (sc.s_io_match.p) return EPPSCORE_OK;
+  if (capturing)
+    return fail(e, EPPSCORE_ERR_CAPACITY,
+                "the first in-order call on a stream allocates its slice scratch: make one call outside the CUDA-graph capture "
+                "first");
+  int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
+  if (sc.rows > 0) rows = std::min(rows, sc.rows);
+  CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
+  CK(e, sc.s_io_total.reserve((size_t)rows * 2));
+  CK(e, sc.s_io_minmax.reserve((size_t)rows * 32 * EPPSCORE_MAX_PROFILES));
+  CK(e, sc.s_io_room.reserve((size_t)rows * 4));
+  sc.io_rows = rows;
+  return EPPSCORE_OK;
+}
+
 // A slice's per-request arguments of the walk.
 void inorder_slice(InOrderArgs& a, const DevBatch& q) {
   a.R = q.R;
@@ -1637,18 +1664,7 @@ void inorder_slice(InOrderArgs& a, const DevBatch& q) {
 // so the next slice continues from them.  lat: the latency form (inorder_pick_lat_kernel), whose input token counts are those
 // schedule_device counted into sc.s_fields when the batch supplies none.
 int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, bool lat) {
-  if (!sc.s_io_match.p) {
-    if (is_capturing(s))
-      return fail(e, EPPSCORE_ERR_CAPACITY,
-                  "the first eppscore_schedule_batch_inorder on a stream allocates its slice scratch: make one call outside the "
-                  "CUDA-graph capture first");
-    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
-    if (sc.rows > 0) rows = std::min(rows, sc.rows);
-    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
-    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
-    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
-    sc.io_rows = rows;
-  }
+  if (int32_t rc = inorder_scratch(e, sc, is_capturing(s)); rc != EPPSCORE_OK) return rc;
   bool minmax = false;
   InOrderArgs a = inorder_args(e, &minmax);
   InOrderLatArgs lt = inorder_lat_args(e);
@@ -1682,30 +1698,56 @@ int32_t schedule_inorder(eppscore_engine* e, const DevBatch& d, cudaStream_t s, 
 // (DeviceIndex::ordered_room), then inorder_index_kernel, which reads each request's match counts from the index as it stands
 // and commits the request's blocks at its pick before the next request probes.  lat: the latency form (inorder_index_lat_kernel),
 // which counts the input tokens of the prompt bytes itself when the batch supplies none.
-int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, const DeviceIndex::OrderedRefs& refs,
-                               bool capturing, bool lat) {
-  const int32_t mb = d.max_blocks;
+// The index form's slice scratch (inorder_scratch, plus a hash scratch of its rows when the batch hashes prompts without
+// hashes_out), and what it refuses of the batch's hash inputs.
+int32_t inorder_hash_scratch(eppscore_engine* e, const DevBatch& d, Scratch& sc, bool capturing) {
   const bool hashing = !d.hashes_in && d.prompt_bytes;
-  if (hashing && mb > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
+  if (hashing && d.max_blocks > EPPSCORE_MAX_BLOCKS) return fail(e, EPPSCORE_ERR_CAPACITY, "max_blocks > 65535");
   if (d.hashes_in && (!d.n_hashes_in || d.hash_stride <= 0)) return fail(e, EPPSCORE_ERR_INVALID, "hashes_in needs n_hashes_in and hash_stride");
-  if (!sc.s_io_match.p) {
-    if (capturing)
-      return fail(e, EPPSCORE_ERR_CAPACITY,
-                  "the first in-order call on a stream allocates its slice scratch: make one call outside the CUDA-graph capture "
-                  "first");
-    int32_t rows = (int32_t)std::max<size_t>(1, kInOrderSliceBytes / ((size_t)e->geo.Mpad * 2));
-    if (sc.rows > 0) rows = std::min(rows, sc.rows);
-    CK(e, sc.s_io_match.reserve((size_t)rows * e->geo.Mpad * 2));
-    CK(e, sc.s_io_total.reserve((size_t)rows * 2));
-    CK(e, sc.s_io_minmax.reserve((size_t)rows * 32));
-    sc.io_rows = rows;
-  }
-  const size_t hash_bytes = hashing && !d.hashes_out ? (size_t)std::min(sc.io_rows, d.R) * mb * 8 : 0;
+  if (int32_t rc = inorder_scratch(e, sc, capturing); rc != EPPSCORE_OK) return rc;
+  const size_t hash_bytes = hashing && !d.hashes_out ? (size_t)std::min(sc.io_rows, d.R) * d.max_blocks * 8 : 0;
   if (hash_bytes > sc.s_hashes.bytes) {
     if (capturing) return fail(e, EPPSCORE_ERR_CAPACITY, "schedule_batch_inorder_index under CUDA-graph capture: the hash scratch "
                                                          "is smaller than this batch needs (make the same call outside the capture first)");
     CK(e, sc.s_hashes.reserve(hash_bytes));
   }
+  return EPPSCORE_OK;
+}
+// The index form's hash stage of slice q: its plain form (hashes and totals into the scratch, or the caller's hashes_out /
+// total_blocks), supplied hashes read where they are, or 0 blocks without prompts; sets ix->hashes / stride.
+int32_t inorder_hash_slice(eppscore_engine* e, const DevBatch& q, cudaStream_t s, Scratch& sc, uint16_t* total, InOrderIndexArgs* ix) {
+  if (!q.hashes_in && q.prompt_bytes) {
+    HashArgs h{};
+    h.R = q.R;
+    h.bytes = q.prompt_bytes;
+    h.off = q.prompt_off;
+    h.len = q.prompt_len;
+    h.seed = q.model_seed;
+    h.block_chars = q.block_chars;
+    h.max_blocks = q.max_blocks;
+    h.hashes = q.hashes_out ? q.hashes_out : sc.s_hashes.as<uint64_t>();
+    h.stride = q.max_blocks;
+    h.n_hashes = total;
+    h.stage_mask = e->hash_stage_mask;
+    e->launches += launch_hash_prompts(h, s, e->sm_count);
+    ix->hashes = h.hashes;
+    ix->stride = q.max_blocks;
+  } else if (q.hashes_in) {
+    CK(e, cudaMemcpyAsync(total, q.n_hashes_in, (size_t)q.R * 2, cudaMemcpyDeviceToDevice, s));
+    ix->hashes = q.hashes_in;
+    ix->stride = q.hash_stride;
+  } else {  // no prompts: every request has 0 blocks
+    CK(e, cudaMemsetAsync(total, 0, (size_t)q.R * 2, s));
+    ix->hashes = nullptr;
+    ix->stride = 1;
+  }
+  CK(e, cudaGetLastError());
+  return EPPSCORE_OK;
+}
+
+int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc, const DeviceIndex::OrderedRefs& refs,
+                               bool capturing, bool lat) {
+  if (int32_t rc = inorder_hash_scratch(e, d, sc, capturing); rc != EPPSCORE_OK) return rc;
   bool wait_snapshot = false;
   if (int32_t rc = reader_begin(e, s, nullptr, &wait_snapshot); rc != EPPSCORE_OK) return rc;
   const bool count = lat && !d.input_tokens && d.prompt_bytes && d.prompt_off;
@@ -1724,32 +1766,7 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
   for (int32_t base = 0; base < d.R; base += sc.io_rows) {
     const DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
     uint16_t* total = q.total_blocks ? q.total_blocks : sc.s_io_total.as<uint16_t>();
-    if (hashing) {
-      HashArgs h{};
-      h.R = q.R;
-      h.bytes = q.prompt_bytes;
-      h.off = q.prompt_off;
-      h.len = q.prompt_len;
-      h.seed = q.model_seed;
-      h.block_chars = q.block_chars;
-      h.max_blocks = mb;
-      h.hashes = q.hashes_out ? q.hashes_out : sc.s_hashes.as<uint64_t>();
-      h.stride = mb;
-      h.n_hashes = total;
-      h.stage_mask = e->hash_stage_mask;
-      e->launches += launch_hash_prompts(h, s, e->sm_count);
-      ix.hashes = h.hashes;
-      ix.stride = mb;
-    } else if (q.hashes_in) {
-      CK(e, cudaMemcpyAsync(total, q.n_hashes_in, (size_t)q.R * 2, cudaMemcpyDeviceToDevice, s));
-      ix.hashes = q.hashes_in;
-      ix.stride = q.hash_stride;
-    } else {  // no prompts: every request has 0 blocks
-      CK(e, cudaMemsetAsync(total, 0, (size_t)q.R * 2, s));
-      ix.hashes = nullptr;
-      ix.stride = 1;
-    }
-    CK(e, cudaGetLastError());
+    if (int32_t rc = inorder_hash_slice(e, q, s, sc, total, &ix); rc != EPPSCORE_OK) return rc;
     if (count)
       e->launches += launch_count_fields(q.prompt_bytes, q.prompt_off, q.prompt_len, q.R, sc.s_fields.as<int32_t>(), s, e->sm_count);
     inorder_lat_slice(lt, q, count ? sc.s_fields.as<int32_t>() : nullptr);
@@ -1773,6 +1790,111 @@ int32_t schedule_inorder_index(eppscore_engine* e, const DevBatch& d, cudaStream
   return EPPSCORE_OK;
 }
 
+// eppscore_schedule_batch_inorder_profiles on device buffers, asynchronous on `s`: the slices of schedule_inorder (refs null,
+// the in-flight form: the batch kernels of one run give the match rows and totals) or of schedule_inorder_index (refs set, the
+// index form: the hash stage, and room for the slice's Σ n_hashes once per Add a request can make), then each run's candidate
+// min / max where its profile reads them, then one profiles walk over the slice.
+int32_t schedule_inorder_profiles(eppscore_engine* e, const DevBatch& d, cudaStream_t s, Scratch& sc,
+                                  const DeviceIndex::OrderedRefs* refs, bool capturing, const eppscore_inorder_profiles& x) {
+  const bool index = refs != nullptr;
+  int32_t rc = index ? inorder_hash_scratch(e, d, sc, capturing) : inorder_scratch(e, sc, capturing);
+  if (rc != EPPSCORE_OK) return rc;
+  bool wait_snapshot = false;
+  if (index && (rc = reader_begin(e, s, nullptr, &wait_snapshot)) != EPPSCORE_OK) return rc;
+  bool unused = false;
+  InOrderArgs a = inorder_args(e, &unused);
+  bool minmax[EPPSCORE_MAX_PROFILES] = {};
+  InOrderArgs ra[EPPSCORE_MAX_PROFILES];
+  InOrderProfArgs pa{};
+  pa.n_runs = d.n_runs;
+  pa.primary = x.primary_run;
+  pa.prefill = x.prefill_run;
+  int32_t slots = 0;
+  for (int i = 0; i < d.n_runs; i++) {
+    ra[i] = inorder_args(e, &minmax[i], d.run[i].profile);
+    InOrderRun& u = pa.run[i];
+    u.n_scorers = ra[i].n_scorers;
+    u.term_base = slots;
+    slots += u.n_scorers;
+    memcpy(u.kind, ra[i].kind, sizeof(u.kind));
+    memcpy(u.weight, ra[i].weight, sizeof(u.weight));
+    memcpy(u.lora_term, ra[i].lora_term, sizeof(u.lora_term));
+    memcpy(u.term, ra[i].term, sizeof(u.term));
+    u.pick_mode = ra[i].pick_mode;
+    u.seed_lo = ra[i].seed_lo;
+    u.seed_hi = ra[i].seed_hi;
+    u.member = ra[i].member;
+  }
+  const int C = e->io_prof_cluster[index];  // (inorder_profiles_prologue checked that the runs' terms fit its shared memory)
+  if (slots < 1) slots = 1;
+  InOrderIndexArgs ix{};
+  if (index) {
+    ix.tv = refs->tv;
+    ix.lv = refs->lv;
+    ix.cap_req = refs->cap_req;
+  }
+  const int adds = x.prefill_run >= 0 ? 2 : 1;
+  for (int32_t base = 0; base < d.R; base += sc.io_rows) {
+    DevBatch q = slice_rows(d, base, std::min(sc.io_rows, d.R - base), (size_t)e->M);
+    uint16_t* total = q.total_blocks ? q.total_blocks : sc.s_io_total.as<uint16_t>();
+    if (index) {
+      if ((rc = inorder_hash_slice(e, q, s, sc, total, &ix)) != EPPSCORE_OK) return rc;
+    } else {  // the match rows and totals: the batch kernels of one run with the prefix scorer (its provisional picks are overwritten)
+      DevBatch one = q;
+      one.n_runs = 1;
+      for (int i = 0; i < d.n_runs; i++)
+        if (cfg_has(e->prof[d.run[i].profile].cfg, EPPSCORE_SCORER_PREFIX)) {
+          one.run[0] = q.run[i];
+          break;
+        }
+      one.match_blocks = sc.s_io_match.as<uint16_t>();
+      one.total_blocks = total;
+      if ((rc = schedule_device(e, one, s, sc)) != EPPSCORE_OK) return rc;
+    }
+    inorder_slice(a, q);
+    a.cand_mask = nullptr;
+    a.match = index ? nullptr : sc.s_io_match.as<uint16_t>();
+    a.total = total;
+    pa.run_mask = q.run_mask;
+    if (wait_snapshot && base == 0) CK(e, cudaStreamWaitEvent(s, e->ev_snapshot, 0));
+    for (int i = 0; i < d.n_runs; i++) {
+      InOrderRun& u = pa.run[i];
+      u.cand_mask = q.run[i].cand_mask;
+      u.pick = q.run[i].pick;
+      u.pick_score = q.run[i].pick_score;
+      u.tie_count = q.run[i].tie_count;
+      u.pick_match = q.run[i].pick_match;
+      u.minmax = nullptr;
+      if (!minmax[i]) continue;
+      InOrderArgs m = ra[i];
+      inorder_slice(m, q);
+      m.cand_mask = q.run[i].cand_mask;
+      m.minmax = sc.s_io_minmax.as<long long>() + (size_t)i * sc.io_rows * 4;
+      u.minmax = m.minmax;
+      e->launches += launch_inorder_minmax(m, s, e->sm_count);
+    }
+    if (index) {
+      const uint16_t* room = total;
+      if (adds == 2) {  // the slice's totals twice: room for the primary's and the prefill's Adds of every request
+        uint16_t* two = sc.s_io_room.as<uint16_t>();
+        CK(e, cudaMemcpyAsync(two, total, (size_t)q.R * 2, cudaMemcpyDeviceToDevice, s));
+        CK(e, cudaMemcpyAsync(two + q.R, total, (size_t)q.R * 2, cudaMemcpyDeviceToDevice, s));
+        room = two;
+      }
+      if ((rc = index_status(e, e->index->ordered_room(q.R * adds, room, s), "schedule_batch_inorder_profiles")) != EPPSCORE_OK) return rc;
+    }
+    const int launched = launch_inorder_profiles(a, index ? &ix : nullptr, pa, C, slots, s);
+    if (launched < 0) {
+      cudaGetLastError();
+      return cuda_fail(e, (cudaError_t)-launched, "inorder_profiles_walk_kernel launch");
+    }
+    e->launches += launched;
+    CK(e, cudaGetLastError());
+    if (index) CK(e, e->index->ordered_end(s, capturing));
+  }
+  return EPPSCORE_OK;
+}
+
 int32_t run_make_room(eppscore_engine* e, cudaStream_t st, int64_t R, bool capturing);
 int32_t run_copy_back(eppscore_engine* e, cudaStream_t st, bool capturing);
 int32_t count_reads_wait(eppscore_engine* e, cudaStream_t st);
@@ -1782,10 +1904,11 @@ int32_t count_reads_wait(eppscore_engine* e, cudaStream_t st);
 // scheduled in arrival order against the in-flight counters (schedule_inorder), with `tokens` its requests' estimates; with
 // `ordered` also against the prefix index, committing as it goes (schedule_inorder_index), with pick_match [R] (optional) its
 // output; with `running` also with the latency scorer against the running-request queues, adding as it goes when it has keys.
+// `prof`: the runs are scheduled together in arrival order (schedule_inorder_profiles), in the index form when `ordered` is set.
 int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
                        const eppscore_topk* topk, bool wide = false, bool inorder = false, const int64_t* tokens = nullptr,
                        const DeviceIndex::OrderedRefs* ordered = nullptr, uint16_t* pick_match = nullptr,
-                       const eppscore_inorder_running* running = nullptr) {
+                       const eppscore_inorder_running* running = nullptr, const eppscore_inorder_profiles* prof = nullptr) {
   if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
   if (b->R == 0) return EPPSCORE_OK;
   CK(e, cudaSetDevice(e->device));
@@ -1795,6 +1918,10 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
   d.pick_match = pick_match;
   d.request_key = running ? running->request_key : nullptr;
   d.added_out = running ? running->added_out : nullptr;
+  if (prof) {
+    d.run_mask = prof->run_mask;
+    for (int i = 0; i < n_runs; i++) d.run[i].pick_match = prof->pick_match[i];
+  }
   const size_t M = (size_t)e->M;
   bool any_wide = false;
   for (int i = 0; i < n_runs; i++) any_wide = any_wide || d.run[i].wide;
@@ -1811,8 +1938,9 @@ int32_t schedule_batch(eppscore_engine* e, const eppscore_batch* b, int32_t n_ru
     if (rc == EPPSCORE_OK && adds) rc = run_make_room(e, st, x.R, capturing);
     if (rc != EPPSCORE_OK) return rc;
     if (adds) e->launches += launch_running_compact(e->run_desc.as<RunDev>(), (unsigned long long)e->run_cap, x.R, e->sm_count, st);
-    rc = ordered ? schedule_inorder_index(e, x, st, sc, *ordered, capturing, running != nullptr)
-                 : schedule_inorder(e, x, st, sc, running != nullptr);
+    rc = prof      ? schedule_inorder_profiles(e, x, st, sc, ordered, capturing, *prof)
+         : ordered ? schedule_inorder_index(e, x, st, sc, *ordered, capturing, running != nullptr)
+                   : schedule_inorder(e, x, st, sc, running != nullptr);
     if (rc == EPPSCORE_OK && adds) {
       e->launches += launch_running_finalize(e->run_desc.as<RunDev>(), e->cfg.max_endpoints, st);
       e->run_bound_live += x.R;
@@ -2069,6 +2197,35 @@ int32_t eppscore_schedule_batch_inorder(eppscore_engine* e, const eppscore_batch
 
 namespace {
 
+// The index form of an in-order call, after its prologue: run(refs) schedules the batch as an index mutation on the stream it
+// runs on, ordered like eppscore_commit_picks_device.
+template <class Run>
+int32_t inorder_index_mutation(eppscore_engine* e, const eppscore_batch* b, const int32_t* lru_capacity, const char* what, Run run) {
+  int32_t rc = EPPSCORE_OK;
+  cudaStream_t cs = b->location == 1 && b->stream ? (cudaStream_t)b->stream : e->stream;
+  const bool capturing = is_capturing(cs);
+  if (capturing && !e->index->reserved())
+    return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + " under CUDA-graph capture: reserve the prefix index before capturing "
+                                          "commits (eppscore_prefix_reserve)");
+  if (capturing && lru_capacity)
+    return fail(e, EPPSCORE_ERR_INVALID, std::string(what) + " under CUDA-graph capture: lru_capacity must be NULL (create the "
+                                         "endpoints' LRUs outside the capture, e.g. eppscore_prefix_add with n = 0)");
+  if (!capturing && (rc = index_skips(e, false, what)) != EPPSCORE_OK) return rc;
+  std::vector<int32_t> caps;
+  if ((rc = pad_caps(e, lru_capacity, &caps)) != EPPSCORE_OK) return rc;
+  if (!capturing) {  // after every earlier batch that reads the index and every earlier mutation (inside a capture: the graph's edges)
+    if ((rc = pending_wait(e, cs)) != EPPSCORE_OK) return rc;
+    if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
+  }
+  DeviceIndex::OrderedRefs refs{};
+  if ((rc = index_status(e, e->index->ordered_begin(caps.empty() ? nullptr : caps.data(), cs, &refs), what)) != EPPSCORE_OK) return rc;
+  rc = run(&refs);
+  if (rc != EPPSCORE_OK || capturing) return rc;
+  CK(e, cudaEventRecord(e->ev_table, cs));  // later readers on other streams, and later mutations on the engine stream, follow it
+  if (cs != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_table, 0));
+  return EPPSCORE_OK;
+}
+
 // eppscore_schedule_batch_inorder_index, and the index form of eppscore_schedule_batch_inorder_latency (q non-null)
 int32_t inorder_index_call(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens, const eppscore_inorder_index* x,
                            const eppscore_inorder_running* q, const char* what) {
@@ -2076,29 +2233,9 @@ int32_t inorder_index_call(eppscore_engine* e, const eppscore_batch* b, const in
   bool done = false;
   int32_t rc = inorder_prologue(e, b, what, true, q, &done);
   if (rc != EPPSCORE_OK || done) return rc;
-  // the call is an index mutation on the stream the batch runs on: ordered like eppscore_commit_picks_device
-  cudaStream_t cs = b->location == 1 && b->stream ? (cudaStream_t)b->stream : e->stream;
-  const bool capturing = is_capturing(cs);
-  if (capturing && !e->index->reserved())
-    return fail(e, EPPSCORE_ERR_CAPACITY, std::string(what) + " under CUDA-graph capture: reserve the prefix index before capturing "
-                                          "commits (eppscore_prefix_reserve)");
-  if (capturing && x->lru_capacity)
-    return fail(e, EPPSCORE_ERR_INVALID, std::string(what) + " under CUDA-graph capture: lru_capacity must be NULL (create the "
-                                         "endpoints' LRUs outside the capture, e.g. eppscore_prefix_add with n = 0)");
-  if (!capturing && (rc = index_skips(e, false, what)) != EPPSCORE_OK) return rc;
-  std::vector<int32_t> caps;
-  if ((rc = pad_caps(e, x->lru_capacity, &caps)) != EPPSCORE_OK) return rc;
-  if (!capturing) {  // after every earlier batch that reads the index and every earlier mutation (inside a capture: the graph's edges)
-    if ((rc = pending_wait(e, cs)) != EPPSCORE_OK) return rc;
-    if (cs != e->stream) CK(e, cudaStreamWaitEvent(cs, e->ev_table, 0));
-  }
-  DeviceIndex::OrderedRefs refs{};
-  if ((rc = index_status(e, e->index->ordered_begin(caps.empty() ? nullptr : caps.data(), cs, &refs), what)) != EPPSCORE_OK) return rc;
-  rc = schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, &refs, x->pick_match, q);
-  if (rc != EPPSCORE_OK || capturing) return rc;
-  CK(e, cudaEventRecord(e->ev_table, cs));  // later readers on other streams, and later mutations on the engine stream, follow it
-  if (cs != e->stream) CK(e, cudaStreamWaitEvent(e->stream, e->ev_table, 0));
-  return EPPSCORE_OK;
+  return inorder_index_mutation(e, b, x->lru_capacity, what, [&](const DeviceIndex::OrderedRefs* refs) {
+    return schedule_batch(e, b, 1, nullptr, nullptr, false, true, tokens, refs, x->pick_match, q);
+  });
 }
 
 }  // namespace
@@ -2235,6 +2372,82 @@ int32_t eppscore_schedule_batch_profiles_topk(eppscore_engine* e, const eppscore
   for (int32_t i = 0; i < n_runs; i++)
     if ((rc = check_topk(e, topk[i], 0, e->cfg.max_endpoints, "[0, max_endpoints]")) != EPPSCORE_OK) return rc;
   return schedule_batch(e, b, n_runs, runs, topk);
+}
+
+}  // extern "C"
+
+namespace {
+
+static_assert(kMaxRuns == EPPSCORE_MAX_PROFILES, "InOrderProfArgs holds one run per profile");
+
+// What eppscore_schedule_batch_inorder_profiles refuses, and its walk's cluster shape and shared memory per form (decided once
+// per engine, before the first call launches anything).  *done: nothing to run (R == 0).
+int32_t inorder_profiles_prologue(eppscore_engine* e, const eppscore_batch* b, int32_t n_runs, const eppscore_profile_run* runs,
+                                  const eppscore_inorder_profiles* x, bool* done) {
+  *done = false;
+  const std::string w = "schedule_batch_inorder_profiles";
+  if (!x || x->struct_size != sizeof(eppscore_inorder_profiles))
+    return fail(e, EPPSCORE_ERR_INVALID, "inorder_profiles NULL or struct_size mismatch");
+  if (x->index != 0 && x->index != 1) return fail(e, EPPSCORE_ERR_INVALID, w + ": index must be 0 or 1");
+  int32_t rc = check_profile_runs(e, b, n_runs, runs);
+  if (rc != EPPSCORE_OK) return rc;
+  if (x->primary_run < 0 || x->primary_run >= n_runs) return fail(e, EPPSCORE_ERR_INVALID, w + ": primary_run outside [0, n_runs)");
+  if (x->prefill_run < -1 || x->prefill_run >= n_runs || x->prefill_run == x->primary_run)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": prefill_run must be -1 or another run in [0, n_runs)");
+  for (int32_t i = 0; i < n_runs; i++) {
+    const eppscore_profile_run& r = runs[i];
+    if (r.scores_out || r.pred_out || r.filter_mask_out)
+      return fail(e, EPPSCORE_ERR_INVALID, w + ": a run's scores_out, pred_out and filter_mask_out are not available");
+    const eppscore_config& c = e->prof[r.profile].cfg;
+    if (cfg_has(c, EPPSCORE_SCORER_LATENCY))
+      return fail(e, EPPSCORE_ERR_INVALID, w + ": a run's profile has the latency scorer, whose inputs are PreRequest state the call does not order");
+    if (c.n_filters > 0)
+      return fail(e, EPPSCORE_ERR_INVALID, w + ": the device filters (prefix-cache-affinity, slo-headroom-tier) are not ordered");
+  }
+  if (e->have_snapshot && e->snapshot_has_tokens)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": the snapshot supplies inflight_tokens; the in-order view needs the engine's counters");
+  if (b->dense_feat || b->match_blocks)
+    return fail(e, EPPSCORE_ERR_INVALID, w + ": dense_feat and match_blocks are not available");
+  if (b->R < 0) return fail(e, EPPSCORE_ERR_INVALID, "R < 0");
+  if (b->location != 0 && b->location != 1) return fail(e, EPPSCORE_ERR_INVALID, "location must be 0 or 1");
+  if (b->R == 0) {
+    *done = true;
+    return EPPSCORE_OK;
+  }
+  if (!e->have_snapshot) return fail(e, EPPSCORE_ERR_NO_SNAPSHOT, w + " before set_snapshot");
+  if (b->prompt_bytes && !b->prompt_off) return fail(e, EPPSCORE_ERR_INVALID, "prompt_off required with prompt_bytes");
+  CK(e, cudaSetDevice(e->device));
+  int32_t& shape = e->io_prof_cluster[x->index];
+  if (shape == 0) {
+    const int C = inorder_profiles_cluster_size(e->geo.Mpad, x->index == 1, &e->io_prof_smem[x->index]);
+    if (C < 0) return cuda_fail(e, (cudaError_t)-C, "inorder_profiles_walk_kernel cluster attributes");
+    if (C == 0)
+      return fail(e, EPPSCORE_ERR_CAPACITY, w + ": no thread-block cluster of this device holds max_endpoints "
+                                                "endpoints (8192 needs the non-portable cluster size 16)");
+    shape = C;
+  }
+  int slots = 0;
+  for (int32_t i = 0; i < n_runs; i++) slots += e->prof[runs[i].profile].cfg.n_scorers;
+  if (inorder_profiles_smem(e->geo.Mpad, shape, x->index == 1, std::max(slots, 1)) > e->io_prof_smem[x->index])
+    return fail(e, EPPSCORE_ERR_CAPACITY, w + ": the runs' " + std::to_string(slots) +
+                                              " scorers do not fit the walk's shared memory on this device");
+  return EPPSCORE_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t eppscore_schedule_batch_inorder_profiles(eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens, int32_t n_runs,
+                                                 const eppscore_profile_run* runs, const eppscore_inorder_profiles* x) {
+  if (!e) return EPPSCORE_ERR_INVALID;
+  bool done = false;
+  const int32_t rc = inorder_profiles_prologue(e, b, n_runs, runs, x, &done);
+  if (rc != EPPSCORE_OK || done) return rc;
+  if (x->index == 0) return schedule_batch(e, b, n_runs, runs, nullptr, false, true, tokens, nullptr, nullptr, nullptr, x);
+  return inorder_index_mutation(e, b, x->lru_capacity, "schedule_batch_inorder_profiles", [&](const DeviceIndex::OrderedRefs* refs) {
+    return schedule_batch(e, b, n_runs, runs, nullptr, false, true, tokens, refs, nullptr, nullptr, x);
+  });
 }
 
 int32_t eppscore_hash_prompts(eppscore_engine* e, int32_t R, int32_t location, const uint8_t* prompt_bytes,

@@ -17,6 +17,11 @@
 //                          queues (eppscore_schedule_batch_inorder_latency): each thread keeps its endpoint's running count and
 //                          minimum tpot in registers, the cluster reduces request r's tier and headroom ranges (one more
 //                          barrier.cluster), and the owner of the pick adds request r to its queue (requestcontrol_hooks.go:73-86).
+//   inorder_profiles_kernel, inorder_index_profiles_kernel   either walk over several profile runs
+//                          (eppscore_schedule_batch_inorder_profiles): each thread scores its endpoint once per run in that
+//                          run's profile order, every CTA publishes one winner per run behind the request's one
+//                          barrier.cluster, and when the primary run picked, each run's pick owner adds the request's tokens and
+//                          the owners of the primary and prefill picks run the index's commit program for those two Adds.
 #include <cooperative_groups.h>
 
 #include "device_common.cuh"
@@ -147,11 +152,20 @@ struct InOrderHits {
   uint32_t first[2];                            // first miss of the current round (double-buffered, reset one round ahead)
 };
 
+// A run's pick of one request in the profiles walk.
+struct InOrderPick {
+  double score;
+  int32_t m, cnt;
+};
+
 // The walk, in the in-flight form (IDX false: inorder_pick_kernel) or the index form (IDX true: inorder_index_kernel, CTAs of
 // kCommitThreads threads; dynamic shared memory = the terms, then the CommitSmem of IndexProgram).  LAT: with the latency scorer
 // (the _lat kernels): the terms are followed by the kLatStatic static tile slots of each thread's endpoint, before the CommitSmem.
-template <bool RND, bool IDX, bool LAT>
-__device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrderIndexArgs& ix, const InOrderLatArgs& lt) {
+// PROF: over the runs of pa (the _profiles kernels; RND unused, each run's picker is read at run time): the terms of run i sit
+// in slots [term_base, term_base + n_scorers), Σ n_scorers slots before the CommitSmem.
+template <bool RND, bool IDX, bool LAT, bool PROF = false>
+__device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrderIndexArgs& ix, const InOrderLatArgs& lt,
+                                             const InOrderProfArgs* pa = nullptr) {
   constexpr int kTermSlots = kMaxSteps + (LAT ? kLatStatic : 0);
   extern __shared__ __align__(16) double s_term[];  // [n_scorers][blockDim.x]: the request-independent terms of each thread's endpoint
   __shared__ InOrderBest s_warp[kInOrderWarps];
@@ -163,7 +177,19 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
   const bool real = m < a.M;
   const int tie_mode = a.tie_mode;
 
-  for (int s = 0; s < a.n_scorers; s++) s_term[(size_t)s * T + tid] = (real && a.term[s]) ? a.term[s][m] : 0.0;
+  if constexpr (!PROF)
+    for (int s = 0; s < a.n_scorers; s++) s_term[(size_t)s * T + tid] = (real && a.term[s]) ? a.term[s][m] : 0.0;
+  uint32_t members = 0;  // PROF: bit i = this endpoint is in run i's profile subset
+  int slots = kTermSlots;
+  if constexpr (PROF) {
+#pragma unroll 1
+    for (int i = 0; i < pa->n_runs; i++) {
+      const InOrderRun& u = pa->run[i];
+      for (int s = 0; s < u.n_scorers; s++) s_term[(size_t)(u.term_base + s) * T + tid] = (real && u.term[s]) ? u.term[s][m] : 0.0;
+      if (real && (!u.member || ((__ldg(u.member + (m >> 5)) >> (m & 31)) & 1u))) members |= 1u << i;
+    }
+    slots = pa->run[pa->n_runs - 1].term_base + pa->run[pa->n_runs - 1].n_scorers;
+  }
   const long long q0 = (real && a.queue) ? a.queue[m] : 0LL, q1 = (real && a.running) ? a.running[m] : 0LL;
   const bool member = real && (!a.member || ((__ldg(a.member + (m >> 5)) >> (m & 31)) & 1u));
   long long tok = m < a.Mpad ? a.inflight_tok[m] : 0, req = m < a.Mpad ? a.inflight_req[m] : 0;
@@ -195,6 +221,20 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
     }
     if (a.tokens) x.tokens = __ldg(reinterpret_cast<const long long*>(a.tokens) + r);
     return x;
+  };
+  // PROF: request r's candidate bit of each run at this endpoint: subset ∧ run_mask ∧ the run's cand_mask
+  auto load_cands = [&](auto r) {  // (generic: instantiated by the PROF walk alone)
+    uint32_t b = 0;
+    if (r >= a.R) return b;
+    const uint32_t rm = pa->run_mask ? (uint32_t)__ldg(pa->run_mask + r) : 0xFu;
+#pragma unroll 1
+    for (int i = 0; i < pa->n_runs; i++) {
+      const uint32_t* cm = pa->run[i].cand_mask;
+      bool c = ((members & rm) >> i) & 1u;
+      if (c && cm) c = (__ldg(cm + (size_t)r * a.mask_words + (m >> 5)) >> (m & 31)) & 1u;
+      b |= (uint32_t)c << i;
+    }
+    return b;
   };
 
   // LAT: this thread's endpoint in the latency fold-in.  The static tile slots go to shared memory; lim (slot 6) and the idle
@@ -252,11 +292,15 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
 
   cluster.sync();  // every CTA of the cluster is running before any reads another's shared memory
   InOrderReq cur = load(0);
+  uint32_t cands = 0;
+  if constexpr (PROF) cands = load_cands(0);
   InOrderLatReq lcur{};  // (loaded one request ahead in the in-flight form; the index form has no registers to spare for that,
                          // and its probes cover the loads)
   if constexpr (LAT && !IDX) lcur = load_lat(0);
   for (int r = 0; r < a.R; r++) {
     const InOrderReq nxt = load(r + 1);
+    uint32_t cands_nxt = 0;
+    if constexpr (PROF) cands_nxt = load_cands(r + 1);
     InOrderLatReq lnxt{};
     if constexpr (LAT && IDX) lcur = load_lat(r);
     if constexpr (LAT && !IDX) lnxt = load_lat(r + 1);
@@ -342,6 +386,146 @@ __device__ __forceinline__ void inorder_walk(const InOrderArgs& a, const InOrder
         const double rel = maxq > 0 ? __ddiv_rn(__ll2double_rn(maxq - q), __ll2double_rn(maxq)) : 1.0;
         lat_w = __double2ll_rz(round(__dmul_rn(100.0, __dadd_rn(__dadd_rn(s_lat[tid], __dmul_rn(L.wq, rel)), pt))));
       }
+    }
+    if constexpr (PROF) {
+      // ---- Each run: its score in its profile order, its candidate, and this warp's winner (the run's picker, uniform) ----
+      __shared__ InOrderBest s_pwarp[kMaxRuns][kInOrderWarps];
+      __shared__ InOrderBest s_pcta[2][kMaxRuns];  // the CTA's winner per run of the last two requests (read cluster-wide)
+      __shared__ InOrderPick s_pick[kMaxRuns];
+      const int n_runs = pa->n_runs;
+#pragma unroll 1
+      for (int i = 0; i < n_runs; i++) {
+        const InOrderRun& u = pa->run[i];
+        long long mn0 = 0, mx0 = 0, mn1 = 0, mx1 = 0;  // (read at the request: a second run's min / max would not fit one ahead)
+        if (u.minmax) {
+          const long long* mm = u.minmax + (size_t)r * 4;
+          mn0 = __ldg(mm);
+          mx0 = __ldg(mm + 1);
+          mn1 = __ldg(mm + 2);
+          mx1 = __ldg(mm + 3);
+        }
+        double acc = 0.0;
+        for (int s = 0; s < u.n_scorers; s++) {
+          const int kind = u.kind[s];
+          const double w = u.weight[s];
+          double term;
+          if (kind == 6) {
+            term = __dmul_rn(tl, w);
+          } else if (kind == 0 || kind == 4) {
+            const bool queue = kind == 0;
+            const long long mn = queue ? mn0 : mn1, mx = queue ? mx0 : mx1, qv = queue ? q0 : q1;
+            term = mx == mn ? __dmul_rn(1.0, w) : __dmul_rn(clamp01(__ddiv_rn(__ll2double_rn(mx - qv), __ll2double_rn(mx - mn))), w);
+          } else if (kind == 2) {
+            term = prefix_term_direct(cur.c, cur.total, w);
+          } else if (kind == 3) {
+            term = u.lora_term[s][cur.cls];
+          } else if (kind >= 16) {
+            term = __dmul_rn(0.0, w);
+          } else {
+            term = s_term[(size_t)(u.term_base + s) * T + tid];
+          }
+          acc = __dadd_rn(acc, term);
+        }
+        const bool rnd = u.pick_mode != 0;
+        const uint32_t areq = tie_areq(a.request_base + r, u.seed_lo);
+        InOrderBest x = inorder_none();
+        if ((cands >> i) & 1u) {
+          const uint32_t pr = tie_prio(areq, m, u.seed_hi);
+          if (rnd) {
+            rbest_update(x.all, (double)pr, acc, m);
+            if (u.pick_mode == 1 && acc > 0.0) rbest_update(x.pos, ares_key(pr, m, acc), acc, m);
+          } else {
+            best_update(x.b, acc, m, tie_mode, areq, u.seed_hi);
+          }
+        }
+        if (rnd) inorder_warp_reduce<true>(x, tie_mode);
+        else inorder_warp_reduce<false>(x, tie_mode);
+        if (lane == 0) s_pwarp[i][warp] = x;
+      }
+      __syncthreads();
+      // ---- The CTA's winner of each run (warp w reduces runs w, w + nwarps, ...), then one barrier.cluster for all runs ----
+      for (int i = warp; i < n_runs; i += nwarps) {
+        const bool rnd = pa->run[i].pick_mode != 0;
+        InOrderBest x = lane < nwarps ? s_pwarp[i][lane] : inorder_none();
+        if (rnd) inorder_warp_reduce<true>(x, tie_mode);
+        else inorder_warp_reduce<false>(x, tie_mode);
+        if (lane == 0) s_pcta[r & 1][i] = x;
+      }
+      cluster.sync();  // barrier.cluster: the CTA winners of request r, every run, are visible cluster-wide
+      for (int i = warp; i < n_runs; i += nwarps) {
+        const InOrderRun& u = pa->run[i];
+        const bool rnd = u.pick_mode != 0;
+        InOrderBest x = lane < C ? *cluster.map_shared_rank(&s_pcta[r & 1][i], lane) : inorder_none();
+        InOrderPick p;
+        if (rnd) {
+          inorder_warp_reduce<true>(x, tie_mode);
+          const RBest& wb = x.pos.m >= 0 ? x.pos : x.all;  // no positive score: the random picker (weightedrandom/picker.go:113-116)
+          p = InOrderPick{wb.score, wb.m, wb.n};
+        } else {
+          inorder_warp_reduce<false>(x, tie_mode);
+          p = InOrderPick{x.b.score, x.b.m, x.b.cnt};
+        }
+        if (lane == 0) {
+          s_pick[i] = p;
+          if (cluster.block_rank() == 0) {
+            u.pick[r] = p.m;
+            u.pick_score[r] = p.m >= 0 ? p.score : 0.0;
+            u.tie_count[r] = p.cnt;
+          }
+        }
+      }
+      __syncthreads();  // every run's pick of request r is in s_pick
+      // ---- PreRequest, when the primary run picked (no PreRequest for a failed schedule): requests += 1 and tokens += tokens[r]
+      // on every run's pick (producer.go:106-119), PrefixCacheMatchInfo at each pick before the request's Adds
+      // (plugin.go:199-204), then indexer.Add at the primary pick and at the prefill pick (plugin.go:177-197) ----
+      const int p0 = s_pick[pa->primary].m;
+      const int p1 = pa->prefill >= 0 ? s_pick[pa->prefill].m : -1;
+      bool moved = false;
+#pragma unroll 1
+      for (int i = 0; i < n_runs; i++) {
+        const int pk = p0 >= 0 ? s_pick[i].m : -1;
+        if (pk == m) {
+          tok += cur.tokens;
+          req += 1;
+          moved = true;
+        }
+        uint16_t* pm = pa->run[i].pick_match;
+        if (pm && (pk >= 0 ? pk == m : m == 0)) pm[r] = pk >= 0 ? (uint16_t)cur.c : (uint16_t)0;
+      }
+      if (moved) tl = token_load_score(tok, a.token_threshold);
+      if constexpr (IDX) {
+        const int rank = (int)cluster.block_rank();
+        const bool own0 = p0 >= 0 && p0 / T == rank, own1 = p1 >= 0 && p1 / T == rank && p1 != p0;  // CTA-uniform
+        if (own0 || own1) {
+          __shared__ int32_t s_adds[2];
+          if (tid == 0) {  // (read inside the program's first parallel section, behind its barrier)
+            s_adds[0] = p0;
+            s_adds[1] = p1;
+          }
+          CommitArgs ca{};
+          ca.R = 1;
+          ca.pick = &s_adds[0];
+          ca.hashes = ix.hashes + (size_t)r * ix.stride;
+          ca.n_hashes = a.total + r;
+          ca.stride = ix.stride;
+          ca.cap_req = ix.cap_req;
+          ca.n_picks = p1 >= 0 ? 2 : 1;
+          ca.more_picks[0] = &s_adds[1];
+          CommitSmem* sm = reinterpret_cast<CommitSmem*>(s_term + (size_t)slots * T);
+          if (own0) {  // both Adds when both picks are this endpoint, primary first
+            IndexProgram<DevX> prog(dx, ix.tv, ix.lv, sm, (uint32_t)p0);
+            prog.commit(ca);
+          }
+          if (own1) {
+            IndexProgram<DevX> prog(dx, ix.tv, ix.lv, sm, (uint32_t)p1);
+            prog.commit(ca);
+          }
+        }
+        cluster.sync();  // request r's Adds are visible to every CTA's probes of request r + 1
+      }
+      cands = cands_nxt;
+      cur = nxt;
+      continue;
     }
     // ---- Score (scheduler_profile.go:151-174): profile order from 0.0, the operations of score_matrix_kernel ----
     double acc = 0.0;
@@ -645,6 +829,69 @@ int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C
   }
   const cudaLaunchConfig_t cfg = index_config(C, s, at);
   return launched_one(cudaLaunchKernelEx(&cfg, inorder_index_kernel<false>, a, ix));
+}
+
+template <bool IDX>
+__global__ void __launch_bounds__(kInOrderMaxThreads, 1) inorder_profiles_walk_kernel(const __grid_constant__ InOrderArgs a,
+                                                                                      const __grid_constant__ InOrderIndexArgs ix,
+                                                                                      const __grid_constant__ InOrderProfArgs p) {
+  inorder_walk<false, IDX, false, true>(a, ix, InOrderLatArgs{}, &p);
+}
+
+// The profiles walk: the cluster shapes of the single-profile walks (the in-flight form's CTAs of Mpad / C threads, the index
+// form's of kCommitThreads), with Σ n_scorers term slots per thread, then (index form) the CommitSmem.  The kernels are opted in to
+// the device's whole shared memory less their static part; a call whose runs need more is refused before any launch.
+size_t inorder_profiles_smem(int Mpad, int C, bool index, int slots) {
+  return index ? (size_t)slots * 8 * kCommitThreads + sizeof(CommitSmem) : (size_t)slots * 8 * (Mpad / C);
+}
+
+static cudaLaunchConfig_t profiles_config(int Mpad, int C, bool index, size_t smem, cudaStream_t s, cudaLaunchAttribute* at) {
+  cudaLaunchConfig_t cfg = index ? index_config(C, s, at) : pick_config<false>(Mpad, C, s, at);
+  cfg.dynamicSmemBytes = smem;
+  return cfg;
+}
+
+// > 0: CTAs per cluster (and *smem_max the dynamic shared memory the kernel may use); 0: no cluster shape fits; -(cudaError_t)
+int inorder_profiles_cluster_size(int Mpad, bool index, size_t* smem_max) {
+  const void* kernel = index ? (const void*)inorder_profiles_walk_kernel<true> : (const void*)inorder_profiles_walk_kernel<false>;
+  int dev = 0, optin = 0;
+  cudaFuncAttributes fa{};
+  cudaError_t c = cudaGetDevice(&dev);
+  if (c == cudaSuccess) c = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (c == cudaSuccess) c = cudaFuncGetAttributes(&fa, kernel);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+  const int dyn = optin - (int)fa.sharedSizeBytes;
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn);
+  if (c != cudaSuccess) return -(int)c;
+  *smem_max = (size_t)dyn;
+  // the largest shape first, with the shared memory of the smallest call (one run of one scorer): a call past it is refused
+  for (int cmax = 16; cmax >= (index ? 16 : 8); cmax /= 2) {
+    int C;
+    if (index) {
+      C = Mpad <= kCommitThreads ? 1 : (Mpad + kCommitThreads - 1) / kCommitThreads;
+    } else {
+      C = Mpad / 256;
+      if (C < 1) C = 1;
+      if (C > cmax) C = cmax;
+      if (Mpad / C > kInOrderMaxThreads) continue;
+    }
+    if (C > 16) return 0;
+    cudaLaunchAttribute at[1];
+    const cudaLaunchConfig_t cfg = profiles_config(Mpad, C, index, inorder_profiles_smem(Mpad, C, index, 1), nullptr, at);
+    int clusters = 0;
+    c = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
+    if (c == cudaSuccess && clusters >= 1) return C;
+    cudaGetLastError();
+  }
+  return 0;
+}
+
+int launch_inorder_profiles(const InOrderArgs& a, const InOrderIndexArgs* ix, const InOrderProfArgs& p, int C, int slots, cudaStream_t s) {
+  if (a.R <= 0) return 0;
+  cudaLaunchAttribute at[1];
+  const cudaLaunchConfig_t cfg = profiles_config(a.Mpad, C, ix != nullptr, inorder_profiles_smem(a.Mpad, C, ix != nullptr, slots), s, at);
+  return launched_one(ix ? cudaLaunchKernelEx(&cfg, inorder_profiles_walk_kernel<true>, a, *ix, p)
+                         : cudaLaunchKernelEx(&cfg, inorder_profiles_walk_kernel<false>, a, InOrderIndexArgs{}, p));
 }
 
 }  // namespace eppscore

@@ -351,6 +351,37 @@ struct InOrderIndexArgs {
 };
 int inorder_index_cluster_size(int Mpad, bool lat = false);  // as inorder_cluster_size, for launch_inorder_index's CTAs of kCommitThreads
 int launch_inorder_index(const InOrderArgs& a, const InOrderIndexArgs& ix, int C, cudaStream_t s, const InOrderLatArgs* lt = nullptr);
+// Several profiles in the walk (eppscore_schedule_batch_inorder_profiles): per run, what InOrderArgs holds for profile 0, read
+// by every thread for its endpoint each request.  The InOrderArgs of the launch carry the request- and engine-wide fields (its
+// per-profile fields are unused).
+struct InOrderRun {
+  int32_t n_scorers;
+  int32_t term_base;                   // the run's first term slot in the walk's shared-memory staging (Σ earlier n_scorers)
+  int32_t kind[kMaxSteps];
+  double weight[kMaxSteps];
+  double lora_term[kMaxSteps][4];
+  const double* term[kMaxSteps];
+  int32_t pick_mode;
+  uint32_t seed_lo, seed_hi;           // the profile's derived tie seed
+  const uint32_t* cand_mask;           // [R][mask_words] or null
+  const uint32_t* member;              // the profile's endpoint subset, or null
+  const long long* minmax;             // [R][4] over the run's candidates, or null
+  int32_t* pick;
+  double* pick_score;
+  int32_t* tie_count;
+  uint16_t* pick_match;                // [R] or null
+};
+constexpr int kMaxRuns = 4;  // EPPSCORE_MAX_PROFILES
+struct InOrderProfArgs {
+  int32_t n_runs, primary, prefill;    // prefill -1: no second Add
+  const uint8_t* run_mask;             // [R] bit i: run i runs for request r, or null (every run)
+  InOrderRun run[kMaxRuns];
+};
+// Dynamic shared memory of the profiles walk with `slots` term slots (Σ n_scorers); the device's opt-in limit bounds it.
+size_t inorder_profiles_smem(int Mpad, int C, bool index, int slots);
+// CTAs per cluster of the profiles walk of either form, as inorder_cluster_size / inorder_index_cluster_size
+int inorder_profiles_cluster_size(int Mpad, bool index, size_t* smem_max);
+int launch_inorder_profiles(const InOrderArgs& a, const InOrderIndexArgs* ix, const InOrderProfArgs& p, int C, int slots, cudaStream_t s);
 
 // predicted-latency producer's running-request queues (running_kernel.cu).  Table slot: {key, meta}, meta = endpoint + 1
 // (| kRunTomb once removed), {0, 0} empty; tpot[] holds the entry's tpot bits, owner[] / rm[] the (gen << 32 | r) bids of

@@ -368,7 +368,7 @@ class Engine:
     def schedule_profiles(self, R, runs, *, prompt_bytes=None, prompt_off=None, prompt_len=None, model_seed=None, hashes_in=None,
                           n_hashes_in=None, hash_stride=0, adapter_id=None, dense_feat=None, dense_total=None, block_chars=0,
                           max_blocks=0, request_base=0, want_match=False, want_total=True, want_hashes=False, input_tokens=None,
-                          ttft_slo=None, tpot_slo=None, device=False, stream=None, out=None):
+                          ttft_slo=None, tpot_slo=None, device=False, stream=None, out=None, _inorder=None):
         """eppscore_schedule_batch_profiles: one hash stage, then one Filter -> Score -> Pick per run.  runs: list of dicts
         {"profile": id, "cand_mask": optional, "want_scores" / "want_pred" / "want_filter_mask": optional bools (host mode)};
         in device mode each run dict also holds its preallocated outputs (pick, pick_score, tie_count, optional scores_out,
@@ -439,7 +439,19 @@ class Engine:
                     setattr(x, k, v.ctypes.data)
             res_runs.append(o)
 
+        if _inorder is not None:  # schedule_inorder_profiles: (tokens, InOrderProfiles)
+            tok, x = a.ptr(_inorder[0], np.int64), _inorder[1]
+            x.run_mask = a.ptr(_inorder[2], np.uint8)
+            for i, run in enumerate(runs):
+                if device:
+                    x.pick_match[i] = a.ptr(run.get("pick_match"), None)
+                else:
+                    res_runs[i]["pick_match"] = np.zeros(max(R, 1), np.uint16)
+                    x.pick_match[i] = res_runs[i]["pick_match"].ctypes.data
+
         def call():
+            if _inorder is not None:
+                return self._lib.eppscore_schedule_batch_inorder_profiles(self._h, C.byref(b), tok, len(runs), arr, C.byref(x))
             if with_lists:
                 return self._lib.eppscore_schedule_batch_profiles_topk(self._h, C.byref(b), len(runs), arr, tarr)
             return self._lib.eppscore_schedule_batch_profiles(self._h, C.byref(b), len(runs), arr)
@@ -462,7 +474,34 @@ class Engine:
         for k, v in res.items():
             setattr(b, k, v.ctypes.data)
         self._check(call())
+        if _inorder is not None:
+            for o in res_runs:
+                o["pick_match"] = o["pick_match"][:R]
         return res, res_runs
+
+    def schedule_inorder_profiles(self, R, runs, tokens=None, index=False, primary_run=0, prefill_run=-1, run_mask=None,
+                                  lru_capacity=None, **kw):
+        """eppscore_schedule_batch_inorder_profiles: `schedule_profiles` with request r's runs scored against the in-flight load
+        (index=True: and the prefix index) that requests 0..r-1 left, and, when the primary run picked, each run's pick counted
+        with tokens[r] (int64[R], None = 0) and the primary and prefill picks' Adds made inside the call (do not commit the batch
+        again).  run_mask: uint8[R], bit i = run i runs for request r (None: every run).  lru_capacity: host int32[M] or None.
+        Takes the arguments of `schedule_profiles` except match_blocks and the runs' R x M outputs and lists.  Host mode returns
+        (batch outputs, [run outputs]) with each run's pick_match uint16[R]; device mode fills the runs' outputs (pick_match when
+        the run dict has it) asynchronously on `stream`."""
+        if kw.get("want_match") or kw.get("dense_feat") is not None:
+            raise ValueError("schedule_inorder_profiles does not take want_match or dense_feat")
+        for run in runs:
+            for k in ("want_scores", "want_pred", "want_filter_mask", "topk"):
+                if run.get(k):
+                    raise ValueError(f"schedule_inorder_profiles does not take a run's {k}")
+        x = capi.InOrderProfiles()
+        x.struct_size = C.sizeof(capi.InOrderProfiles)
+        x.index = 1 if index else 0
+        x.primary_run = primary_run
+        x.prefill_run = prefill_run
+        caps = None if lru_capacity is None else np.ascontiguousarray(lru_capacity, np.int32)
+        x.lru_capacity = None if caps is None else caps.ctypes.data
+        return self.schedule_profiles(R, runs, _inorder=(tokens, x, run_mask), **kw)
 
     @staticmethod
     def _topk(k, endpoints, scores) -> TopK:

@@ -157,6 +157,12 @@ extern "C" int32_t eppscore_schedule_batch_inorder_latency(struct eppscore_engin
                                                            const eppscore_inorder_index* x, const eppscore_inorder_running* q)
     __attribute__((weak));
 inline bool EngineHasInOrderLatency() { return &eppscore_schedule_batch_inorder_latency != nullptr; }
+// eppscore_schedule_batch_inorder_profiles (either in-order call over several profiles) likewise: EngineHasInOrderProfiles() tells.
+// Without it a Profiles config with SchedulerConfig::InOrderInFlightLoad is refused.
+extern "C" int32_t eppscore_schedule_batch_inorder_profiles(struct eppscore_engine* e, const eppscore_batch* b, const int64_t* tokens,
+                                                            int32_t n_runs, const eppscore_profile_run* runs,
+                                                            const eppscore_inorder_profiles* x) __attribute__((weak));
+inline bool EngineHasInOrderProfiles() { return &eppscore_schedule_batch_inorder_profiles != nullptr; }
 
 inline bool EngineHasInFlightLoad() {
   return &eppscore_estimate_tokens != nullptr && &eppscore_inflight_add != nullptr && &eppscore_inflight_release != nullptr &&
@@ -370,8 +376,14 @@ struct SchedulerConfig {
   // sequence does (inflightload/producer.go:101-120 before token_load.go:83-111), instead of one load view per batch.  The
   // call adds each request's estimate to its TargetEndpoints[0] while it schedules, so PreRequest does not add it again;
   // ResponseComplete releases it as before.  The counters after ScheduleBatch + PreRequest are those of the per-request
-  // sequence.  Refused with a latency scorer, with the Profiles list, with MaxNumOfEndpoints > 1, without InFlightLoad and with
-  // an engine library without the call.
+  // sequence.  Refused with a latency scorer, with MaxNumOfEndpoints > 1, without InFlightLoad and with an engine library without
+  // the call.  With the Profiles list (every profile with MaxNumOfEndpoints 1, no latency scorer and no device filters) each
+  // engine batch, LoRA pieces in order, is one eppscore_schedule_batch_inorder_profiles call: the runs are the profiles in order,
+  // each request's run mask is the handler's first Pick, the primary run is the first profile and the prefill run the profile
+  // named "prefill".  The call counts each request on every profile's target when the first profile picked, so PreRequest adds
+  // no load.  A request whose ProcessResults names another primary profile gets an error, but its load (and with
+  // InOrderPrefixIndex its blocks) was already recorded at the first profile's target.  Needs an engine library with
+  // eppscore_schedule_batch_inorder_profiles.
   bool InOrderInFlightLoad = false;
   // Opt-in (off by default), with InOrderInFlightLoad and the approximate-prefix producer (prefix hashing on): every engine batch
   // goes through eppscore_schedule_batch_inorder_index, so request r is also scored against the prefix index as requests
@@ -380,7 +392,9 @@ struct SchedulerConfig {
   // target's PrefixCacheMatchInfo is the pick's match as the request was scored, before its own Add (plugin.go:199-204).  A
   // batch cut into LoRA pieces runs its pieces in order, each committing before the next is scheduled.  Refused with
   // LatencyPredictionInfo (eppscore_predict_latency after the batch would read the index the batch left), without
-  // InOrderInFlightLoad or prefix hashing, and with an engine library without the call.
+  // InOrderInFlightLoad or prefix hashing, and with an engine library without the call.  With the Profiles list it is the index
+  // form of that call: the primary and the "prefill" targets get their Adds inside it, PreRequest commits nothing, and with
+  // PrefixMatchInfo every profile's target gets its run's pick_match.
   bool InOrderPrefixIndex = false;
   // Opt-in (off by default), with InOrderInFlightLoad and a profile with a latency scorer: every engine batch goes through
   // eppscore_schedule_batch_inorder_latency (its index form with InOrderPrefixIndex), so request r's latency scorer sees the
@@ -502,13 +516,26 @@ class Scheduler {
     inflight_ = cfg.InFlightLoad != nullptr;
     if (cfg0.InOrderInFlightLoad) {
       if (!inflight_) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs the inflight-load-producer (InFlightLoad)");
-      if (!cfg0.Profiles.empty()) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad serves the single-profile config, not the Profiles list");
       if (cfg.Profile.picker().MaxNumOfEndpoints > 1) throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs maxNumOfEndpoints == 1");
+      for (const auto& np : cfg0.Profiles) {
+        if (np.second.picker().MaxNumOfEndpoints != 1)
+          throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs maxNumOfEndpoints == 1 (profile '" + np.first + "')");
+        for (const auto& w : np.second.scorers())
+          if (dynamic_cast<const LatencyScorer*>(w.Scorer_.get()))
+            throw SchedulingError("SchedulerConfig::InOrderInFlightLoad cannot order the latency scorer's inputs (profile '" + np.first + "')");
+        if (!np.second.device_filters().empty())
+          throw SchedulingError("SchedulerConfig::InOrderInFlightLoad does not order the device filters (profile '" + np.first + "')");
+      }
+      if (!cfg0.Profiles.empty() && cfg0.Profiles[0].first == "prefill")
+        throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs the first profile (the primary) to be other than \"prefill\"");
+      if (!cfg0.Profiles.empty() && !EngineHasInOrderProfiles())
+        throw SchedulingError("SchedulerConfig::InOrderInFlightLoad with several profiles needs an engine library with "
+                              "eppscore_schedule_batch_inorder_profiles");
       if (!cfg0.InOrderRunningRequests)
         for (const auto& w : sc)
           if (dynamic_cast<const LatencyScorer*>(w.Scorer_.get()))
             throw SchedulingError("SchedulerConfig::InOrderInFlightLoad cannot order the latency scorer's inputs");
-      if (!EngineHasInOrderLoad())
+      if (cfg0.Profiles.empty() && !EngineHasInOrderLoad())
         throw SchedulingError("SchedulerConfig::InOrderInFlightLoad needs an engine library with eppscore_schedule_batch_inorder");
       inorder_ = true;
     }
@@ -518,7 +545,7 @@ class Scheduler {
       if (cfg.LatencyPredictionInfo)
         throw SchedulingError("SchedulerConfig::InOrderPrefixIndex cannot give LatencyPredictionInfo: the prediction would read the "
                               "prefix index the batch left");
-      if (!(cfg0.InOrderRunningRequests ? EngineHasInOrderLatency() : EngineHasInOrderPrefixIndex()))  // (the route's one call)
+      if (cfg0.Profiles.empty() && !(cfg0.InOrderRunningRequests ? EngineHasInOrderLatency() : EngineHasInOrderPrefixIndex()))  // (the route's one call)
         throw SchedulingError("SchedulerConfig::InOrderPrefixIndex needs an engine library with eppscore_schedule_batch_inorder_index");
       inorder_index_ = true;
     }
@@ -1447,6 +1474,10 @@ class Scheduler {
     std::vector<unsigned> distinct;
     for (int r = 0; r < R; r++)
       if (out[r].error.empty() && sets[r] && std::find(distinct.begin(), distinct.end(), sets[r]) == distinct.end()) distinct.push_back(sets[r]);
+    if (inorder_) {
+      if (M > 0) ScheduleInOrderProfiles(requests, endpoints, sets, out, got, ids, Mx, mw, g, set_base);
+      distinct.clear();
+    }
     for (unsigned S : distinct) {
       if (M == 0) break;  // no endpoints: every profile fails (scheduler_profile.go:119-121)
       std::vector<int> rows;
@@ -1545,12 +1576,104 @@ class Scheduler {
       } catch (const SchedulingError& ex) {
         out[r].error = ex.what();
       }
+      if (inorder_ && out[r].error.empty() && out[r].result.PrimaryProfileName != names[0])  // (its load and Adds are at names[0]'s target)
+        out[r].error = "the in-order batch route records PreRequest at the first profile's target ('" + names[0] +
+                       "'), but ProcessResults named '" + out[r].result.PrimaryProfileName + "' the primary profile";
       if (cfg_.LatencyPredictionInfo) AttachLatency(out[r], last_.lat[(size_t)r], endpoints, ids);
     }
     last_endpoints_ = &endpoints;
     last_ids_ = ids;
     last_rows_ = Mx;
     return out;
+  }
+
+  // The in-order form of ScheduleBatchProfiles (SchedulerConfig::InOrderInFlightLoad): the requests the handler gave a profile
+  // set go through ONE eppscore_schedule_batch_inorder_profiles call, every profile a run (run i = profile i), with the set as
+  // each request's run mask; the index form with InOrderPrefixIndex.  Fills got[r] for the profiles of request r's set.
+  void ScheduleInOrderProfiles(const std::vector<InferenceRequest>& requests, const std::vector<Endpoint>& endpoints,
+                               const std::vector<unsigned>& sets, const std::vector<BatchItem>& out,
+                               std::vector<std::map<std::string, ProfileRunResult>>& got, const std::vector<int>& ids, int Mx, int mw,
+                               const PrefixGeometry& g, std::map<unsigned, int64_t>& set_base) {
+    const int R = (int)requests.size(), P = (int)cfg_.Profiles.size(), M = (int)endpoints.size();
+    std::vector<int> rows;
+    for (int r = 0; r < R; r++)
+      if (out[r].error.empty() && sets[r]) rows.push_back(r);
+    const int n = (int)rows.size();
+    if (n == 0) return;
+    std::vector<int> pos_of_id((size_t)Mx, -1);
+    for (int m = 0; m < M; m++) pos_of_id[(size_t)ids[m]] = m;
+    const PackedRequests packed = Pack(requests, rows);
+    std::vector<uint64_t> hashes((size_t)n * g.stride, 0);
+    std::vector<uint16_t> nh((size_t)n, 0);
+    std::vector<std::vector<uint32_t>> masks((size_t)P);
+    std::vector<std::vector<int32_t>> pick((size_t)P, std::vector<int32_t>((size_t)n)), ties = pick;
+    std::vector<std::vector<double>> score((size_t)P, std::vector<double>((size_t)n));
+    std::vector<std::vector<uint16_t>> match((size_t)P, std::vector<uint16_t>((size_t)n, 0));
+    std::vector<eppscore_profile_run> runs((size_t)P);
+    eppscore_inorder_profiles x{};
+    x.struct_size = sizeof(x);
+    x.index = inorder_index_ ? 1 : 0;
+    x.primary_run = 0;
+    x.prefill_run = -1;
+    for (int p = 0; p < P; p++) {
+      if (cfg_.Profiles[(size_t)p].first == "prefill") x.prefill_run = p;
+      eppscore_profile_run& u = runs[(size_t)p];
+      u = eppscore_profile_run{};
+      u.struct_size = sizeof(u);
+      u.profile = p;
+      const auto& filters = cfg_.Profiles[(size_t)p].second.filters();
+      if (!filters.empty() || Mx != M) {  // host filters and rows without an endpoint in this list
+        masks[(size_t)p] = CandidateMask(filters, requests, rows, endpoints, ids, mw);
+        u.cand_mask = masks[(size_t)p].data();
+      }
+      u.pick = pick[(size_t)p].data();
+      u.pick_score = score[(size_t)p].data();
+      u.tie_count = ties[(size_t)p].data();
+      x.pick_match[p] = match[(size_t)p].data();
+    }
+    std::vector<uint8_t> run_mask((size_t)n);
+    std::vector<int64_t> size((size_t)n);
+    std::vector<int32_t> hint((size_t)n), chars((size_t)n);
+    for (int i = 0; i < n; i++) {
+      run_mask[(size_t)i] = (uint8_t)sets[(size_t)rows[i]];
+      size[(size_t)i] = last_.size[(size_t)rows[i]];
+      hint[(size_t)i] = last_.hint[(size_t)rows[i]];
+      chars[(size_t)i] = last_.chars[(size_t)rows[i]];
+    }
+    x.run_mask = run_mask.data();
+    last_endpoints_ = &endpoints;  // (LruCapacities reads the batch's list)
+    last_ids_ = ids;
+    last_rows_ = Mx;
+    const std::vector<int32_t> caps = LruCapacities();
+    if (inorder_index_) x.lru_capacity = caps.data();
+    const std::vector<int64_t> est = EstimateTokens(n, size.data(), hint.data(), chars.data());
+    eppscore_batch b = BatchOf(packed, g, nh.data(), hashes.data());
+    b.request_base = set_base[0u];  // (no profile set is 0: one count for the in-order calls of a batch)
+    set_base[0u] += n;
+    Check(eppscore_schedule_batch_inorder_profiles(eng_, &b, est.data(), P, runs.data(), &x), "eppscore_schedule_batch_inorder_profiles");
+    const bool with_match = inorder_index_ && cfg_.PrefixMatchInfo && g.want_prefix;
+    if (with_match && g.block_tokens > 0xFFFF) throw SchedulingError("PrefixCacheMatchInfo: block size above 65535 tokens");
+    for (int i = 0; i < n; i++) {
+      const int r = rows[i];
+      last_.nh[(size_t)r] = nh[(size_t)i];
+      std::copy(hashes.begin() + (size_t)i * g.stride, hashes.begin() + (size_t)(i + 1) * g.stride, last_.hashes.begin() + (size_t)r * g.stride);
+      for (int p = 0; p < P; p++) {
+        if (!(sets[(size_t)r] & (1u << p))) continue;
+        ProfileRunResult& pr = got[(size_t)r][cfg_.Profiles[(size_t)p].first];
+        const int32_t id = pick[(size_t)p][(size_t)i];
+        if (id < 0) continue;
+        ScoredEndpoint se = Scored(id, score[(size_t)p][(size_t)i], endpoints, pos_of_id, "picked");
+        se.TieCount = ties[(size_t)p][(size_t)i];
+        if (with_match) se.PrefixMatch = PrefixCacheMatchInfo{match[(size_t)p][(size_t)i], nh[(size_t)i], (uint16_t)g.block_tokens};
+        pr.TargetEndpoints.push_back(se);
+      }
+    }
+    if (cfg_.PrefixMatchInfo && !with_match) {  // the in-flight form: the index is the one the batch was scored against
+      TargetRuns truns((size_t)n);
+      for (int i = 0; i < n; i++)
+        for (auto& kv : got[(size_t)rows[i]]) truns[(size_t)i].emplace_back(kv.first, &kv.second);
+      FillTargetInfo(truns, rows, requests, endpoints, ids, hashes.data(), nh.data(), packed, g);
+    }
   }
 
   // PreRequest with several profiles: the primary profile's target, then the "prefill" profile's, recorded in the prefix index
@@ -1577,13 +1700,13 @@ class Scheduler {
         load_req.push_back(r);
       }
     }
-    if (!last_.hashes.empty()) {
+    if (!last_.hashes.empty() && !inorder_index_) {  // (in order against the index: ScheduleBatch committed the batch already)
       const int32_t* picks[2] = {primary.data(), prefill.data()};
       Check(eppscore_commit_picks_profiles(eng_, R, has_prefill ? 2 : 1, picks, last_.hashes.data(), last_.nh.data(), last_.stride,
                                            LruCapacities().data(), 0, 0, nullptr),
             "eppscore_commit_picks_profiles");
     }
-    if (inflight_ && (int)last_.size.size() == R && !load_ep.empty()) {
+    if (inflight_ && !inorder_ && (int)last_.size.size() == R && !load_ep.empty()) {  // (in order: ScheduleBatch counted them)
       const std::vector<int64_t> est = EstimateTokens(R, last_.size.data(), last_.hint.data(), last_.chars.data());
       std::vector<int64_t> tok(load_ep.size());
       for (size_t i = 0; i < load_ep.size(); i++) tok[i] = est[(size_t)load_req[i]];

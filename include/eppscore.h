@@ -368,7 +368,8 @@ int32_t eppscore_schedule_batch_topk_wide(struct eppscore_engine *e, const eppsc
  * holds max_endpoints endpoints (8192 needs the non-portable cluster size 16).
  * Not ordered: the prefix index (request r+1 does not see the blocks request r adds; commit after the call, or use
  * eppscore_schedule_batch_inorder_index), the latency scorer's running queues (use eppscore_schedule_batch_inorder_latency),
- * top-k lists, several profiles, and requests on other GPU shards (each engine orders its own batch).
+ * top-k lists, several profiles (eppscore_schedule_batch_inorder_profiles), and requests on other GPU shards (each engine orders
+ * its own batch).
  * ERR_INVALID before anything is launched: a profile 0 with the latency scorer, a current snapshot that supplies
  * inflight_tokens, dense_feat / scores_out / match_blocks / pred_out / filter_mask_out set, and what eppscore_schedule_batch
  * refuses.  ERR_NO_SNAPSHOT before eppscore_set_snapshot. */
@@ -407,8 +408,8 @@ typedef struct eppscore_inorder_index {
  * requests in order: each request's blocks are probed up to the first miss, every endpoint's thread counts the hit blocks whose
  * set holds it, the request is scored and picked as in eppscore_schedule_batch_inorder, and the CTA that owns the pick runs the
  * index's commit program for that one Add before the cluster barrier that the next request's probes wait for.
- * Not covered: several picks per request (the "prefill" profile's Add), several profiles and top-k lists, the latency scorer's
- * running queues (eppscore_schedule_batch_inorder_latency with x), and replication across GPU shards (each engine commits its own batch inside the call; replaying an
+ * Not covered: several picks per request and several profiles (eppscore_schedule_batch_inorder_profiles), top-k lists, the
+ * latency scorer's running queues (eppscore_schedule_batch_inorder_latency with x), and replication across GPU shards (each engine commits its own batch inside the call; replaying an
  * all-gathered commit stream on top would apply its commits twice, so sharding.gather_commit_stream belongs to the
  * batch-wide path).  ERR_INVALID: x NULL or a wrong struct_size, and what eppscore_schedule_batch_inorder refuses. */
 int32_t eppscore_schedule_batch_inorder_index(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens,
@@ -498,6 +499,49 @@ int32_t eppscore_schedule_batch_profiles(struct eppscore_engine *e, const eppsco
  * NULL arrays with k > 0. */
 int32_t eppscore_schedule_batch_profiles_topk(struct eppscore_engine *e, const eppscore_batch *b, int32_t n_runs,
                                               const eppscore_profile_run *runs, const eppscore_topk *topk);
+
+/* The arrival-order side of eppscore_schedule_batch_inorder_profiles. */
+typedef struct eppscore_inorder_profiles {
+  int32_t struct_size;               /* sizeof(eppscore_inorder_profiles) */
+  int32_t index;                     /* 0: the in-flight form; 1: also ordered against the prefix index, committing as it goes */
+  int32_t primary_run;               /* the run whose pick gates PreRequest and receives the first Add */
+  int32_t prefill_run;               /* -1, or the run whose pick receives the second Add (approximateprefix/plugin.go:180-183) */
+  const uint8_t *run_mask;           /* optional [R] where b->location says: bit i = run i runs for request r (ProfileHandler.Pick);
+                                        NULL = every run for every request */
+  const int32_t *lru_capacity;       /* HOST [M] CacheNumBlocks (index form), NULL/<=0 = default; NULL under capture */
+  uint16_t *pick_match[EPPSCORE_MAX_PROFILES]; /* optional per run [R]: matchBlocks at that run's pick before request r's Adds */
+} eppscore_inorder_profiles;
+
+/* Several profiles in arrival order (prefill/decode disaggregation): every output (each run's pick / pick_score / tie_count and
+ * pick_match, total_blocks, hashes_out), the in-flight counters and, in the index form, the whole prefix index afterwards (every
+ * LRU oldest -> newest, every set, len(hashToPods)) equal, bit for bit, what this loop gives:
+ *     for r in 0 .. R-1:
+ *         eppscore_schedule_batch_profiles(request r alone, request_base = b->request_base + r,
+ *                                          the runs whose bit is set in run_mask[r]; the others get pick -1)
+ *         if pick[primary_run][r] >= 0:                  (the reference runs no PreRequest when scheduling fails)
+ *             pick_match[i][r] = eppscore_prefix_match(request r's hashes, at pick[i][r])   for every run i that picked
+ *             eppscore_inflight_add(one entry per run that picked, tokens[r] each)         (inflightload/producer.go:106-119)
+ *             [index] eppscore_commit_picks_profiles(1, {pick[primary_run][r], pick[prefill_run][r]}, ..., x->lru_capacity)
+ * pick_match is 0 where the loop records none.  Every run of request r is scored against what requests 0..r-1 left; none sees
+ * request r's own Adds.  Two runs on one endpoint count it twice and Add twice, as the reference does.  Run i draws its
+ * stochastic picks and seeded ties with its profile's derived seed, as eppscore_schedule_batch_profiles does.  With one run,
+ * primary_run 0 and prefill_run -1 the outputs equal eppscore_schedule_batch_inorder (index 0) or
+ * eppscore_schedule_batch_inorder_index (index 1) on that profile.
+ * Locations, slicing, the capture rule (one call outside a capture first; in the index form a reserved index), the room per slice
+ * (in the index form: the slice's Σ n_hashes once per Add a request can make) and the ordering as a producer update and an
+ * index mutation are those of the single-profile in-order calls.  Per slice: the match rows (in-flight form) or the hash stage
+ * (index form), each run's candidate min / max where its profile reads them, then one thread-block cluster walks the requests:
+ * each thread scores its endpoint once per run, in that run's profile order, and the CTAs publish one winner per run behind the
+ * request's one cluster barrier.  The walk stages Σ n_scorers request-independent terms per thread in shared memory (with the
+ * index's commit state in the index form): runs that do not fit the device get ERR_CAPACITY before any launch.
+ * ERR_INVALID before any launch: x NULL or a wrong struct_size, index outside {0, 1}, what eppscore_schedule_batch_profiles
+ * refuses, primary_run or prefill_run out of range or equal, a run with scores_out, pred_out or filter_mask_out, a run whose
+ * profile has the latency scorer or device filters, dense_feat or match_blocks set, and a snapshot that supplies
+ * inflight_tokens.  ERR_NO_SNAPSHOT before eppscore_set_snapshot.
+ * Not covered: top-k lists, the latency scorer's running queues, device filters, and order across GPU shards. */
+int32_t eppscore_schedule_batch_inorder_profiles(struct eppscore_engine *e, const eppscore_batch *b, const int64_t *tokens,
+                                                 int32_t n_runs, const eppscore_profile_run *runs,
+                                                 const eppscore_inorder_profiles *x);
 
 /* ---- stand-alone stages (same kernels; for parity tests and hosts that only want one stage) ---- */
 /* hashPrompt for R prompts (hashing.go:34-98). hashes_out [R*max_blocks], n_hashes_out [R]. */
